@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- the headline measurement (BASELINE.json metric) of the B200-native LightCTR hot path.
+"""bench.py -- the headline measurement of the H100-native LightCTR hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload fm_c2|ffm_c3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload fm_c2|ffm_c3] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path (gather -> interaction -> loss -> scatter-add -> updater) over one batch of
@@ -37,7 +37,7 @@ N_FIELDS = 39
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, gpu_index=0, period_ms=100):
         super().__init__(daemon=True)
@@ -105,8 +105,8 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def measured_tensor_peak():
@@ -115,7 +115,7 @@ def measured_tensor_peak():
         d = json.load(open(p))
         if "bf16_tflops" in d:
             return d["bf16_tflops"], "measured burst cuBLAS bf16 (MEASURED_PEAKS.json)"
-    return 1600.0, "fallback (B200_PROFILING.md)"
+    return 989.0, "H100 SXM data sheet (dense bf16)"
 
 
 def make_batches(wl, n_batches, seed_offset=0):
@@ -197,6 +197,37 @@ def ncu_traffic(wname, kernel):
     return None, None
 
 
+DUMP_BYTES = 64 << 20  # everything --dump-outputs writes, .npy headers included
+
+
+def dump_outputs(ctx, wl, out_dir):
+    """--dump-outputs: what the last timed step left in the model, as .npy files in out_dir, DUMP_BYTES in all.  A training
+    step's result is the updated model: NFM's dense layers in full (mlp<l>_weight.npy [out][in], mlp<l>_bias.npy, float32);
+    W.npy and V.npy (float32) hold the embedding bias and embedding row of every feature when the tables fit the rest of
+    the budget, else of a fixed sample of features (the same ids every run: seeded, sorted ascending), whose ids are in
+    feature_ids.npy (float64, counted in the budget).  The benchmark's inputs are seeded, so two builds run with the same
+    arguments can be compared file for file."""
+    out = {}
+    if wl["model"] == "nfm":
+        dims = [wl["k"]] + list(wl["hidden"]) + [1]
+        for li in range(len(dims) - 1):
+            w, b = ctx.mlp_download(li, dims[li], dims[li + 1])
+            out["mlp%d_weight" % li], out["mlp%d_bias" % li] = w.reshape(dims[li + 1], dims[li]), b
+    W, V = ctx.download_params()
+    F = W.size
+    V = V.reshape(F, -1)
+    header = 128  # bytes of a .npy header for these shapes
+    room = DUMP_BYTES - sum(a.nbytes for a in out.values()) - header * (len(out) + 3)
+    n = min(F, room // (4 * (V.shape[1] + 1) + 8))  # per feature: its V row and W entry (float32) and its id (float64)
+    if n <= 0:
+        raise SystemExit("bench.py: --dump-outputs: the dense layers alone exceed %d bytes" % DUMP_BYTES)
+    ids = np.arange(F) if n == F else np.sort(np.random.default_rng(20240).choice(F, n, replace=False))
+    out.update(W=W[ids], V=V[ids], feature_ids=ids.astype(np.float64))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a))
+
+
 def check_against_oracle(ctx, wl, batch, Fc):
     """--check: step 0 of the benched batch against the CPU oracle from the same (downloaded) parameters."""
     from oracle import api
@@ -220,8 +251,9 @@ def check_against_oracle(ctx, wl, batch, Fc):
     return out
 
 
-def measure(wname, wl, args, rank, world, local_rank, dist, steps, warmup, do_e2e=True, split_global=0):
-    """One workload on this process group: K device-timed steps on resident batches (+ the end-to-end arm)."""
+def measure(wname, wl, args, rank, world, local_rank, dist, steps, warmup, do_e2e=True, split_global=0, dump_dir=None):
+    """One workload on this process group: K device-timed steps on resident batches (+ the end-to-end arm); dump_dir:
+    where to write the model the timed steps left behind (dump_outputs)."""
     import torch
     from lightctr_b200 import capi
     model = {"fm": capi.MODEL_FM, "ffm": capi.MODEL_FFM, "nfm": capi.MODEL_NFM}[wl["model"]]
@@ -264,7 +296,7 @@ def measure(wname, wl, args, rank, world, local_rank, dist, steps, warmup, do_e2
     if args.check and world == 1:
         check = check_against_oracle(ctx, wl_b, batches[0], Fc)
     stream = torch.cuda.ExternalStream(ctx.stream())
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
     do_flush = os.environ.get("LCTR_BENCH_NOFLUSH", "0") != "1"
 
     def one_step(i, timed_events=None):
@@ -272,9 +304,9 @@ def measure(wname, wl, args, rank, world, local_rank, dist, steps, warmup, do_e2
             if do_flush:
                 flush.zero_()
             if world > 1 and do_flush:
-                # the 256 MB flush saturates THIS GPU's memory system for ~80 us; a peer that is already inside its step
-                # would have its NVLink stores into this GPU queue behind it (measured: 3 MB pull / push kernels stretched
-                # from ~10 to ~45 us).  Ranks therefore leave the flush together; the timed region starts after it.
+                # the 256 MB flush saturates THIS GPU's memory system for a while; a peer that is already inside its step
+                # would have its NVLink stores into this GPU queue behind it and its pull / push kernels would stretch.
+                # Ranks therefore leave the flush together; the timed region starts after it.
                 stream.synchronize()
                 dist.barrier()
             if timed_events is not None:
@@ -307,6 +339,8 @@ def measure(wname, wl, args, rank, world, local_rank, dist, steps, warmup, do_e2
         dist.barrier()
     t_wall = time.time() - t_wall0
     launches = ctx.launch_count() - launches0
+    if dump_dir and rank == 0:
+        dump_outputs(ctx, wl, dump_dir)
     ctx.profile(True)
     ctx.profile_read(reset=True)
     for i in range(steps):
@@ -397,9 +431,13 @@ def main():
     ap.add_argument("--check", action="store_true", help="compare step 0 of the benched batch with the CPU oracle")
     ap.add_argument("--batch", type=int, default=0, help="override the workload's rows per GPU per step (sweeps; "
                     "the headline configs are the defaults)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the parameters they produced to DIR/<name>.npy (see dump_outputs)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if args.dump_outputs and world > 1:
+        raise SystemExit("bench.py: --dump-outputs is for one GPU (the tables of N > 1 are sharded over the ranks)")
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     wname = args.workload or "fm_c2"
     wl = dict(WORKLOADS[wname])
@@ -436,7 +474,7 @@ def main():
     if world > 1:
         import torch.distributed as dist
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
-    m = measure(wname, wl, args, rank, world, local_rank, dist, args.steps, args.warmup)
+    m = measure(wname, wl, args, rank, world, local_rank, dist, args.steps, args.warmup, dump_dir=args.dump_outputs)
     value, ms_per_step, prof, B, Fc, det, nnz_mean = m["value"], m["ms_per_step"], m["prof"], m["B"], m["Fc"], m["det"], m["nnz_mean"]
     mlp_bf16 = m["mlp_bf16"]
     k = wl["k"]
@@ -477,7 +515,7 @@ def main():
         tpeak, tsrc = measured_tensor_peak()
         achieved = flops / (ms / cnt * 1e-3) / 1e12
         umma = os.environ.get("LCTR_MLP_UMMA", "1") != "0"
-        roof = {"bound": "tensor", "kernel": ("mlp (nfm_mlp_umma_kernel: tcgen05.mma, TMEM accumulators; + dense Adagrad)" if umma
+        roof = {"bound": "tensor", "kernel": ("mlp (nfm_mlp_umma_kernel: wgmma, register accumulators; + dense Adagrad)" if umma
                                               else "mlp (nfm_mlp_fused_kernel: mma.sync; + dense Adagrad)"), "achieved": achieved, "peak": tpeak,
                 "unit": "TFLOP/s", "frac": achieved / tpeak, "traffic": None, "peak_source": tsrc,
                 "algorithmic_flops_per_launch": flops, "kernel_ms": ms / cnt}
@@ -510,7 +548,7 @@ def main():
                        "kernel_buckets": "kernels_ms / roofline.kernel_ms: a second pass of the same steps with per-launch CUDA events (the timed region carries one event pair per step only)",
                        "batch_per_gpu": B,
                        "global_batch": world * B, "nnz_per_row": n,
-                       **({"mlp": ("bf16 tcgen05.mma with TMEM accumulators, fused fwd+bwd per 128-sample CTA" if os.environ.get("LCTR_MLP_UMMA", "1") != "0"
+                       **({"mlp": ("bf16 wgmma with register accumulators, fused fwd+bwd per 128-sample CTA" if os.environ.get("LCTR_MLP_UMMA", "1") != "0"
                                    else "bf16 mma.sync, fused fwd+bwd per 128-sample tile") if mlp_bf16 else "fp32 reference-order"}
                           if wl["model"] == "nfm" else {}),
                        "backward": bw_desc,

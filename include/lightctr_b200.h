@@ -1,4 +1,4 @@
-/* include/lightctr_b200.h -- the drop-in boundary (C ABI) of the B200-native LightCTR hot path.
+/* include/lightctr_b200.h -- the drop-in boundary (C ABI) of the H100-native LightCTR hot path.
  *
  * The reference (cnkuangshi/LightCTR) has no FFI: its "API" is C++ inheritance
  * (FM_Algo_Abst::Train() fm_algo_abst.h:137, Train_FM_Algo/Train_FFM_Algo/Train_NFM_Algo ctors

@@ -1,4 +1,4 @@
-"""Build the sm_100a shared library (lightctr_b200/lib/liblightctr_b200.so) with nvcc, in-tree.
+"""Build the sm_90a shared library (lightctr_b200/lib/liblightctr_b200.so) with nvcc, in-tree.
 
     python -m lightctr_b200.build [--force] [--verbose]
 """
@@ -14,7 +14,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false: the reference is built without FMA (-mavx only, Makefile:3); keeping mul and add
 # separately rounded keeps per-coordinate updates comparable bit-for-bit.  All kernels here are
 # memory-bound, so contraction would buy nothing.
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
          "-ccbin", "/usr/bin/g++", "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function", "-shared", "-cudart", "shared"]
 
 

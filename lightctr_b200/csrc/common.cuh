@@ -1,4 +1,4 @@
-// lightctr_b200/csrc/common.cuh -- shared device/host helpers for the sm_100a kernels.
+// lightctr_b200/csrc/common.cuh -- shared device/host helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -175,11 +175,11 @@ struct lctr_ctx {
     void* dense_allreduce_user = nullptr;
     int mlp_tm = 0;             // bf16 mode: samples per CTA tile (128 or 64)
     size_t mlp_smem = 0;        // bf16 mode: dynamic shared memory per CTA
-    int mlp_umma = 0;           // bf16 mode: the tcgen05 kernel (mlp_umma.cu) takes this chain
+    int mlp_umma = 0;           // bf16 mode: the wgmma kernel (mlp_umma.cu) takes this chain
     size_t mlp_umma_smem = 0;
     int mlp_has_mask = 0;       // any dropout mask entry == 0
     int mlp_skip_update = 0;    // LCTR_MLP_SKIP_UPDATE=1: leave the dense gradients in place (tests read them)
-    int sm_count = 148;
+    int sm_count = 132;
     int64_t launches = 0;
     const unsigned long long* apply_wait_flags = nullptr;  // multi-GPU owner: flags the sparse apply polls before it starts
     int apply_wait_n = 0;
@@ -230,7 +230,7 @@ __device__ __forceinline__ void red_add_f32(float* addr, float v) {
 __device__ __forceinline__ float4 ldg_f4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 // Gather loads whose ISSUE ORDER matters: as volatile asm they stay where the source puts them (all gathers of a pass
 // back to back), where plain __ldg loads were sunk next to their uses -- one dependent round trip per row instead of
-// one per pass (seen in the SASS of the forward kernel, profiles/README.md).
+// one per pass (visible in the SASS of the forward kernel).
 __device__ __forceinline__ float4 ldg_f4_pinned(const float* p) {
     float4 v;
     asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));

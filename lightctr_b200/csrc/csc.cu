@@ -1,8 +1,7 @@
 // lightctr_b200/csrc/csc.cu -- feature-major view of a batch built ON THE DEVICE at upload, and the
 // atomic-free backward + fused updater that consumes it (cfg.deterministic == 2, the streamed-batch default).
 //
-// Why: the RED scatter of fm.cu issues 17 fp32 atomic adds per nnz and is bound by the L2 atomic units
-// (profiles/README.md: 133 G adds/s, 42 us for 313 K nnz).  Grouping the entries by feature id turns the scatter
+// Why: the RED scatter of fm.cu issues 17 fp32 atomic adds per nnz and is bound by the L2 atomic units.  Grouping the entries by feature id turns the scatter
 // into a segmented reduction: each unique fid's gradient is summed in registers by one lane group and the
 // updater is applied on the spot -- no update_g traffic, no atomics on floats, no touched map, no apply pass.
 // The grouping depends only on the batch (not on the parameters), so it runs on the upload stream and overlaps

@@ -16,8 +16,7 @@
 //     straight into o's key inbox with posted stores + a generation flag (send_keys_kernel).  From then on a row of the
 //     exchange is addressed by p = o * cap_pair + its position in that list, by requester and owner alike: the entries of
 //     the batch are re-indexed to p (remap_entries_kernel), so the cache rows of one owner and the gradient rows for one
-//     owner are CONTIGUOUS and both transfers are long coalesced streams instead of scattered 64 B packets (the first
-//     version of this protocol wrote pulled rows to scattered cache slots: 48 us for the 3 MB of an FM C2 step).
+//     owner are CONTIGUOUS and both transfers are long coalesced streams instead of scattered 64 B packets.
 //   step
 //     1 serve   OWNER-driven pull: I read the key lists my peers posted and WRITE the rows they asked for into their
 //               caches (posted peer stores instead of read round trips), then raise "rows delivered" on each peer
@@ -28,7 +27,7 @@
 //               landed" flags                                                                    (push_rows_kernel)
 //     4 owner   inbox rows are added into update_g with local REDs (waits for the flags)          (merge_kernel)
 //               sparse updater on the shard                                                      (opt.cu)
-// Launches per step: 6; the barriers of the r01 protocol are flags written at the tail of one kernel and polled at the
+// Launches per step: 6; the barriers between the phases are flags written at the tail of one kernel and polled at the
 // head of the next -- no barrier launches, no host involvement.
 #include <stdlib.h>
 #include <string.h>
@@ -102,8 +101,8 @@ __device__ __forceinline__ unsigned long long* flag_ptr(unsigned char* arena, co
     return reinterpret_cast<unsigned long long*>(arena + A.flags) + (size_t)row * kMaxWorld + col;
 }
 // System-scope fences are executed by the few threads that poll / raise flags, never by whole CTAs: membar.sys drains the
-// issuing SM's outstanding peer traffic, and hundreds of CTAs x 256 threads doing it cost ~40 us per kernel (measured: the
-// pull / push kernels of an FM C2 step, 3 MB each, took 46 us with per-thread fences).  The CTA barrier before / after
+// issuing SM's outstanding peer traffic, so hundreds of CTAs x 256 threads doing it would serialise every kernel behind
+// its own fences.  The CTA barrier before / after
 // makes the fence cumulative over the other threads' accesses (PTX memory model: causality order through bar.sync).
 __device__ __forceinline__ void wait_flags(unsigned char* my_arena, const ArenaLayout& A, int row, int world,
                                            unsigned long long value) {
@@ -120,8 +119,8 @@ __device__ __forceinline__ void wait_flags(unsigned char* my_arena, const ArenaL
 __device__ int g_dbg_mode = 0;  // LCTR_DIST_DEBUG bit0: serve_pull skips the row copies (timing experiment only)
 // Blocks fence their stores at DEVICE scope and count in; only the last block (which has observed every other block's
 // count) issues the system-scope fence before raising the flags -- cumulativity carries the other blocks' peer stores
-// along.  One membar.sys per kernel instead of one per CTA: 41 -> 24 us for the FM C2 pull (LCTR_DIST_FENCE=sys restores
-// the per-block system fences).
+// along.  One membar.sys per kernel instead of one per CTA (LCTR_DIST_FENCE=sys restores the per-block system fences; the
+// choice was timed on B200s and has not been re-measured on H100s).
 __device__ int g_block_fence_sys = 0;
 __device__ __forceinline__ void raise_flags_last_block(const PeerTable& P, const ArenaLayout& A, int row, int me, int world,
                                                        unsigned long long value, unsigned int* ctr) {

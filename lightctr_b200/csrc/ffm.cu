@@ -1,4 +1,4 @@
-// lightctr_b200/csrc/ffm.cu -- field-aware FM forward + backward fused per sample, sm_100a.
+// lightctr_b200/csrc/ffm.cu -- field-aware FM forward + backward fused per sample, sm_90a.
 //
 // Reference semantics: Train_FFM_Algo::batchGradCompute / accumWVGrad (train/train_ffm_algo.cpp:51-118):
 //     pred   = sum_i W[f_i] x_i + sum_{i<j} <V[f_i, fld_j], V[f_j, fld_i]> x_i x_j
@@ -276,8 +276,8 @@ __global__ void ffm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint
 // are requested at once -- one bulk copy per row, all completing on ONE mbarrier armed with the chunk's byte count -- so
 // CR whole rows are in flight per CTA at no register cost and without per-thread load instructions, and the gradient
 // phase reads the rows from shared memory again instead of gathering them a second time.
-// (A first version streamed single rows through a 16-stage full/empty ring fed by a producer warp: the two mbarrier
-// hand-shakes per row cost more than the 16 B of work a consumer thread has per row; 510 vs 425 us on C3.)
+// (A ring of single rows fed by a producer warp pays two mbarrier hand-shakes per row, more than the 16 B of work a
+// consumer thread has per row.)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -512,8 +512,8 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
     const int A = Fc * k / vec;
     LCTR_CHECK(A <= 1024, "FFM row of %d slots exceeds one CTA (Fc=%d k=%d)", A, Fc, k);
     const int tpb = std::max(64, (A + 31) / 32 * 32);
-    // TMA bulk reduce-add of whole gradient rows is built but off by default: measured 554 us vs 532 us for the vector
-    // REDs on C3 -- both hit the same L2 reduction rate (~0.75 TB/s of fp32 adds), see profiles/README.md
+    // TMA bulk reduce-add of whole gradient rows is built but off by default: on B200s it was no faster than the vector
+    // REDs (both end in the same L2 reductions); not re-measured on H100s.
     static const bool use_bulk = getenv("LCTR_FFM_BULK") && atoi(getenv("LCTR_FFM_BULK")) == 1;
     const bool bulk = use_bulk && train && vec == 4 && (Fc * k * 4) % 16 == 0;
     const size_t smem = ((size_t)Fc * A * vec * 4 + (size_t)Fc * 4 + 80 * 4 + (size_t)kFfmStage * 10 + 15) / 16 * 16 +
@@ -535,10 +535,9 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
         return 0;
     }
     // LCTR_FFM_TMA=1 selects the TMA-staged kernel (cp.async.bulk rows + mbarrier).  It is parity-green but NOT the
-    // default: ncu (profiles/ncu_r02_ffm_c3_summary.txt) shows both kernels are ISSUE-bound, not memory-bound (C3:
-    // 26 K / 16 K warp instructions per sample, DRAM at 2-3 % of peak); staging whole rows in shared memory cuts the
-    // instruction count by 37 % but leaves 2 CTAs = 4 warps per SM next to the field-pair tile, against 16 warps of the
-    // register-staged kernel: 664 vs 437 us on C3, 6.10 vs 5.74 ms on C5.
+    // default: both kernels are issue-bound rather than memory-bound, and staging whole rows in shared memory cuts the
+    // instruction count but leaves 2 CTAs = 4 warps per SM next to the field-pair tile, against 16 warps of the
+    // register-staged kernel, which was the faster of the two on B200s.  The choice has not been re-measured on H100s.
     static const bool use_tma = getenv("LCTR_FFM_TMA") && atoi(getenv("LCTR_FFM_TMA")) == 1;
     if (use_tma && train && vec == 4 && !bulk) {
         // rows per chunk: as many as leave 3 (narrow rows) or 2 CTAs per SM, at least 40, at most 96

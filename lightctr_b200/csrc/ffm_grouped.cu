@@ -1,7 +1,7 @@
 // lightctr_b200/csrc/ffm_grouped.cu -- feature-grouped (atomic-free) FFM backward with the updater fused in.
 //
 // Why: the fused kernel of ffm.cu scatters every entry's Fc*k-float gradient row with REDs and is bound by the L2
-// reduction rate (~0.75 TB/s of fp32 adds: 532 us on C3, 8.2 ms on C5, profiles/README.md).  The gradient row of an
+// reduction rate of fp32 adds.  The gradient row of an
 // entry i of sample s (field a = fld_i) is
 //     g_i[b] = d_s x_i ( T_s[a][b] - [b == a] x_i R_i[a] ) + l2 c_{i,b} R_i[b]        (ffm.cu header; reference
 //     train_ffm_algo.cpp:81-118), c_{i,b} = cnt_s[b] - [b == a],

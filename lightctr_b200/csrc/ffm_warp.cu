@@ -1,9 +1,8 @@
 // lightctr_b200/csrc/ffm_warp.cu -- the FFM training step (train/train_ffm_algo.cpp:51-118), one WARP per sample.
 //
 // Same factorisation and the same terms as ffm.cu (per-sample field-pair sums T[a][slot] = sum over the sample's entries
-// of field a of x * row[slot]; slot = (target field b, 4-float part)), but organised around the instruction count: ncu
-// showed the CTA-per-sample kernel issue bound at 26 K warp instructions per C3 sample (profiles/ncu_r02_ffm_c3_summary.txt:
-// 39 of 64 threads own a slot, every entry pays a block-wide index staging, shared-memory read-modify-writes of T,
+// of field a of x * row[slot]; slot = (target field b, 4-float part)), but organised around the instruction count: the
+// CTA-per-sample kernel is issue bound (39 of 64 threads own a slot, every entry pays a block-wide index staging, shared-memory read-modify-writes of T,
 // thread-0 scalar work and two __syncthreads per chunk).  Here
 //   * a warp owns a sample and its own T tile in shared memory: no block barrier anywhere in the sample loop;
 //   * lane j reads the (fid, field, x, W[fid]) of entry j of a 32-entry chunk -- the wide sum, the gW REDs and the touched

@@ -1,4 +1,4 @@
-// lightctr_b200/csrc/fm.cu -- FM / NFM embedding gather (forward) and scatter-add (backward), sm_100a.
+// lightctr_b200/csrc/fm.cu -- FM / NFM embedding gather (forward) and scatter-add (backward), sm_90a.
 //
 // Reference semantics: Train_FM_Algo::batchGradCompute / accumWVGrad (train/train_fm_algo.cpp:63-118)
 // and the wide + bi-interaction / accumWideGrad / accumDeepGrad parts of Train_NFM_Algo
@@ -406,7 +406,7 @@ static int fwd_go(lctr_ctx* c, Slot& s, bool nfm, int64_t rb, int64_t re, double
     static const bool want_coalesced = !(getenv("LCTR_FWD_COALESCED") && atoi(getenv("LCTR_FWD_COALESCED")) == 0);
     const bool co = kCoalesced && want_coalesced;
     // coalesced kernel: 4 warps per CTA (its 8 row gathers per pass are all in flight: ~70 registers per thread, and
-    // at batch 4096 / 148 SMs = 27.7 warps per SM every sample must be resident in ONE wave)
+    // at batch 4096 / 132 SMs = 31 warps per SM every sample must be resident in ONE wave)
     const int wpb = co ? 4 : 8;
     const unsigned grid = (unsigned)((re - rb + wpb - 1) / wpb);
     const size_t smem = co ? (size_t)wpb * (K + 2) * 68 * sizeof(float) : (size_t)wpb * 64 * (K + 4) * sizeof(float);

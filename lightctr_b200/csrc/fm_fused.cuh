@@ -1,4 +1,4 @@
-// lightctr_b200/csrc/fm_fused.cuh -- order-free FM step kernels (cfg.deterministic == 0), sm_100a.
+// lightctr_b200/csrc/fm_fused.cuh -- order-free FM step kernels (cfg.deterministic == 0), sm_90a.
 //
 // Reference semantics: Train_FM_Algo::batchGradCompute + accumWVGrad + ApplyGrad (train/train_fm_algo.cpp:63-126).
 // The in-order kernels of fm.cu reproduce the reference's arithmetic SEQUENCE (needed for multi-epoch 1e-5 parity);
@@ -17,11 +17,12 @@
 //                     and state rows, G re-zeroed in the same pass (replaces compact_touched + apply of opt.cu).
 // HBM/L2-bound integer + fp32 work: no tensor cores by design.
 //
-// What bounds the scatter (scripts/lab/fm_lab.cu, profiles/lab_r02_*.txt): fp32 REDs into L2 sustain 430-830 G adds/s when
-// the target rows are spread, but ops on ONE address serialise at ~4-6 ns each -- the hottest id of a Criteo-shaped batch
-// sits in every row, so 4096 rows cost ~25 us however few bytes move (a W-only RED pass takes as long as the full V+W
-// pass).  Hence HOT slots: ids whose multiplicity in a sample of the batch predicts >= ~128 occurrences get kHotRep
-// replica rows (Ghot) that the warps address round-robin; the updater folds the replicas.  The same serialisation hits
+// What bounds the scatter (scripts/lab/fm_lab.cu): fp32 REDs into L2 run at a high rate when the target rows are spread,
+// but ops on ONE address serialise -- the hottest id of a Criteo-shaped batch sits in every row, so the pass costs time in
+// proportion to the rows however few bytes move (a W-only RED pass takes as long as the full V+W pass).  Hence HOT slots:
+// ids whose multiplicity in a sample of the batch predicts >= ~128 occurrences get kHotRep replica rows (Ghot) that the
+// warps address round-robin; the updater folds the replicas.  The threshold and kHotRep were tuned on B200s and have not
+// been re-measured on H100s.  The same serialisation hits
 // plain byte stores, so the mark kernel only writes marks it does not already see set.
 #pragma once
 #include "opt.cuh"
@@ -43,8 +44,7 @@ __device__ __forceinline__ uint32_t ldg_u32_pinned(const uint32_t* p) {
 // ---------------------------------------------------------------------------------------------------------------
 // Each CTA walks a CONTIGUOUS range of entries and keeps a direct-mapped tag table of the ids it has already marked:
 // the hot ids of the small-vocabulary fields recur in every row, and tens of thousands of byte stores (or loads) aimed
-// at the same few 128 B lines serialise in one L2 slice (lab: 30 us of plain stores / 218 us of load-then-store for the
-// 313 K entries of a 4096-row batch); the filter forwards each id once per CTA.
+// at the same few 128 B lines serialise in one L2 slice; the filter forwards each id once per CTA.
 // The mark of id f lives at position (f % 128) * T + f / 128 (T = ceil(F / 128)): ids that are neighbours in value --
 // the dense, hot low end of every field's vocabulary -- land T bytes apart, i.e. in different lines and L2 slices.
 constexpr int kMarkTags = 2048;
@@ -202,7 +202,7 @@ slotmap_assign_kernel(const uint32_t* __restrict__ fid, const int64_t* __restric
 // Persistent warps: warp w of the grid takes samples w, w + NW, w + 2 NW, ...; the row_ptr pairs of its next 32 samples
 // are fetched with one load, and the index loads of sample t+1 are issued before sample t's rows are consumed, so that
 // per sample only ONE dependent round trip (the row gather itself) is exposed instead of three (row_ptr -> indices ->
-// rows: the chain that held every r01 forward variant at 21 us / batch 4096).
+// rows).
 template <int K, bool HAS_VAL, int MODE, bool SAME_IDX, int MINB = 4>
 __global__ void __launch_bounds__(128, MINB)
 fm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ pidx, const uint32_t* __restrict__ gidx,

@@ -1,4 +1,4 @@
-// lightctr_b200/csrc/mlp_umma.cuh -- launch parameters of the tcgen05 dense-layer kernel (mlp_umma.cu)
+// lightctr_b200/csrc/mlp_umma.cuh -- launch parameters of the wgmma dense-layer kernel (mlp_umma.cu)
 #pragma once
 #include <cuda_bf16.h>
 
@@ -20,7 +20,7 @@ struct Dev {
     int x_off[kMaxDense];                   // byte offset of X_l = input of layer l, [128 x in_l] chunk-major; X_0 = z
     int w_off[kMaxDense];                   // byte offset of W_l, [out_l x in_l] chunk-major
     int vec_off[kMaxDense];                 // element offset of layer l in the concatenated bias vector
-    int wl_off, bias_off, part_off, bar_off;
+    int wl_off, bias_off, bar_off;
     unsigned long long* trace;              // LCTR_MLP_UMMA_TRACE=1: clock64 stamps of CTA 0 per phase, else null
 };
 

@@ -1,4 +1,4 @@
-// lightctr_b200/csrc/opt.cu -- sparse per-coordinate updaters (Adagrad / FTRL / Adam), sm_100a.
+// lightctr_b200/csrc/opt.cu -- sparse per-coordinate updaters (Adagrad / FTRL / Adam), sm_90a.
 //
 // Reference: AdagradUpdater_Num::update (util/gradientUpdater.h:139-150), FTRLUpdater::update
 // (:252-273), AdamUpdater_Num::update (util/momentumUpdater.h:187-210), applied by
@@ -87,9 +87,8 @@ compact_touched_kernel(uint8_t* __restrict__ touched, size_t F, uint32_t* __rest
 // (gradient, weight, state of U rows per lane group) are issued before the first update is computed, so one
 // HBM/L2 round trip covers 32/LPR*U rows.  The last block re-arms the list counter.
 // OPT: the updater as a compile-time constant (-1 = decide at run time).  With the five updaters' double-precision
-// divisions and square roots inlined U * (SPL * VEC + 1) times the run-time version is 8.7 K SASS instructions and 177
-// registers: ncu showed `stall no_instruction` (instruction-cache misses) as its top stall and one resident CTA per SM
-// (profiles/ncu_r01_fm_c2_v2_summary.txt).  The VEC = 4 instances are therefore specialised per updater.
+// divisions and square roots inlined U * (SPL * VEC + 1) times the run-time version is a very long kernel with
+// one resident CTA per SM whose top stall is instruction-cache misses.  The VEC = 4 instances are therefore specialised per updater.
 template <int LPR, int VEC, int SPL, int U, int OPT>
 __global__ void __launch_bounds__(256, (OPT >= 0 ? 2 : 1))
 apply_kernel(const uint32_t* __restrict__ list, unsigned int* __restrict__ n_list, unsigned int* __restrict__ done,

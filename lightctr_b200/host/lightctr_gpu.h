@@ -11,7 +11,7 @@
 //                         dl_algo_abst.h:25-246 (minibatch-batched: see the comment above Layer_Base below)
 //     Distributed_Algo_Abst   LightCTR/distributed_algo_abst.h:86-292 (one process per GPU instead of ZeroMQ workers)
 //     GradientUpdater / MomentumUpdater statics   LightCTR/util/gradientUpdater.h:36-42, main.cpp:64-73
-// but every Train()/Predict() lowers to the C ABI of include/lightctr_b200.h (CUDA, sm_100a).  A caller
+// but every Train()/Predict() lowers to the C ABI of include/lightctr_b200.h (CUDA, sm_90a).  A caller
 // such as the reference's main.cpp:144-162,228-253 compiles unchanged against this header inside
 // `namespace lightctr_b200` (see INTEGRATION.md).  Error behaviour follows the reference: print + exit(1)
 // (fm_algo_abst.h:79-82).  Host-side randomness uses libc rand() in the reference's call order

@@ -1,8 +1,8 @@
-// scripts/lab/fm_lab.cu -- kernel lab for the FM step (round 2): times the candidate kernels of
+// scripts/lab/fm_lab.cu -- kernel lab for the FM step: times the candidate kernels of
 // lightctr_b200/csrc/fm_fused.cuh and a family of RED micro-benchmarks on a dumped synthetic batch
 // (scripts/lab/dump_batch.py), with the L2 flushed before every timed launch.  Not part of the product.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -fmad=false -lineinfo -o scripts/lab/fm_lab scripts/lab/fm_lab.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -fmad=false -lineinfo -o scripts/lab/fm_lab scripts/lab/fm_lab.cu
 //   scripts/lab/fm_lab /tmp/lab_F1000000_B4096.bin [K=16]
 #include <algorithm>
 #include <cmath>

@@ -7,11 +7,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-REF_DATA = "/root/reference/data"
-
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -20,9 +18,3 @@ def oracle_api():
     api.build(ref=True)
     return api
 
-
-def has_reference():
-    return os.path.isdir(REF_DATA)
-
-
-needs_reference = pytest.mark.skipif(not has_reference(), reason="/root/reference not present (GPU box)")

@@ -89,8 +89,8 @@ def _emulate(torch, capi, rp, fid, label, W, V, k, layers, act, masks):
     return p.numpy(), [(g[0].numpy(), g[1].numpy()) for g in grads], dz.numpy()
 
 
-# which kernel takes the chain: "umma" = tcgen05 / TMEM (mlp_umma.cu: hidden widths multiples of 64, every layer's dW
-# expressible with M = 128, no dropout mask), "mma" = the mma.sync kernel of mlp_bf16.cu (everything else)
+# which kernel takes the chain: "umma" = wgmma (mlp_umma.cu: hidden widths multiples of 64, no dropout mask), "mma" = the
+# mma.sync kernel of mlp_bf16.cu (everything else)
 @pytest.mark.parametrize("hidden,act_name,rows,masked,kernel", [((64, 32), "sigmoid", 300, False, "mma"),
                                                                 ((256, 128, 64), "sigmoid", 257, False, "umma"),
                                                                 ((256, 128, 64), "tanh", 200, False, "umma"),
@@ -100,7 +100,7 @@ def _emulate(torch, capi, rp, fid, label, W, V, k, layers, act, masks):
 def test_bf16_mlp_matches_emulation(hidden, act_name, rows, masked, kernel, capfd, monkeypatch):
     torch = pytest.importorskip("torch")
     from lightctr_b200 import capi
-    monkeypatch.setenv("LCTR_MLP_UMMA_TRACE", "1")  # the tcgen05 kernel reports its phase timings on stderr when it runs
+    monkeypatch.setenv("LCTR_MLP_UMMA_TRACE", "1")  # the wgmma kernel reports its phase timings on stderr when it runs
     F, k = 3000, 16
     act = capi.ACT_SIGMOID if act_name == "sigmoid" else capi.ACT_TANH
     dims = [k] + list(hidden) + [1]
@@ -134,8 +134,8 @@ def test_bf16_mlp_matches_emulation(hidden, act_name, rows, masked, kernel, capf
     c.close()
 
 
-def test_tcgen05_and_mma_sync_kernels_agree(monkeypatch):
-    """The two tensor-core kernels (mlp_umma.cu: tcgen05.mma + TMEM; mlp_bf16.cu: mma.sync) round at the same points; on the
+def test_wgmma_and_mma_sync_kernels_agree(monkeypatch):
+    """The two tensor-core kernels (mlp_umma.cu: wgmma.mma_async; mlp_bf16.cu: mma.sync) round at the same points; on the
     C4 chain they must agree to a few bf16 ulps of single activations (the sigmoid is 1/(1+2^t) on MUFU in one and
     __expf/__fdividef in the other)."""
     from lightctr_b200 import capi
