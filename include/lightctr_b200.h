@@ -41,6 +41,7 @@ enum { LCTR_OPT_ADAGRAD = 0, LCTR_OPT_FTRL = 1, LCTR_OPT_ADAM = 2, LCTR_OPT_RMSP
        LCTR_OPT_PS_SGD = 5, LCTR_OPT_PS_ADAGRAD = 6, LCTR_OPT_PS_DCASGD = 7, LCTR_OPT_PS_DCASGDA = 8 };
 enum { LCTR_ACT_SIGMOID = 0, LCTR_ACT_TANH = 1 };
 enum { LCTR_MLP_FP32 = 0, LCTR_MLP_BF16 = 1 };
+enum { LCTR_KEYS_DENSE = 0, LCTR_KEYS_HASHED = 1 };
 
 #define LCTR_MAX_LAYERS 8
 
@@ -78,7 +79,11 @@ typedef struct lctr_cfg {
      *     arbitrary order and are accumulated in double precision, so the fp32 result is order-independent.
      *     Whole-slot steps only; FM with k in {4, 8, 16, 32}, FFM with k % 4 == 0 and field_cnt * k <= 512. */
     int32_t deterministic;
-    int32_t reserved0;
+    /* LCTR_KEYS_DENSE (0): fids index the tables directly, feature_cnt = max fid + 1.
+     * LCTR_KEYS_HASHED (1): batches carry uint64_t hashed keys (lctr_upload_batch_keys); the library maps each key to a
+     * table row, creating and initialising rows on first sight.  feature_cnt is then the row CAPACITY (< 2^32 - 1); one
+     * GPU and deterministic = 0 only. */
+    int32_t key_mode;
     uint64_t csc_row_block;
     float ema_rate;           /* GradientUpdater::__global_ema_rate (RMSpropUpdater_Num, gradientUpdater.h:200-233); 0 => 0.99 (main.cpp:66) */
     uint32_t reserved[3];
@@ -110,6 +115,34 @@ int lctr_upload_opt_state(lctr_ctx* ctx, const float* s1, const float* s2);
  * 1.0f (the shipped data).  Indexing is bit-exact w.r.t. the reference parser. */
 int lctr_upload_batch(lctr_ctx* ctx, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr,
                       const uint32_t* fid, const uint16_t* field, const float* val, const int32_t* label);
+
+/* ---- keyed mode (cfg.key_mode = LCTR_KEYS_HASHED) ------------------------------------------- */
+/* Replaces the host-side vocabulary a caller would otherwise build to renumber hashed ids into 0..F-1; the reference
+ * keeps such a map only on its parameter server (size_t keys, created on first touch, distribut/paramserver.h:315-339).
+ * The table rows are what the row-indexed calls see: lctr_upload_params / lctr_download_params and the opt-state
+ * transfers take `capacity` rows (rows not allocated yet read as zero); train_step, predict, eval and the MLP calls work
+ * unchanged.  lctr_upload_batch, lctr_train_batch and lctr_train_batch_async are refused on a keyed context.
+ *
+ * Keyed twin of lctr_upload_batch (same validation of row_ptr and field).  insert = 1 (training): a key seen for the first
+ * time gets the next free row, initialised as W = 0, V = scale * N(0,1) drawn from a hash of (seed, key, element) -- the
+ * values depend on the key only, never on its row or on arrival order; they are NOT the reference's rand() stream -- and
+ * the optimizer state lctr_create gives.  insert = 0 (prediction): unseen keys map to a null row of zeros that is never
+ * updated, i.e. the feature is dropped (predict/fm_predict.cpp:122); lctr_train_step refuses such a slot.  Wide&Deep reads
+ * the first id of each field, which may then be the null row (the reference's server would create a fresh tensor).  A
+ * batch whose new keys exceed the capacity fails naming it: keys inserted before keep their rows, the slot is unusable
+ * until uploaded again.  The key 0xFFFFFFFFFFFFFFFF is reserved. */
+int lctr_upload_batch_keys(lctr_ctx* ctx, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr,
+                           const uint64_t* key, const uint16_t* field, const float* val, const int32_t* label, int insert);
+/* row of each key, -1 when absent; never inserts */
+int lctr_lookup_keys(lctr_ctx* ctx, int64_t n, const uint64_t* keys, int64_t* rows);
+/* row -> key map of rows [0, *n_rows); keys may be NULL to query the count, otherwise it must hold cap >= *n_rows */
+int lctr_download_keys(lctr_ctx* ctx, uint64_t* keys, uint64_t cap, uint64_t* n_rows);
+/* parameters of the given keys (replaces lctr_upload_params for keyed tables).  Absent keys get consecutive rows in
+ * array order (seeding keys[i] in order on a fresh context gives row i) and the optimizer state lctr_create gives; present
+ * keys keep their row and state.  W (n) / V (n * rowlen) may be NULL.  A duplicate key is an error. */
+int lctr_upload_keyed_params(lctr_ctx* ctx, int64_t n, const uint64_t* keys, const float* W, const float* V);
+/* lazy-init parameters of new rows; defaults seed 0, scale 1 / sqrt(k) (the reference's scale, fm_algo_abst.h:62-65) */
+int lctr_set_key_init(lctr_ctx* ctx, uint64_t seed, float scale);
 
 /* ---- the hot path --------------------------------------------------------------------------- */
 /* One reference "batch": forward (gather + interaction [+ MLP]) -> loss -> backward scatter-add ->
@@ -171,7 +204,7 @@ int lctr_mlp_download_grad(lctr_ctx* ctx, int layer, float* dweight, float* dbia
  * export this rank's table handles, gather them, import all peers'. */
 int lctr_ipc_export(lctr_ctx* ctx, void* handles_out, size_t cap, size_t* bytes);
 int lctr_ipc_import(lctr_ctx* ctx, const void* all_handles, size_t bytes_per_rank);
-/* device memory of the context in bytes: table shard + updater state, and (world > 1) the exchange arena, caches and
+/* device memory of the context in bytes: table shard + updater state (+ the key table in keyed mode), and (world > 1) the exchange arena, caches and
  * inboxes -- owner-sharding keeps the second number O(keys of a batch), not O(feature_cnt) */
 int lctr_device_bytes(lctr_ctx* ctx, uint64_t* shard_bytes, uint64_t* exchange_bytes);
 /* Data-parallel dense layers (world > 1, NFM): the per-rank weightDelta / biasDelta of the batch must be summed over
@@ -198,6 +231,18 @@ typedef struct lctr_dataset {
 } lctr_dataset;
 int lctr_load_libffm(const char* path, uint64_t field_cnt_in, uint64_t feature_cnt_in, lctr_dataset** out);
 int lctr_free_dataset(lctr_dataset* d);
+/* the same parser for keyed contexts: ids keep their full %zu width as uint64_t keys (no >= 2^32 rejection) */
+typedef struct lctr_keyed_dataset {
+    int64_t rows, nnz, label_cnt;
+    uint64_t field_cnt;
+    int64_t* row_ptr;
+    uint64_t* key;
+    uint16_t* field;
+    float* val;
+    int32_t* label;
+} lctr_keyed_dataset;
+int lctr_load_libffm_keys(const char* path, uint64_t field_cnt_in, lctr_keyed_dataset** out);
+int lctr_free_keyed_dataset(lctr_keyed_dataset* d);
 /* binary CSR cache of a parsed file: the sscanf-per-token parse is paid once (SURVEY.md 8f-2) */
 int lctr_save_dataset_bin(const lctr_dataset* d, const char* path);
 int lctr_load_dataset_bin(const char* path, lctr_dataset** out);

@@ -18,6 +18,8 @@ PIPE_DEPTH = 3  # LCTR_PIPE_DEPTH: tickets of train_batch_async that may be outs
 OPT_PS_SGD, OPT_PS_ADAGRAD, OPT_PS_DCASGD, OPT_PS_DCASGDA = 5, 6, 7, 8
 ACT_SIGMOID, ACT_TANH = 0, 1
 MLP_FP32, MLP_BF16 = 0, 1
+KEYS_DENSE, KEYS_HASHED = 0, 1
+RESERVED_KEY = (1 << 64) - 1  # the key table's empty marker: never a valid key
 MAX_LAYERS = 8
 ABI_VERSION = 1
 
@@ -29,6 +31,8 @@ SYMBOLS = [
     "lctr_mlp_forward", "lctr_mlp_backward", "lctr_mlp_apply", "lctr_mlp_upload", "lctr_mlp_download", "lctr_mlp_set_mask", "lctr_mlp_download_grad", "lctr_set_dense_allreduce", "lctr_save_checkpoint", "lctr_load_checkpoint",
     "lctr_save_dataset_bin", "lctr_load_dataset_bin", "lctr_eval", "lctr_upload_pred", "lctr_ipc_export", "lctr_ipc_import",
     "lctr_dense_grad_buffer", "lctr_device_bytes", "lctr_load_libffm", "lctr_free_dataset", "lctr_launch_count", "lctr_stream", "lctr_profile", "lctr_profile_read",
+    "lctr_upload_batch_keys", "lctr_lookup_keys", "lctr_download_keys", "lctr_upload_keyed_params", "lctr_set_key_init",
+    "lctr_load_libffm_keys", "lctr_free_keyed_dataset",
 ]
 
 
@@ -40,7 +44,7 @@ class Cfg(C.Structure):
                 ("ftrl_beta", C.c_float), ("ftrl_lambda1", C.c_float), ("ftrl_lambda2", C.c_float),
                 ("n_hidden", C.c_int32), ("hidden", C.c_uint32 * MAX_LAYERS), ("activation", C.c_int32),
                 ("mlp_precision", C.c_int32), ("max_rows", C.c_uint64), ("max_nnz", C.c_uint64), ("rank", C.c_int32),
-                ("world", C.c_int32), ("deterministic", C.c_int32), ("reserved0", C.c_int32),
+                ("world", C.c_int32), ("deterministic", C.c_int32), ("key_mode", C.c_int32),
                 ("csc_row_block", C.c_uint64), ("ema_rate", C.c_float), ("reserved", C.c_uint32 * 3)]
 
 
@@ -48,6 +52,12 @@ class DatasetC(C.Structure):
     _fields_ = [("rows", C.c_int64), ("nnz", C.c_int64), ("label_cnt", C.c_int64), ("feature_cnt", C.c_uint64),
                 ("field_cnt", C.c_uint64), ("row_ptr", C.POINTER(C.c_int64)), ("fid", C.POINTER(C.c_uint32)),
                 ("field", C.POINTER(C.c_uint16)), ("val", C.POINTER(C.c_float)), ("label", C.POINTER(C.c_int32))]
+
+
+class KeyedDatasetC(C.Structure):
+    _fields_ = [("rows", C.c_int64), ("nnz", C.c_int64), ("label_cnt", C.c_int64), ("field_cnt", C.c_uint64),
+                ("row_ptr", C.POINTER(C.c_int64)), ("key", C.POINTER(C.c_uint64)), ("field", C.POINTER(C.c_uint16)),
+                ("val", C.POINTER(C.c_float)), ("label", C.POINTER(C.c_int32))]
 
 
 _lib = None
@@ -105,6 +115,13 @@ def load_library():
     L.lctr_stream.restype = vp
     L.lctr_profile.argtypes = [vp, C.c_int]
     L.lctr_profile_read.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int, C.c_int]
+    L.lctr_upload_batch_keys.argtypes = [vp, C.c_int, i64, i64, vp, vp, vp, vp, vp, C.c_int]
+    L.lctr_lookup_keys.argtypes = [vp, i64, vp, vp]
+    L.lctr_download_keys.argtypes = [vp, vp, C.c_uint64, C.POINTER(C.c_uint64)]
+    L.lctr_upload_keyed_params.argtypes = [vp, i64, vp, f32p, f32p]
+    L.lctr_set_key_init.argtypes = [vp, C.c_uint64, C.c_float]
+    L.lctr_load_libffm_keys.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.POINTER(KeyedDatasetC))]
+    L.lctr_free_keyed_dataset.argtypes = [C.POINTER(KeyedDatasetC)]
     _lib = L
     return L
 
@@ -153,6 +170,37 @@ def load_libffm(path, field_cnt=0, feature_cnt=0):
     return out
 
 
+class KeyedHostDataset:
+    """CSR arrays as produced by lctr_load_libffm_keys: `key` holds the ids at their full 64-bit width."""
+
+    def __init__(self, row_ptr, key, field, val, label, field_cnt):
+        self.row_ptr = np.ascontiguousarray(row_ptr, np.int64)
+        self.key = np.ascontiguousarray(key, np.uint64)
+        self.field = None if field is None else np.ascontiguousarray(field, np.uint16)
+        self.val = None if val is None else np.ascontiguousarray(val, np.float32)
+        self.label = np.ascontiguousarray(label, np.int32)
+        self.field_cnt = int(field_cnt)
+
+    rows = property(lambda self: len(self.row_ptr) - 1)
+    nnz = property(lambda self: len(self.key))
+
+
+def load_libffm_keys(path, field_cnt=0):
+    """The libffm parser of load_libffm with 64-bit ids, for keyed contexts."""
+    L = load_library()
+    dp = C.POINTER(KeyedDatasetC)()
+    _chk(L.lctr_load_libffm_keys(path.encode(), field_cnt, C.byref(dp)))
+    d = dp.contents
+    n, r, lc = d.nnz, d.rows, d.label_cnt
+    out = KeyedHostDataset(np.ctypeslib.as_array(d.row_ptr, (r + 1,)).copy(),
+                           np.ctypeslib.as_array(d.key, (max(n, 1),))[:n].copy(),
+                           np.ctypeslib.as_array(d.field, (max(n, 1),))[:n].copy(),
+                           np.ctypeslib.as_array(d.val, (max(n, 1),))[:n].copy(),
+                           np.ctypeslib.as_array(d.label, (max(lc, 1),))[:lc].copy(), d.field_cnt)
+    L.lctr_free_keyed_dataset(dp)
+    return out
+
+
 def _dataset_from_c(d):
     n, r, lc = d.nnz, d.rows, d.label_cnt
     return HostDataset(np.ctypeslib.as_array(d.row_ptr, (r + 1,)).copy(),
@@ -191,7 +239,8 @@ class Context:
     def __init__(self, model, feature_cnt, factor_cnt, field_cnt=0, optimizer=OPT_ADAGRAD, lr=0.05, l2=0.001,
                  minibatch_size=0, momentum=0.8, momentum_adam2=0.999, hidden=(), activation=ACT_SIGMOID,
                  mlp_precision=MLP_FP32, device=0, rank=0, world=1, deterministic=0, csc_row_block=0, max_rows=0,
-                 max_nnz=0, ema_rate=0.99):
+                 max_nnz=0, ema_rate=0.99, key_mode=KEYS_DENSE):
+        """key_mode=KEYS_HASHED: batches carry uint64 keys (upload_batch_keys) and feature_cnt is the row capacity."""
         L = load_library()
         cfg = Cfg()
         cfg.abi_version = ABI_VERSION
@@ -207,6 +256,7 @@ class Context:
         cfg.rank, cfg.world = rank, world
         cfg.deterministic, cfg.csc_row_block = deterministic, csc_row_block
         cfg.max_rows, cfg.max_nnz = max_rows, max_nnz
+        cfg.key_mode = key_mode
         self.cfg = cfg
         self.h = C.c_void_p()
         _chk(L.lctr_create(C.byref(cfg), C.byref(self.h)))
@@ -262,6 +312,41 @@ class Context:
         _chk(self.L.lctr_upload_batch(self.h, slot, rows, nnz, *[_p(a) for a in keep]))
         self.sync()  # host arrays may be pageable temporaries
         self.slot_rows[slot] = rows
+
+    def upload_batch_keys(self, slot, row_ptr, key, field, val, label, insert=True):
+        """keyed twin of upload_batch: key (uint64) per entry; insert=False maps unseen keys to the null row"""
+        rows, nnz = len(row_ptr) - 1, len(key)
+        keep = [np.ascontiguousarray(row_ptr, np.int64), np.ascontiguousarray(key, np.uint64),
+                None if field is None else np.ascontiguousarray(field, np.uint16),
+                None if val is None else np.ascontiguousarray(val, np.float32), np.ascontiguousarray(label, np.int32)]
+        self.slot_rows[slot] = 0
+        _chk(self.L.lctr_upload_batch_keys(self.h, slot, rows, nnz, *[_p(a) for a in keep], 1 if insert else 0))
+        self.sync()
+        self.slot_rows[slot] = rows
+
+    def lookup_keys(self, keys):
+        """row of each key (int64), -1 where absent"""
+        k = np.ascontiguousarray(keys, np.uint64)
+        out = np.empty(len(k), np.int64)
+        _chk(self.L.lctr_lookup_keys(self.h, len(k), _p(k), _p(out)))
+        return out
+
+    def download_keys(self):
+        """row -> key map (uint64) of the rows in use"""
+        n = C.c_uint64()
+        _chk(self.L.lctr_download_keys(self.h, None, 0, C.byref(n)))
+        out = np.empty(n.value, np.uint64)
+        _chk(self.L.lctr_download_keys(self.h, _p(out), len(out), C.byref(n)))
+        return out[:n.value]
+
+    def upload_keyed_params(self, keys, W=None, V=None):
+        k = np.ascontiguousarray(keys, np.uint64)
+        W = None if W is None else np.ascontiguousarray(W, np.float32)
+        V = None if V is None else np.ascontiguousarray(V, np.float32)
+        _chk(self.L.lctr_upload_keyed_params(self.h, len(k), _p(k), _p(W), _p(V)))
+
+    def set_key_init(self, seed, scale):
+        _chk(self.L.lctr_set_key_init(self.h, seed, scale))
 
     def upload_dataset(self, slot, ds, all_ones_as_null=True):
         val = ds.val
@@ -380,16 +465,18 @@ class Context:
         _chk(self.L.lctr_mlp_set_mask(self.h, layer, m.ctypes.data))
 
     PROF_NAMES = ["fm_forward", "fm_backward_red", "apply", "ffm_fused", "fm_backward_csc", "mlp", "dist_mark", "dist_compact",
-                  "dist_pull", "dist_push", "dist_barrier0", "dist_merge", "dist_barrier1", "csc_build", "fm_fused", "apply_compact"]
+                  "dist_pull", "dist_push", "dist_barrier0", "dist_merge", "dist_barrier1", "csc_build", "fm_fused", "apply_compact",
+                  "keys_translate"]
 
     def profile(self, enable=True):
         _chk(self.L.lctr_profile(self.h, 1 if enable else 0))
 
     def profile_read(self, reset=True):
-        ms = (C.c_double * 16)()
-        cnt = (C.c_int64 * 16)()
-        _chk(self.L.lctr_profile_read(self.h, ms, cnt, 16, 1 if reset else 0))
-        return {self.PROF_NAMES[i]: (ms[i], cnt[i]) for i in range(16) if cnt[i] > 0}
+        n = len(self.PROF_NAMES)
+        ms = (C.c_double * n)()
+        cnt = (C.c_int64 * n)()
+        _chk(self.L.lctr_profile_read(self.h, ms, cnt, n, 1 if reset else 0))
+        return {self.PROF_NAMES[i]: (ms[i], cnt[i]) for i in range(n) if cnt[i] > 0}
 
     def ipc_export(self):
         n = C.c_size_t()

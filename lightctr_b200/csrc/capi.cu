@@ -174,6 +174,14 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
     LCTR_CHECK(cfg->model >= LCTR_MODEL_FM && cfg->model <= LCTR_MODEL_WND, "lctr_create: bad model %d", cfg->model);
     LCTR_CHECK(cfg->optimizer >= LCTR_OPT_ADAGRAD && cfg->optimizer <= LCTR_OPT_PS_DCASGDA, "lctr_create: bad optimizer %d",
                cfg->optimizer);
+    LCTR_CHECK(cfg->key_mode == LCTR_KEYS_DENSE || cfg->key_mode == LCTR_KEYS_HASHED, "lctr_create: bad key_mode %d", cfg->key_mode);
+    if (cfg->key_mode == LCTR_KEYS_HASHED) {
+        // the owner map of several GPUs would have to be keyed too; exact-order modes build their feature-major view on
+        // the host from host ids, which a keyed upload does not have
+        LCTR_CHECK(cfg->world <= 1, "lctr_create: keyed mode is single-GPU (world %d)", cfg->world);
+        LCTR_CHECK(cfg->deterministic == 0, "lctr_create: keyed mode needs deterministic = 0 (got %d)", cfg->deterministic);
+        LCTR_CHECK(cfg->feature_cnt > 0 && cfg->feature_cnt < (1ull << 32) - 1, "lctr_create: keyed capacity (feature_cnt) out of range");
+    }
     LCTR_CHECK(cfg->feature_cnt > 0 && cfg->feature_cnt < (1ull << 32), "lctr_create: feature_cnt out of range");
     LCTR_CHECK(cfg->factor_cnt > 0, "lctr_create: factor_cnt must be > 0");
     LCTR_CHECK(cfg->model != LCTR_MODEL_FFM || cfg->field_cnt > 0, "lctr_create: FFM needs field_cnt > 0");
@@ -196,7 +204,7 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
         c->cfg.ftrl_alpha = 0.15f; c->cfg.ftrl_lambda1 = 1.0f; c->cfg.ftrl_beta = 1.0f; c->cfg.ftrl_lambda2 = 1.0f;
     }
     if (c->cfg.world <= 0) { c->cfg.world = 1; c->cfg.rank = 0; }
-    c->F = cfg->feature_cnt;
+    c->F = cfg->feature_cnt + (cfg->key_mode == LCTR_KEYS_HASHED ? 1 : 0);  // keyed: + the null row of unseen keys
     c->Fl = (c->F + (size_t)c->cfg.world - 1) / (size_t)c->cfg.world;
     LCTR_CHECK(c->cfg.world == 1 || !cfg->deterministic, "lctr_create: deterministic modes are single-GPU only");
     LCTR_CHECK(cfg->deterministic >= 0 && cfg->deterministic <= 2, "lctr_create: deterministic must be 0, 1 or 2");
@@ -251,6 +259,7 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
     if (cfg->model == LCTR_MODEL_NFM || cfg->model == LCTR_MODEL_WND) {
         if (mlp_alloc(c)) { lctr_destroy(c); return 1; }
     }
+    if (cfg->key_mode == LCTR_KEYS_HASHED && keys_alloc(c)) { lctr_destroy(c); return 1; }
     { const char* e = getenv("LCTR_CSC_IN_STEP"); c->csc_in_step = e && e[0] == '1'; }
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     *out = c;
@@ -278,6 +287,7 @@ int lctr_destroy(lctr_ctx* c) {
     dist_free(c);
     fused_free(c);
     csc_scratch_free(c);
+    keys_free(c);
     if (c->h_stats) cudaFreeHost(c->h_stats);
     if (c->h_stat_ring) cudaFreeHost(c->h_stat_ring);
     for (int p = 0; p < kPipe; p++) {
@@ -310,8 +320,8 @@ int lctr_upload_params(lctr_ctx* c, const float* W, const float* V) {
     LCTR_CHECK(c, "null ctx");
     const int R = c->cfg.world, me = c->cfg.rank;
     if (R == 1) {
-        if (W) LCTR_CUDA(cudaMemcpyAsync(c->W, W, c->F * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-        if (V) LCTR_CUDA(cudaMemcpyAsync(c->V, V, c->F * c->rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        if (W) LCTR_CUDA(cudaMemcpyAsync(c->W, W, api_rows(c) * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        if (V) LCTR_CUDA(cudaMemcpyAsync(c->V, V, api_rows(c) * c->rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     } else {
         std::vector<float> w, v;
         if (W) {
@@ -335,8 +345,8 @@ int lctr_download_params(lctr_ctx* c, float* W, float* V) {
     LCTR_CHECK(c, "null ctx");
     const int R = c->cfg.world, me = c->cfg.rank;
     if (R == 1) {
-        if (W) LCTR_CUDA(cudaMemcpyAsync(W, c->W, c->F * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-        if (V) LCTR_CUDA(cudaMemcpyAsync(V, c->V, c->F * c->rowlen * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        if (W) LCTR_CUDA(cudaMemcpyAsync(W, c->W, api_rows(c) * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        if (V) LCTR_CUDA(cudaMemcpyAsync(V, c->V, api_rows(c) * c->rowlen * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
         return 0;
     }
@@ -362,14 +372,14 @@ int lctr_fill_params(lctr_ctx* c, uint64_t seed, float scale) {
 int lctr_download_opt_state(lctr_ctx* c, float* s1, float* s2) {
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(c->cfg.world == 1, "optimizer-state transfer is single-GPU only");
-    const size_t nv = c->F * c->rowlen;
+    const size_t F = api_rows(c), nv = F * c->rowlen;
     if (s1) {
-        LCTR_CUDA(cudaMemcpyAsync(s1, c->s1W, c->F * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-        LCTR_CUDA(cudaMemcpyAsync(s1 + c->F, c->s1V, nv * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(s1, c->s1W, F * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(s1 + F, c->s1V, nv * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     }
     if (s2 && c->s2W) {
-        LCTR_CUDA(cudaMemcpyAsync(s2, c->s2W, c->F * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-        LCTR_CUDA(cudaMemcpyAsync(s2 + c->F, c->s2V, nv * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(s2, c->s2W, F * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(s2 + F, c->s2V, nv * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     }
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
@@ -377,24 +387,26 @@ int lctr_download_opt_state(lctr_ctx* c, float* s1, float* s2) {
 int lctr_upload_opt_state(lctr_ctx* c, const float* s1, const float* s2) {
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(c->cfg.world == 1, "optimizer-state transfer is single-GPU only (the state arrays are sharded by owner)");
-    const size_t nv = c->F * c->rowlen;
+    const size_t F = api_rows(c), nv = F * c->rowlen;
     if (s1) {
-        LCTR_CUDA(cudaMemcpyAsync(c->s1W, s1, c->F * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-        LCTR_CUDA(cudaMemcpyAsync(c->s1V, s1 + c->F, nv * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(c->s1W, s1, F * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(c->s1V, s1 + F, nv * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     }
     if (s2 && c->s2W) {
-        LCTR_CUDA(cudaMemcpyAsync(c->s2W, s2, c->F * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-        LCTR_CUDA(cudaMemcpyAsync(c->s2V, s2 + c->F, nv * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(c->s2W, s2, F * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(c->s2V, s2 + F, nv * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     }
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }
 
+// fid_resident: the slot's fid array already holds the batch (keyed uploads translate into it before this runs)
 static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr,
-                           const uint32_t* fid, const uint16_t* field, const float* val, const int32_t* label) {
+                           const uint32_t* fid, const uint16_t* field, const float* val, const int32_t* label,
+                           bool fid_resident = false) {
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
-    LCTR_CHECK(rows >= 0 && nnz >= 0 && row_ptr && (nnz == 0 || fid) && (rows == 0 || label), "upload_batch: null input");
+    LCTR_CHECK(rows >= 0 && nnz >= 0 && row_ptr && (nnz == 0 || fid || fid_resident) && (rows == 0 || label), "upload_batch: null input");
     LCTR_CHECK((c->cfg.model != LCTR_MODEL_FFM && c->cfg.model != LCTR_MODEL_WND) || field || nnz == 0,
                "upload_batch: FFM / Wide&Deep need the field array");
     Slot& s = c->slots[slot];
@@ -408,7 +420,7 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
     s.has_field = field != nullptr;
     LCTR_CUDA(cudaMemcpyAsync(s.row_ptr, row_ptr, (size_t)(rows + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
     if (nnz) {
-        LCTR_CUDA(cudaMemcpyAsync(s.fid, fid, (size_t)nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        if (!fid_resident) LCTR_CUDA(cudaMemcpyAsync(s.fid, fid, (size_t)nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
         if (field) LCTR_CUDA(cudaMemcpyAsync(s.field, field, (size_t)nnz * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
         if (val) LCTR_CUDA(cudaMemcpyAsync(s.val, val, (size_t)nnz * sizeof(float), cudaMemcpyHostToDevice, st));
     }
@@ -424,6 +436,7 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
         }
     }
     s.fused_valid = false;
+    s.key_state = SLOT_KEYS_OK;
     if ((fused_supported(c) || c->cfg.world > 1) && rows > 0 && nnz > 0) {  // fused_supported: FM and NFM, one GPU
         // slot map of the batch: the gradient rows of the order-free fused step; on several GPUs also the key set of the
         // pull / push exchange, whose per-owner lists go out right away (posted stores, overlapping the previous step)
@@ -446,6 +459,7 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
 int lctr_upload_batch(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
                       const uint16_t* field, const float* val, const int32_t* label) {
     LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(!c->keys, "lctr_upload_batch: keyed context (key_mode = LCTR_KEYS_HASHED): use lctr_upload_batch_keys");
     // Resident datasets are validated once, on the host: an out-of-range id would otherwise surface as an illegal
     // address inside a gather (the reference indexes W / V unchecked too, fm_algo_abst.h:146-151, but there feature_cnt
     // is derived from the same file).  The streamed entry points (lctr_train_batch[_async]) trust their caller.
@@ -463,6 +477,42 @@ int lctr_upload_batch(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const in
     return upload_batch_on(c, c->stream, slot, rows, nnz, row_ptr, fid, field, val, label);
 }
 
+int lctr_upload_batch_keys(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint64_t* key,
+                           const uint16_t* field, const float* val, const int32_t* label, int insert) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(c->keys, "lctr_upload_batch_keys: the context was not created with key_mode = LCTR_KEYS_HASHED");
+    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
+    LCTR_CHECK(rows >= 0 && nnz >= 0 && row_ptr && (nnz == 0 || key) && (rows == 0 || label), "upload_batch_keys: null input");
+    LCTR_CHECK(row_ptr[0] == 0 && row_ptr[rows] == nnz, "upload_batch_keys: row_ptr must run from 0 to nnz (%lld .. %lld, nnz %lld)",
+               (long long)row_ptr[0], (long long)row_ptr[rows], (long long)nnz);
+    for (int64_t r = 0; r < rows; r++)
+        LCTR_CHECK(row_ptr[r] <= row_ptr[r + 1], "upload_batch_keys: row_ptr decreases at row %lld", (long long)r);
+    for (int64_t i = 0; i < nnz; i++)
+        LCTR_CHECK(key[i] != ~0ull, "upload_batch_keys: key %llu at entry %lld is reserved (the empty marker of the key table)",
+                   (unsigned long long)key[i], (long long)i);
+    if ((c->cfg.model == LCTR_MODEL_FFM || c->cfg.model == LCTR_MODEL_WND) && field)
+        for (int64_t i = 0; i < nnz; i++)
+            LCTR_CHECK(field[i] < c->cfg.field_cnt, "upload_batch_keys: field %u at entry %lld >= field_cnt %u", (unsigned)field[i],
+                       (long long)i, c->cfg.field_cnt);
+    LCTR_CHECK((c->cfg.model != LCTR_MODEL_FFM && c->cfg.model != LCTR_MODEL_WND) || field || nnz == 0,
+               "upload_batch_keys: FFM / Wide&Deep need the field array");
+    Slot& s = c->slots[slot];
+    if (rows > s.cap_rows || nnz > s.cap_nnz) {
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));  // buffers about to be reallocated may still be in use
+        if (slot_reserve(c, s, rows, nnz)) return 1;
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    }
+    s.key_state = SLOT_KEYS_INVALID;  // until the whole upload has succeeded
+    s.fused_valid = false;
+    if (keys_translate(c, key, nnz, insert != 0, s.fid)) return 1;
+    if (upload_batch_on(c, c->stream, slot, rows, nnz, row_ptr, nullptr, field, val, label, true)) {
+        s.key_state = SLOT_KEYS_INVALID;
+        return 1;
+    }
+    s.key_state = insert ? SLOT_KEYS_OK : SLOT_KEYS_LOOKUP;
+    return 0;
+}
+
 static int read_stats(lctr_ctx* c, uint64_t step, float* loss_sum, float* acc_cnt) {
     if (!loss_sum && !acc_cnt) return 0;
     if (c->cfg.world > 1 && dist_check_overflow(c)) return 1;
@@ -478,6 +528,9 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
     Slot& s = c->slots[slot];
+    LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "train_step: slot %d holds no usable batch (its last keyed upload failed)", slot);
+    LCTR_CHECK(s.key_state != SLOT_KEYS_LOOKUP, "train_step: slot %d was uploaded with insert = 0 (lookup only: unseen keys "
+                                                "sit on the null row, which is never trained)", slot);
     LCTR_CHECK(rb >= 0 && re <= s.rows && rb <= re, "train_step: rows [%lld,%lld) outside slot (%lld rows)",
                (long long)rb, (long long)re, (long long)s.rows);
     LCTR_CHECK(c->cfg.world == 1 || c->cfg.minibatch_size > 0,
@@ -557,6 +610,8 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
 
 int lctr_train_batch(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
                      const uint16_t* field, const float* val, const int32_t* label, float* loss_sum, float* acc_cnt) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(!c->keys, "lctr_train_batch: keyed context: upload with lctr_upload_batch_keys, then lctr_train_step");
     if (lctr_upload_batch(c, 0, rows, nnz, row_ptr, fid, field, val, label)) return 1;
     return lctr_train_step(c, 0, 0, rows, loss_sum, acc_cnt);
 }
@@ -687,6 +742,7 @@ static int train_batch_async_graph(lctr_ctx* c, int64_t rows, int64_t nnz, const
 int lctr_train_batch_async(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
                            const uint16_t* field, const float* val, const int32_t* label, uint64_t* ticket) {
     LCTR_CHECK(c && ticket, "null argument");
+    LCTR_CHECK(!c->keys, "lctr_train_batch_async: the streamed pipeline takes no keyed batches (lctr_upload_batch_keys + lctr_train_step)");
     LCTR_CHECK(c->cfg.deterministic != 1, "streamed batches need cfg.deterministic 0 (RED scatter) or 2 (device grouping)");
     if (pipe_init(c)) return 1;
     LCTR_CHECK(c->pipe_issued - c->pipe_waited < (uint64_t)kPipe, "more than %d streamed batches outstanding: call lctr_wait first", kPipe);
@@ -739,6 +795,7 @@ int lctr_predict(lctr_ctx* c, int slot, int quirk_sumvx_slot, float* pctr) {
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
     Slot& s = c->slots[slot];
+    LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "lctr_predict: slot %d holds no usable batch (its last keyed upload failed)", slot);
     int rc = 0;
     if (c->cfg.model == LCTR_MODEL_WND) {
         // Distributed_Algo_Abst::Predict (distributed_algo_abst.h:163-174): a forward pass over the slot; with several

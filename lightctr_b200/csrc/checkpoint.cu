@@ -16,7 +16,7 @@ namespace lctr {
 
 struct CkptHeader {
     char magic[8];  // "LCTRCKP1"
-    int32_t model, optimizer, n_layers, reserved;
+    int32_t model, optimizer, n_layers, reserved;  // reserved: cfg.key_mode (0 for dense tables)
     uint64_t feature_cnt, field_cnt, factor_cnt, adam_iter, step;
     int32_t in[LCTR_MAX_LAYERS + 1], out[LCTR_MAX_LAYERS + 1];
 };
@@ -65,6 +65,7 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
     h.model = c->cfg.model; h.optimizer = c->cfg.optimizer; h.n_layers = c->n_layers;
     h.feature_cnt = c->F; h.field_cnt = c->cfg.field_cnt; h.factor_cnt = c->cfg.factor_cnt;
     h.adam_iter = c->adam_iter; h.step = c->step;
+    h.reserved = c->cfg.key_mode;
     for (int l = 0; l < c->n_layers; l++) { h.in[l] = c->layers[l].in; h.out[l] = c->layers[l].out; }
     int rc = put(f, &h, sizeof(h)) ? 0 : 1;
     const size_t nv = c->F * c->rowlen;
@@ -77,6 +78,12 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
         const size_t nw = (size_t)L.out * L.in;
         rc = dev_to_file(c, f, L.w, nw) || dev_to_file(c, f, L.b, L.out) || dev_to_file(c, f, L.acc_w, nw) ||
              dev_to_file(c, f, L.acc_b, L.out) || dev_to_file(c, f, L.mask, L.out);
+    }
+    if (!rc && c->keys) {  // keyed tables: row count, then the key of every row (the table is rebuilt from it on load)
+        std::vector<uint64_t> keys;
+        rc = keys_download(c, keys);
+        const uint64_t n = keys.size();
+        if (!rc) rc = !(put(f, &n, sizeof(n)) && put(f, keys.data(), n * sizeof(uint64_t)));
     }
     if (fclose(f) != 0) rc = 1;
     if (rc) {
@@ -105,11 +112,12 @@ int lctr_load_checkpoint(lctr_ctx* c, const char* path) {
         return 1;
     }
     bool same = h.model == c->cfg.model && h.optimizer == c->cfg.optimizer && h.n_layers == c->n_layers &&
-                h.feature_cnt == c->F && h.field_cnt == c->cfg.field_cnt && h.factor_cnt == c->cfg.factor_cnt;
+                h.feature_cnt == c->F && h.field_cnt == c->cfg.field_cnt && h.factor_cnt == c->cfg.factor_cnt &&
+                h.reserved == c->cfg.key_mode;
     for (int l = 0; l < c->n_layers && same; l++) same = h.in[l] == c->layers[l].in && h.out[l] == c->layers[l].out;
     if (!same) {
         fclose(f);
-        set_error("checkpoint %s was written by a different trainer (model/optimizer/feature_cnt/field_cnt/factor_cnt/layers)", path);
+        set_error("checkpoint %s was written by a different trainer (model/optimizer/feature_cnt/field_cnt/factor_cnt/layers/key_mode)", path);
         return 1;
     }
     const size_t nv = c->F * c->rowlen;
@@ -123,6 +131,18 @@ int lctr_load_checkpoint(lctr_ctx* c, const char* path) {
         rc = file_to_dev(c, f, L.w, nw) || file_to_dev(c, f, L.b, L.out) || file_to_dev(c, f, L.acc_w, nw) ||
              file_to_dev(c, f, L.acc_b, L.out) || file_to_dev(c, f, L.mask, L.out);
         if (!rc) rc = mlp_bf16_refresh(c, l);
+    }
+    if (!rc && c->keys) {
+        uint64_t n = 0;
+        std::vector<uint64_t> keys;
+        if (!get(f, &n, sizeof(n)) || n > c->F - 1) {
+            rc = 1;
+            set_error("checkpoint %s: missing or inconsistent key section", path);
+        } else {
+            keys.resize(n);
+            if (!get(f, keys.data(), n * sizeof(uint64_t))) { rc = 1; set_error("checkpoint %s: short read of the keys", path); }
+            else rc = keys_restore(c, keys.data(), n);
+        }
     }
     fclose(f);
     if (rc) return 1;

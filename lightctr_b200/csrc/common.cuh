@@ -32,8 +32,8 @@ void set_error(const char* fmt, ...);
 
 constexpr int kNumSlots = 8;
 constexpr int kPipe = LCTR_PIPE_DEPTH;  // streamed pipeline: batches in flight (the last kPipe slots are its buffers)
-constexpr int kNumProf = 16;  // per-kernel timing buckets
-enum { PROF_FM_FWD = 0, PROF_FM_BWD_RED = 1, PROF_APPLY = 2, PROF_FFM_FUSED = 3, PROF_FM_BWD_CSC = 4, PROF_MLP = 5, PROF_DIST_MARK = 6, PROF_DIST_COMPACT = 7, PROF_DIST_PULL = 8, PROF_DIST_PUSH = 9, PROF_DIST_BAR0 = 10, PROF_DIST_MERGE = 11, PROF_DIST_BAR1 = 12, PROF_CSC_BUILD = 13, PROF_FM_FUSED = 14, PROF_APPLY_COMPACT = 15 };
+constexpr int kNumProf = 17;  // per-kernel timing buckets
+enum { PROF_FM_FWD = 0, PROF_FM_BWD_RED = 1, PROF_APPLY = 2, PROF_FFM_FUSED = 3, PROF_FM_BWD_CSC = 4, PROF_MLP = 5, PROF_DIST_MARK = 6, PROF_DIST_COMPACT = 7, PROF_DIST_PULL = 8, PROF_DIST_PUSH = 9, PROF_DIST_BAR0 = 10, PROF_DIST_MERGE = 11, PROF_DIST_BAR1 = 12, PROF_CSC_BUILD = 13, PROF_FM_FUSED = 14, PROF_APPLY_COMPACT = 15, PROF_KEYS = 16 };
 constexpr int kStatRing = 64;
 constexpr int kHotRep = 32;      // fm_fused: replica rows per hot slot of the batch-compact gradient buffer
 constexpr int kHotMax = 2048;    // hot slots per batch (ids beyond the cap stay ordinary slots)
@@ -85,7 +85,11 @@ struct Slot {
     uint32_t *hot_of = nullptr, *hot_slot = nullptr;
     unsigned int* n_hot = nullptr;
     bool fused_valid = false;
+    // keyed mode (keys.cu): SLOT_KEYS_LOOKUP = uploaded with insert = 0 (predict only); SLOT_KEYS_INVALID = the last
+    // keyed upload failed, nothing may run on the slot until it is uploaded again
+    int key_state = 0;
 };
+enum { SLOT_KEYS_OK = 0, SLOT_KEYS_LOOKUP = 1, SLOT_KEYS_INVALID = 2 };
 
 // captured graphs of one slot of the streamed pipeline (capi.cu)
 struct PipeGraph {
@@ -113,6 +117,7 @@ struct MlpLayer {
 
 namespace lctr {
 struct DistState;
+struct KeyTable;
 struct OptParams;
 // slot map scratch + batch-compact gradient buffers of the order-free fused FM step (fm_fused.cu); the slot map part is
 // also what the multi-GPU exchange is keyed by (dist.cu)
@@ -143,6 +148,7 @@ struct lctr_ctx {
     float *cW = nullptr, *cV = nullptr, *cgW = nullptr, *cgV = nullptr;
     lctr::DistState* dist = nullptr;
     lctr::FusedState* fused = nullptr;  // order-free fused FM step (fm_fused.cu)
+    lctr::KeyTable* keys = nullptr;     // keyed mode (keys.cu): key -> row table; F = capacity + 1 (the null row)
     size_t dist_rows = 0;               // world > 1: rows of the exchange index space (gradient / cache rows are indexed by it)
     uint32_t* touch_list = nullptr;      // compacted fids of the step (stage A of the sparse apply)
     unsigned int* n_touch = nullptr;     // list length (device)
@@ -398,5 +404,14 @@ int mlp_bf16_prepare(lctr_ctx* c);
 int mlp_bf16_refresh(lctr_ctx* c, int layer);
 int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor);
 int launch_nfm_mlp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor);
+// keyed mode (keys.cu)
+int keys_alloc(lctr_ctx* c);
+void keys_free(lctr_ctx* c);
+size_t keys_bytes(const lctr_ctx* c);
+int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid);
+int keys_restore(lctr_ctx* c, const uint64_t* row_key, uint64_t n);
+int keys_download(lctr_ctx* c, std::vector<uint64_t>& out);
+// rows of the row-indexed parameter / optimizer-state transfers: F, or the capacity in keyed mode (the null row stays out)
+inline size_t api_rows(const lctr_ctx* c) { return c->keys ? c->F - 1 : c->F; }
 
 }  // namespace lctr

@@ -788,11 +788,12 @@ int lctr_ipc_import(lctr_ctx* c, const void* all_handles, size_t bytes_per_rank)
     return 0;
 }
 
-/* device memory of this context in bytes: table shard + updater state + multi-GPU arena / caches (DESIGN.md 6) */
+/* device memory of this context in bytes: table shard + updater state (+ the key table in keyed mode) + multi-GPU arena /
+ * caches (DESIGN.md 6) */
 int lctr_device_bytes(lctr_ctx* c, uint64_t* shard_bytes, uint64_t* exchange_bytes) {
     LCTR_CHECK(c, "null ctx");
     const bool two = c->s2W != nullptr;
-    if (shard_bytes) *shard_bytes = (uint64_t)(c->Fl * (c->rowlen + 1) * sizeof(float) * (two ? 4 : 3) + c->Fl);
+    if (shard_bytes) *shard_bytes = (uint64_t)(c->Fl * (c->rowlen + 1) * sizeof(float) * (two ? 4 : 3) + c->Fl + keys_bytes(c));
     if (exchange_bytes) *exchange_bytes = (uint64_t)dist_bytes(c);
     return 0;
 }

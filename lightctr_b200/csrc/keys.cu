@@ -1,0 +1,497 @@
+// lightctr_b200/csrc/keys.cu -- keyed mode (cfg.key_mode = LCTR_KEYS_HASHED): batches carry 64-bit hashed feature keys and
+// the library owns the key -> row map, creating and initialising a row the first time a key is met.  The reference has
+// this capability on its distributed path only: its parameter server keys parameters by size_t in an unordered_map and
+// creates a key on first touch (distribut/paramserver.h:315-339, :40-47; distributed_algo_abst.h:70-72).  Here the map is
+// a device hash table and translation happens at upload, so a slot holds ordinary u32 row ids afterwards and every
+// kernel of the dense path runs on it unchanged.
+//
+// Table: open addressing over T = 2^m >= 2 * capacity slots, each a u64 key (~0 = empty, so that key value is reserved)
+// and a u32 row.  Home group = fmix64(key) mod (T / 16); probing walks whole 128-byte groups of 16 keys, one 16-lane
+// tile per key (one coalesced load and two ballots per group).  Slots only ever go from empty to a key, so a group with
+// an empty slot and no match ends a lookup.  fmix64 is the MurmurHash3 finaliser the reference uses for PS sharding
+// (common/hash.h:51-58), without its 32-bit truncation.
+//
+// Upload (insert = 1) is three launches on the ctx stream:
+//   1. key_insert_kernel: a tile that finds no match claims the first empty slot of the group with a 64-bit atomicCAS; the
+//      winner takes a row from an atomicAdd counter and records it in the list of new rows.  A key met again in the same
+//      batch finds the claimed slot with a plain load once the CAS has landed, so batch-local duplicates cost atomics only
+//      while their first claim is in flight, and keys already in the table cost none.
+//   2. key_init_kernel: one warp per new row (FFM rows are Fc * k floats) writes W = 0, V, and the optimizer state
+//      lctr_create gives (0, or the 1e-7 accumulator of the PS Adagrad / DCASGDA rules, paramserver.h:323).
+//   3. key_find_kernel: the translated row of every entry into the slot's fid array -- a second launch, so no tile ever
+//      waits on another tile's row inside a kernel.
+// Lookup-only uploads (insert = 0) run step 3 alone: absent keys map to the null row (index capacity), all zeros and
+// never updated, which drops a feature the model never trained on (the reference's rule, predict/fm_predict.cpp:122).
+//
+// Capacity: the claim that draws row >= capacity stores kNoRow for its key and raises a flag; the upload fails naming the
+// capacity and the slot is unusable until it is uploaded again.  Keys inserted before keep their rows; a key stored with
+// kNoRow fails every later insert-upload that meets it the same way, and looks up as absent.
+//
+// Lazy init of V: V[row][j] = scale * N(0,1), the Box-Muller of fill_params_kernel (capi.cu) with its element counter
+// replaced by fmix64(key) * rowlen + j, and uniforms whose fp32 arithmetic is exact (u1 never reaches 1, where
+// sqrt(-2 log u1) is steepest):
+//     h = fmix64((fmix64(key) * rowlen + j) * 0x9E3779B97F4A7C15 + seed)          (all arithmetic mod 2^64)
+//     u1 = ((h & 0x7fffff) + 0.5) * 2^-23,  u2 = ((h >> 24) & 0xffffff) * 2^-24    (fp32)
+//     V = scale * sqrtf(-2 logf(u1)) * cosf(6.2831853 u2)
+// so the values depend on (seed, key, j) only -- never on the row a key got or on the order keys arrived in.  This is a
+// different stream from the reference's rand()-driven GaussRand (fm_algo_abst.h:62-65); only the scale default,
+// 1 / sqrt(k), is the reference's.
+#include <algorithm>
+#include <vector>
+
+#include "common.cuh"
+
+namespace lctr {
+
+constexpr unsigned long long kEmptyKey = ~0ull;
+constexpr uint32_t kNoRow = 0xffffffffu;
+constexpr int kGroup = 16;  // slots per 128-byte probe group
+
+struct KeyTable {
+    unsigned long long* key = nullptr;      // [T] slot keys, kEmptyKey = free
+    uint32_t* row = nullptr;                // [T] row of the slot's key, kNoRow when the capacity was exhausted
+    unsigned long long* row_key = nullptr;  // [capacity] key of each row
+    unsigned long long* count = nullptr;    // rows claimed (may pass capacity: claims that got no row)
+    unsigned int* flags = nullptr;          // [0] capacity exhausted, [1] table full, [2] new rows of this upload
+    unsigned int* h_flags = nullptr;        // pinned mirror of flags
+    uint32_t* new_rows = nullptr;           // rows created by this upload
+    unsigned long long* d_keys = nullptr;   // staging of the keys of one call
+    int64_t* d_rows = nullptr;              // lookup results / fixed rows of one call
+    size_t cap_scratch = 0;
+    size_t T = 0, cap = 0;
+    unsigned long long seed = 0;
+    float scale = 1.f;
+};
+
+struct KeyView {
+    unsigned long long* key;
+    uint32_t* row;
+    unsigned long long* row_key;
+    unsigned long long* count;
+    unsigned int* flags;
+    uint32_t* new_rows;
+    size_t ngroups, cap;
+};
+
+static KeyView view(const KeyTable* t) {
+    return KeyView{t->key, t->row, t->row_key, t->count, t->flags, t->new_rows, t->T / kGroup, t->cap};
+}
+
+__host__ __device__ __forceinline__ unsigned long long fmix64(unsigned long long k) {
+    k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
+    return k;
+}
+
+// Finds the slot of `key` or claims one for it.  Returns the slot, or -1 when the table has no free slot left on the
+// probe path.  *claimed: this tile's CAS put the key there (all lanes).  Table words are read with ld.cg: other tiles of
+// the same launch insert concurrently, and a stale "empty" is corrected by the CAS that follows it.
+__device__ __forceinline__ long long tile_claim(const KeyView& t, unsigned long long key, int sub, unsigned gmask, bool* claimed) {
+    const size_t home = (size_t)(fmix64(key) & (t.ngroups - 1));
+    *claimed = false;
+    for (size_t step = 0; step < t.ngroups; step++) {
+        const size_t base = ((home + step) & (t.ngroups - 1)) * kGroup;
+        unsigned long long k = __ldcg(t.key + base + sub);
+        while (true) {
+            const unsigned hit = __ballot_sync(gmask, k == key) & gmask;
+            if (hit) return (long long)(base + ((__ffs(hit) - 1) & (kGroup - 1)));
+            const unsigned empty = __ballot_sync(gmask, k == kEmptyKey) & gmask;
+            if (!empty) break;
+            const int leader = __ffs(empty) - 1, lsub = leader & (kGroup - 1);
+            unsigned long long old = 0;
+            if ((int)(threadIdx.x & 31) == leader) old = atomicCAS(t.key + base + lsub, kEmptyKey, key);
+            old = __shfl_sync(gmask, old, leader);
+            if (old == kEmptyKey) { *claimed = true; return (long long)(base + lsub); }
+            if (old == key) return (long long)(base + lsub);
+            if (sub == lsub) k = old;  // lost the slot to another key: look at the group again
+        }
+    }
+    return -1;
+}
+
+// read-only probe (no insert may run concurrently): slot of `key` or -1
+__device__ __forceinline__ long long tile_find(const KeyView& t, unsigned long long key, int sub, unsigned gmask) {
+    if (key == kEmptyKey) return -1;
+    const size_t home = (size_t)(fmix64(key) & (t.ngroups - 1));
+    for (size_t step = 0; step < t.ngroups; step++) {
+        const size_t base = ((home + step) & (t.ngroups - 1)) * kGroup;
+        const unsigned long long k = __ldg(t.key + base + sub);
+        const unsigned hit = __ballot_sync(gmask, k == key) & gmask;
+        if (hit) return (long long)(base + ((__ffs(hit) - 1) & (kGroup - 1)));
+        if (__ballot_sync(gmask, k == kEmptyKey) & gmask) return -1;
+    }
+    return -1;
+}
+
+// 1. claim a slot and a row for every key not yet in the table (one 16-lane tile per key)
+__global__ void __launch_bounds__(256) key_insert_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;  // whole tiles leave together
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const unsigned long long key = keys[i];
+    bool claimed;
+    const long long pos = tile_claim(t, key, sub, gmask, &claimed);
+    if (sub != 0) return;
+    if (pos < 0) { t.flags[1] = 1u; return; }
+    if (!claimed) return;
+    const unsigned long long r = atomicAdd(t.count, 1ull);
+    if (r < t.cap) {
+        t.row[pos] = (uint32_t)r;
+        t.row_key[r] = key;
+        t.new_rows[atomicAdd(&t.flags[2], 1u)] = (uint32_t)r;
+    } else {
+        t.row[pos] = kNoRow;
+        t.flags[0] = 1u;
+    }
+}
+
+// keys with caller-chosen rows (lctr_upload_keyed_params, checkpoint restore): every key gets rows[i]; `record` appends the
+// row to the new-row list for key_init_kernel.
+__global__ void __launch_bounds__(256) key_insert_fixed_kernel(const unsigned long long* __restrict__ keys, const int64_t* __restrict__ rows,
+                                                               int64_t n, KeyView t, int record) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const unsigned long long key = keys[i];
+    bool claimed;
+    const long long pos = tile_claim(t, key, sub, gmask, &claimed);
+    if (sub != 0) return;
+    if (pos < 0) { t.flags[1] = 1u; return; }
+    const uint32_t r = (uint32_t)rows[i];
+    t.row[pos] = r;
+    t.row_key[r] = key;
+    if (record) t.new_rows[atomicAdd(&t.flags[2], 1u)] = r;
+}
+
+__device__ __forceinline__ float key_gauss(unsigned long long hk, size_t rowlen, size_t j, unsigned long long seed, float scale) {
+    const unsigned long long g = hk * (unsigned long long)rowlen + (unsigned long long)j;
+    const unsigned long long h = fmix64(g * 0x9E3779B97F4A7C15ull + seed);
+    // every step exact in fp32 up to logf / cosf; u1 lies in (0, 1) and is never 1
+    const float u1 = ((float)(unsigned)(h & 0x7fffffu) + 0.5f) * 1.1920928955078125e-07f;  // 2^-23
+    const float u2 = (float)(unsigned)((h >> 24) & 0xffffffu) * 5.9604644775390625e-08f;   // 2^-24
+    return scale * sqrtf(-2.0f * logf(u1)) * cosf(6.2831853f * u2);
+}
+
+// 2. lazy init of the rows created by this upload: one warp per row
+__global__ void __launch_bounds__(256) key_init_kernel(KeyView t, float* __restrict__ W, float* __restrict__ V, float* __restrict__ s1W,
+                                                       float* __restrict__ s1V, float* __restrict__ s2W, float* __restrict__ s2V,
+                                                       size_t rowlen, float s1_init, unsigned long long seed, float scale) {
+    const unsigned n = t.flags[2];
+    const int lane = threadIdx.x & 31;
+    const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
+    for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n; w += nwarps) {
+        const uint32_t r = t.new_rows[w];
+        const unsigned long long hk = fmix64(t.row_key[r]);
+        const size_t o = (size_t)r * rowlen;
+        for (size_t j = lane; j < rowlen; j += 32) {
+            V[o + j] = key_gauss(hk, rowlen, j, seed, scale);
+            s1V[o + j] = s1_init;
+            if (s2V) s2V[o + j] = 0.f;
+        }
+        if (lane == 0) {
+            W[r] = 0.f;
+            s1W[r] = s1_init;
+            if (s2W) s2W[r] = 0.f;
+        }
+    }
+}
+
+// 3. translation: MODE 0 -> u32 row per entry into a slot (absent: the null row; kNoRow: capacity flag + null row);
+//    MODE 1 -> int64 row per key, -1 when absent or without a row
+template <int MODE>
+__global__ void __launch_bounds__(256) key_find_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t,
+                                                       uint32_t* __restrict__ fid, int64_t* __restrict__ rows, int insert) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const long long pos = tile_find(t, keys[i], sub, gmask);
+    if (sub != 0) return;
+    const uint32_t r = pos >= 0 ? __ldg(t.row + pos) : kNoRow;
+    if (MODE == 0) {
+        if (r == kNoRow && insert) t.flags[pos >= 0 ? 0 : 1] = 1u;
+        fid[i] = r == kNoRow ? (uint32_t)t.cap : r;
+    } else {
+        rows[i] = r == kNoRow ? -1 : (int64_t)r;
+    }
+}
+
+// parameters of rows given by index: warp per key
+__global__ void __launch_bounds__(256) key_scatter_params_kernel(const int64_t* __restrict__ rows, int64_t n, const float* __restrict__ Win,
+                                                                 const float* __restrict__ Vin, float* __restrict__ W, float* __restrict__ V,
+                                                                 size_t rowlen) {
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x / 32);
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; i < n; i += nwarps) {
+        const size_t r = (size_t)rows[i];
+        if (Vin) for (size_t j = lane; j < rowlen; j += 32) V[r * rowlen + j] = Vin[(size_t)i * rowlen + j];
+        if (Win && lane == 0) W[r] = Win[i];
+    }
+}
+
+static unsigned tile_grid(int64_t n) { return (unsigned)std::max<int64_t>(1, (n * kGroup + 255) / 256); }
+
+static int scratch_reserve(lctr_ctx* c, size_t n) {
+    KeyTable* t = c->keys;
+    if (n <= t->cap_scratch) return 0;
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    const size_t cap = std::max(n, t->cap_scratch + t->cap_scratch / 2);
+    cudaFree(t->d_keys); cudaFree(t->d_rows); cudaFree(t->new_rows);
+    t->d_keys = nullptr; t->d_rows = nullptr; t->new_rows = nullptr; t->cap_scratch = 0;
+    LCTR_CUDA(cudaMalloc((void**)&t->d_keys, cap * sizeof(unsigned long long)));
+    LCTR_CUDA(cudaMalloc((void**)&t->d_rows, cap * sizeof(int64_t)));
+    LCTR_CUDA(cudaMalloc((void**)&t->new_rows, cap * sizeof(uint32_t)));
+    t->cap_scratch = cap;
+    return 0;
+}
+
+static int init_new_rows(lctr_ctx* c, int64_t max_new) {
+    KeyTable* t = c->keys;
+    const float s1 = (c->cfg.optimizer == LCTR_OPT_PS_ADAGRAD || c->cfg.optimizer == LCTR_OPT_PS_DCASGDA) ? 1e-7f : 0.f;
+    const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((max_new + 7) / 8, (int64_t)c->sm_count * 16));
+    key_init_kernel<<<grid, 256, 0, c->stream>>>(view(t), c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, c->rowlen, s1, t->seed, t->scale);
+    c->launches++;
+    LCTR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+static int read_flags(lctr_ctx* c) {
+    KeyTable* t = c->keys;
+    LCTR_CUDA(cudaMemcpyAsync(t->h_flags, t->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+static uint64_t rows_in_use(lctr_ctx* c, int* rc) {
+    unsigned long long n = 0;
+    *rc = cudaMemcpyAsync(&n, c->keys->count, sizeof(n), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
+          cudaStreamSynchronize(c->stream) != cudaSuccess;
+    if (*rc) set_error("key table: cannot read the row count");
+    return std::min<uint64_t>(n, c->keys->cap);
+}
+
+static int check_keys_host(const uint64_t* keys, int64_t n, const char* who) {
+    for (int64_t i = 0; i < n; i++)
+        LCTR_CHECK(keys[i] != kEmptyKey, "%s: key %llu at entry %lld is reserved (the empty marker of the key table)", who,
+                   (unsigned long long)keys[i], (long long)i);
+    return 0;
+}
+
+int keys_alloc(lctr_ctx* c) {
+    KeyTable* t = new KeyTable();
+    c->keys = t;
+    t->cap = c->F - 1;
+    size_t T = kGroup;
+    while (T < 2 * t->cap) T <<= 1;
+    t->T = T;
+    t->scale = (float)(1.0 / sqrt((double)c->cfg.factor_cnt));
+    LCTR_CUDA(cudaMalloc((void**)&t->key, T * sizeof(unsigned long long)));
+    LCTR_CUDA(cudaMalloc((void**)&t->row, T * sizeof(uint32_t)));
+    LCTR_CUDA(cudaMalloc((void**)&t->row_key, t->cap * sizeof(unsigned long long)));
+    LCTR_CUDA(cudaMalloc((void**)&t->count, sizeof(unsigned long long)));
+    LCTR_CUDA(cudaMalloc((void**)&t->flags, 3 * sizeof(unsigned int)));
+    LCTR_CUDA(cudaMallocHost((void**)&t->h_flags, 3 * sizeof(unsigned int)));
+    LCTR_CUDA(cudaMemsetAsync(t->key, 0xff, T * sizeof(unsigned long long), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->row, 0xff, T * sizeof(uint32_t), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->count, 0, sizeof(unsigned long long), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    return 0;
+}
+
+void keys_free(lctr_ctx* c) {
+    KeyTable* t = c->keys;
+    if (!t) return;
+    cudaFree(t->key); cudaFree(t->row); cudaFree(t->row_key); cudaFree(t->count); cudaFree(t->flags);
+    cudaFree(t->new_rows); cudaFree(t->d_keys); cudaFree(t->d_rows);
+    if (t->h_flags) cudaFreeHost(t->h_flags);
+    delete t;
+    c->keys = nullptr;
+}
+
+size_t keys_bytes(const lctr_ctx* c) {
+    const KeyTable* t = c->keys;
+    return t ? t->T * (sizeof(unsigned long long) + sizeof(uint32_t)) + t->cap * sizeof(unsigned long long) : 0;
+}
+
+// keys of one upload -> rows in fid (device, n entries); insert: create and initialise rows for new keys first
+int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid) {
+    KeyTable* t = c->keys;
+    if (n == 0) return 0;
+    if (scratch_reserve(c, (size_t)n)) return 1;
+    LCTR_CUDA(cudaMemcpyAsync(t->d_keys, h_keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    {
+        ProfScope prof(c, PROF_KEYS);
+        if (insert) {
+            key_insert_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t));
+            c->launches++;
+            LCTR_CUDA(cudaGetLastError());
+            if (init_new_rows(c, std::min<int64_t>(n, (int64_t)t->cap))) return 1;
+        }
+        key_find_kernel<0><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0);
+        c->launches++;
+        LCTR_CUDA(cudaGetLastError());
+    }
+    if (read_flags(c)) return 1;
+    LCTR_CHECK(!t->h_flags[1], "key table: no free slot on a probe path (%zu slots for capacity %zu)", t->T, t->cap);
+    LCTR_CHECK(!t->h_flags[0], "key table: capacity of %zu rows (cfg.feature_cnt) exhausted; the batch's new keys do not fit",
+               t->cap);
+    return 0;
+}
+
+static int lookup_dev(lctr_ctx* c, const uint64_t* keys, int64_t n) {
+    KeyTable* t = c->keys;
+    if (scratch_reserve(c, (size_t)n)) return 1;
+    LCTR_CUDA(cudaMemcpyAsync(t->d_keys, keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
+    key_find_kernel<1><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), nullptr, t->d_rows, 0);
+    c->launches++;
+    LCTR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// rebuild from a row -> key array (checkpoint restore): key i gets row i, parameters are left as they are
+int keys_restore(lctr_ctx* c, const uint64_t* row_key, uint64_t n) {
+    KeyTable* t = c->keys;
+    LCTR_CHECK(n <= t->cap, "checkpoint: %llu keyed rows exceed the capacity %zu", (unsigned long long)n, t->cap);
+    LCTR_CUDA(cudaMemsetAsync(t->key, 0xff, t->T * sizeof(unsigned long long), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->row, 0xff, t->T * sizeof(uint32_t), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    const unsigned long long cnt = n;
+    LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
+    if (n) {
+        if (scratch_reserve(c, (size_t)n)) return 1;
+        std::vector<int64_t> rows(n);
+        for (uint64_t i = 0; i < n; i++) rows[i] = (int64_t)i;
+        LCTR_CUDA(cudaMemcpyAsync(t->d_keys, row_key, n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(t->d_rows, rows.data(), n * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
+        key_insert_fixed_kernel<<<tile_grid((int64_t)n), 256, 0, c->stream>>>(t->d_keys, t->d_rows, (int64_t)n, view(t), 0);
+        c->launches++;
+        LCTR_CUDA(cudaGetLastError());
+    }
+    if (read_flags(c)) return 1;
+    LCTR_CHECK(!t->h_flags[1], "checkpoint: key table full while restoring %llu keys", (unsigned long long)n);
+    return 0;
+}
+
+int keys_download(lctr_ctx* c, std::vector<uint64_t>& out) {
+    int rc = 0;
+    const uint64_t n = rows_in_use(c, &rc);
+    if (rc) return 1;
+    out.resize(n);
+    if (n) LCTR_CUDA(cudaMemcpyAsync(out.data(), c->keys->row_key, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+}  // namespace lctr
+
+using namespace lctr;
+
+extern "C" {
+
+int lctr_lookup_keys(lctr_ctx* c, int64_t n, const uint64_t* keys, int64_t* rows) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(c->keys, "lctr_lookup_keys: the context was not created with key_mode = LCTR_KEYS_HASHED");
+    LCTR_CHECK(n >= 0 && (n == 0 || (keys && rows)), "lctr_lookup_keys: null argument");
+    if (n == 0) return 0;
+    if (lookup_dev(c, keys, n)) return 1;
+    LCTR_CUDA(cudaMemcpyAsync(rows, c->keys->d_rows, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int lctr_download_keys(lctr_ctx* c, uint64_t* keys, uint64_t cap, uint64_t* n_rows) {
+    LCTR_CHECK(c && n_rows, "null argument");
+    LCTR_CHECK(c->keys, "lctr_download_keys: the context was not created with key_mode = LCTR_KEYS_HASHED");
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    int rc = 0;
+    const uint64_t n = rows_in_use(c, &rc);
+    if (rc) return 1;
+    *n_rows = n;
+    if (!keys) return 0;
+    LCTR_CHECK(cap >= n, "lctr_download_keys: room for %llu keys, the table has %llu rows", (unsigned long long)cap,
+               (unsigned long long)n);
+    if (n) LCTR_CUDA(cudaMemcpyAsync(keys, c->keys->row_key, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int lctr_upload_keyed_params(lctr_ctx* c, int64_t n, const uint64_t* keys, const float* W, const float* V) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(c->keys, "lctr_upload_keyed_params: the context was not created with key_mode = LCTR_KEYS_HASHED");
+    LCTR_CHECK(n >= 0 && (n == 0 || keys), "lctr_upload_keyed_params: null argument");
+    if (n == 0) return 0;
+    if (check_keys_host(keys, n, "lctr_upload_keyed_params")) return 1;
+    {
+        std::vector<uint64_t> sorted(keys, keys + n);
+        std::sort(sorted.begin(), sorted.end());
+        const auto d = std::adjacent_find(sorted.begin(), sorted.end());
+        LCTR_CHECK(d == sorted.end(), "lctr_upload_keyed_params: key %llu appears more than once", (unsigned long long)*d);
+    }
+    KeyTable* t = c->keys;
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    if (lookup_dev(c, keys, n)) return 1;
+    std::vector<int64_t> rows((size_t)n);
+    LCTR_CUDA(cudaMemcpyAsync(rows.data(), t->d_rows, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    int rc = 0;
+    const uint64_t used = rows_in_use(c, &rc);
+    if (rc) return 1;
+    // absent keys: consecutive rows in array order
+    std::vector<uint64_t> new_keys;
+    std::vector<int64_t> new_rows;
+    for (int64_t i = 0; i < n; i++)
+        if (rows[(size_t)i] < 0) {
+            rows[(size_t)i] = (int64_t)(used + new_keys.size());
+            new_keys.push_back(keys[i]);
+            new_rows.push_back(rows[(size_t)i]);
+        }
+    LCTR_CHECK(used + new_keys.size() <= t->cap, "lctr_upload_keyed_params: %zu new keys do not fit the capacity of %zu rows (%llu in use)",
+               new_keys.size(), t->cap, (unsigned long long)used);
+    const int64_t m = (int64_t)new_keys.size();
+    if (m) {
+        LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(t->d_keys, new_keys.data(), (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(t->d_rows, new_rows.data(), (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
+        key_insert_fixed_kernel<<<tile_grid(m), 256, 0, c->stream>>>(t->d_keys, t->d_rows, m, view(t), 1);
+        c->launches++;
+        LCTR_CUDA(cudaGetLastError());
+        if (init_new_rows(c, m)) return 1;
+        const unsigned long long cnt = used + (uint64_t)m;
+        LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
+        if (read_flags(c)) return 1;
+        LCTR_CHECK(!t->h_flags[1], "lctr_upload_keyed_params: key table full");
+    }
+    if (W || V) {
+        float *dW = nullptr, *dV = nullptr;
+        LCTR_CUDA(cudaMemcpyAsync(t->d_rows, rows.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
+        if (W) {
+            LCTR_CUDA(cudaMalloc((void**)&dW, (size_t)n * sizeof(float)));
+            LCTR_CUDA(cudaMemcpyAsync(dW, W, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        }
+        if (V) {
+            LCTR_CUDA(cudaMalloc((void**)&dV, (size_t)n * c->rowlen * sizeof(float)));
+            LCTR_CUDA(cudaMemcpyAsync(dV, V, (size_t)n * c->rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        }
+        const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 7) / 8, (int64_t)c->sm_count * 16));
+        key_scatter_params_kernel<<<grid, 256, 0, c->stream>>>(t->d_rows, n, dW, dV, c->W, c->V, c->rowlen);
+        c->launches++;
+        const cudaError_t e = cudaGetLastError();
+        cudaStreamSynchronize(c->stream);
+        cudaFree(dW); cudaFree(dV);
+        LCTR_CUDA(e);
+    }
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int lctr_set_key_init(lctr_ctx* c, uint64_t seed, float scale) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(c->keys, "lctr_set_key_init: the context was not created with key_mode = LCTR_KEYS_HASHED");
+    c->keys->seed = seed;
+    c->keys->scale = scale;
+    return 0;
+}
+
+}  // extern "C"

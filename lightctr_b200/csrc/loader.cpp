@@ -71,10 +71,20 @@ inline bool fast_label(const char* p, int* y, int* nchar) {
     return true;
 }
 
-}  // namespace
+// The parse itself, shared by the dense and the keyed loader.  Id = uint32_t: ids >= 2^32 are an error (the dense
+// tables are indexed by them); Id = uint64_t: ids keep the full %zu width (keyed mode hashes them into rows).
+template <typename Id>
+struct Parsed {
+    std::vector<int64_t> row_ptr{0};
+    std::vector<Id> ids;
+    std::vector<uint16_t> fields;
+    std::vector<float> vals;
+    std::vector<int32_t> labels;
+    uint64_t feature_cnt = 0, field_cnt = 0;
+};
 
-extern "C" int lctr_load_libffm(const char* path, uint64_t field_cnt, uint64_t feature_cnt, lctr_dataset** out) {
-    if (!path || !out) { lctr::set_error("lctr_load_libffm: null argument"); return 1; }
+template <typename Id>
+static int parse_libffm(const char* path, Parsed<Id>& out) {
     FILE* f = fopen(path, "rb");
     if (!f) { lctr::set_error("open file error! (%s)", path); return 1; }  // fm_algo_abst.h:79-82
     std::string buf;
@@ -84,11 +94,13 @@ extern "C" int lctr_load_libffm(const char* path, uint64_t field_cnt, uint64_t f
         while ((n = fread(tmp, 1, sizeof(tmp), f)) > 0) buf.append(tmp, n);
     }
     fclose(f);
-    std::vector<int64_t> row_ptr(1, 0);
-    std::vector<uint32_t> fids;
-    std::vector<uint16_t> fields;
-    std::vector<float> vals;
-    std::vector<int32_t> labels;
+    std::vector<int64_t>& row_ptr = out.row_ptr;
+    std::vector<Id>& fids = out.ids;
+    std::vector<uint16_t>& fields = out.fields;
+    std::vector<float>& vals = out.vals;
+    std::vector<int32_t>& labels = out.labels;
+    uint64_t& feature_cnt = out.feature_cnt;
+    uint64_t& field_cnt = out.field_cnt;
     int nchar = 0, y = 0;
     size_t fid = 0, fieldid = 0;
     float val = 0;
@@ -116,11 +128,11 @@ extern "C" int lctr_load_libffm(const char* path, uint64_t field_cnt, uint64_t f
                     if (!(sscanf(p, "%zu:%zu:%f%n", &fieldid, &fid, &val, &nchar) >= 2)) break;
                 }
                 p += nchar + 1;
-                if (fid >= (1ull << 32) || fieldid >= (1ull << 16)) {
+                if ((sizeof(Id) < 8 && fid >= (1ull << 32)) || fieldid >= (1ull << 16)) {
                     lctr::set_error("lctr_load_libffm: fid %zu / field %zu exceed the device index types (u32/u16)", fid, fieldid);
                     return 1;
                 }
-                fids.push_back((uint32_t)fid);
+                fids.push_back((Id)fid);
                 fields.push_back((uint16_t)fieldid);
                 vals.push_back(val);
                 if (fid + 1 > feature_cnt) feature_cnt = fid + 1;
@@ -130,27 +142,61 @@ extern "C" int lctr_load_libffm(const char* path, uint64_t field_cnt, uint64_t f
         if (fids.size() == row_start) continue;
         row_ptr.push_back((int64_t)fids.size());
     }
+    return 0;
+}
+
+template <typename T>
+static T* copy_out(const std::vector<T>& v) {
+    T* p = (T*)malloc(sizeof(T) * (v.size() ? v.size() : 1));
+    if (v.size()) memcpy(p, v.data(), sizeof(T) * v.size());
+    return p;
+}
+
+}  // namespace
+
+extern "C" int lctr_load_libffm(const char* path, uint64_t field_cnt, uint64_t feature_cnt, lctr_dataset** out) {
+    if (!path || !out) { lctr::set_error("lctr_load_libffm: null argument"); return 1; }
+    Parsed<uint32_t> r;
+    r.feature_cnt = feature_cnt;
+    r.field_cnt = field_cnt;
+    if (parse_libffm(path, r)) return 1;
     lctr_dataset* d = (lctr_dataset*)calloc(1, sizeof(lctr_dataset));
-    d->rows = (int64_t)row_ptr.size() - 1;
-    d->nnz = (int64_t)fids.size();
-    d->label_cnt = (int64_t)labels.size();
-    d->feature_cnt = feature_cnt;
-    d->field_cnt = field_cnt;
-    d->row_ptr = (int64_t*)malloc(sizeof(int64_t) * row_ptr.size());
-    memcpy(d->row_ptr, row_ptr.data(), sizeof(int64_t) * row_ptr.size());
-    const size_t nn = fids.size() ? fids.size() : 1;
-    d->fid = (uint32_t*)malloc(sizeof(uint32_t) * nn);
-    d->field = (uint16_t*)malloc(sizeof(uint16_t) * nn);
-    d->val = (float*)malloc(sizeof(float) * nn);
-    const size_t nl2 = labels.size() ? labels.size() : 1;
-    d->label = (int32_t*)malloc(sizeof(int32_t) * nl2);
-    if (fids.size()) {
-        memcpy(d->fid, fids.data(), sizeof(uint32_t) * fids.size());
-        memcpy(d->field, fields.data(), sizeof(uint16_t) * fields.size());
-        memcpy(d->val, vals.data(), sizeof(float) * vals.size());
-    }
-    if (labels.size()) memcpy(d->label, labels.data(), sizeof(int32_t) * labels.size());
+    d->rows = (int64_t)r.row_ptr.size() - 1;
+    d->nnz = (int64_t)r.ids.size();
+    d->label_cnt = (int64_t)r.labels.size();
+    d->feature_cnt = r.feature_cnt;
+    d->field_cnt = r.field_cnt;
+    d->row_ptr = copy_out(r.row_ptr);
+    d->fid = copy_out(r.ids);
+    d->field = copy_out(r.fields);
+    d->val = copy_out(r.vals);
+    d->label = copy_out(r.labels);
     *out = d;
+    return 0;
+}
+
+extern "C" int lctr_load_libffm_keys(const char* path, uint64_t field_cnt, lctr_keyed_dataset** out) {
+    if (!path || !out) { lctr::set_error("lctr_load_libffm_keys: null argument"); return 1; }
+    Parsed<uint64_t> r;
+    r.field_cnt = field_cnt;
+    if (parse_libffm(path, r)) return 1;
+    lctr_keyed_dataset* d = (lctr_keyed_dataset*)calloc(1, sizeof(lctr_keyed_dataset));
+    d->rows = (int64_t)r.row_ptr.size() - 1;
+    d->nnz = (int64_t)r.ids.size();
+    d->label_cnt = (int64_t)r.labels.size();
+    d->field_cnt = r.field_cnt;
+    d->row_ptr = copy_out(r.row_ptr);
+    d->key = copy_out(r.ids);
+    d->field = copy_out(r.fields);
+    d->val = copy_out(r.vals);
+    d->label = copy_out(r.labels);
+    *out = d;
+    return 0;
+}
+
+extern "C" int lctr_free_keyed_dataset(lctr_keyed_dataset* d) {
+    if (!d) return 0;
+    free(d->row_ptr); free(d->key); free(d->field); free(d->val); free(d->label); free(d);
     return 0;
 }
 

@@ -1,0 +1,151 @@
+#!/usr/bin/env python
+"""Keyed mode against dense mode on one GPU: the same workload and batches, ids fed as 64-bit keys fmix64(fid) into a keyed
+context of capacity F (cfg.key_mode = LCTR_KEYS_HASHED), alternated with the dense context in one process.
+
+    python scripts/bench_keys.py [--workload fm_c2|ffm_c3|nfm_c4] [--steps K] [--warmup W] [--rounds R]
+
+Prints ONE JSON line:
+  keyed_ms_per_step / dense_ms_per_step   device-timed step (one CUDA-event pair per step, L2 flushed before each step,
+                                          as bench.py times `value`), one entry per round;
+  translate_us_per_batch                  device time of the upload-side insert + lazy init + translate launches (the
+                                          library's per-launch events, L2 not flushed): first upload of each batch
+                                          ("first_sight": new keys get rows; "first_batch": the first one, on an empty
+                                          table) and a second upload of the same batches ("all_known": probes only);
+  table_bytes                             key table (slots of u64 key + u32 row, u64 key per row) and lctr_device_bytes;
+  gpu                                     card name and power limit, read in the same run.
+Writes nothing to the tree.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True  # the tree may be read-only
+
+import numpy as np  # noqa: E402
+
+from bench import N_FIELDS, WORKLOADS, make_batches  # noqa: E402
+
+
+def fmix64(x):
+    """MurmurHash3's 64-bit finaliser (a bijection of uint64)"""
+    k = np.asarray(x, np.uint64).copy()
+    with np.errstate(over="ignore"):
+        k ^= k >> np.uint64(33)
+        k *= np.uint64(0xff51afd7ed558ccd)
+        k ^= k >> np.uint64(33)
+        k *= np.uint64(0xc4ceb9fe1a85ec53)
+        k ^= k >> np.uint64(33)
+    return k
+
+
+def gpu_info():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return out[0] if out else None
+    except Exception:
+        return None
+
+
+def run(wl, batches, keyed, steps, warmup):
+    import torch
+    from lightctr_b200 import capi
+    model = {"fm": capi.MODEL_FM, "ffm": capi.MODEL_FFM, "nfm": capi.MODEL_NFM}[wl["model"]]
+    opt = {"adagrad": capi.OPT_ADAGRAD, "ftrl": capi.OPT_FTRL}[wl["opt"]]
+    F, k, B = wl["F"], wl["k"], wl["batch"]
+    Fc = N_FIELDS if wl["model"] == "ffm" else 0
+    ctx = capi.Context(model, F, k, Fc, optimizer=opt, max_nnz=B * 100, hidden=wl.get("hidden", ()),
+                       mlp_precision=capi.MLP_BF16 if wl["model"] == "nfm" else capi.MLP_FP32,
+                       key_mode=capi.KEYS_HASHED if keyed else capi.KEYS_DENSE)
+    if wl["model"] == "nfm":  # the dense layers as bench.py initialises them
+        rng0 = np.random.default_rng(99)
+        dims = [k] + list(wl["hidden"]) + [1]
+        for li in range(len(dims) - 1):
+            ctx.mlp_upload(li, (rng0.random((dims[li + 1], dims[li]), dtype=np.float32) - 0.5), np.zeros(dims[li + 1], np.float32))
+    out = {}
+    if keyed:  # rows get W = 0, V ~ N(0,1)/sqrt(k) when their key is first uploaded
+        ctx.set_key_init(1234, float(1.0 / np.sqrt(k)))
+        keys = [fmix64(b[1]) for b in batches]
+        ctx.profile(True)
+        per = {}
+        for phase in ("first_sight", "all_known"):
+            per[phase] = []
+            for i, (rp, fid, fld, lab) in enumerate(batches):
+                ctx.profile_read(reset=True)
+                ctx.upload_batch_keys(i, rp, keys[i], fld if Fc else None, None, lab)
+                per[phase].append(ctx.profile_read(reset=True)["keys_translate"][0])
+        ctx.profile(False)
+        out["translate_us_per_batch"] = {"first_sight": 1e3 * float(np.mean(per["first_sight"])),
+                                         "first_batch": 1e3 * per["first_sight"][0],
+                                         "all_known": 1e3 * float(np.mean(per["all_known"])), "batches": len(batches),
+                                         "rows_created": int(len(ctx.download_keys()))}
+        T = 16
+        while T < 2 * F:
+            T *= 2
+        out["table_bytes"] = {"key_table": T * 12 + F * 8, "shard": ctx.device_bytes()[0]}
+    else:
+        ctx.fill_params(1234, float(1.0 / np.sqrt(k)))
+        for i, (rp, fid, fld, lab) in enumerate(batches):
+            ctx.upload_batch(i, rp, fid, fld if Fc else None, None, lab)
+    stream = torch.cuda.ExternalStream(ctx.stream())
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
+    NB = len(batches)
+
+    def step(i, ev=None):
+        with torch.cuda.stream(stream):
+            flush.zero_()
+            if ev:
+                ev[0].record(stream)
+        ctx.train_step(i % NB, want_stats=False)
+        if ev:
+            with torch.cuda.stream(stream):
+                ev[1].record(stream)
+
+    for i in range(max(warmup, 3)):
+        step(i)
+    ctx.sync()
+    evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
+    for i in range(steps):
+        step(i, evs[i])
+    ctx.sync()
+    torch.cuda.synchronize()
+    out["ms_per_step"] = float(np.mean([a.elapsed_time(b) for a, b in evs]))
+    ctx.close()
+    del flush
+    torch.cuda.empty_cache()
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="fm_c2", choices=["fm_c2", "ffm_c3", "nfm_c4"])
+    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--rounds", type=int, default=2, help="dense / keyed alternations")
+    args = ap.parse_args()
+    import torch
+    from lightctr_b200 import build as lbuild
+    lbuild.build()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_keys.py: no CUDA device (the product has no CPU path)")
+    wl = dict(WORKLOADS[args.workload])
+    batches = make_batches(wl, wl.get("nb", 8))
+    line = {"workload": wl["desc"], "keys": "key = fmix64(fid), keyed context of capacity F", "gpu": gpu_info(),
+            "steps": args.steps, "dense_ms_per_step": [], "keyed_ms_per_step": [], "translate_us_per_batch": []}
+    for _ in range(args.rounds):
+        d = run(wl, batches, False, args.steps, args.warmup)
+        kd = run(wl, batches, True, args.steps, args.warmup)
+        line["dense_ms_per_step"].append(d["ms_per_step"])
+        line["keyed_ms_per_step"].append(kd["ms_per_step"])
+        line["translate_us_per_batch"].append(kd["translate_us_per_batch"])
+        line["table_bytes"] = kd["table_bytes"]
+    print(json.dumps(line))
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
