@@ -86,7 +86,10 @@ typedef struct lctr_cfg {
     int32_t key_mode;
     uint64_t csc_row_block;
     float ema_rate;           /* GradientUpdater::__global_ema_rate (RMSpropUpdater_Num, gradientUpdater.h:200-233); 0 => 0.99 (main.cpp:66) */
-    uint32_t reserved[3];
+    /* keyed mode only: 1 = every row records the insert-upload that last met it (8 B per row), which lctr_evict_keys
+     * needs; 0 = no record (refused on a dense context when non-zero) */
+    int32_t key_evict;
+    uint32_t reserved[2];
 } lctr_cfg;
 
 const char* lctr_last_error(void);
@@ -143,6 +146,26 @@ int lctr_download_keys(lctr_ctx* ctx, uint64_t* keys, uint64_t cap, uint64_t* n_
 int lctr_upload_keyed_params(lctr_ctx* ctx, int64_t n, const uint64_t* keys, const float* W, const float* V);
 /* lazy-init parameters of new rows; defaults seed 0, scale 1 / sqrt(k) (the reference's scale, fm_algo_abst.h:62-65) */
 int lctr_set_key_init(lctr_ctx* ctx, uint64_t seed, float scale);
+/* Eviction of idle rows (cfg.key_evict = 1), so that a drifting key stream can train within a fixed capacity.
+ * Clock: every lctr_upload_batch_keys with insert = 1 advances a u64 counter by one, then stamps every row it meets (new or
+ * not) with the new value; lctr_upload_keyed_params stamps the rows it names with the current value; lookup-only uploads
+ * and lctr_lookup_keys stamp nothing.  The age of a row is clock - stamp (0: met by the latest insert-upload).
+ * lctr_evict_keys frees
+ *   1. every row older than max_idle;
+ *   2. if more than max_rows rows remain, also the oldest: only rows younger than a* stay, a* the largest age for which
+ *      that set holds at most max_rows rows (rows that tie at the cutoff leave together).  UINT64_MAX = no limit.
+ * keys_out / W_out / V_out (each may be NULL) receive the evicted keys in ascending order of their old row, their W (n)
+ * and V (n * rowlen); when any is given, cap_out must be >= the number evicted, else the call fails and nothing changes.
+ * *n_evicted receives that number.  Survivors are renumbered by one fixed rule: with n_live survivors, a survivor below
+ * row n_live keeps its row; the j-th survivor at or above n_live (ascending) moves into the j-th evicted row below n_live
+ * (ascending), carrying W, V, the optimizer state and its stamp bit for bit.  Rows [n_live, rows in use) return to the
+ * state lctr_create gives and the table is rebuilt from the survivors, so keys stored without a row after a capacity
+ * overflow are forgotten.  When a row was freed, every resident keyed slot becomes stale: train_step and predict refuse
+ * it until it is uploaded again.  An evicted key that comes back is a new key: lazy-init values (which depend on the key
+ * only) and fresh optimizer state; re-uploading exported rows with lctr_upload_keyed_params restores W and V, also with
+ * fresh optimizer state.  Refused on a dense context and on a keyed context created with key_evict = 0. */
+int lctr_evict_keys(lctr_ctx* ctx, uint64_t max_idle, uint64_t max_rows, uint64_t* keys_out, float* W_out, float* V_out,
+                    uint64_t cap_out, uint64_t* n_evicted);
 
 /* ---- the hot path --------------------------------------------------------------------------- */
 /* One reference "batch": forward (gather + interaction [+ MLP]) -> loss -> backward scatter-add ->
@@ -204,7 +227,8 @@ int lctr_mlp_download_grad(lctr_ctx* ctx, int layer, float* dweight, float* dbia
  * export this rank's table handles, gather them, import all peers'. */
 int lctr_ipc_export(lctr_ctx* ctx, void* handles_out, size_t cap, size_t* bytes);
 int lctr_ipc_import(lctr_ctx* ctx, const void* all_handles, size_t bytes_per_rank);
-/* device memory of the context in bytes: table shard + updater state (+ the key table in keyed mode), and (world > 1) the exchange arena, caches and
+/* device memory of the context in bytes: table shard + updater state (+ the key table in keyed mode, + 8 B per row of
+ * stamps with key_evict = 1; per-call scratch is not counted), and (world > 1) the exchange arena, caches and
  * inboxes -- owner-sharding keeps the second number O(keys of a batch), not O(feature_cnt) */
 int lctr_device_bytes(lctr_ctx* ctx, uint64_t* shard_bytes, uint64_t* exchange_bytes);
 /* Data-parallel dense layers (world > 1, NFM): the per-rank weightDelta / biasDelta of the batch must be summed over

@@ -32,8 +32,9 @@ SYMBOLS = [
     "lctr_save_dataset_bin", "lctr_load_dataset_bin", "lctr_eval", "lctr_upload_pred", "lctr_ipc_export", "lctr_ipc_import",
     "lctr_dense_grad_buffer", "lctr_device_bytes", "lctr_load_libffm", "lctr_free_dataset", "lctr_launch_count", "lctr_stream", "lctr_profile", "lctr_profile_read",
     "lctr_upload_batch_keys", "lctr_lookup_keys", "lctr_download_keys", "lctr_upload_keyed_params", "lctr_set_key_init",
-    "lctr_load_libffm_keys", "lctr_free_keyed_dataset",
+    "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys",
 ]
+NO_LIMIT = (1 << 64) - 1  # lctr_evict_keys: UINT64_MAX = no limit
 
 
 class Cfg(C.Structure):
@@ -45,7 +46,8 @@ class Cfg(C.Structure):
                 ("n_hidden", C.c_int32), ("hidden", C.c_uint32 * MAX_LAYERS), ("activation", C.c_int32),
                 ("mlp_precision", C.c_int32), ("max_rows", C.c_uint64), ("max_nnz", C.c_uint64), ("rank", C.c_int32),
                 ("world", C.c_int32), ("deterministic", C.c_int32), ("key_mode", C.c_int32),
-                ("csc_row_block", C.c_uint64), ("ema_rate", C.c_float), ("reserved", C.c_uint32 * 3)]
+                ("csc_row_block", C.c_uint64), ("ema_rate", C.c_float), ("key_evict", C.c_int32),
+                ("reserved", C.c_uint32 * 2)]
 
 
 class DatasetC(C.Structure):
@@ -122,6 +124,7 @@ def load_library():
     L.lctr_set_key_init.argtypes = [vp, C.c_uint64, C.c_float]
     L.lctr_load_libffm_keys.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.POINTER(KeyedDatasetC))]
     L.lctr_free_keyed_dataset.argtypes = [C.POINTER(KeyedDatasetC)]
+    L.lctr_evict_keys.argtypes = [vp, C.c_uint64, C.c_uint64, vp, f32p, f32p, C.c_uint64, C.POINTER(C.c_uint64)]
     _lib = L
     return L
 
@@ -239,8 +242,9 @@ class Context:
     def __init__(self, model, feature_cnt, factor_cnt, field_cnt=0, optimizer=OPT_ADAGRAD, lr=0.05, l2=0.001,
                  minibatch_size=0, momentum=0.8, momentum_adam2=0.999, hidden=(), activation=ACT_SIGMOID,
                  mlp_precision=MLP_FP32, device=0, rank=0, world=1, deterministic=0, csc_row_block=0, max_rows=0,
-                 max_nnz=0, ema_rate=0.99, key_mode=KEYS_DENSE):
-        """key_mode=KEYS_HASHED: batches carry uint64 keys (upload_batch_keys) and feature_cnt is the row capacity."""
+                 max_nnz=0, ema_rate=0.99, key_mode=KEYS_DENSE, key_evict=False):
+        """key_mode=KEYS_HASHED: batches carry uint64 keys (upload_batch_keys) and feature_cnt is the row capacity.
+        key_evict=True (keyed only): rows record the insert-upload that last met them, for evict_keys."""
         L = load_library()
         cfg = Cfg()
         cfg.abi_version = ABI_VERSION
@@ -257,6 +261,7 @@ class Context:
         cfg.deterministic, cfg.csc_row_block = deterministic, csc_row_block
         cfg.max_rows, cfg.max_nnz = max_rows, max_nnz
         cfg.key_mode = key_mode
+        cfg.key_evict = 1 if key_evict else 0
         self.cfg = cfg
         self.h = C.c_void_p()
         _chk(L.lctr_create(C.byref(cfg), C.byref(self.h)))
@@ -347,6 +352,24 @@ class Context:
 
     def set_key_init(self, seed, scale):
         _chk(self.L.lctr_set_key_init(self.h, seed, scale))
+
+    def evict_keys(self, max_idle=None, max_rows=None, export=False):
+        """Free rows idle for more than max_idle insert-uploads, then the oldest beyond max_rows (None = no limit).
+        Returns the number evicted, or with export=True (keys, W, V) of the evicted rows in ascending order of their
+        old row (V flat, rowlen floats per key)."""
+        idle = NO_LIMIT if max_idle is None else int(max_idle)
+        rows = NO_LIMIT if max_rows is None else int(max_rows)
+        n = C.c_uint64()
+        if not export:
+            _chk(self.L.lctr_evict_keys(self.h, idle, rows, None, None, None, 0, C.byref(n)))
+            return n.value
+        cap = len(self.download_keys())  # at most the rows in use can leave
+        keys = np.empty(max(cap, 1), np.uint64)
+        W = np.empty(max(cap, 1), np.float32)
+        V = np.empty(max(cap, 1) * self.rowlen, np.float32)
+        _chk(self.L.lctr_evict_keys(self.h, idle, rows, _p(keys), _p(W), _p(V), cap, C.byref(n)))
+        m = n.value
+        return keys[:m].copy(), W[:m].copy(), V[:m * self.rowlen].copy()
 
     def upload_dataset(self, slot, ds, all_ones_as_null=True):
         val = ds.val

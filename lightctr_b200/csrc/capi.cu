@@ -182,6 +182,9 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
         LCTR_CHECK(cfg->deterministic == 0, "lctr_create: keyed mode needs deterministic = 0 (got %d)", cfg->deterministic);
         LCTR_CHECK(cfg->feature_cnt > 0 && cfg->feature_cnt < (1ull << 32) - 1, "lctr_create: keyed capacity (feature_cnt) out of range");
     }
+    LCTR_CHECK(cfg->key_evict == 0 || cfg->key_evict == 1, "lctr_create: bad key_evict %d", cfg->key_evict);
+    LCTR_CHECK(cfg->key_evict == 0 || cfg->key_mode == LCTR_KEYS_HASHED,
+               "lctr_create: key_evict = 1 needs key_mode = LCTR_KEYS_HASHED (a dense table has no rows to free)");
     LCTR_CHECK(cfg->feature_cnt > 0 && cfg->feature_cnt < (1ull << 32), "lctr_create: feature_cnt out of range");
     LCTR_CHECK(cfg->factor_cnt > 0, "lctr_create: factor_cnt must be > 0");
     LCTR_CHECK(cfg->model != LCTR_MODEL_FFM || cfg->field_cnt > 0, "lctr_create: FFM needs field_cnt > 0");
@@ -531,6 +534,8 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
     LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "train_step: slot %d holds no usable batch (its last keyed upload failed)", slot);
     LCTR_CHECK(s.key_state != SLOT_KEYS_LOOKUP, "train_step: slot %d was uploaded with insert = 0 (lookup only: unseen keys "
                                                 "sit on the null row, which is never trained)", slot);
+    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "train_step: slot %d is stale: lctr_evict_keys renumbered rows after it was "
+                                               "uploaded; upload it again", slot);
     LCTR_CHECK(rb >= 0 && re <= s.rows && rb <= re, "train_step: rows [%lld,%lld) outside slot (%lld rows)",
                (long long)rb, (long long)re, (long long)s.rows);
     LCTR_CHECK(c->cfg.world == 1 || c->cfg.minibatch_size > 0,
@@ -796,6 +801,8 @@ int lctr_predict(lctr_ctx* c, int slot, int quirk_sumvx_slot, float* pctr) {
     LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
     Slot& s = c->slots[slot];
     LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "lctr_predict: slot %d holds no usable batch (its last keyed upload failed)", slot);
+    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "lctr_predict: slot %d is stale: lctr_evict_keys renumbered rows after it was "
+                                               "uploaded; upload it again", slot);
     int rc = 0;
     if (c->cfg.model == LCTR_MODEL_WND) {
         // Distributed_Algo_Abst::Predict (distributed_algo_abst.h:163-174): a forward pass over the slot; with several

@@ -16,10 +16,13 @@ namespace lctr {
 
 struct CkptHeader {
     char magic[8];  // "LCTRCKP1"
-    int32_t model, optimizer, n_layers, reserved;  // reserved: cfg.key_mode (0 for dense tables)
+    int32_t model, optimizer, n_layers, reserved;  // reserved: key_word(cfg) (0 for dense tables)
     uint64_t feature_cnt, field_cnt, factor_cnt, adam_iter, step;
     int32_t in[LCTR_MAX_LAYERS + 1], out[LCTR_MAX_LAYERS + 1];
 };
+
+// cfg.key_mode in the low byte, cfg.key_evict in bit 8: dense and untracked keyed files keep the value they always had
+static int32_t key_word(const lctr_cfg& cfg) { return cfg.key_mode | (cfg.key_evict ? 0x100 : 0); }
 
 static bool put(FILE* f, const void* p, size_t n) { return n == 0 || fwrite(p, 1, n, f) == n; }
 static bool get(FILE* f, void* p, size_t n) { return n == 0 || fread(p, 1, n, f) == n; }
@@ -65,7 +68,7 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
     h.model = c->cfg.model; h.optimizer = c->cfg.optimizer; h.n_layers = c->n_layers;
     h.feature_cnt = c->F; h.field_cnt = c->cfg.field_cnt; h.factor_cnt = c->cfg.factor_cnt;
     h.adam_iter = c->adam_iter; h.step = c->step;
-    h.reserved = c->cfg.key_mode;
+    h.reserved = key_word(c->cfg);
     for (int l = 0; l < c->n_layers; l++) { h.in[l] = c->layers[l].in; h.out[l] = c->layers[l].out; }
     int rc = put(f, &h, sizeof(h)) ? 0 : 1;
     const size_t nv = c->F * c->rowlen;
@@ -84,6 +87,12 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
         rc = keys_download(c, keys);
         const uint64_t n = keys.size();
         if (!rc) rc = !(put(f, &n, sizeof(n)) && put(f, keys.data(), n * sizeof(uint64_t)));
+        if (!rc && keys_tracked(c)) {  // key_evict = 1: the upload clock, then the stamp of every row
+            std::vector<uint64_t> stamps;
+            uint64_t clock = 0;
+            rc = keys_download_stamps(c, n, stamps, &clock);
+            if (!rc) rc = !(put(f, &clock, sizeof(clock)) && put(f, stamps.data(), n * sizeof(uint64_t)));
+        }
     }
     if (fclose(f) != 0) rc = 1;
     if (rc) {
@@ -113,11 +122,11 @@ int lctr_load_checkpoint(lctr_ctx* c, const char* path) {
     }
     bool same = h.model == c->cfg.model && h.optimizer == c->cfg.optimizer && h.n_layers == c->n_layers &&
                 h.feature_cnt == c->F && h.field_cnt == c->cfg.field_cnt && h.factor_cnt == c->cfg.factor_cnt &&
-                h.reserved == c->cfg.key_mode;
+                h.reserved == key_word(c->cfg);
     for (int l = 0; l < c->n_layers && same; l++) same = h.in[l] == c->layers[l].in && h.out[l] == c->layers[l].out;
     if (!same) {
         fclose(f);
-        set_error("checkpoint %s was written by a different trainer (model/optimizer/feature_cnt/field_cnt/factor_cnt/layers/key_mode)", path);
+        set_error("checkpoint %s was written by a different trainer (model/optimizer/feature_cnt/field_cnt/factor_cnt/layers/key_mode/key_evict)", path);
         return 1;
     }
     const size_t nv = c->F * c->rowlen;
@@ -142,6 +151,16 @@ int lctr_load_checkpoint(lctr_ctx* c, const char* path) {
             keys.resize(n);
             if (!get(f, keys.data(), n * sizeof(uint64_t))) { rc = 1; set_error("checkpoint %s: short read of the keys", path); }
             else rc = keys_restore(c, keys.data(), n);
+        }
+        if (!rc && keys_tracked(c)) {
+            uint64_t clock = 0;
+            std::vector<uint64_t> stamps(n);
+            if (!get(f, &clock, sizeof(clock)) || !get(f, stamps.data(), n * sizeof(uint64_t))) {
+                rc = 1;
+                set_error("checkpoint %s: short read of the row stamps", path);
+            } else {
+                rc = keys_restore_stamps(c, stamps.data(), n, clock);
+            }
         }
     }
     fclose(f);

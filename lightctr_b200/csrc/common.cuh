@@ -86,10 +86,11 @@ struct Slot {
     unsigned int* n_hot = nullptr;
     bool fused_valid = false;
     // keyed mode (keys.cu): SLOT_KEYS_LOOKUP = uploaded with insert = 0 (predict only); SLOT_KEYS_INVALID = the last
-    // keyed upload failed, nothing may run on the slot until it is uploaded again
+    // keyed upload failed, nothing may run on the slot until it is uploaded again; SLOT_KEYS_STALE = lctr_evict_keys
+    // renumbered rows after the upload, so the slot's row ids are out of date until it is uploaded again
     int key_state = 0;
 };
-enum { SLOT_KEYS_OK = 0, SLOT_KEYS_LOOKUP = 1, SLOT_KEYS_INVALID = 2 };
+enum { SLOT_KEYS_OK = 0, SLOT_KEYS_LOOKUP = 1, SLOT_KEYS_INVALID = 2, SLOT_KEYS_STALE = 3 };
 
 // captured graphs of one slot of the streamed pipeline (capi.cu)
 struct PipeGraph {
@@ -411,6 +412,10 @@ size_t keys_bytes(const lctr_ctx* c);
 int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid);
 int keys_restore(lctr_ctx* c, const uint64_t* row_key, uint64_t n);
 int keys_download(lctr_ctx* c, std::vector<uint64_t>& out);
+// key_evict = 1: the upload clock and the stamps of rows [0, n) (checkpoints)
+bool keys_tracked(const lctr_ctx* c);
+int keys_download_stamps(lctr_ctx* c, uint64_t n, std::vector<uint64_t>& stamps, uint64_t* clock);
+int keys_restore_stamps(lctr_ctx* c, const uint64_t* stamps, uint64_t n, uint64_t clock);
 // rows of the row-indexed parameter / optimizer-state transfers: F, or the capacity in keyed mode (the null row stays out)
 inline size_t api_rows(const lctr_ctx* c) { return c->keys ? c->F - 1 : c->F; }
 

@@ -36,6 +36,24 @@
 // so the values depend on (seed, key, j) only -- never on the row a key got or on the order keys arrived in.  This is a
 // different stream from the reference's rand()-driven GaussRand (fm_algo_abst.h:62-65); only the scale default,
 // 1 / sqrt(k), is the reference's.
+//
+// Eviction (cfg.key_evict = 1; the reference's server map only grows, paramserver.h:315-339).  A host u64 clock advances
+// once per insert-upload, and key_find_kernel<0> of that upload stores it into last_seen[row] of every entry it
+// translates (plain stores: duplicates write the same value).  Untracked contexts pass a null stamp pointer, a uniform
+// branch.  lctr_evict_keys then runs on the ctx stream:
+//   survey     survivors of the max_idle rule and their largest age (two counters back to the host);
+//   select     only when max_rows binds: exact radix select of the age of rank max_rows among the survivors, 16-bit
+//              digits from the top significant bit of the largest age (usually one 65,536-bin pass), warp-aggregated
+//              histogram + a one-block pick of the digit; the host reads back (digit, count below) per pass;
+//   count/scan one flag per row, recomputed from the stamp wherever needed; per-1024-row counts, a one-block scan of
+//              them, then E(r) = evicted rows below r for r in [0, n] and the evicted-row list ev[E(r)] = r;
+//   export     gather of the evicted rows' key, W and V (before anything moves);
+//   move       survivor r >= n_live goes to ev[(r - n_live) - (E(r) - E(n_live))], the holes below n_live in order:
+//              sources all >= n_live, destinations all < n_live, so one launch moves every row with no ordering hazard;
+//   reset      rows [n_live, n) back to the state lctr_create gives;
+//   rebuild    table emptied and rows [0, n_live) re-inserted with row = index (key_insert_fixed_kernel).
+// The per-row arrays that do not move: gW / gV and `touched` are zero between steps, fused->slot_of and touch_list are
+// scratch written by each step before it reads them.  Slots hold row ids of the old numbering and become stale.
 #include <algorithm>
 #include <vector>
 
@@ -46,6 +64,8 @@ namespace lctr {
 constexpr unsigned long long kEmptyKey = ~0ull;
 constexpr uint32_t kNoRow = 0xffffffffu;
 constexpr int kGroup = 16;  // slots per 128-byte probe group
+constexpr int kEvTile = 1024;  // rows per block of the eviction count / index kernels
+constexpr int kEvBins = 1 << 16;  // radix-select digit
 
 struct KeyTable {
     unsigned long long* key = nullptr;      // [T] slot keys, kEmptyKey = free
@@ -61,6 +81,16 @@ struct KeyTable {
     size_t T = 0, cap = 0;
     unsigned long long seed = 0;
     float scale = 1.f;
+    // key_evict = 1
+    unsigned long long* last_seen = nullptr;  // [capacity] clock of the insert-upload that last met the row
+    unsigned long long clock = 0;             // insert-uploads so far
+    // scratch of lctr_evict_keys, allocated by its first call
+    uint32_t* ev_scan = nullptr;              // [capacity + 1] E(r)
+    uint32_t* ev_rows = nullptr;              // [capacity] evicted rows, ascending
+    uint32_t* ev_tiles = nullptr;             // [capacity / kEvTile + 1] per-tile counts -> offsets
+    unsigned int* ev_hist = nullptr;          // [65536] digit histogram of the radix select
+    unsigned long long* ev_res = nullptr;     // [4] counters read back by the host
+    unsigned long long* h_res = nullptr;      // pinned mirror
 };
 
 struct KeyView {
@@ -146,8 +176,9 @@ __global__ void __launch_bounds__(256) key_insert_kernel(const unsigned long lon
 }
 
 // keys with caller-chosen rows (lctr_upload_keyed_params, checkpoint restore): every key gets rows[i]; `record` appends the
-// row to the new-row list for key_init_kernel.
-__global__ void __launch_bounds__(256) key_insert_fixed_kernel(const unsigned long long* __restrict__ keys, const int64_t* __restrict__ rows,
+// row to the new-row list for key_init_kernel.  rows == nullptr: key i gets row i and keys is the row -> key map itself
+// (the rebuild after an eviction), which is then left as it is.
+__global__ void __launch_bounds__(256) key_insert_fixed_kernel(const unsigned long long* keys, const int64_t* __restrict__ rows,
                                                                int64_t n, KeyView t, int record) {
     const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
     if (i >= n) return;
@@ -158,9 +189,9 @@ __global__ void __launch_bounds__(256) key_insert_fixed_kernel(const unsigned lo
     const long long pos = tile_claim(t, key, sub, gmask, &claimed);
     if (sub != 0) return;
     if (pos < 0) { t.flags[1] = 1u; return; }
-    const uint32_t r = (uint32_t)rows[i];
+    const uint32_t r = rows ? (uint32_t)rows[i] : (uint32_t)i;
     t.row[pos] = r;
-    t.row_key[r] = key;
+    if (rows) t.row_key[r] = key;
     if (record) t.new_rows[atomicAdd(&t.flags[2], 1u)] = r;
 }
 
@@ -197,11 +228,13 @@ __global__ void __launch_bounds__(256) key_init_kernel(KeyView t, float* __restr
     }
 }
 
-// 3. translation: MODE 0 -> u32 row per entry into a slot (absent: the null row; kNoRow: capacity flag + null row);
+// 3. translation: MODE 0 -> u32 row per entry into a slot (absent: the null row; kNoRow: capacity flag + null row), and
+//    with a stamp array (tracked context, insert-upload) last_seen[row] = clock;
 //    MODE 1 -> int64 row per key, -1 when absent or without a row
 template <int MODE>
 __global__ void __launch_bounds__(256) key_find_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t,
-                                                       uint32_t* __restrict__ fid, int64_t* __restrict__ rows, int insert) {
+                                                       uint32_t* __restrict__ fid, int64_t* __restrict__ rows, int insert,
+                                                       unsigned long long* __restrict__ last_seen, unsigned long long clock) {
     const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
     if (i >= n) return;
     const int sub = threadIdx.x & (kGroup - 1);
@@ -211,6 +244,8 @@ __global__ void __launch_bounds__(256) key_find_kernel(const unsigned long long*
     const uint32_t r = pos >= 0 ? __ldg(t.row + pos) : kNoRow;
     if (MODE == 0) {
         if (r == kNoRow && insert) t.flags[pos >= 0 ? 0 : 1] = 1u;
+        // hot rows appear in many entries of a batch: entries that find the stamp already written skip the store
+        if (last_seen && r != kNoRow && __ldcg(last_seen + r) != clock) last_seen[r] = clock;
         fid[i] = r == kNoRow ? (uint32_t)t.cap : r;
     } else {
         rows[i] = r == kNoRow ? -1 : (int64_t)r;
@@ -230,6 +265,246 @@ __global__ void __launch_bounds__(256) key_scatter_params_kernel(const int64_t* 
     }
 }
 
+// stamps of rows given by index (lctr_upload_keyed_params)
+__global__ void __launch_bounds__(256) key_stamp_rows_kernel(const int64_t* __restrict__ rows, int64_t n,
+                                                             unsigned long long* __restrict__ last_seen, unsigned long long clock) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        last_seen[rows[i]] = clock;
+}
+
+// ---- eviction ----------------------------------------------------------------------------------------------------------
+// a row leaves when its age exceeds max_idle, or (limit) reaches the cutoff a* of the max_rows rule
+struct EvictRule {
+    unsigned long long clock, max_idle, cut;
+    int limit;
+};
+__device__ __forceinline__ bool row_evicted(const EvictRule& e, unsigned long long stamp) {
+    const unsigned long long age = e.clock - stamp;
+    return age > e.max_idle || (e.limit && age >= e.cut);
+}
+
+// the per-row arrays that move with a row
+struct RowArrays {
+    float *W, *V, *s1W, *s1V, *s2W, *s2V;
+    unsigned long long *row_key, *last_seen;
+};
+
+// res[0] += rows with age <= max_idle, res[1] = max(res[1], their largest age)
+__global__ void __launch_bounds__(256) evict_survey_kernel(const unsigned long long* __restrict__ last_seen, size_t n,
+                                                           unsigned long long clock, unsigned long long max_idle,
+                                                           unsigned long long* __restrict__ res) {
+    unsigned long long cnt = 0, mx = 0;
+    for (size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (size_t)gridDim.x * blockDim.x) {
+        const unsigned long long age = clock - last_seen[r];
+        if (age <= max_idle) { cnt++; mx = age > mx ? age : mx; }
+    }
+    for (int o = 16; o; o >>= 1) {
+        cnt += __shfl_xor_sync(~0u, cnt, o);
+        const unsigned long long m = __shfl_xor_sync(~0u, mx, o);
+        mx = m > mx ? m : mx;
+    }
+    if ((threadIdx.x & 31) == 0 && cnt) {
+        atomicAdd(res, cnt);
+        atomicMax(res + 1, mx);
+    }
+}
+
+// one radix-select pass: histogram of digit (age >> shift) & (2^width - 1) over the survivors whose bits above
+// pshift equal prefix (pshift >= 64: no condition).  Ages cluster on a few values, so lanes with the same digit add once.
+__global__ void __launch_bounds__(256) evict_hist_kernel(const unsigned long long* __restrict__ last_seen, size_t n,
+                                                         unsigned long long clock, unsigned long long max_idle, int shift,
+                                                         int width, int pshift, unsigned long long prefix,
+                                                         unsigned int* __restrict__ hist) {
+    const int lane = threadIdx.x & 31;
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t r0 = (size_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); r0 < n; r0 += stride) {  // warp-uniform
+        const size_t r = r0 + lane;
+        bool in = false;
+        unsigned bin = 0;
+        if (r < n) {
+            const unsigned long long age = clock - last_seen[r];
+            in = age <= max_idle && (pshift >= 64 || (age >> pshift) == prefix);
+            bin = (unsigned)(age >> shift) & ((1u << width) - 1u);
+        }
+        const unsigned act = __ballot_sync(~0u, in);
+        if (in) {
+            const unsigned peers = __match_any_sync(act, bin);
+            if (lane == __ffs(peers) - 1) atomicAdd(hist + bin, (unsigned)__popc(peers));
+        }
+    }
+}
+
+// the digit holding rank `rank` (0-based, ascending): res[0] = digit, res[1] = count of the smaller digits
+__global__ void __launch_bounds__(1024) evict_pick_kernel(const unsigned int* __restrict__ hist, int nbins,
+                                                          unsigned long long rank, unsigned long long* __restrict__ res) {
+    __shared__ unsigned long long part[1024];
+    const int per = (nbins + 1023) / 1024;
+    const int b0 = (int)threadIdx.x * per, b1 = min(b0 + per, nbins);
+    unsigned long long s = 0;
+    for (int b = b0; b < b1; b++) s += hist[b];
+    part[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {
+        const unsigned long long v = threadIdx.x >= (unsigned)o ? part[threadIdx.x - o] : 0ull;
+        __syncthreads();
+        part[threadIdx.x] += v;
+        __syncthreads();
+    }
+    const unsigned long long incl = part[threadIdx.x], excl = incl - s;
+    if (excl <= rank && rank < incl) {  // exactly one thread: rank < total
+        unsigned long long below = excl;
+        for (int b = b0; b < b1; b++) {
+            const unsigned long long h = hist[b];
+            if (rank < below + h) { res[0] = (unsigned long long)b; res[1] = below; break; }
+            below += h;
+        }
+    }
+}
+
+// inclusive scan of one value per thread over a 1024-thread block; *total = the block's sum
+__device__ __forceinline__ unsigned block_scan_incl(unsigned v, unsigned* ws, unsigned* total) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    unsigned x = v;
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned y = __shfl_up_sync(~0u, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) ws[w] = x;
+    __syncthreads();
+    if (w == 0) {
+        unsigned s = ws[lane];
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned y = __shfl_up_sync(~0u, s, o);
+            if (lane >= o) s += y;
+        }
+        ws[lane] = s;
+    }
+    __syncthreads();
+    const unsigned out = x + (w ? ws[w - 1] : 0u);
+    *total = ws[31];
+    __syncthreads();  // ws is reused by the next call
+    return out;
+}
+
+// evicted rows per tile of kEvTile rows (tiles cover [0, n])
+__global__ void __launch_bounds__(kEvTile) evict_count_kernel(const unsigned long long* __restrict__ last_seen, size_t n,
+                                                              EvictRule e, uint32_t* __restrict__ tiles) {
+    const size_t r = (size_t)blockIdx.x * kEvTile + threadIdx.x;
+    const int cnt = __syncthreads_count(r < n && row_evicted(e, last_seen[r]));
+    if (threadIdx.x == 0) tiles[blockIdx.x] = (uint32_t)cnt;
+}
+
+// tile counts -> exclusive offsets in place (one block); res[0] = evicted rows in all
+__global__ void __launch_bounds__(1024) evict_scan_tiles_kernel(uint32_t* __restrict__ tiles, size_t ntiles,
+                                                                unsigned long long* __restrict__ res) {
+    __shared__ unsigned ws[32];
+    unsigned carry = 0;
+    for (size_t base = 0; base < ntiles; base += 1024) {
+        const size_t i = base + threadIdx.x;
+        const unsigned v = i < ntiles ? tiles[i] : 0u;
+        unsigned tot;
+        const unsigned incl = block_scan_incl(v, ws, &tot);
+        if (i < ntiles) tiles[i] = carry + incl - v;
+        carry += tot;
+    }
+    if (threadIdx.x == 0) res[0] = carry;
+}
+
+// E(r) for r in [0, n] and the evicted-row list ev_rows[E(r)] = r
+__global__ void __launch_bounds__(kEvTile) evict_index_kernel(const unsigned long long* __restrict__ last_seen, size_t n,
+                                                              EvictRule e, const uint32_t* __restrict__ tiles,
+                                                              uint32_t* __restrict__ scan, uint32_t* __restrict__ ev_rows) {
+    __shared__ unsigned ws[32];
+    const size_t r = (size_t)blockIdx.x * kEvTile + threadIdx.x;
+    const unsigned f = r < n && row_evicted(e, last_seen[r]);
+    unsigned tot;
+    const unsigned E = tiles[blockIdx.x] + block_scan_incl(f, ws, &tot) - f;
+    if (r <= n) scan[r] = E;
+    if (f) ev_rows[E] = (uint32_t)r;
+}
+
+// export of the evicted rows (warp per row): key, W, V into dense device buffers, each may be null
+__global__ void __launch_bounds__(256) evict_export_kernel(const uint32_t* __restrict__ ev_rows, size_t m, const unsigned long long* __restrict__ row_key,
+                                                           const float* __restrict__ W, const float* __restrict__ V, size_t rowlen,
+                                                           unsigned long long* __restrict__ keys_out, float* __restrict__ W_out,
+                                                           float* __restrict__ V_out) {
+    const int lane = threadIdx.x & 31;
+    const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
+    for (size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; i < m; i += nwarps) {
+        const size_t r = ev_rows[i];
+        if (V_out) for (size_t j = lane; j < rowlen; j += 32) V_out[i * rowlen + j] = V[r * rowlen + j];
+        if (lane == 0) {
+            if (keys_out) keys_out[i] = row_key[r];
+            if (W_out) W_out[i] = W[r];
+        }
+    }
+}
+
+// copy of one rowlen-float row by a warp, 16-byte accesses when rowlen % 4 == 0 (rows are then 16-byte aligned)
+template <bool VEC4>
+__device__ __forceinline__ void warp_copy_row(float* __restrict__ a, size_t d, size_t s, size_t rowlen, int lane) {
+    if (VEC4) {
+        float4* dst = reinterpret_cast<float4*>(a + d * rowlen);
+        const float4* src = reinterpret_cast<const float4*>(a + s * rowlen);
+        for (size_t j = lane; j < rowlen / 4; j += 32) dst[j] = src[j];
+    } else {
+        for (size_t j = lane; j < rowlen; j += 32) a[d * rowlen + j] = a[s * rowlen + j];
+    }
+}
+template <bool VEC4>
+__device__ __forceinline__ void warp_fill_row(float* __restrict__ a, size_t d, size_t rowlen, float v, int lane) {
+    if (VEC4) {
+        float4* dst = reinterpret_cast<float4*>(a + d * rowlen);
+        for (size_t j = lane; j < rowlen / 4; j += 32) dst[j] = make_float4(v, v, v, v);
+    } else {
+        for (size_t j = lane; j < rowlen; j += 32) a[d * rowlen + j] = v;
+    }
+}
+
+// survivors at or above n_live into the holes below it (warp per row of [n_live, n); evicted rows there skip)
+template <bool VEC4>
+__global__ void __launch_bounds__(256) evict_move_kernel(RowArrays a, size_t rowlen, size_t n_live, size_t n,
+                                                         const uint32_t* __restrict__ scan, const uint32_t* __restrict__ ev_rows) {
+    const int lane = threadIdx.x & 31;
+    const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
+    const uint32_t e_live = scan[n_live];
+    for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n - n_live; w += nwarps) {
+        const size_t r = n_live + w;
+        const uint32_t E = scan[r];
+        if (scan[r + 1] != E) continue;  // evicted
+        const size_t d = ev_rows[(r - n_live) - (E - e_live)];
+        warp_copy_row<VEC4>(a.V, d, r, rowlen, lane);
+        warp_copy_row<VEC4>(a.s1V, d, r, rowlen, lane);
+        if (a.s2V) warp_copy_row<VEC4>(a.s2V, d, r, rowlen, lane);
+        if (lane == 0) {
+            a.W[d] = a.W[r];
+            a.s1W[d] = a.s1W[r];
+            if (a.s2W) a.s2W[d] = a.s2W[r];
+            a.row_key[d] = a.row_key[r];
+            a.last_seen[d] = a.last_seen[r];
+        }
+    }
+}
+
+// rows [lo, hi) back to the state lctr_create gives (warp per row)
+template <bool VEC4>
+__global__ void __launch_bounds__(256) evict_reset_kernel(RowArrays a, size_t rowlen, size_t lo, size_t hi, float s1_init) {
+    const int lane = threadIdx.x & 31;
+    const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
+    for (size_t r = lo + ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; r < hi; r += nwarps) {
+        warp_fill_row<VEC4>(a.V, r, rowlen, 0.f, lane);
+        warp_fill_row<VEC4>(a.s1V, r, rowlen, s1_init, lane);
+        if (a.s2V) warp_fill_row<VEC4>(a.s2V, r, rowlen, 0.f, lane);
+        if (lane == 0) {
+            a.W[r] = 0.f;
+            a.s1W[r] = s1_init;
+            if (a.s2W) a.s2W[r] = 0.f;
+            a.row_key[r] = kEmptyKey;
+            a.last_seen[r] = 0;
+        }
+    }
+}
+
 static unsigned tile_grid(int64_t n) { return (unsigned)std::max<int64_t>(1, (n * kGroup + 255) / 256); }
 
 static int scratch_reserve(lctr_ctx* c, size_t n) {
@@ -246,9 +521,14 @@ static int scratch_reserve(lctr_ctx* c, size_t n) {
     return 0;
 }
 
+// the s1 value lctr_create gives every row
+static float s1_init(const lctr_ctx* c) {
+    return (c->cfg.optimizer == LCTR_OPT_PS_ADAGRAD || c->cfg.optimizer == LCTR_OPT_PS_DCASGDA) ? 1e-7f : 0.f;
+}
+
 static int init_new_rows(lctr_ctx* c, int64_t max_new) {
     KeyTable* t = c->keys;
-    const float s1 = (c->cfg.optimizer == LCTR_OPT_PS_ADAGRAD || c->cfg.optimizer == LCTR_OPT_PS_DCASGDA) ? 1e-7f : 0.f;
+    const float s1 = s1_init(c);
     const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((max_new + 7) / 8, (int64_t)c->sm_count * 16));
     key_init_kernel<<<grid, 256, 0, c->stream>>>(view(t), c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, c->rowlen, s1, t->seed, t->scale);
     c->launches++;
@@ -296,6 +576,10 @@ int keys_alloc(lctr_ctx* c) {
     LCTR_CUDA(cudaMemsetAsync(t->row, 0xff, T * sizeof(uint32_t), c->stream));
     LCTR_CUDA(cudaMemsetAsync(t->count, 0, sizeof(unsigned long long), c->stream));
     LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    if (c->cfg.key_evict) {
+        LCTR_CUDA(cudaMalloc((void**)&t->last_seen, t->cap * sizeof(unsigned long long)));
+        LCTR_CUDA(cudaMemsetAsync(t->last_seen, 0, t->cap * sizeof(unsigned long long), c->stream));
+    }
     return 0;
 }
 
@@ -304,19 +588,27 @@ void keys_free(lctr_ctx* c) {
     if (!t) return;
     cudaFree(t->key); cudaFree(t->row); cudaFree(t->row_key); cudaFree(t->count); cudaFree(t->flags);
     cudaFree(t->new_rows); cudaFree(t->d_keys); cudaFree(t->d_rows);
+    cudaFree(t->last_seen); cudaFree(t->ev_scan); cudaFree(t->ev_rows); cudaFree(t->ev_tiles); cudaFree(t->ev_hist);
+    cudaFree(t->ev_res);
     if (t->h_flags) cudaFreeHost(t->h_flags);
+    if (t->h_res) cudaFreeHost(t->h_res);
     delete t;
     c->keys = nullptr;
 }
 
+bool keys_tracked(const lctr_ctx* c) { return c->keys && c->keys->last_seen; }
+
 size_t keys_bytes(const lctr_ctx* c) {
     const KeyTable* t = c->keys;
-    return t ? t->T * (sizeof(unsigned long long) + sizeof(uint32_t)) + t->cap * sizeof(unsigned long long) : 0;
+    if (!t) return 0;
+    return t->T * (sizeof(unsigned long long) + sizeof(uint32_t)) + t->cap * sizeof(unsigned long long) +
+           (t->last_seen ? t->cap * sizeof(unsigned long long) : 0);
 }
 
 // keys of one upload -> rows in fid (device, n entries); insert: create and initialise rows for new keys first
 int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid) {
     KeyTable* t = c->keys;
+    if (insert) t->clock++;  // the clock counts insert-uploads, empty ones included
     if (n == 0) return 0;
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, h_keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
@@ -329,7 +621,8 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
             LCTR_CUDA(cudaGetLastError());
             if (init_new_rows(c, std::min<int64_t>(n, (int64_t)t->cap))) return 1;
         }
-        key_find_kernel<0><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0);
+        key_find_kernel<0><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0,
+                                                                insert ? t->last_seen : nullptr, t->clock);
         c->launches++;
         LCTR_CUDA(cudaGetLastError());
     }
@@ -344,7 +637,7 @@ static int lookup_dev(lctr_ctx* c, const uint64_t* keys, int64_t n) {
     KeyTable* t = c->keys;
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
-    key_find_kernel<1><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), nullptr, t->d_rows, 0);
+    key_find_kernel<1><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), nullptr, t->d_rows, 0, nullptr, 0);
     c->launches++;
     LCTR_CUDA(cudaGetLastError());
     return 0;
@@ -381,6 +674,75 @@ int keys_download(lctr_ctx* c, std::vector<uint64_t>& out) {
     out.resize(n);
     if (n) LCTR_CUDA(cudaMemcpyAsync(out.data(), c->keys->row_key, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int keys_download_stamps(lctr_ctx* c, uint64_t n, std::vector<uint64_t>& stamps, uint64_t* clock) {
+    KeyTable* t = c->keys;
+    stamps.resize(n);
+    *clock = t->clock;
+    if (n) LCTR_CUDA(cudaMemcpyAsync(stamps.data(), t->last_seen, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int keys_restore_stamps(lctr_ctx* c, const uint64_t* stamps, uint64_t n, uint64_t clock) {
+    KeyTable* t = c->keys;
+    LCTR_CHECK(n <= t->cap, "checkpoint: %llu stamps exceed the capacity %zu", (unsigned long long)n, t->cap);
+    LCTR_CUDA(cudaMemsetAsync(t->last_seen, 0, t->cap * sizeof(uint64_t), c->stream));
+    if (n) LCTR_CUDA(cudaMemcpyAsync(t->last_seen, stamps, n * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    t->clock = clock;
+    return 0;
+}
+
+static int evict_scratch(lctr_ctx* c) {
+    KeyTable* t = c->keys;
+    if (t->ev_scan) return 0;
+    LCTR_CUDA(cudaMalloc((void**)&t->ev_scan, (t->cap + 1) * sizeof(uint32_t)));
+    LCTR_CUDA(cudaMalloc((void**)&t->ev_rows, t->cap * sizeof(uint32_t)));
+    LCTR_CUDA(cudaMalloc((void**)&t->ev_tiles, (t->cap / kEvTile + 1) * sizeof(uint32_t)));
+    LCTR_CUDA(cudaMalloc((void**)&t->ev_hist, kEvBins * sizeof(unsigned int)));
+    LCTR_CUDA(cudaMalloc((void**)&t->ev_res, 4 * sizeof(unsigned long long)));
+    LCTR_CUDA(cudaMallocHost((void**)&t->h_res, 4 * sizeof(unsigned long long)));
+    return 0;
+}
+
+static int read_res(lctr_ctx* c, int n) {
+    KeyTable* t = c->keys;
+    LCTR_CUDA(cudaMemcpyAsync(t->h_res, t->ev_res, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+#define LCTR_LAUNCHED()                  \
+    do {                                 \
+        c->launches++;                   \
+        LCTR_CUDA(cudaGetLastError());   \
+    } while (0)
+
+// the age of rank `rank` (0-based, ascending) among the rows of age <= max_idle, of which the largest is max_age
+static int radix_select_age(lctr_ctx* c, size_t n, unsigned long long max_idle, unsigned long long max_age,
+                            unsigned long long rank, unsigned long long* out) {
+    KeyTable* t = c->keys;
+    const int bits = std::max(1, 64 - __builtin_clzll(max_age | 1ull));
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
+    unsigned long long prefix = 0;
+    int pshift = 64, shift = bits;  // bits above `bits` are zero for every survivor: no prefix condition on the first pass
+    while (shift > 0) {
+        const int width = std::min(16, shift);
+        shift -= width;
+        LCTR_CUDA(cudaMemsetAsync(t->ev_hist, 0, ((size_t)1 << width) * sizeof(unsigned int), c->stream));
+        evict_hist_kernel<<<grid, 256, 0, c->stream>>>(t->last_seen, n, t->clock, max_idle, shift, width, pshift, prefix, t->ev_hist);
+        LCTR_LAUNCHED();
+        evict_pick_kernel<<<1, 1024, 0, c->stream>>>(t->ev_hist, 1 << width, rank, t->ev_res);
+        LCTR_LAUNCHED();
+        if (read_res(c, 2)) return 1;
+        prefix = (prefix << width) | t->h_res[0];
+        rank -= t->h_res[1];
+        pshift = shift;
+    }
+    *out = prefix;
     return 0;
 }
 
@@ -463,9 +825,16 @@ int lctr_upload_keyed_params(lctr_ctx* c, int64_t n, const uint64_t* keys, const
         if (read_flags(c)) return 1;
         LCTR_CHECK(!t->h_flags[1], "lctr_upload_keyed_params: key table full");
     }
+    if (t->last_seen || W || V)
+        LCTR_CUDA(cudaMemcpyAsync(t->d_rows, rows.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
+    if (t->last_seen) {  // every named row counts as met at the current clock
+        const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)c->sm_count * 8));
+        key_stamp_rows_kernel<<<grid, 256, 0, c->stream>>>(t->d_rows, n, t->last_seen, t->clock);
+        c->launches++;
+        LCTR_CUDA(cudaGetLastError());
+    }
     if (W || V) {
         float *dW = nullptr, *dV = nullptr;
-        LCTR_CUDA(cudaMemcpyAsync(t->d_rows, rows.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
         if (W) {
             LCTR_CUDA(cudaMalloc((void**)&dW, (size_t)n * sizeof(float)));
             LCTR_CUDA(cudaMemcpyAsync(dW, W, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
@@ -491,6 +860,97 @@ int lctr_set_key_init(lctr_ctx* c, uint64_t seed, float scale) {
     LCTR_CHECK(c->keys, "lctr_set_key_init: the context was not created with key_mode = LCTR_KEYS_HASHED");
     c->keys->seed = seed;
     c->keys->scale = scale;
+    return 0;
+}
+
+int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t* keys_out, float* W_out, float* V_out,
+                    uint64_t cap_out, uint64_t* n_evicted) {
+    LCTR_CHECK(c && n_evicted, "null argument");
+    LCTR_CHECK(c->keys, "lctr_evict_keys: the context was not created with key_mode = LCTR_KEYS_HASHED");
+    LCTR_CHECK(c->keys->last_seen, "lctr_evict_keys: the context was not created with key_evict = 1 (rows record no last use)");
+    KeyTable* t = c->keys;
+    *n_evicted = 0;
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    int rc = 0;
+    const size_t n = rows_in_use(c, &rc);
+    if (rc) return 1;
+    if (n == 0) return 0;
+    if (evict_scratch(c)) return 1;
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
+
+    // 1 + 2: the rule
+    LCTR_CUDA(cudaMemsetAsync(t->ev_res, 0, 2 * sizeof(unsigned long long), c->stream));
+    evict_survey_kernel<<<grid, 256, 0, c->stream>>>(t->last_seen, n, t->clock, max_idle, t->ev_res);
+    LCTR_LAUNCHED();
+    if (read_res(c, 2)) return 1;
+    const unsigned long long survivors = t->h_res[0], max_age = t->h_res[1];
+    EvictRule e{t->clock, max_idle, 0ull, 0};
+    if (survivors > max_rows) {
+        if (radix_select_age(c, n, max_idle, max_age, max_rows, &e.cut)) return 1;
+        e.limit = 1;
+    }
+
+    // count and scan
+    const size_t ntiles = n / kEvTile + 1;  // tiles cover [0, n]: E(n) is needed too
+    evict_count_kernel<<<(unsigned)ntiles, kEvTile, 0, c->stream>>>(t->last_seen, n, e, t->ev_tiles);
+    LCTR_LAUNCHED();
+    evict_scan_tiles_kernel<<<1, 1024, 0, c->stream>>>(t->ev_tiles, ntiles, t->ev_res);
+    LCTR_LAUNCHED();
+    if (read_res(c, 1)) return 1;
+    const size_t m = (size_t)t->h_res[0];
+    if (m == 0) return 0;  // nothing leaves: the table, its rows and the slots stay as they are
+    const bool exporting = keys_out || W_out || V_out;
+    LCTR_CHECK(!exporting || cap_out >= m, "lctr_evict_keys: room for %llu evicted rows, %zu would leave (nothing was changed)",
+               (unsigned long long)cap_out, m);
+    const size_t n_live = n - m;
+    evict_index_kernel<<<(unsigned)ntiles, kEvTile, 0, c->stream>>>(t->last_seen, n, e, t->ev_tiles, t->ev_scan, t->ev_rows);
+    LCTR_LAUNCHED();
+
+    const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
+    if (exporting) {  // gathered before anything moves
+        unsigned long long* dK = nullptr;
+        float *dW = nullptr, *dV = nullptr;
+        cudaError_t err = cudaSuccess;
+        if (keys_out && err == cudaSuccess) err = cudaMalloc((void**)&dK, m * sizeof(unsigned long long));
+        if (W_out && err == cudaSuccess) err = cudaMalloc((void**)&dW, m * sizeof(float));
+        if (V_out && err == cudaSuccess) err = cudaMalloc((void**)&dV, m * c->rowlen * sizeof(float));
+        if (err == cudaSuccess) {
+            evict_export_kernel<<<mgrid, 256, 0, c->stream>>>(t->ev_rows, m, t->row_key, c->W, c->V, c->rowlen, dK, dW, dV);
+            c->launches++;
+            err = cudaGetLastError();
+        }
+        if (err == cudaSuccess && dK) err = cudaMemcpyAsync(keys_out, dK, m * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
+        if (err == cudaSuccess && dW) err = cudaMemcpyAsync(W_out, dW, m * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
+        if (err == cudaSuccess && dV) err = cudaMemcpyAsync(V_out, dV, m * c->rowlen * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
+        const cudaError_t es = cudaStreamSynchronize(c->stream);
+        cudaFree(dK); cudaFree(dW); cudaFree(dV);
+        LCTR_CUDA(err);
+        LCTR_CUDA(es);
+    }
+
+    // move, reset, rebuild
+    const RowArrays a{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, t->row_key, t->last_seen};
+    const bool vec4 = (c->rowlen & 3) == 0;  // 16-byte rows: FM / NFM k % 4 == 0, FFM Fc * k % 4 == 0
+    if (vec4) evict_move_kernel<true><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, t->ev_scan, t->ev_rows);
+    else evict_move_kernel<false><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, t->ev_scan, t->ev_rows);
+    LCTR_LAUNCHED();
+    if (vec4) evict_reset_kernel<true><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, s1_init(c));
+    else evict_reset_kernel<false><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, s1_init(c));
+    LCTR_LAUNCHED();
+    LCTR_CUDA(cudaMemsetAsync(t->key, 0xff, t->T * sizeof(unsigned long long), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->row, 0xff, t->T * sizeof(uint32_t), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    if (n_live) {
+        key_insert_fixed_kernel<<<tile_grid((int64_t)n_live), 256, 0, c->stream>>>(t->row_key, nullptr, (int64_t)n_live, view(t), 0);
+        LCTR_LAUNCHED();
+    }
+    const unsigned long long cnt = n_live;
+    LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
+    if (read_flags(c)) return 1;
+    LCTR_CHECK(!t->h_flags[1], "lctr_evict_keys: key table full while re-inserting %zu keys", n_live);
+    for (int s = 0; s < kNumSlots; s++)  // their row ids belong to the old numbering
+        if (c->slots[s].key_state != SLOT_KEYS_INVALID) c->slots[s].key_state = SLOT_KEYS_STALE;
+    *n_evicted = m;
     return 0;
 }
 

@@ -2,7 +2,7 @@
 """Keyed mode against dense mode on one GPU: the same workload and batches, ids fed as 64-bit keys fmix64(fid) into a keyed
 context of capacity F (cfg.key_mode = LCTR_KEYS_HASHED), alternated with the dense context in one process.
 
-    python scripts/bench_keys.py [--workload fm_c2|ffm_c3|nfm_c4] [--steps K] [--warmup W] [--rounds R]
+    python scripts/bench_keys.py [--workload fm_c2|ffm_c3|nfm_c4] [--steps K] [--warmup W] [--rounds R] [--evict]
 
 Prints ONE JSON line:
   keyed_ms_per_step / dense_ms_per_step   device-timed step (one CUDA-event pair per step, L2 flushed before each step,
@@ -13,13 +13,24 @@ Prints ONE JSON line:
                                           table) and a second upload of the same batches ("all_known": probes only);
   table_bytes                             key table (slots of u64 key + u32 row, u64 key per row) and lctr_device_bytes;
   gpu                                     card name and power limit, read in the same run.
-Writes nothing to the tree.
+With --evict (row eviction, cfg.key_evict; the workload is then always fm_c2: capacity 1M, k = 16, Adagrad) the line
+instead holds, per round:
+  translate_us_per_batch                  as above for keyed contexts with key_evict = 1 ("tracked", stamps stored by the
+                                          translate launch) and 0 ("untracked"), alternated;
+  ms_per_step                             step time of the dense, untracked and tracked contexts, alternated;
+  evict_ms                                host clock around lctr_evict_keys (it ends in a stream synchronise) on a full
+                                          table of 1M rows whose ages are spread uniformly over 0..99, evicting 10 %, 25 %
+                                          and 50 % of them through max_rows, with and without export of keys, W and V;
+  rows_moved                              survivors renumbered by each of those calls.
+Writes nothing to the tree (the full table is restored from a checkpoint in a temporary directory).
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import tempfile
+import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -51,7 +62,7 @@ def gpu_info():
         return None
 
 
-def run(wl, batches, keyed, steps, warmup):
+def run(wl, batches, keyed, steps, warmup, key_evict=False):
     import torch
     from lightctr_b200 import capi
     model = {"fm": capi.MODEL_FM, "ffm": capi.MODEL_FFM, "nfm": capi.MODEL_NFM}[wl["model"]]
@@ -60,7 +71,7 @@ def run(wl, batches, keyed, steps, warmup):
     Fc = N_FIELDS if wl["model"] == "ffm" else 0
     ctx = capi.Context(model, F, k, Fc, optimizer=opt, max_nnz=B * 100, hidden=wl.get("hidden", ()),
                        mlp_precision=capi.MLP_BF16 if wl["model"] == "nfm" else capi.MLP_FP32,
-                       key_mode=capi.KEYS_HASHED if keyed else capi.KEYS_DENSE)
+                       key_mode=capi.KEYS_HASHED if keyed else capi.KEYS_DENSE, key_evict=key_evict)
     if wl["model"] == "nfm":  # the dense layers as bench.py initialises them
         rng0 = np.random.default_rng(99)
         dims = [k] + list(wl["hidden"]) + [1]
@@ -120,18 +131,82 @@ def run(wl, batches, keyed, steps, warmup):
     return out
 
 
+def evict_times(wl, rounds, fractions=(0.10, 0.25, 0.50)):
+    """lctr_evict_keys on a full 1M-row table with ages spread over 0..99, restored from one checkpoint before each call"""
+    import ctypes as C
+    from lightctr_b200 import capi
+    F, k = wl["F"], wl["k"]
+    ctx = capi.Context(capi.MODEL_FM, F, k, optimizer=capi.OPT_ADAGRAD, key_mode=capi.KEYS_HASHED, key_evict=True)
+    ctx.set_key_init(1234, float(1.0 / np.sqrt(k)))
+    keys = fmix64(np.arange(F, dtype=np.uint64) + np.uint64(1 << 40))
+    ctx.upload_keyed_params(keys)  # every row, lazily initialised
+    perm = np.random.default_rng(7).permutation(F)
+    one = np.array([0, 1], np.int64)
+    for chunk in np.array_split(perm, 100):  # one insert-upload per chunk, then that chunk is stamped with its clock
+        ctx.upload_batch_keys(0, one, keys[chunk[:1]], None, None, np.array([1], np.int32))
+        ctx.upload_keyed_params(keys[chunk])
+    out = {"rows": F, "evict_ms": {}, "rows_moved": {}}
+    kbuf, wbuf, vbuf = np.empty(F, np.uint64), np.empty(F, np.float32), np.empty(F * k, np.float32)
+    n = C.c_uint64()
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "full.ckpt")
+        ctx.save_checkpoint(path)
+        rows0 = ctx.lookup_keys(keys)
+        ctx.evict_keys(max_rows=F)  # allocates the eviction scratch; frees nothing
+        for f in fractions:
+            for export in (False, True):
+                name = "%d%%%s" % (round(f * 100), "_export" if export else "")
+                out["evict_ms"][name] = []
+                for _ in range(rounds):
+                    ctx.load_checkpoint(path)
+                    ptrs = (kbuf.ctypes.data, wbuf.ctypes.data, vbuf.ctypes.data) if export else (None, None, None)
+                    t0 = time.perf_counter()
+                    rc = ctx.L.lctr_evict_keys(ctx.h, capi.NO_LIMIT, int(F * (1 - f)), *ptrs, F if export else 0, C.byref(n))
+                    dt = time.perf_counter() - t0
+                    if rc:
+                        raise RuntimeError(capi.load_library().lctr_last_error().decode())
+                    out["evict_ms"][name].append(1e3 * dt)
+                rows1 = ctx.lookup_keys(keys)
+                out["rows_moved"]["%d%%" % round(f * 100)] = int(np.sum((rows1 >= 0) & (rows1 != rows0)))
+                out.setdefault("rows_evicted", {})["%d%%" % round(f * 100)] = int(n.value)
+    ctx.close()
+    return out
+
+
+def main_evict(args):
+    wl = dict(WORKLOADS["fm_c2"])
+    batches = make_batches(wl, wl.get("nb", 8))
+    line = {"workload": wl["desc"] + ", keyed capacity 1M", "keys": "key = fmix64(fid)", "gpu": gpu_info(), "steps": args.steps,
+            "translate_us_per_batch": {"tracked": [], "untracked": []},
+            "ms_per_step": {"dense": [], "untracked": [], "tracked": []}}
+    for r in range(args.rounds):
+        order = (False, True) if r % 2 == 0 else (True, False)
+        for tracked in order:
+            kd = run(wl, batches, True, args.steps, args.warmup, key_evict=tracked)
+            name = "tracked" if tracked else "untracked"
+            line["translate_us_per_batch"][name].append(kd["translate_us_per_batch"])
+            line["ms_per_step"][name].append(kd["ms_per_step"])
+        line["ms_per_step"]["dense"].append(run(wl, batches, False, args.steps, args.warmup)["ms_per_step"])
+    line.update(evict_times(wl, max(args.rounds, 3)))
+    print(json.dumps(line))
+    return 0
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="fm_c2", choices=["fm_c2", "ffm_c3", "nfm_c4"])
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=2, help="dense / keyed alternations")
+    ap.add_argument("--evict", action="store_true", help="row eviction (key_evict) instead: see the module docstring")
     args = ap.parse_args()
     import torch
     from lightctr_b200 import build as lbuild
     lbuild.build()
     if not torch.cuda.is_available():
         raise SystemExit("bench_keys.py: no CUDA device (the product has no CPU path)")
+    if args.evict:
+        return main_evict(args)
     wl = dict(WORKLOADS[args.workload])
     batches = make_batches(wl, wl.get("nb", 8))
     line = {"workload": wl["desc"], "keys": "key = fmix64(fid), keyed context of capacity F", "gpu": gpu_info(),
