@@ -81,13 +81,13 @@ typedef struct lctr_cfg {
     int32_t deterministic;
     /* LCTR_KEYS_DENSE (0): fids index the tables directly, feature_cnt = max fid + 1.
      * LCTR_KEYS_HASHED (1): batches carry uint64_t hashed keys (lctr_upload_batch_keys); the library maps each key to a
-     * table row, creating and initialising rows on first sight.  feature_cnt is then the row CAPACITY (< 2^32 - 1); one
-     * GPU and deterministic = 0 only. */
+     * table row, creating and initialising rows on first sight.  feature_cnt is then the row CAPACITY (< 2^32 - 1, and
+     * >= world); deterministic = 0 only.  world > 1: the key table is sharded, see "keyed mode on several GPUs" below. */
     int32_t key_mode;
     uint64_t csc_row_block;
     float ema_rate;           /* GradientUpdater::__global_ema_rate (RMSpropUpdater_Num, gradientUpdater.h:200-233); 0 => 0.99 (main.cpp:66) */
     /* keyed mode only: 1 = every row records the insert-upload that last met it (8 B per row), which lctr_evict_keys
-     * needs; 0 = no record (refused on a dense context when non-zero) */
+     * needs; 0 = no record (refused on a dense context when non-zero, and with world > 1) */
     int32_t key_evict;
     uint32_t reserved[2];
 } lctr_cfg;
@@ -166,6 +166,28 @@ int lctr_set_key_init(lctr_ctx* ctx, uint64_t seed, float scale);
  * fresh optimizer state.  Refused on a dense context and on a keyed context created with key_evict = 0. */
 int lctr_evict_keys(lctr_ctx* ctx, uint64_t max_idle, uint64_t max_rows, uint64_t* keys_out, float* W_out, float* V_out,
                     uint64_t cap_out, uint64_t* n_evicted);
+/* Keyed mode on several GPUs (world > 1; the reference's parameter servers key by size_t and create on first touch,
+ * distribut/paramserver.h:315-339).
+ * Owner rule: key k lives on rank fmix64(k) >> (64 - log2 world) (the top bits of MurmurHash3's 64-bit finaliser); the
+ * owner's table takes its home slot from the low bits.  Local row l of rank o is global row l * world + o -- the dense
+ * convention -- so lctr_upload_params / lctr_download_params with full arrays of feature_cnt rows keep working, and rank o
+ * holds at most the number of global rows < feature_cnt it owns.
+ * lctr_upload_batch_keys (insert = 1) is COLLECTIVE: every rank calls it for the same slot, in the same order, each with
+ * its own batch (steps are collective in the same way).  Each rank dedupes its batch's keys, sends each owner its keys,
+ * and as owner creates and initialises the rows of the keys it received (values as on one GPU: they depend on the key
+ * only, so a sharded run starts from what a single-GPU keyed run starts from).  Every rank then reads every owner's status
+ * and fails the upload with the same message, naming the first failing owner (shard capacity exhausted, key table full);
+ * keys inserted before keep their rows, and the slot is unusable until it is uploaded again, as on one GPU.  A rank whose
+ * own arguments are refused still takes part with an empty, refused list, so its peers fail the upload at once.  The
+ * waits of the upload are bounded (a few seconds): the ranks must enter it about together, else it fails as timed out.
+ * cfg.max_nnz must be > 0: it bounds the entries of a batch and its distinct keys, and sizes the per-batch key tables.
+ * Per rank, no communication: lctr_download_keys gives the rank's own local row -> key map; lctr_lookup_keys gives the
+ * GLOBAL row of the keys this rank holds, -1 otherwise; lctr_upload_keyed_params takes from the arrays only the keys this
+ * rank owns, in array order, so the same call on every rank seeds the sharded table; lctr_set_key_init must be called
+ * with the same values on every rank.  lctr_device_bytes counts the shard's key table in the shard figure and the batch
+ * dedupe table and inbox key arrays in the exchange figure.
+ * Refused with world > 1: key_evict = 1 (at lctr_create), insert = 0 uploads (lctr_predict is single-GPU) and
+ * checkpoints. */
 
 /* ---- the hot path --------------------------------------------------------------------------- */
 /* One reference "batch": forward (gather + interaction [+ MLP]) -> loss -> backward scatter-add ->

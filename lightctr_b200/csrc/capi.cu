@@ -176,9 +176,15 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
                cfg->optimizer);
     LCTR_CHECK(cfg->key_mode == LCTR_KEYS_DENSE || cfg->key_mode == LCTR_KEYS_HASHED, "lctr_create: bad key_mode %d", cfg->key_mode);
     if (cfg->key_mode == LCTR_KEYS_HASHED) {
-        // the owner map of several GPUs would have to be keyed too; exact-order modes build their feature-major view on
-        // the host from host ids, which a keyed upload does not have
-        LCTR_CHECK(cfg->world <= 1, "lctr_create: keyed mode is single-GPU (world %d)", cfg->world);
+        // exact-order modes build their feature-major view on the host from host ids, which a keyed upload does not have;
+        // on several GPUs an eviction would renumber rows across the shards, which needs a collective of its own
+        LCTR_CHECK(cfg->world <= 1 || cfg->max_nnz > 0,
+                   "lctr_create: keyed mode on several GPUs (world %d) needs cfg.max_nnz > 0, which sizes the per-batch key "
+                   "tables; without it keyed mode is single-GPU", cfg->world);
+        LCTR_CHECK(cfg->world <= 1 || cfg->key_evict == 0,
+                   "lctr_create: key_evict = 1 is single-GPU (world %d): evicting from a sharded keyed table is not supported", cfg->world);
+        LCTR_CHECK(cfg->world <= 1 || cfg->feature_cnt >= (uint64_t)cfg->world,
+                   "lctr_create: keyed capacity (feature_cnt %llu) below world %d", (unsigned long long)cfg->feature_cnt, cfg->world);
         LCTR_CHECK(cfg->deterministic == 0, "lctr_create: keyed mode needs deterministic = 0 (got %d)", cfg->deterministic);
         LCTR_CHECK(cfg->feature_cnt > 0 && cfg->feature_cnt < (1ull << 32) - 1, "lctr_create: keyed capacity (feature_cnt) out of range");
     }
@@ -329,12 +335,12 @@ int lctr_upload_params(lctr_ctx* c, const float* W, const float* V) {
         std::vector<float> w, v;
         if (W) {
             w.assign(c->Fl, 0.f);
-            for (size_t f = (size_t)me, l = 0; f < c->F; f += R, l++) w[l] = W[f];
+            for (size_t f = (size_t)me, l = 0; f < api_rows(c); f += R, l++) w[l] = W[f];
             LCTR_CUDA(cudaMemcpyAsync(c->W, w.data(), c->Fl * sizeof(float), cudaMemcpyHostToDevice, c->stream));
         }
         if (V) {
             v.assign(c->Fl * c->rowlen, 0.f);
-            for (size_t f = (size_t)me, l = 0; f < c->F; f += R, l++)
+            for (size_t f = (size_t)me, l = 0; f < api_rows(c); f += R, l++)
                 memcpy(&v[l * c->rowlen], V + f * c->rowlen, c->rowlen * sizeof(float));
             LCTR_CUDA(cudaMemcpyAsync(c->V, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
         }
@@ -357,7 +363,7 @@ int lctr_download_params(lctr_ctx* c, float* W, float* V) {
     LCTR_CUDA(cudaMemcpyAsync(w.data(), c->W, w.size() * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaMemcpyAsync(v.data(), c->V, v.size() * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    for (size_t f = (size_t)me, l = 0; f < c->F; f += R, l++) {
+    for (size_t f = (size_t)me, l = 0; f < api_rows(c); f += R, l++) {
         if (W) W[f] = w[l];
         if (V) memcpy(V + f * c->rowlen, &v[l * c->rowlen], c->rowlen * sizeof(float));
     }
@@ -480,11 +486,9 @@ int lctr_upload_batch(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const in
     return upload_batch_on(c, c->stream, slot, rows, nnz, row_ptr, fid, field, val, label);
 }
 
-int lctr_upload_batch_keys(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint64_t* key,
-                           const uint16_t* field, const float* val, const int32_t* label, int insert) {
-    LCTR_CHECK(c, "null ctx");
-    LCTR_CHECK(c->keys, "lctr_upload_batch_keys: the context was not created with key_mode = LCTR_KEYS_HASHED");
-    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
+// the arguments of a keyed upload, checked on the host before anything is sent
+static int check_batch_keys(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint64_t* key,
+                            const uint16_t* field, const int32_t* label) {
     LCTR_CHECK(rows >= 0 && nnz >= 0 && row_ptr && (nnz == 0 || key) && (rows == 0 || label), "upload_batch_keys: null input");
     LCTR_CHECK(row_ptr[0] == 0 && row_ptr[rows] == nnz, "upload_batch_keys: row_ptr must run from 0 to nnz (%lld .. %lld, nnz %lld)",
                (long long)row_ptr[0], (long long)row_ptr[rows], (long long)nnz);
@@ -499,6 +503,67 @@ int lctr_upload_batch_keys(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, con
                        (long long)i, c->cfg.field_cnt);
     LCTR_CHECK((c->cfg.model != LCTR_MODEL_FFM && c->cfg.model != LCTR_MODEL_WND) || field || nnz == 0,
                "upload_batch_keys: FFM / Wide&Deep need the field array");
+    return 0;
+}
+
+// world > 1: a collective call (every rank, same slot, same order).  Requester: dedupe, slot map, keyed lists to the owners;
+// owner: translation of what it received (dist.cu).  A rank whose own part fails still takes part with a refusal, so every
+// rank returns: its own error, or the first failing owner's status, which every rank reports alike.
+static int upload_batch_keys_dist(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint64_t* key,
+                                  const uint16_t* field, const float* val, const int32_t* label, int insert) {
+    if (dist_keys_begin(c)) return 1;
+    Slot& s = c->slots[slot];
+    s.key_state = SLOT_KEYS_INVALID;  // until every owner has translated the batch
+    s.fused_valid = false;
+    int rc = check_batch_keys(c, rows, nnz, row_ptr, key, field, label);
+    if (!rc && !insert) {
+        set_error("lctr_upload_batch_keys: insert = 0 is single-GPU (lookup-only slots serve lctr_predict, which a sharded "
+                  "context refuses)");
+        rc = 1;
+    }
+    if (!rc && (rows == 0 || nnz == 0)) {
+        set_error("lctr_upload_batch_keys: empty batch (%lld rows, %lld entries) on a multi-GPU context", (long long)rows,
+                  (long long)nnz);
+        rc = 1;
+    }
+    if (!rc && std::min<int64_t>(nnz, (int64_t)c->F) > (int64_t)std::min<uint64_t>(c->cfg.max_nnz ? c->cfg.max_nnz : c->F, c->F)) {
+        set_error("lctr_upload_batch_keys: batch of %lld entries exceeds the key capacity of the multi-GPU context (cfg.max_nnz)",
+                  (long long)nnz);
+        rc = 1;
+    }
+    if (!rc && (rows > s.cap_rows || nnz > s.cap_nnz)) {
+        rc = cudaStreamSynchronize(c->stream) != cudaSuccess || slot_reserve(c, s, rows, nnz) ||
+             cudaStreamSynchronize(c->stream) != cudaSuccess;
+        if (rc && g_err.empty()) set_error("lctr_upload_batch_keys: slot buffers could not be reserved");
+    }
+    if (!rc) rc = dist_keys_dedupe(c, s, key, nnz);
+    if (!rc) rc = upload_batch_on(c, c->stream, slot, rows, nnz, row_ptr, nullptr, field, val, label, true);
+    std::string own;
+    if (rc) {
+        own = g_err;
+        s.key_state = SLOT_KEYS_INVALID;
+        if (dist_keys_refuse(c, slot)) return 1;
+    }
+    const int xrc = dist_keys_translate(c, slot);
+    if (rc) {
+        g_err = own;
+        return 1;
+    }
+    if (xrc) {
+        s.key_state = SLOT_KEYS_INVALID;
+        return 1;
+    }
+    s.key_state = SLOT_KEYS_OK;
+    return 0;
+}
+
+int lctr_upload_batch_keys(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint64_t* key,
+                           const uint16_t* field, const float* val, const int32_t* label, int insert) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(c->keys, "lctr_upload_batch_keys: the context was not created with key_mode = LCTR_KEYS_HASHED");
+    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
+    if (c->cfg.world > 1) return upload_batch_keys_dist(c, slot, rows, nnz, row_ptr, key, field, val, label, insert);
+    if (check_batch_keys(c, rows, nnz, row_ptr, key, field, label)) return 1;
     Slot& s = c->slots[slot];
     if (rows > s.cap_rows || nnz > s.cap_nnz) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));  // buffers about to be reallocated may still be in use

@@ -374,6 +374,11 @@ int dist_send_keys(lctr_ctx* c, Slot& s, int slot, cudaStream_t st);            
 int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait);           // owner-driven pull of the step's rows
 int dist_post_step(lctr_ctx* c, Slot& s, int slot, int64_t rows_divisor);         // push gradients, owner-side merge + update
 int dist_check_overflow(lctr_ctx* c);
+// keyed contexts (collective upload): begin, requester dedupe into s.fid, refusal in place of the lists, owner translation
+int dist_keys_begin(lctr_ctx* c);
+int dist_keys_dedupe(lctr_ctx* c, Slot& s, const uint64_t* h_keys, int64_t nnz);
+int dist_keys_refuse(lctr_ctx* c, int slot);
+int dist_keys_translate(lctr_ctx* c, int slot);
 size_t dist_bytes(const lctr_ctx* c);
 __global__ void compact_touched_kernel(uint8_t* touched, size_t F, uint32_t* list, unsigned int* n_list,
                                        const unsigned long long* wait_flags, int n_wait, unsigned long long wait_epoch);

@@ -27,6 +27,8 @@
 //               landed" flags                                                                    (push_rows_kernel)
 //     4 owner   inbox rows are added into update_g with local REDs (waits for the flags)          (merge_kernel)
 //               sparse updater on the shard                                                      (opt.cu)
+// Keyed contexts (cfg.key_mode = LCTR_KEYS_HASHED) change the upload only: the batch's keys are deduped into batch-local
+// ids, the lists carry the keys, and each owner translates them into its shard's rows before the step (see "keyed upload").
 // Launches per step: 6; the barriers between the phases are flags written at the tail of one kernel and polled at the
 // head of the next -- no barrier launches, no host involvement.
 #include <stdlib.h>
@@ -35,6 +37,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "keys.cuh"
 #include "opt.cuh"
 
 namespace lctr {
@@ -55,15 +58,21 @@ struct ArenaLayout {
     size_t flags;        // u64 [3 + kNumSlots][kMaxWorld]: row 0 rows delivered, 1 pushes landed, 3 + s keys of slot s
     size_t key_inbox;    // [kNumSlots][2][world] regions (2: parity of the slot's upload generation -- a list may still be read
                          // by a slower owner's merge when its sender already uploads the slot's next batch):
-                         // 64 B header {u32 count} + cap_pair x uint2 {row, requester slot}
+                         // 64 B header {u32 count, u32 requester status (keyed)} + cap_pair x uint2 {row, requester slot}
+                         // (+ keyed contexts: cap_pair x u64 keys at key_keys)
     size_t key_region;   // bytes per region
+    size_t key_keys;     // keyed: offset of the key array inside a region
     size_t cacheW;       // world * cap_pair floats (row p)
     size_t cacheV;       // world * cap_pair x rowlen floats
     size_t grad_inbox;   // [world] regions of cap_pair x recw floats
     size_t grad_region;  // bytes per region
     size_t total;
 };
-enum { FLAG_PULLED = 0, FLAG_PUSHED = 1, FLAG_KEYS = 3 };
+enum { FLAG_PULLED = 0, FLAG_PUSHED = 1, FLAG_XLATED = 2, FLAG_KEYS = 3 };
+// statuses of a keyed upload (code << 8 | rank): raised by every owner on every requester in FLAG_XLATED as seq << 16 | status
+enum { XS_OK = 0, XS_REFUSED = 1, XS_INBOX = 2, XS_TIMEOUT = 3, XS_CAPACITY = 4, XS_TABLE_FULL = 5 };
+// bound of every wait of the keyed upload: ~4 s at the H100's boost clock (longer at lower clocks)
+constexpr long long kXlateWaitCycles = 1ll << 33;
 
 struct DistState {
     int rank = 0, world = 1, shift = 0;
@@ -95,6 +104,21 @@ struct DistState {
     unsigned long long epoch = 0;
     unsigned long long gen[kNumSlots] = {0};
     size_t bytes = 0;                 // device memory this module allocated
+    // keyed contexts (cfg.key_mode = LCTR_KEYS_HASHED): requester-side dedupe of a batch's keys into batch-local ids u,
+    // an open-addressing table of bt_T >= 2 * cap_keys slots cleared by the list of the slots it claimed
+    bool keyed = false;
+    unsigned long long* bt_key = nullptr;     // [bt_T] slot keys, kEmptyKey = free
+    uint32_t* bt_row = nullptr;               // [bt_T] batch-local id of the slot's key
+    uint32_t* bt_claimed = nullptr;           // [bt_T] slots claimed by the running dedupe
+    unsigned long long* bt_cnt = nullptr;     // keys claimed (the batch's U when <= cap_keys)
+    unsigned int* bt_flags = nullptr;         // [3] U > cap_keys, table full, (unused)
+    unsigned long long* batch_key = nullptr;  // [cap_keys] key of batch-local id u
+    unsigned long long* bt_stage = nullptr;   // the batch's keys, one per entry
+    size_t bt_T = 0, bt_stage_cap = 0;
+    unsigned int* xstat = nullptr;            // owner side: status of the running translation (wait kernel -> the others)
+    unsigned long long* xres = nullptr;       // [kMaxWorld] status every owner raised for this rank's upload
+    unsigned long long xseq = 0;              // keyed uploads so far (the same on every rank: the upload is collective)
+    bool posted = false;                      // this upload's lists (or its refusal) are out
 };
 
 __device__ __forceinline__ unsigned long long* flag_ptr(unsigned char* arena, const ArenaLayout& A, int row, int col) {
@@ -144,10 +168,13 @@ __device__ __forceinline__ void raise_flags_last_block(const PeerTable& P, const
 // upload: per owner, the list of shard-local rows -> the owner's key inbox; rows of the exchange are then addressed by
 // p = owner * cap_pair + position in that list, on both sides
 // ---------------------------------------------------------------------------------------------------------------
+// KEYED: uniq holds batch-local ids u; the owner comes from the top bits of fmix64(batch_key[u]), the pair is posted as
+// {~0 (translated by the owner), requester slot} and the key goes to the key array of the same region
+template <bool KEYED>
 __global__ void __launch_bounds__(256)
 send_keys_kernel(const uint32_t* __restrict__ uniq, const unsigned int* __restrict__ n_uniq, PeerTable P, ArenaLayout A,
                  int me, int world, int slot, int shift, unsigned cap_pair, unsigned int* __restrict__ send_cnt,
-                 uint32_t* __restrict__ opos, int* __restrict__ overflow) {
+                 uint32_t* __restrict__ opos, int* __restrict__ overflow, const unsigned long long* __restrict__ batch_key) {
     __shared__ unsigned s_cnt[kMaxWorld], s_base[kMaxWorld];
     const unsigned n = *n_uniq;
     const unsigned mask = (unsigned)world - 1;
@@ -157,9 +184,15 @@ send_keys_kernel(const uint32_t* __restrict__ uniq, const unsigned int* __restri
         const unsigned i = c0 + threadIdx.x;
         uint32_t f = 0;
         unsigned o = 0, rk = 0;
+        unsigned long long key = 0;
         if (i < n) {
             f = uniq[i];
-            o = f & mask;
+            if (KEYED) {
+                key = batch_key[f];
+                o = owner_of_key(key, shift);
+            } else {
+                o = f & mask;
+            }
             rk = atomicAdd(&s_cnt[o], 1u);
         }
         __syncthreads();
@@ -168,8 +201,14 @@ send_keys_kernel(const uint32_t* __restrict__ uniq, const unsigned int* __restri
         if (i < n) {
             const unsigned j = s_base[o] + rk;
             if (j < cap_pair) {
-                uint2* pairs = reinterpret_cast<uint2*>(P.p[o].arena + A.key_inbox + ((size_t)slot * world + me) * A.key_region + 64);
-                pairs[j] = make_uint2(f >> shift, i);
+                unsigned char* region = P.p[o].arena + A.key_inbox + ((size_t)slot * world + me) * A.key_region;
+                uint2* pairs = reinterpret_cast<uint2*>(region + 64);
+                if (KEYED) {
+                    pairs[j] = make_uint2(kNoRow, i);
+                    reinterpret_cast<unsigned long long*>(region + A.key_keys)[j] = key;
+                } else {
+                    pairs[j] = make_uint2(f >> shift, i);
+                }
                 opos[i] = o * cap_pair + j;
             } else {
                 *overflow = 1;  // reported at the next host synchronisation; the row index stays in bounds
@@ -181,15 +220,18 @@ send_keys_kernel(const uint32_t* __restrict__ uniq, const unsigned int* __restri
     if (threadIdx.x == 0) __threadfence_system();  // after the loop's last CTA barrier: cumulative over the CTA's stores
 }
 // counts into the owners' headers (and kept locally for the push), counters re-armed, then the generation flag of
-// (slot, me) on every owner
+// (slot, me) on every owner.  Keyed contexts (overflow != nullptr) also post the requester status in hdr[1]: 1 = this rank
+// refused its batch (the lists are empty), 2 = a list outgrew its region.
 __global__ void send_keys_finish_kernel(PeerTable P, ArenaLayout A, int me, int world, int slot, int flag_slot, unsigned cap_pair,
-                                        unsigned int* send_cnt, unsigned int* seg_cnt, unsigned long long gen) {
+                                        unsigned int* send_cnt, unsigned int* seg_cnt, unsigned long long gen,
+                                        const int* overflow, int refused) {
     const int o = threadIdx.x;
     __threadfence_system();
     if (o < world) {
         unsigned int* hdr = reinterpret_cast<unsigned int*>(P.p[o].arena + A.key_inbox + ((size_t)slot * world + me) * A.key_region);
-        const unsigned n = min(send_cnt[o], cap_pair);
+        const unsigned n = refused ? 0u : min(send_cnt[o], cap_pair);
         hdr[0] = n;
+        if (overflow) hdr[1] = refused ? 1u : (*overflow ? 2u : 0u);
         seg_cnt[o] = n;
         send_cnt[o] = 0;
         __threadfence_system();
@@ -225,6 +267,151 @@ clear_hot_p_kernel(const uint32_t* __restrict__ opos_prev, const uint32_t* __res
                    uint32_t* __restrict__ hot_p) {
     for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n_prev; i += gridDim.x * blockDim.x)
         if (hot_of_prev[i] != 0xffffffffu) hot_p[opos_prev[i]] = 0xffffffffu;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// keyed upload (cfg.key_mode = LCTR_KEYS_HASHED).  Requester: the batch's keys -> batch-local ids u in [0, U) (the slot
+// map and the send run on them unchanged, batch_key[u] gives the owner and the key that travels).  Owner: every key it
+// received -> its local row (claimed and lazily initialised on first sight), written into pairs[j].x of its own inbox, so
+// that serve / merge / union / updater kernels run unmodified; then a status flag on every requester.  Owner-side only,
+// posted stores only: no rank probes or inserts into a peer's table.
+// ---------------------------------------------------------------------------------------------------------------
+// dedupe: claim a slot per distinct key; the claimer takes the next id and records the slot for the clear
+__global__ void __launch_bounds__(256) batch_insert_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t,
+                                                           uint32_t* __restrict__ claimed_slots) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;  // whole tiles leave together
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const unsigned long long key = keys[i];
+    bool claimed;
+    const long long pos = tile_claim(t, key, sub, gmask, &claimed);
+    if (sub != 0) return;
+    if (pos < 0) { t.flags[1] = 1u; return; }
+    if (!claimed) return;
+    const unsigned long long u = atomicAdd(t.count, 1ull);  // < table slots: every claim holds its own slot
+    claimed_slots[u] = (uint32_t)pos;
+    if (u < t.cap) {
+        t.row[pos] = (uint32_t)u;
+        t.row_key[u] = key;
+    } else {
+        t.row[pos] = kNoRow;
+        t.flags[0] = 1u;
+    }
+}
+// batch-local id of every entry into the slot's fid array (0 for a key without an id: the upload fails then)
+__global__ void __launch_bounds__(256) batch_find_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t,
+                                                         uint32_t* __restrict__ fid) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const long long pos = tile_find(t, keys[i], sub, gmask);
+    if (sub != 0) return;
+    const uint32_t u = pos >= 0 ? __ldg(t.row + pos) : kNoRow;
+    fid[i] = u == kNoRow ? 0u : u;
+}
+// the slots the dedupe claimed back to empty
+__global__ void __launch_bounds__(256) batch_clear_kernel(KeyView t, const uint32_t* __restrict__ claimed_slots, size_t T) {
+    const size_t n = min((size_t)*t.count, T);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t pos = claimed_slots[i];
+        t.key[pos] = kEmptyKey;
+        t.row[pos] = kNoRow;
+    }
+}
+
+__device__ __forceinline__ unsigned char* key_region_of(const PeerTable& P, const ArenaLayout& A, int rank, int slot2, int world, int q) {
+    return P.p[rank].arena + A.key_inbox + ((size_t)slot2 * world + q) * A.key_region;
+}
+
+// owner: every requester's lists of this (slot, generation) have landed, or a bounded wait has run out; a requester that
+// refused its batch or overflowed a region fails the translation.  *xstat = first problem in rank order (0: none).
+__global__ void xlate_wait_kernel(PeerTable P, ArenaLayout A, int me, int world, int slot2, int flag_slot, unsigned long long gen,
+                                  unsigned int* xstat) {
+    __shared__ unsigned st[kMaxWorld];
+    const int q = threadIdx.x;
+    if (q < world) {
+        const volatile unsigned long long* f = flag_ptr(P.p[me].arena, A, FLAG_KEYS + flag_slot, q);
+        const long long t0 = clock64();
+        bool late = false;
+        while (*f < gen) {
+            if (clock64() - t0 > kXlateWaitCycles) { late = true; break; }
+            __nanosleep(256);
+        }
+        unsigned code = XS_OK;
+        if (late) {
+            code = XS_TIMEOUT;
+        } else {
+            __threadfence();
+            const unsigned rs = reinterpret_cast<const volatile unsigned int*>(key_region_of(P, A, me, slot2, world, q))[1];
+            code = rs == 1u ? XS_REFUSED : (rs == 2u ? XS_INBOX : XS_OK);
+        }
+        st[q] = code == XS_OK ? 0u : (code << 8 | (unsigned)q);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned first = 0;
+        for (int r = world - 1; r >= 0; r--) if (st[r]) first = st[r];
+        *xstat = first;
+    }
+}
+
+// owner: MODE 0 claims a row for every received key (the key table's insert, new rows recorded for key_init_kernel);
+// MODE 1 writes the local row of each into pairs[j].x (0 in place of a key left without a row; the upload fails then)
+template <int MODE>
+__global__ void __launch_bounds__(256) xlate_keys_kernel(PeerTable P, ArenaLayout A, int me, int world, int slot2,
+                                                         const unsigned int* __restrict__ xstat, KeyView t) {
+    if (*xstat) return;
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const unsigned tile0 = (blockIdx.x * blockDim.x + threadIdx.x) / kGroup, ntiles = gridDim.x * blockDim.x / kGroup;
+    for (int q = 0; q < world; q++) {
+        unsigned char* region = key_region_of(P, A, me, slot2, world, q);
+        const unsigned n = *reinterpret_cast<const volatile unsigned int*>(region);
+        const unsigned long long* keys = reinterpret_cast<const unsigned long long*>(region + A.key_keys);
+        uint2* pairs = reinterpret_cast<uint2*>(region + 64);
+        for (unsigned j = tile0; j < n; j += ntiles) {  // the 16 lanes of a tile share j
+            if (MODE == 0) {
+                tile_insert(t, keys[j], sub, gmask);
+            } else {
+                const long long pos = tile_find(t, keys[j], sub, gmask);
+                if (sub == 0) {
+                    uint32_t r = pos >= 0 ? __ldg(t.row + pos) : kNoRow;
+                    if (r == kNoRow) { t.flags[pos >= 0 ? 0 : 1] = 1u; r = 0; }
+                    pairs[j].x = r;
+                }
+            }
+        }
+    }
+}
+
+// owner: its status (the wait's, else the table's) on every requester as seq << 16 | status; then, as requester, the
+// statuses every owner raised for me (bounded wait) into xres[owner]
+__global__ void xlate_finish_kernel(PeerTable P, ArenaLayout A, int me, int world, unsigned long long seq,
+                                    const unsigned int* __restrict__ xstat, const unsigned int* __restrict__ tflags,
+                                    unsigned long long* __restrict__ xres) {
+    __shared__ unsigned s_st;
+    if (threadIdx.x == 0) {
+        unsigned st = *xstat;
+        if (!st) st = tflags[1] ? (XS_TABLE_FULL << 8 | (unsigned)me) : (tflags[0] ? (XS_CAPACITY << 8 | (unsigned)me) : 0u);
+        s_st = st;
+    }
+    __syncthreads();
+    const int o = threadIdx.x;
+    if (o < world) {
+        volatile unsigned long long* f = flag_ptr(P.p[o].arena, A, FLAG_XLATED, me);
+        *f = seq << 16 | s_st;
+        __threadfence_system();
+        const volatile unsigned long long* g = flag_ptr(P.p[me].arena, A, FLAG_XLATED, o);
+        const long long t0 = clock64();
+        unsigned long long v;
+        while (((v = *g) >> 16) < seq) {
+            if (clock64() - t0 > kXlateWaitCycles) { v = seq << 16 | (XS_TIMEOUT << 8 | (unsigned)o); break; }
+            __nanosleep(256);
+        }
+        xres[o] = v & 0xffffull;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -525,6 +712,7 @@ int dist_alloc(lctr_ctx* c) {
     DistState* d = new DistState();
     c->dist = d;
     d->rank = c->cfg.rank; d->world = R;
+    d->keyed = c->cfg.key_mode == LCTR_KEYS_HASHED;
     while ((1 << d->shift) < R) d->shift++;
     if (const char* de = getenv("LCTR_DIST_DEBUG")) {
         const int m = atoi(de);
@@ -537,14 +725,16 @@ int dist_alloc(lctr_ctx* c) {
     LCTR_CHECK(c->rowlen % 4 == 0, "multi-GPU exchange moves rows in 16 B slices: rowlen %zu must be a multiple of 4", c->rowlen);
     // keys of one batch: at most its entry count (cfg.max_nnz), at most the id space
     d->cap_keys = c->cfg.max_nnz ? std::min<size_t>(c->cfg.max_nnz, c->F) : c->F;
-    // keys one requester sends one owner: U / R on average (owner = fid mod R, binomially tight); 1.5x that plus slack
+    // keys one requester sends one owner: U / R on average (owner = fid mod R, or the top bits of fmix64(key): binomially
+    // tight either way); 1.5x that plus slack
     d->cap_pair = std::min<size_t>(c->Fl, 3 * d->cap_keys / (2 * R) + 4096);
     d->rows_x = (size_t)R * d->cap_pair;
     d->recw = (int)((c->rowlen + 4 + 3) / 4 * 4);
     ArenaLayout& A = d->A;
     size_t off = 0;
     A.flags = off; off = align_up(off + (size_t)(3 + kNumSlots) * kMaxWorld * sizeof(unsigned long long), 256);
-    A.key_region = align_up(64 + d->cap_pair * sizeof(uint2), 256);
+    A.key_keys = 64 + d->cap_pair * sizeof(uint2);
+    A.key_region = align_up(A.key_keys + (d->keyed ? d->cap_pair * sizeof(unsigned long long) : 0), 256);
     A.key_inbox = off; off += A.key_region * kNumSlots * 2 * R;
     A.cacheW = off; off = align_up(off + d->rows_x * sizeof(float), 256);
     A.cacheV = off; off = align_up(off + d->rows_x * c->rowlen * sizeof(float), 256);
@@ -586,6 +776,22 @@ int dist_alloc(lctr_ctx* c) {
         LCTR_CUDA(cudaMemsetAsync(d->cgV, 0, d->rows_x * c->rowlen * sizeof(float), c->stream));
         d->bytes += d->rows_x * (c->rowlen + 1) * sizeof(float);
     }
+    if (d->keyed) {  // the requester's batch table (2x the key capacity of a batch, a power of two) and the status words
+        size_t T = kGroup;
+        while (T < 2 * d->cap_keys) T <<= 1;
+        d->bt_T = T;
+        LCTR_CUDA(cudaMalloc((void**)&d->bt_key, T * sizeof(unsigned long long)));
+        LCTR_CUDA(cudaMalloc((void**)&d->bt_row, T * sizeof(uint32_t)));
+        LCTR_CUDA(cudaMalloc((void**)&d->bt_claimed, T * sizeof(uint32_t)));
+        LCTR_CUDA(cudaMalloc((void**)&d->bt_cnt, sizeof(unsigned long long)));
+        LCTR_CUDA(cudaMalloc((void**)&d->bt_flags, 3 * sizeof(unsigned int)));
+        LCTR_CUDA(cudaMalloc((void**)&d->batch_key, d->cap_keys * sizeof(unsigned long long)));
+        LCTR_CUDA(cudaMalloc((void**)&d->xstat, sizeof(unsigned int)));
+        LCTR_CUDA(cudaMalloc((void**)&d->xres, kMaxWorld * sizeof(unsigned long long)));
+        LCTR_CUDA(cudaMemsetAsync(d->bt_key, 0xff, T * sizeof(unsigned long long), c->stream));
+        LCTR_CUDA(cudaMemsetAsync(d->bt_row, 0xff, T * sizeof(uint32_t), c->stream));
+        d->bytes += T * (sizeof(unsigned long long) + 2 * sizeof(uint32_t)) + d->cap_keys * sizeof(unsigned long long);
+    }
     c->dist_rows = d->rows_x;
     // compute view: the batch-compact cache and gradient rows (indexed by exchange row p)
     c->cW = reinterpret_cast<float*>(d->arena + A.cacheW);
@@ -609,6 +815,10 @@ int dist_free(lctr_ctx* c) {
     if (d->own_uniq) { cudaFree(d->own_uniq); cudaFree(d->own_pos); cudaFree(d->n_own); cudaFree(d->posmap); cudaFree(d->own_mark); }
     if (d->cgW) cudaFree(d->cgW);
     if (d->cgV) cudaFree(d->cgV);
+    if (d->keyed) {
+        cudaFree(d->bt_key); cudaFree(d->bt_row); cudaFree(d->bt_claimed); cudaFree(d->bt_cnt); cudaFree(d->bt_flags);
+        cudaFree(d->batch_key); cudaFree(d->bt_stage); cudaFree(d->xstat); cudaFree(d->xres);
+    }
     c->cW = c->cV = c->cgW = c->cgV = nullptr;
     delete d;
     c->dist = nullptr;
@@ -636,14 +846,138 @@ int dist_send_keys(lctr_ctx* c, Slot& s, int slot, cudaStream_t st) {
     uint32_t* opos = d->opos + (size_t)slot * d->cap_keys;
     uint32_t* hot_p = d->hot_p ? d->hot_p + (size_t)slot * d->rows_x : nullptr;
     if (hot_p) LCTR_CUDA(cudaMemsetAsync(hot_p, 0xff, d->rows_x * sizeof(uint32_t), st));  // the previous batch's hot rows
-    send_keys_kernel<<<grid, 256, 0, st>>>(s.uniq, s.n_uniq, d->peers, d->A, d->rank, d->world, slot2, d->shift, (unsigned)d->cap_pair,
-                                           d->send_cnt, opos, d->overflow);
+    if (d->keyed) {  // an overflow fails this upload only (reported through the owners' statuses)
+        LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), st));
+        send_keys_kernel<true><<<grid, 256, 0, st>>>(s.uniq, s.n_uniq, d->peers, d->A, d->rank, d->world, slot2, d->shift,
+                                                     (unsigned)d->cap_pair, d->send_cnt, opos, d->overflow, d->batch_key);
+    } else {
+        send_keys_kernel<false><<<grid, 256, 0, st>>>(s.uniq, s.n_uniq, d->peers, d->A, d->rank, d->world, slot2, d->shift,
+                                                      (unsigned)d->cap_pair, d->send_cnt, opos, d->overflow, nullptr);
+    }
     send_keys_finish_kernel<<<1, 32, 0, st>>>(d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair, d->send_cnt,
-                                              d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot]);
+                                              d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow : nullptr, 0);
+    d->posted = d->keyed;
     const unsigned rg = (unsigned)std::max<int64_t>(1, std::min<int64_t>((s.nnz + 255) / 256, (int64_t)c->sm_count * 8));
     remap_entries_kernel<<<rg, 256, 0, st>>>(nullptr, s.nnz, opos, s.ent_pslot, s.ent_slot, hot_p ? s.hot_of : nullptr, s.n_uniq, hot_p);
     c->launches += 3;
     LCTR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ---- keyed upload, host side (capi.cu: lctr_upload_batch_keys on world > 1) -------------------------------------------
+int dist_keys_begin(lctr_ctx* c) {
+    DistState* d = c->dist;
+    LCTR_CHECK(d->imported, "multi-GPU upload before lctr_ipc_import");
+    d->posted = false;
+    return 0;
+}
+
+// the batch's keys -> batch-local ids in s.fid (device), U of them; fails (nothing sent yet) when U > cap_keys
+int dist_keys_dedupe(lctr_ctx* c, Slot& s, const uint64_t* h_keys, int64_t nnz) {
+    DistState* d = c->dist;
+    if ((size_t)nnz > d->bt_stage_cap) {
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
+        cudaFree(d->bt_stage);
+        d->bt_stage = nullptr;
+        d->bt_stage_cap = 0;
+        const size_t cap = (size_t)nnz + (size_t)nnz / 2;
+        LCTR_CUDA(cudaMalloc((void**)&d->bt_stage, cap * sizeof(unsigned long long)));
+        d->bt_stage_cap = cap;
+    }
+    LCTR_CUDA(cudaMemcpyAsync(d->bt_stage, h_keys, (size_t)nnz * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
+    LCTR_CUDA(cudaMemsetAsync(d->bt_cnt, 0, sizeof(unsigned long long), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(d->bt_flags, 0, 3 * sizeof(unsigned int), c->stream));
+    const KeyView bt{d->bt_key, d->bt_row, d->batch_key, d->bt_cnt, d->bt_flags, nullptr, d->bt_T / kGroup, d->cap_keys};
+    const unsigned tg = (unsigned)std::max<int64_t>(1, (nnz * kGroup + 255) / 256);
+    const unsigned cg = (unsigned)std::max<int64_t>(1, std::min<int64_t>((std::min<int64_t>(nnz, (int64_t)d->bt_T) + 255) / 256,
+                                                                         (int64_t)c->sm_count * 8));
+    {
+        ProfScope prof(c, PROF_KEYS);
+        batch_insert_kernel<<<tg, 256, 0, c->stream>>>(d->bt_stage, nnz, bt, d->bt_claimed);
+        batch_find_kernel<<<tg, 256, 0, c->stream>>>(d->bt_stage, nnz, bt, s.fid);
+        batch_clear_kernel<<<cg, 256, 0, c->stream>>>(bt, d->bt_claimed, d->bt_T);
+    }
+    c->launches += 3;
+    LCTR_CUDA(cudaGetLastError());
+    unsigned long long u = 0;
+    unsigned int fl[3] = {0, 0, 0};
+    LCTR_CUDA(cudaMemcpyAsync(&u, d->bt_cnt, sizeof(u), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaMemcpyAsync(fl, d->bt_flags, sizeof(fl), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    LCTR_CHECK(!fl[1] && u <= d->cap_keys, "lctr_upload_batch_keys: the batch has %llu distinct keys, more than the key capacity "
+               "%zu of the multi-GPU context (cfg.max_nnz, at most feature_cnt + 1)", u, d->cap_keys);
+    return 0;
+}
+
+// a rank that cannot send its batch still posts empty lists, marked refused, so that every peer fails the upload at once
+int dist_keys_refuse(lctr_ctx* c, int slot) {
+    DistState* d = c->dist;
+    if (d->posted) return 0;
+    d->gen[slot]++;
+    const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
+    send_keys_finish_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair,
+                                                     d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->overflow, 1);
+    c->launches++;
+    LCTR_CUDA(cudaGetLastError());
+    d->posted = true;
+    return 0;
+}
+
+// owner side of the upload: translate what every requester sent me, raise my status on each, collect every owner's
+// status for my own lists.  Returns non-zero with the message every rank composes alike when an owner failed.
+int dist_keys_translate(lctr_ctx* c, int slot) {
+    DistState* d = c->dist;
+    const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
+    d->posted = false;
+    d->xseq++;
+    KeyView t = keys_view(c);
+    if (keys_reserve_new_rows(c, std::min(d->rows_x, keys_capacity(c)))) return 1;
+    t = keys_view(c);  // the scratch may have moved
+    LCTR_CUDA(cudaMemsetAsync(t.flags, 0, 3 * sizeof(unsigned int), c->stream));
+    const unsigned tg = (unsigned)std::max<int64_t>(1, std::min<int64_t>(((int64_t)d->rows_x * kGroup + 255) / 256,
+                                                                         (int64_t)c->sm_count * 16));
+    {
+        ProfScope prof(c, PROF_KEYS);
+        xlate_wait_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, slot, d->gen[slot], d->xstat);
+        xlate_keys_kernel<0><<<tg, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, d->xstat, t);
+        c->launches += 2;
+        LCTR_CUDA(cudaGetLastError());
+        if (keys_init_new_rows(c, (int64_t)std::min(d->rows_x, keys_capacity(c)))) return 1;
+        xlate_keys_kernel<1><<<tg, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, d->xstat, t);
+        xlate_finish_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, d->xseq, d->xstat, t.flags, d->xres);
+        c->launches += 2;
+        LCTR_CUDA(cudaGetLastError());
+    }
+    unsigned long long res[kMaxWorld] = {0};
+    LCTR_CUDA(cudaMemcpyAsync(res, d->xres, (size_t)d->world * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    for (int o = 0; o < d->world; o++) {
+        if (!res[o]) continue;
+        const unsigned code = (unsigned)(res[o] >> 8), r = (unsigned)(res[o] & 0xff);
+        const unsigned long long fc = c->cfg.feature_cnt;
+        switch (code) {
+            case XS_CAPACITY:
+                set_error("lctr_upload_batch_keys: owner rank %u: key shard capacity of %llu rows exhausted; the batch's new keys "
+                          "do not fit (cfg.feature_cnt %llu over %d ranks)", r, (fc + d->world - 1 - r) / d->world, fc, d->world);
+                break;
+            case XS_TABLE_FULL:
+                set_error("lctr_upload_batch_keys: owner rank %u: no free slot on a probe path of its key table", r);
+                break;
+            case XS_REFUSED:
+                set_error("lctr_upload_batch_keys: rank %u refused its part of this collective upload (its own error names "
+                          "the reason)", r);
+                break;
+            case XS_INBOX:
+                set_error("lctr_upload_batch_keys: rank %u: a per-owner key list outgrew its inbox (%zu records, bounded by "
+                          "cfg.max_nnz and by the rows of a shard)", r, d->cap_pair);
+                break;
+            default:
+                set_error("lctr_upload_batch_keys: timed out waiting for rank %u (every rank must make the same collective "
+                          "upload calls)", r);
+                break;
+        }
+        return 1;
+    }
     return 0;
 }
 

@@ -37,6 +37,11 @@
 // different stream from the reference's rand()-driven GaussRand (fm_algo_abst.h:62-65); only the scale default,
 // 1 / sqrt(k), is the reference's.
 //
+// Several GPUs (world > 1): each rank's table is the shard of the keys it owns (top bits of fmix64(key), keys.cuh) with
+// the capacity of the global rows < feature_cnt that rank holds; dist.cu translates the keys an upload sends each owner
+// with the insert and init above, and the per-rank calls below take only the owned keys (lctr_upload_keyed_params) or
+// return global rows (lctr_lookup_keys).
+//
 // Eviction (cfg.key_evict = 1; the reference's server map only grows, paramserver.h:315-339).  A host u64 clock advances
 // once per insert-upload, and key_find_kernel<0> of that upload stores it into last_seen[row] of every entry it
 // translates (plain stores: duplicates write the same value).  Untracked contexts pass a null stamp pointer, a uniform
@@ -57,13 +62,10 @@
 #include <algorithm>
 #include <vector>
 
-#include "common.cuh"
+#include "keys.cuh"
 
 namespace lctr {
 
-constexpr unsigned long long kEmptyKey = ~0ull;
-constexpr uint32_t kNoRow = 0xffffffffu;
-constexpr int kGroup = 16;  // slots per 128-byte probe group
 constexpr int kEvTile = 1024;  // rows per block of the eviction count / index kernels
 constexpr int kEvBins = 1 << 16;  // radix-select digit
 
@@ -93,63 +95,8 @@ struct KeyTable {
     unsigned long long* h_res = nullptr;      // pinned mirror
 };
 
-struct KeyView {
-    unsigned long long* key;
-    uint32_t* row;
-    unsigned long long* row_key;
-    unsigned long long* count;
-    unsigned int* flags;
-    uint32_t* new_rows;
-    size_t ngroups, cap;
-};
-
 static KeyView view(const KeyTable* t) {
     return KeyView{t->key, t->row, t->row_key, t->count, t->flags, t->new_rows, t->T / kGroup, t->cap};
-}
-
-__host__ __device__ __forceinline__ unsigned long long fmix64(unsigned long long k) {
-    k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
-    return k;
-}
-
-// Finds the slot of `key` or claims one for it.  Returns the slot, or -1 when the table has no free slot left on the
-// probe path.  *claimed: this tile's CAS put the key there (all lanes).  Table words are read with ld.cg: other tiles of
-// the same launch insert concurrently, and a stale "empty" is corrected by the CAS that follows it.
-__device__ __forceinline__ long long tile_claim(const KeyView& t, unsigned long long key, int sub, unsigned gmask, bool* claimed) {
-    const size_t home = (size_t)(fmix64(key) & (t.ngroups - 1));
-    *claimed = false;
-    for (size_t step = 0; step < t.ngroups; step++) {
-        const size_t base = ((home + step) & (t.ngroups - 1)) * kGroup;
-        unsigned long long k = __ldcg(t.key + base + sub);
-        while (true) {
-            const unsigned hit = __ballot_sync(gmask, k == key) & gmask;
-            if (hit) return (long long)(base + ((__ffs(hit) - 1) & (kGroup - 1)));
-            const unsigned empty = __ballot_sync(gmask, k == kEmptyKey) & gmask;
-            if (!empty) break;
-            const int leader = __ffs(empty) - 1, lsub = leader & (kGroup - 1);
-            unsigned long long old = 0;
-            if ((int)(threadIdx.x & 31) == leader) old = atomicCAS(t.key + base + lsub, kEmptyKey, key);
-            old = __shfl_sync(gmask, old, leader);
-            if (old == kEmptyKey) { *claimed = true; return (long long)(base + lsub); }
-            if (old == key) return (long long)(base + lsub);
-            if (sub == lsub) k = old;  // lost the slot to another key: look at the group again
-        }
-    }
-    return -1;
-}
-
-// read-only probe (no insert may run concurrently): slot of `key` or -1
-__device__ __forceinline__ long long tile_find(const KeyView& t, unsigned long long key, int sub, unsigned gmask) {
-    if (key == kEmptyKey) return -1;
-    const size_t home = (size_t)(fmix64(key) & (t.ngroups - 1));
-    for (size_t step = 0; step < t.ngroups; step++) {
-        const size_t base = ((home + step) & (t.ngroups - 1)) * kGroup;
-        const unsigned long long k = __ldg(t.key + base + sub);
-        const unsigned hit = __ballot_sync(gmask, k == key) & gmask;
-        if (hit) return (long long)(base + ((__ffs(hit) - 1) & (kGroup - 1)));
-        if (__ballot_sync(gmask, k == kEmptyKey) & gmask) return -1;
-    }
-    return -1;
 }
 
 // 1. claim a slot and a row for every key not yet in the table (one 16-lane tile per key)
@@ -158,21 +105,7 @@ __global__ void __launch_bounds__(256) key_insert_kernel(const unsigned long lon
     if (i >= n) return;  // whole tiles leave together
     const int sub = threadIdx.x & (kGroup - 1);
     const unsigned gmask = 0xffffu << (threadIdx.x & 16);
-    const unsigned long long key = keys[i];
-    bool claimed;
-    const long long pos = tile_claim(t, key, sub, gmask, &claimed);
-    if (sub != 0) return;
-    if (pos < 0) { t.flags[1] = 1u; return; }
-    if (!claimed) return;
-    const unsigned long long r = atomicAdd(t.count, 1ull);
-    if (r < t.cap) {
-        t.row[pos] = (uint32_t)r;
-        t.row_key[r] = key;
-        t.new_rows[atomicAdd(&t.flags[2], 1u)] = (uint32_t)r;
-    } else {
-        t.row[pos] = kNoRow;
-        t.flags[0] = 1u;
-    }
+    tile_insert(t, keys[i], sub, gmask);
 }
 
 // keys with caller-chosen rows (lctr_upload_keyed_params, checkpoint restore): every key gets rows[i]; `record` appends the
@@ -561,7 +494,9 @@ static int check_keys_host(const uint64_t* keys, int64_t n, const char* who) {
 int keys_alloc(lctr_ctx* c) {
     KeyTable* t = new KeyTable();
     c->keys = t;
-    t->cap = c->F - 1;
+    // several GPUs: this rank's shard holds the global rows l * world + rank below feature_cnt (dist.cu: placement)
+    const size_t R = (size_t)c->cfg.world, me = (size_t)c->cfg.rank;
+    t->cap = R > 1 ? (c->F - 1 + R - 1 - me) / R : c->F - 1;
     size_t T = kGroup;
     while (T < 2 * t->cap) T <<= 1;
     t->T = T;
@@ -597,6 +532,11 @@ void keys_free(lctr_ctx* c) {
 }
 
 bool keys_tracked(const lctr_ctx* c) { return c->keys && c->keys->last_seen; }
+
+KeyView keys_view(lctr_ctx* c) { return view(c->keys); }
+int keys_reserve_new_rows(lctr_ctx* c, size_t n) { return scratch_reserve(c, n); }
+int keys_init_new_rows(lctr_ctx* c, int64_t max_new) { return init_new_rows(c, max_new); }
+size_t keys_capacity(const lctr_ctx* c) { return c->keys->cap; }
 
 size_t keys_bytes(const lctr_ctx* c) {
     const KeyTable* t = c->keys;
@@ -760,6 +700,9 @@ int lctr_lookup_keys(lctr_ctx* c, int64_t n, const uint64_t* keys, int64_t* rows
     if (lookup_dev(c, keys, n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(rows, c->keys->d_rows, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    if (c->cfg.world > 1)  // local row l of this rank is global row l * world + rank; keys it does not hold stay -1
+        for (int64_t i = 0; i < n; i++)
+            if (rows[i] >= 0) rows[i] = rows[i] * c->cfg.world + c->cfg.rank;
     return 0;
 }
 
@@ -779,6 +722,8 @@ int lctr_download_keys(lctr_ctx* c, uint64_t* keys, uint64_t cap, uint64_t* n_ro
     return 0;
 }
 
+static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* keys, const float* W, const float* V);
+
 int lctr_upload_keyed_params(lctr_ctx* c, int64_t n, const uint64_t* keys, const float* W, const float* V) {
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(c->keys, "lctr_upload_keyed_params: the context was not created with key_mode = LCTR_KEYS_HASHED");
@@ -791,6 +736,24 @@ int lctr_upload_keyed_params(lctr_ctx* c, int64_t n, const uint64_t* keys, const
         const auto d = std::adjacent_find(sorted.begin(), sorted.end());
         LCTR_CHECK(d == sorted.end(), "lctr_upload_keyed_params: key %llu appears more than once", (unsigned long long)*d);
     }
+    if (c->cfg.world <= 1) return upload_keyed_params_local(c, n, keys, W, V);
+    // several GPUs: only the keys this rank owns, in array order, so the same call on every rank seeds the sharded table
+    int shift = 0;
+    while ((1 << shift) < c->cfg.world) shift++;
+    std::vector<uint64_t> mk;
+    std::vector<float> mw, mv;
+    for (int64_t i = 0; i < n; i++) {
+        if (owner_of_key(keys[i], shift) != (unsigned)c->cfg.rank) continue;
+        mk.push_back(keys[i]);
+        if (W) mw.push_back(W[i]);
+        if (V) mv.insert(mv.end(), V + (size_t)i * c->rowlen, V + (size_t)(i + 1) * c->rowlen);
+    }
+    if (mk.empty()) return 0;
+    return upload_keyed_params_local(c, (int64_t)mk.size(), mk.data(), W ? mw.data() : nullptr, V ? mv.data() : nullptr);
+}
+
+// the keys of one rank's table (all of them on one GPU), validated by the caller
+static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* keys, const float* W, const float* V) {
     KeyTable* t = c->keys;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     if (lookup_dev(c, keys, n)) return 1;

@@ -76,3 +76,40 @@ def merge_shards(parts, world, n_rows):
     for r, p in enumerate(parts):
         out[r::world] = p.reshape(n_rows, rowlen)[r::world]
     return out.reshape(-1)
+
+
+def fmix64(x):
+    """MurmurHash3's 64-bit finaliser, mod 2^64 (csrc/keys.cuh: fmix64)."""
+    k = np.array(x, dtype=np.uint64, copy=True)
+    with np.errstate(over="ignore"):
+        k ^= k >> np.uint64(33)
+        k *= np.uint64(0xff51afd7ed558ccd)
+        k ^= k >> np.uint64(33)
+        k *= np.uint64(0xc4ceb9fe1a85ec53)
+        k ^= k >> np.uint64(33)
+    return k
+
+
+def owner_of_key(keys, world):
+    """Rank that owns each hashed key of a keyed context on `world` (a power of two) ranks: the top log2(world) bits of
+    fmix64(key) (csrc/keys.cuh: owner_of_key).  Its row l there is global row l * world + rank."""
+    assert world >= 1 and world & (world - 1) == 0, world
+    shift = world.bit_length() - 1
+    if shift == 0:
+        return np.zeros(np.shape(keys), np.int64)
+    return (fmix64(keys) >> np.uint64(64 - shift)).astype(np.int64)
+
+
+def merge_keyed_shards(keys, W, V, world):
+    """key -> (W, V row) of a sharded keyed table.  keys[r] is rank r's download_keys() (its local rows in order), W[r] /
+    V[r] its download_params() arrays, in which local row l sits at global row l * world + r."""
+    out = {}
+    for r in range(world):
+        kr = np.asarray(keys[r], np.uint64)
+        g = np.arange(len(kr), dtype=np.int64) * world + r
+        rowlen = len(V[r]) // len(W[r])
+        Vr = np.asarray(V[r]).reshape(-1, rowlen)
+        for key, w, v in zip(kr.tolist(), np.asarray(W[r])[g], Vr[g]):
+            assert key not in out, "key %d held by more than one rank" % key
+            out[key] = (w, v)
+    return out
