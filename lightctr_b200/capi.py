@@ -32,7 +32,7 @@ SYMBOLS = [
     "lctr_save_dataset_bin", "lctr_load_dataset_bin", "lctr_eval", "lctr_upload_pred", "lctr_ipc_export", "lctr_ipc_import",
     "lctr_dense_grad_buffer", "lctr_device_bytes", "lctr_load_libffm", "lctr_free_dataset", "lctr_launch_count", "lctr_stream", "lctr_profile", "lctr_profile_read",
     "lctr_upload_batch_keys", "lctr_lookup_keys", "lctr_download_keys", "lctr_upload_keyed_params", "lctr_set_key_init",
-    "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys",
+    "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys", "lctr_load_checkpoint_shards",
 ]
 NO_LIMIT = (1 << 64) - 1  # lctr_evict_keys: UINT64_MAX = no limit
 
@@ -104,6 +104,7 @@ def load_library():
     L.lctr_upload_pred.argtypes = [vp, C.c_int, f32p]
     L.lctr_save_checkpoint.argtypes = [vp, C.c_char_p]
     L.lctr_load_checkpoint.argtypes = [vp, C.c_char_p]
+    L.lctr_load_checkpoint_shards.argtypes = [vp, C.c_int, C.POINTER(C.c_char_p)]
     L.lctr_save_dataset_bin.argtypes = [C.POINTER(DatasetC), C.c_char_p]
     L.lctr_load_dataset_bin.argtypes = [C.c_char_p, C.POINTER(C.POINTER(DatasetC))]
     L.lctr_ipc_export.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -462,6 +463,12 @@ class Context:
 
     def load_checkpoint(self, path):
         _chk(self.L.lctr_load_checkpoint(self.h, path.encode()))
+
+    def load_checkpoint_shards(self, paths):
+        """The files of one save (ranks 0..n-1 of a world-n run, or one single-GPU file) into this context, whatever its
+        world: this rank takes the rows it owns."""
+        arr = (C.c_char_p * len(paths))(*[p.encode() for p in paths])
+        _chk(self.L.lctr_load_checkpoint_shards(self.h, len(paths), arr))
 
     def mlp_download_grad(self, layer, n_in, n_out):
         w, b = np.empty(n_in * n_out, np.float32), np.empty(n_out, np.float32)

@@ -378,9 +378,49 @@ int lctr_fill_params(lctr_ctx* c, uint64_t seed, float scale) {
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }
+// world > 1: the rows a rank owns are the prefix [0, n) of its shard (local row l = global row l * world + rank); the
+// opt-state transfers move that prefix between the shard and the full global arrays [W part | V part]
+static size_t owned_rows(const lctr_ctx* c) {
+    const size_t F = api_rows(c), R = (size_t)c->cfg.world, me = (size_t)c->cfg.rank;
+    return me < F ? (F - me + R - 1) / R : 0;
+}
+static int shard_to_global(lctr_ctx* c, float* out, const float* dW, const float* dV) {
+    const size_t F = api_rows(c), R = (size_t)c->cfg.world, n = owned_rows(c), k = c->rowlen;
+    std::vector<float> w(n), v(n * k);
+    if (n) {
+        LCTR_CUDA(cudaMemcpyAsync(w.data(), dW, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(v.data(), dV, n * k * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    }
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    for (size_t l = 0, f = (size_t)c->cfg.rank; l < n; l++, f += R) {
+        out[f] = w[l];
+        memcpy(out + F + f * k, &v[l * k], k * sizeof(float));
+    }
+    return 0;
+}
+static int global_to_shard(lctr_ctx* c, const float* in, float* dW, float* dV) {
+    const size_t F = api_rows(c), R = (size_t)c->cfg.world, n = owned_rows(c), k = c->rowlen;
+    std::vector<float> w(n), v(n * k);
+    for (size_t l = 0, f = (size_t)c->cfg.rank; l < n; l++, f += R) {
+        w[l] = in[f];
+        memcpy(&v[l * k], in + F + f * k, k * sizeof(float));
+    }
+    if (n) {
+        LCTR_CUDA(cudaMemcpyAsync(dW, w.data(), n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(dV, v.data(), n * k * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    }
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
 int lctr_download_opt_state(lctr_ctx* c, float* s1, float* s2) {
     LCTR_CHECK(c, "null ctx");
-    LCTR_CHECK(c->cfg.world == 1, "optimizer-state transfer is single-GPU only");
+    if (c->cfg.world > 1) {
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
+        if (s1 && shard_to_global(c, s1, c->s1W, c->s1V)) return 1;
+        if (s2 && c->s2W && shard_to_global(c, s2, c->s2W, c->s2V)) return 1;
+        return 0;
+    }
     const size_t F = api_rows(c), nv = F * c->rowlen;
     if (s1) {
         LCTR_CUDA(cudaMemcpyAsync(s1, c->s1W, F * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
@@ -395,7 +435,11 @@ int lctr_download_opt_state(lctr_ctx* c, float* s1, float* s2) {
 }
 int lctr_upload_opt_state(lctr_ctx* c, const float* s1, const float* s2) {
     LCTR_CHECK(c, "null ctx");
-    LCTR_CHECK(c->cfg.world == 1, "optimizer-state transfer is single-GPU only (the state arrays are sharded by owner)");
+    if (c->cfg.world > 1) {
+        if (s1 && global_to_shard(c, s1, c->s1W, c->s1V)) return 1;
+        if (s2 && c->s2W && global_to_shard(c, s2, c->s2W, c->s2V)) return 1;
+        return 0;
+    }
     const size_t F = api_rows(c), nv = F * c->rowlen;
     if (s1) {
         LCTR_CUDA(cudaMemcpyAsync(c->s1W, s1, F * sizeof(float), cudaMemcpyHostToDevice, c->stream));
@@ -599,8 +643,8 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
     LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "train_step: slot %d holds no usable batch (its last keyed upload failed)", slot);
     LCTR_CHECK(s.key_state != SLOT_KEYS_LOOKUP, "train_step: slot %d was uploaded with insert = 0 (lookup only: unseen keys "
                                                 "sit on the null row, which is never trained)", slot);
-    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "train_step: slot %d is stale: lctr_evict_keys renumbered rows after it was "
-                                               "uploaded; upload it again", slot);
+    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "train_step: slot %d is stale: lctr_evict_keys or a keyed checkpoint load "
+                                               "renumbered rows after it was uploaded; upload it again", slot);
     LCTR_CHECK(rb >= 0 && re <= s.rows && rb <= re, "train_step: rows [%lld,%lld) outside slot (%lld rows)",
                (long long)rb, (long long)re, (long long)s.rows);
     LCTR_CHECK(c->cfg.world == 1 || c->cfg.minibatch_size > 0,
@@ -866,8 +910,8 @@ int lctr_predict(lctr_ctx* c, int slot, int quirk_sumvx_slot, float* pctr) {
     LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
     Slot& s = c->slots[slot];
     LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "lctr_predict: slot %d holds no usable batch (its last keyed upload failed)", slot);
-    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "lctr_predict: slot %d is stale: lctr_evict_keys renumbered rows after it was "
-                                               "uploaded; upload it again", slot);
+    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "lctr_predict: slot %d is stale: lctr_evict_keys or a keyed checkpoint load "
+                                               "renumbered rows after it was uploaded; upload it again", slot);
     int rc = 0;
     if (c->cfg.model == LCTR_MODEL_WND) {
         // Distributed_Algo_Abst::Predict (distributed_algo_abst.h:163-174): a forward pass over the slot; with several

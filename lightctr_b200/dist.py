@@ -5,6 +5,10 @@ this module only (a) exchanges the CUDA-IPC handles every rank exports, (b) redu
 (c) offers the shard arithmetic used on both sides of the C ABI.  Replaces the reference's master/worker
 bootstrap (distribut/master.h:76-190, dist_machine_abst.h:53-87) for the single-box case.
 """
+import os
+import re
+import struct
+
 import numpy as np
 
 
@@ -113,3 +117,86 @@ def merge_keyed_shards(keys, W, V, world):
             assert key not in out, "key %d held by more than one rank" % key
             out[key] = (w, v)
     return out
+
+
+# ---- checkpoints of sharded trainers (lctr_save_checkpoint per rank, lctr_load_checkpoint[_shards]) --------------------
+_SHARD_NAME = re.compile(r"\.rank(\d+)-of-(\d+)$")
+
+
+def shard_path(prefix, rank, world):
+    """File of rank `rank` in a save of a world-`world` run under `prefix`."""
+    return "%s.rank%d-of-%d" % (prefix, rank, world)
+
+
+def checkpoint_info(path):
+    """(step, adam_iter, world, rank) from the header of a checkpoint file (csrc/checkpoint.cu: CkptHeader, CkptShard);
+    a single-GPU file reads as world 1, rank 0."""
+    with open(path, "rb") as f:
+        head = f.read(136 + 24)
+    if len(head) < 136 or head[:8] not in (b"LCTRCKP1", b"LCTRCKS1"):
+        raise ValueError("%s is not a lightctr_b200 checkpoint" % path)
+    adam_iter, step = struct.unpack_from("<QQ", head, 48)
+    if head[:8] == b"LCTRCKP1":
+        return step, adam_iter, 1, 0
+    if len(head) < 160:
+        raise ValueError("%s: short shard header" % path)
+    world, rank = struct.unpack_from("<ii", head, 136)
+    return step, adam_iter, world, rank
+
+
+def find_shards(prefix):
+    """The files of the save under `prefix`, in rank order: every `prefix.rank<r>-of-<R>` beside it.  Refuses files of
+    two different worlds, a rank given twice, and a set with gaps."""
+    d, base = os.path.split(prefix)
+    found = {}
+    for name in os.listdir(d or "."):
+        if not name.startswith(base + ".rank"):
+            continue
+        m = _SHARD_NAME.search(name[len(base):])
+        if not m or m.start() != 0:
+            continue
+        r, w = int(m.group(1)), int(m.group(2))
+        if (r, w) in found:
+            raise ValueError("rank %d of world %d appears twice under %s: %s, %s" % (r, w, prefix, found[(r, w)], name))
+        found[(r, w)] = name
+    if not found:
+        raise FileNotFoundError("no checkpoint files %s.rank<r>-of-<R>" % prefix)
+    worlds = sorted({w for _, w in found})
+    if len(worlds) > 1:
+        raise ValueError("files of several saves under %s (worlds %s)" % (prefix, worlds))
+    world = worlds[0]
+    missing = [r for r in range(world) if (r, world) not in found]
+    if missing or len(found) != world:
+        raise ValueError("incomplete save under %s: world %d, ranks %s missing" % (prefix, world, missing))
+    return [os.path.join(d, found[(r, world)]) for r in range(world)], world
+
+
+def save_sharded(ctx, prefix, group=None):
+    """Every rank writes its shard to shard_path(prefix, rank, world); the ranks then barrier and check that they all
+    saved the same step."""
+    rank, world = ctx.cfg.rank, ctx.cfg.world
+    path = shard_path(prefix, rank, world)
+    ctx.save_checkpoint(path)
+    if world > 1:
+        import torch.distributed as dist
+        dist.barrier(group)
+        steps = [None] * world
+        dist.all_gather_object(steps, checkpoint_info(path)[:2], group=group)
+        if any(s != steps[0] for s in steps):
+            raise RuntimeError("save_sharded: the ranks saved different (step, adam_iter): %s" % steps)
+    return path
+
+
+def load_sharded(ctx, prefix, group=None):
+    """Load the save under `prefix` into this rank's context, whatever world wrote it: the rank's own file when the world
+    is unchanged, else every file, each rank taking the rows it owns (lctr_load_checkpoint_shards).  Returns the world
+    of the save."""
+    paths, world = find_shards(prefix)
+    if world == ctx.cfg.world:
+        ctx.load_checkpoint(paths[ctx.cfg.rank])
+    else:
+        ctx.load_checkpoint_shards(paths)
+    if ctx.cfg.world > 1:  # nobody starts a collective upload while a peer is still reading
+        import torch.distributed as dist
+        dist.barrier(group)
+    return world
