@@ -309,10 +309,11 @@ int lctr_upload_pred(lctr_ctx* ctx, int slot, const float* pctr);
  * trainer continues exactly where the saved one stopped.  The restoring ctx must have been created with the same cfg.
  * world > 1: every rank saves its own shard to its own path (no communication: the call synchronises the ctx stream, on
  * which every update of the shard runs), in a shard format of its own -- the rows it owns (local row l = global row
- * l * world + rank), its copy of the dense layers, and (keyed) its local row -> key map.  lctr_load_checkpoint then loads
- * the file the same rank of the same world wrote and refuses any other, naming both ranks and worlds.  Keyed loads rebuild
- * the key table, and every resident keyed slot becomes stale (train_step refuses it until it is uploaded again), as after
- * lctr_evict_keys; dense slots stay valid. */
+ * l * world + rank), its copy of the dense layers, and (keyed) its local row -> key map.  lctr_load_checkpoint loads the
+ * file the same rank of the same world wrote (a single-GPU file is rank 0 of world 1) and refuses any other, naming both
+ * ranks and worlds.  On any world, one GPU included: the file is checked (cfg, length, key section) before anything is
+ * written, so a refused load changes nothing; keyed loads rebuild the key table, and every resident keyed slot becomes
+ * stale (train_step refuses it until it is uploaded again), as after lctr_evict_keys; dense slots stay valid. */
 int lctr_save_checkpoint(lctr_ctx* ctx, const char* path);
 int lctr_load_checkpoint(lctr_ctx* ctx, const char* path);
 /* The files of ONE save -- ranks 0..n-1 of a world-n run, or n = 1 and a single-GPU file -- into this context, whatever
@@ -320,7 +321,7 @@ int lctr_load_checkpoint(lctr_ctx* ctx, const char* path);
  * Everything is checked before anything is written, and on failure the context is unchanged: every file has this cfg,
  * the set holds each rank 0..n-1 once, all files carry the same step and adam_iter, and when the world changes (n > 1)
  * the dense layers are bit-identical across the files (Wide&Deep without a dense all-reduce trains per-rank layers, which
- * no rule merges).  With the world unchanged it is lctr_load_checkpoint of this rank's file.
+ * no rule merges).  With the world unchanged it loads this rank's file as lctr_load_checkpoint does.
  * Dense tables: the row sections stream through a bounded device staging buffer.  Keyed tables: this rank's keys under
  * its world take rows 0..m-1 in source order (rank 0's rows ascending, then rank 1's, ...); m above the shard's capacity
  * fails naming the rank; rows past m return to the state lctr_create gives. */

@@ -7,8 +7,10 @@
 //
 // Multi-GPU trainers (world > 1) write one shard file per rank ("LCTRCKS1"): the single-GPU header, a CkptShard, then the
 // same sections over the shard's Fl local rows (local row l = global row l * world + rank) and the rank's own copy of the
-// dense layers.  lctr_load_checkpoint reads a shard back into the same rank of the same world; lctr_load_checkpoint_shards
-// loads a whole save into a context of any world, streaming the row sections through reshard_rows_kernel.
+// dense layers.  Every load reads through ckpt_open, which checks a file against the context before anything is written
+// (a single-GPU file reads as rank 0 of world 1).  lctr_load_checkpoint then loads the file of this rank of this world in
+// place, for every world; lctr_load_checkpoint_shards loads a whole save into a context of any world, streaming the row
+// sections through reshard_rows_kernel when the world changes.
 #include <stdio.h>
 #include <string.h>
 
@@ -69,9 +71,41 @@ static bool same_trainer(const lctr_ctx* c, const CkptHeader& h) {
     return same;
 }
 
-static size_t layer_floats(const lctr_ctx* c) {  // w, b, acc_w, acc_b, mask of every layer
+// The sections of a file after its header(s), in file order: the row sections over the file's rows, the parts of every
+// layer, then for keyed tables the row count and the key of every row, and for key_evict = 1 the upload clock and the
+// stamp of every row.  Everything that walks the format takes the first two from these helpers.
+
+// W, V, s1W, s1V[, s2W, s2V] of this rank's shard
+struct RowSections {
+    float* p[6];
+    int n;  // 4, or 6 when the updater keeps s2
+    size_t rowlen;
+    size_t width(int a) const { return a % 2 ? rowlen : 1; }  // floats per row of section a
+};
+static RowSections row_sections(const lctr_ctx* c) {
+    return {{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V}, c->s2W ? 6 : 4, c->rowlen};
+}
+
+// w, b, acc_w, acc_b, mask of one dense layer and their sizes in floats
+struct LayerParts {
+    float* p[5];
+    size_t n[5];
+};
+static LayerParts layer_parts(const MlpLayer& L) {
+    const size_t nw = (size_t)L.out * L.in, no = (size_t)L.out;
+    return {{L.w, L.b, L.acc_w, L.acc_b, L.mask}, {nw, no, nw, no, no}};
+}
+
+static size_t row_floats(const lctr_ctx* c) {  // one row across the row sections
+    const RowSections rs = row_sections(c);
     size_t n = 0;
-    for (int l = 0; l < c->n_layers; l++) n += 2 * (size_t)c->layers[l].out * c->layers[l].in + 3 * (size_t)c->layers[l].out;
+    for (int a = 0; a < rs.n; a++) n += rs.width(a);
+    return n;
+}
+static size_t layer_floats(const lctr_ctx* c) {  // every layer
+    size_t n = 0;
+    for (int l = 0; l < c->n_layers; l++)
+        for (size_t m : layer_parts(c->layers[l]).n) n += m;
     return n;
 }
 
@@ -100,7 +134,7 @@ static void mark_slots_stale(lctr_ctx* c) {
 static int log2_world(int w) { int s = 0; while ((1 << s) < w) s++; return s; }
 
 // One file of a load, opened and checked against the context before anything is written: header, cfg, shard geometry,
-// file length, and (keyed) its row -> key map, each key owned by the file's rank.
+// file length, (keyed) its row -> key map, each key owned by the file's rank, and (key_evict = 1) the clock and stamps.
 struct CkptFile {
     std::string path;
     FILE* f = nullptr;
@@ -108,14 +142,13 @@ struct CkptFile {
     CkptShard s;             // a single-GPU file reads as world 1, rank 0
     long rows_at = 0;        // offset of the first row section
     std::vector<uint64_t> keys;
+    uint64_t clock = 0;
+    std::vector<uint64_t> stamps;
     CkptFile() = default;
     CkptFile(const CkptFile&) = delete;
     CkptFile& operator=(const CkptFile&) = delete;
     ~CkptFile() { if (f) fclose(f); }
-    size_t arrays(const lctr_ctx* c) const { return c->s2W ? 3 : 2; }  // (W, V) pairs: parameters, s1, s2
-    long layers_at(const lctr_ctx* c) const {
-        return rows_at + (long)(arrays(c) * s.local_rows * (1 + c->rowlen) * sizeof(float));
-    }
+    long layers_at(const lctr_ctx* c) const { return rows_at + (long)(s.local_rows * row_floats(c) * sizeof(float)); }
 };
 
 static int ckpt_open(lctr_ctx* c, const char* path, CkptFile& cf) {
@@ -142,8 +175,7 @@ static int ckpt_open(lctr_ctx* c, const char* path, CkptFile& cf) {
     long end = cf.layers_at(c) + (long)(layer_floats(c) * sizeof(float));
     if (c->keys) {
         uint64_t n = 0;
-        const uint64_t owned = (rows + cf.s.world - 1 - cf.s.rank) / cf.s.world;  // global rows < rows this rank holds
-        LCTR_CHECK(fseek(cf.f, end, SEEK_SET) == 0 && get(cf.f, &n, sizeof(n)) && n <= owned,
+        LCTR_CHECK(fseek(cf.f, end, SEEK_SET) == 0 && get(cf.f, &n, sizeof(n)) && n <= owned_rows(rows, cf.s.world, cf.s.rank),
                    "checkpoint %s: missing or inconsistent key section", path);
         cf.keys.resize(n);
         LCTR_CHECK(get(cf.f, cf.keys.data(), n * sizeof(uint64_t)), "checkpoint %s: short read of the keys", path);
@@ -152,7 +184,13 @@ static int ckpt_open(lctr_ctx* c, const char* path, CkptFile& cf) {
             LCTR_CHECK(cf.keys[i] != kEmptyKey && (int)owner_of_key(cf.keys[i], shift) == cf.s.rank,
                        "checkpoint %s: key %llu at row %llu is not owned by rank %d of world %d (corrupted or mismatched set)",
                        path, (unsigned long long)cf.keys[i], (unsigned long long)i, cf.s.rank, cf.s.world);
-        end += (long)((1 + n) * sizeof(uint64_t)) * (keys_tracked(c) ? 2 : 1);  // + the clock and the stamps
+        end += (long)((1 + n) * sizeof(uint64_t));
+        if (keys_tracked(c)) {
+            cf.stamps.resize(n);
+            LCTR_CHECK(get(cf.f, &cf.clock, sizeof(cf.clock)) && get(cf.f, cf.stamps.data(), n * sizeof(uint64_t)),
+                       "checkpoint %s: short read of the row stamps", path);
+            end += (long)((1 + n) * sizeof(uint64_t));
+        }
     }
     long len = -1;
     if (fseek(cf.f, 0, SEEK_END) == 0) len = ftell(cf.f);
@@ -201,9 +239,6 @@ __global__ void __launch_bounds__(256) reshard_scalars_kernel(const float* __res
         if (d != kNoRow) dst[d] = src[i];
     }
 }
-__global__ void fill_kernel(float* p, size_t n, float v) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
-}
 
 // host + device staging of the resharding load: chunks of `rows` source rows (at most 16 M floats)
 struct Stage {
@@ -240,37 +275,25 @@ static int scatter_section(lctr_ctx* c, Stage& st, FILE* f, float* dst, size_t n
     return 0;
 }
 
-// same world, same rank: the sections land where they were read
+// a file ckpt_open checked, written by this rank of this world: the sections land where they were read
 static int load_shard_in_place(lctr_ctx* c, CkptFile& cf) {
-    FILE* f = cf.f;
-    const size_t nv = c->Fl * c->rowlen;
-    int rc = file_to_dev(c, f, c->W, c->Fl) || file_to_dev(c, f, c->V, nv) || file_to_dev(c, f, c->s1W, c->Fl) ||
-             file_to_dev(c, f, c->s1V, nv);
-    if (!rc && c->s2W) rc = file_to_dev(c, f, c->s2W, c->Fl) || file_to_dev(c, f, c->s2V, nv);
-    for (int l = 0; l < c->n_layers && !rc; l++) {
-        MlpLayer& L = c->layers[l];
-        const size_t nw = (size_t)L.out * L.in;
-        rc = file_to_dev(c, f, L.w, nw) || file_to_dev(c, f, L.b, L.out) || file_to_dev(c, f, L.acc_w, nw) ||
-             file_to_dev(c, f, L.acc_b, L.out) || file_to_dev(c, f, L.mask, L.out);
-        if (!rc) rc = mlp_bf16_refresh(c, l);
-    }
-    if (!rc && c->keys) {
-        rc = keys_restore(c, cf.keys.data(), cf.keys.size());
-        mark_slots_stale(c);
-    }
-    return rc ? 1 : finish_load(c, cf.h);
-}
-
-// world > 1, lctr_load_checkpoint: the shard this rank of this world wrote
-static int load_shard_same_world(lctr_ctx* c, const char* path) {
-    CkptFile cf;
-    if (ckpt_open(c, path, cf)) return 1;
-    LCTR_CHECK(cf.s.world == c->cfg.world && cf.s.rank == c->cfg.rank,
-               "checkpoint %s was written by rank %d of world %d, this context is rank %d of world %d (a save of another "
-               "world loads through lctr_load_checkpoint_shards)", path, cf.s.rank, cf.s.world, c->cfg.rank, c->cfg.world);
     LCTR_CHECK(!c->keys || cf.keys.size() <= keys_capacity(c), "checkpoint %s: %zu keyed rows exceed the shard's capacity %zu",
-               path, cf.keys.size(), keys_capacity(c));
-    return load_shard_in_place(c, cf);
+               cf.path.c_str(), cf.keys.size(), keys_capacity(c));
+    const RowSections rs = row_sections(c);
+    for (int a = 0; a < rs.n; a++)
+        if (file_to_dev(c, cf.f, rs.p[a], c->Fl * rs.width(a))) return 1;
+    for (int l = 0; l < c->n_layers; l++) {
+        const LayerParts lp = layer_parts(c->layers[l]);
+        for (int p = 0; p < 5; p++)
+            if (file_to_dev(c, cf.f, lp.p[p], lp.n[p])) return 1;
+        if (mlp_bf16_refresh(c, l)) return 1;
+    }
+    if (c->keys) {
+        mark_slots_stale(c);
+        if (keys_restore(c, cf.keys.data(), cf.keys.size())) return 1;
+        if (keys_tracked(c) && keys_restore_stamps(c, cf.stamps.data(), cf.stamps.size(), cf.clock)) return 1;
+    }
+    return finish_load(c, cf.h);
 }
 
 }  // namespace lctr
@@ -299,16 +322,11 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
         const CkptShard s{c->cfg.world, c->cfg.rank, api_rows(c), c->Fl};
         rc = put(f, &s, sizeof(s)) ? 0 : 1;
     }
-    const size_t nv = c->Fl * c->rowlen;  // Fl == F on one GPU
-    const bool two = c->s2W != nullptr;
-    rc = rc || dev_to_file(c, f, c->W, c->Fl) || dev_to_file(c, f, c->V, nv) || dev_to_file(c, f, c->s1W, c->Fl) ||
-         dev_to_file(c, f, c->s1V, nv);
-    if (!rc && two) rc = dev_to_file(c, f, c->s2W, c->Fl) || dev_to_file(c, f, c->s2V, nv);
+    const RowSections rs = row_sections(c);
+    for (int a = 0; a < rs.n && !rc; a++) rc = dev_to_file(c, f, rs.p[a], c->Fl * rs.width(a));  // Fl == F on one GPU
     for (int l = 0; l < c->n_layers && !rc; l++) {
-        MlpLayer& L = c->layers[l];
-        const size_t nw = (size_t)L.out * L.in;
-        rc = dev_to_file(c, f, L.w, nw) || dev_to_file(c, f, L.b, L.out) || dev_to_file(c, f, L.acc_w, nw) ||
-             dev_to_file(c, f, L.acc_b, L.out) || dev_to_file(c, f, L.mask, L.out);
+        const LayerParts lp = layer_parts(c->layers[l]);
+        for (int p = 0; p < 5 && !rc; p++) rc = dev_to_file(c, f, lp.p[p], lp.n[p]);
     }
     if (!rc && c->keys) {  // keyed tables: row count, then the key of every row (the table is rebuilt from it on load)
         std::vector<uint64_t> keys;
@@ -339,59 +357,12 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
 int lctr_load_checkpoint(lctr_ctx* c, const char* path) {
     LCTR_CHECK(c && path, "null argument");
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    if (c->cfg.world > 1) return load_shard_same_world(c, path);
-    FILE* f = fopen(path, "rb");
-    LCTR_CHECK(f, "open file error! (%s)", path);
-    CkptHeader h{};
-    if (!get(f, &h, sizeof(h)) || memcmp(h.magic, "LCTRCKP1", 8) != 0) {
-        const bool shard = memcmp(h.magic, "LCTRCKS1", 8) == 0;
-        fclose(f);
-        if (shard) set_error("%s is one rank's shard of a multi-GPU checkpoint: load the whole save with lctr_load_checkpoint_shards", path);
-        else set_error("%s is not a lightctr_b200 checkpoint", path);
-        return 1;
-    }
-    if (!same_trainer(c, h)) {
-        fclose(f);
-        set_error("checkpoint %s was written by a different trainer (model/optimizer/feature_cnt/field_cnt/factor_cnt/layers/key_mode/key_evict)", path);
-        return 1;
-    }
-    const size_t nv = c->F * c->rowlen;
-    const bool two = c->s2W != nullptr;
-    int rc = file_to_dev(c, f, c->W, c->F) || file_to_dev(c, f, c->V, nv) || file_to_dev(c, f, c->s1W, c->F) ||
-             file_to_dev(c, f, c->s1V, nv);
-    if (!rc && two) rc = file_to_dev(c, f, c->s2W, c->F) || file_to_dev(c, f, c->s2V, nv);
-    for (int l = 0; l < c->n_layers && !rc; l++) {
-        MlpLayer& L = c->layers[l];
-        const size_t nw = (size_t)L.out * L.in;
-        rc = file_to_dev(c, f, L.w, nw) || file_to_dev(c, f, L.b, L.out) || file_to_dev(c, f, L.acc_w, nw) ||
-             file_to_dev(c, f, L.acc_b, L.out) || file_to_dev(c, f, L.mask, L.out);
-        if (!rc) rc = mlp_bf16_refresh(c, l);
-    }
-    if (!rc && c->keys) {
-        uint64_t n = 0;
-        std::vector<uint64_t> keys;
-        if (!get(f, &n, sizeof(n)) || n > c->F - 1) {
-            rc = 1;
-            set_error("checkpoint %s: missing or inconsistent key section", path);
-        } else {
-            keys.resize(n);
-            if (!get(f, keys.data(), n * sizeof(uint64_t))) { rc = 1; set_error("checkpoint %s: short read of the keys", path); }
-            else rc = keys_restore(c, keys.data(), n);
-        }
-        if (!rc && keys_tracked(c)) {
-            uint64_t clock = 0;
-            std::vector<uint64_t> stamps(n);
-            if (!get(f, &clock, sizeof(clock)) || !get(f, stamps.data(), n * sizeof(uint64_t))) {
-                rc = 1;
-                set_error("checkpoint %s: short read of the row stamps", path);
-            } else {
-                rc = keys_restore_stamps(c, stamps.data(), n, clock);
-            }
-        }
-    }
-    fclose(f);
-    if (rc) return 1;
-    return finish_load(c, h);
+    CkptFile cf;
+    if (ckpt_open(c, path, cf)) return 1;
+    LCTR_CHECK(cf.s.world == c->cfg.world && cf.s.rank == c->cfg.rank,
+               "checkpoint %s was written by rank %d of world %d, this context is rank %d of world %d (a save of another "
+               "world loads through lctr_load_checkpoint_shards)", path, cf.s.rank, cf.s.world, c->cfg.rank, c->cfg.world);
+    return load_shard_in_place(c, cf);
 }
 
 int lctr_load_checkpoint_shards(lctr_ctx* c, int n, const char* const* paths) {
@@ -420,19 +391,7 @@ int lctr_load_checkpoint_shards(lctr_ctx* c, int n, const char* const* paths) {
                    "lctr_load_checkpoint_shards: rank %d was saved at step %llu (adam_iter %llu), rank 0 at step %llu (adam_iter "
                    "%llu): not one save", r, (unsigned long long)by_rank[r]->h.step, (unsigned long long)by_rank[r]->h.adam_iter,
                    (unsigned long long)h0.step, (unsigned long long)h0.adam_iter);
-    if (n == world) {  // the world is unchanged: this rank's own file, rows in place, its own layers
-        CkptFile& mine = *by_rank[me];
-        if (world == 1) {
-            const std::string path = mine.path;
-            fs.clear();
-            if (lctr_load_checkpoint(c, path.c_str())) return 1;  // the single-GPU loader (stamps included)
-            if (c->keys) mark_slots_stale(c);
-            return 0;
-        }
-        LCTR_CHECK(!c->keys || mine.keys.size() <= keys_capacity(c), "checkpoint %s: %zu keyed rows exceed the shard's capacity %zu",
-                   mine.path.c_str(), mine.keys.size(), keys_capacity(c));
-        return load_shard_in_place(c, mine);
-    }
+    if (n == world) return load_shard_in_place(c, *by_rank[me]);  // the world is unchanged: this rank's own file in place
     // the world changes: the dense layers must be one model
     const size_t nlf = layer_floats(c);
     std::vector<float> layers(nlf), other(nlf);
@@ -463,21 +422,7 @@ int lctr_load_checkpoint_shards(lctr_ctx* c, int n, const char* const* paths) {
                    me, mine.size(), keys_capacity(c));
     }
     // 2. the writes: keyed shards start from the state lctr_create gives (rows past the keys stay so)
-    const size_t nv = c->Fl * c->rowlen;
-    if (c->keys) {
-        const float s1 = (c->cfg.optimizer == LCTR_OPT_PS_ADAGRAD || c->cfg.optimizer == LCTR_OPT_PS_DCASGDA) ? 1e-7f : 0.f;
-        const unsigned grid = (unsigned)c->sm_count * 4;
-        LCTR_CUDA(cudaMemsetAsync(c->W, 0, c->Fl * sizeof(float), c->stream));
-        LCTR_CUDA(cudaMemsetAsync(c->V, 0, nv * sizeof(float), c->stream));
-        fill_kernel<<<grid, 256, 0, c->stream>>>(c->s1W, c->Fl, s1);
-        fill_kernel<<<grid, 256, 0, c->stream>>>(c->s1V, nv, s1);
-        c->launches += 2;
-        LCTR_CUDA(cudaGetLastError());
-        if (c->s2W) {
-            LCTR_CUDA(cudaMemsetAsync(c->s2W, 0, c->Fl * sizeof(float), c->stream));
-            LCTR_CUDA(cudaMemsetAsync(c->s2V, 0, nv * sizeof(float), c->stream));
-        }
-    }
+    if (c->keys && reset_table_rows(c)) return 1;
     Stage st;
     {
         size_t src_rows = 0;
@@ -487,30 +432,27 @@ int lctr_load_checkpoint_shards(lctr_ctx* c, int n, const char* const* paths) {
         LCTR_CUDA(cudaMalloc((void**)&st.d, st.rows * c->rowlen * sizeof(float)));
         if (c->keys) LCTR_CUDA(cudaMalloc((void**)&st.dmap, st.rows * sizeof(uint32_t)));
     }
-    float* dst[6] = {c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V};
+    const RowSections rs = row_sections(c);
     for (int r = 0; r < n; r++) {
         CkptFile& cf = *by_rank[r];
         LCTR_CHECK(fseek(cf.f, cf.rows_at, SEEK_SET) == 0, "checkpoint %s: seek failed", cf.path.c_str());
         const ReshardRule rule{nullptr, 0, api_rows(c), (uint32_t)n, (uint32_t)r, (uint32_t)world, (uint32_t)me};
         const uint32_t* map = c->keys ? maps[r].data() : nullptr;
-        for (size_t a = 0; a < 2 * cf.arrays(c); a++)
-            if (scatter_section(c, st, cf.f, dst[a], cf.s.local_rows, a % 2 ? c->rowlen : 1, rule, map)) return 1;
+        for (int a = 0; a < rs.n; a++)
+            if (scatter_section(c, st, cf.f, rs.p[a], cf.s.local_rows, rs.width(a), rule, map)) return 1;
     }
     const float* src = layers.data();
     for (int l = 0; l < c->n_layers; l++) {
-        MlpLayer& L = c->layers[l];
-        const size_t nw = (size_t)L.out * L.in;
-        float* parts[5] = {L.w, L.b, L.acc_w, L.acc_b, L.mask};
-        const size_t sizes[5] = {nw, (size_t)L.out, nw, (size_t)L.out, (size_t)L.out};
+        const LayerParts lp = layer_parts(c->layers[l]);
         for (int p = 0; p < 5; p++) {
-            LCTR_CUDA(cudaMemcpyAsync(parts[p], src, sizes[p] * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-            src += sizes[p];
+            LCTR_CUDA(cudaMemcpyAsync(lp.p[p], src, lp.n[p] * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+            src += lp.n[p];
         }
         if (mlp_bf16_refresh(c, l)) return 1;
     }
     if (c->keys) {
-        if (keys_restore(c, mine.data(), mine.size())) return 1;
         mark_slots_stale(c);
+        if (keys_restore(c, mine.data(), mine.size())) return 1;
     }
     return finish_load(c, h0);
 }

@@ -423,5 +423,13 @@ int keys_download_stamps(lctr_ctx* c, uint64_t n, std::vector<uint64_t>& stamps,
 int keys_restore_stamps(lctr_ctx* c, const uint64_t* stamps, uint64_t n, uint64_t clock);
 // rows of the row-indexed parameter / optimizer-state transfers: F, or the capacity in keyed mode (the null row stays out)
 inline size_t api_rows(const lctr_ctx* c) { return c->keys ? c->F - 1 : c->F; }
+// global rows < rows that rank holds when global row g lives on rank g % world (at local row g / world); rank < world
+inline size_t owned_rows(size_t rows, size_t world, size_t rank) { return (rows + world - 1 - rank) / world; }
+// the s1 value lctr_create gives every row: the PS Adagrad / DCASGDA rules start data_accum at 1e-7 (paramserver.h:323)
+inline float initial_s1(const lctr_cfg& cf) {
+    return cf.optimizer == LCTR_OPT_PS_ADAGRAD || cf.optimizer == LCTR_OPT_PS_DCASGDA ? 1e-7f : 0.f;
+}
+// W, V, s1 and s2 of this rank's shard back to the state lctr_create gives (capi.cu)
+int reset_table_rows(lctr_ctx* c);
 
 }  // namespace lctr
