@@ -32,7 +32,7 @@ SYMBOLS = [
     "lctr_save_dataset_bin", "lctr_load_dataset_bin", "lctr_eval", "lctr_upload_pred", "lctr_ipc_export", "lctr_ipc_import",
     "lctr_dense_grad_buffer", "lctr_device_bytes", "lctr_load_libffm", "lctr_free_dataset", "lctr_launch_count", "lctr_stream", "lctr_profile", "lctr_profile_read",
     "lctr_upload_batch_keys", "lctr_lookup_keys", "lctr_download_keys", "lctr_upload_keyed_params", "lctr_set_key_init",
-    "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys", "lctr_load_checkpoint_shards",
+    "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys", "lctr_load_checkpoint_shards", "lctr_eval_pred",
 ]
 NO_LIMIT = (1 << 64) - 1  # lctr_evict_keys: UINT64_MAX = no limit
 
@@ -102,6 +102,7 @@ def load_library():
     L.lctr_set_dense_allreduce.argtypes = [vp, ALLREDUCE_FN, vp]
     L.lctr_eval.argtypes = [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int64), C.POINTER(C.c_float)]
     L.lctr_upload_pred.argtypes = [vp, C.c_int, f32p]
+    L.lctr_eval_pred.argtypes = [vp, i64, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_int64), C.POINTER(C.c_float)]
     L.lctr_save_checkpoint.argtypes = [vp, C.c_char_p]
     L.lctr_load_checkpoint.argtypes = [vp, C.c_char_p]
     L.lctr_load_checkpoint_shards.argtypes = [vp, C.c_int, C.POINTER(C.c_char_p)]
@@ -452,6 +453,16 @@ class Context:
         """(summed logloss, correct count, AUC) of the slot's pCTR / labels, computed on the device."""
         loss, correct, auc = C.c_float(), C.c_int64(), C.c_float()
         _chk(self.L.lctr_eval(self.h, slot, C.byref(loss), C.byref(correct), C.byref(auc)))
+        return loss.value, correct.value, auc.value
+
+    def eval_pred(self, pctr, labels):
+        """eval_metrics over host arrays: (summed logloss, correct count, AUC) of pctr against labels, in row order."""
+        p = np.ascontiguousarray(pctr, np.float32)
+        y = np.ascontiguousarray(labels, np.int32)
+        if len(p) != len(y):
+            raise ValueError("eval_pred: %d pCTR values for %d labels" % (len(p), len(y)))
+        loss, correct, auc = C.c_float(), C.c_int64(), C.c_float()
+        _chk(self.L.lctr_eval_pred(self.h, len(p), _p(p), _p(y), C.byref(loss), C.byref(correct), C.byref(auc)))
         return loss.value, correct.value, auc.value
 
     def upload_pred(self, slot, pctr):

@@ -469,9 +469,9 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
     LCTR_CHECK((c->cfg.model != LCTR_MODEL_FFM && c->cfg.model != LCTR_MODEL_WND) || field || nnz == 0,
                "upload_batch: FFM / Wide&Deep need the field array");
     Slot& s = c->slots[slot];
-    if (rows > s.cap_rows || nnz > s.cap_nnz) {
+    if (rows > s.cap_rows || nnz > s.cap_nnz || !s.row_ptr) {  // (!row_ptr: an empty first upload still has row_ptr[0])
         LCTR_CUDA(cudaStreamSynchronize(c->stream));  // buffers about to be reallocated may still be in use
-        if (slot_reserve(c, s, rows, nnz)) return 1;
+        if (slot_reserve(c, s, std::max<int64_t>(rows, 1), nnz)) return 1;
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
     }
     s.rows = rows; s.nnz = nnz;
@@ -501,6 +501,12 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
         // pull / push exchange, whose per-owner lists go out right away (posted stores, overlapping the previous step)
         if (fused_reserve(c, s, nnz) || fused_build_slot(c, s, st, nullptr, rows, nnz)) return 1;
         if (c->cfg.world > 1 && dist_send_keys(c, s, slot, st)) return 1;
+    } else if (c->cfg.world > 1) {
+        // an empty share still posts its (empty) key lists: the peers' serve waits for every rank's lists.  The slot then
+        // takes part in predict (0 rows) and in train steps (no gradients; the push still reads the fused FM / NFM gradient
+        // buffers, which a rank whose every share was empty has not reserved yet)
+        if (fused_reserve(c, s, 0) || dist_send_empty(c, slot, st)) return 1;
+        s.fused_valid = true;
     }
     s.csc_block = 0;
     s.dev_csc = false;
@@ -567,13 +573,8 @@ static int upload_batch_keys_dist(lctr_ctx* c, int slot, int64_t rows, int64_t n
     s.fused_valid = false;
     int rc = check_batch_keys(c, rows, nnz, row_ptr, key, field, label);
     if (!rc && !insert) {
-        set_error("lctr_upload_batch_keys: insert = 0 is single-GPU (lookup-only slots serve lctr_predict, which a sharded "
-                  "context refuses)");
-        rc = 1;
-    }
-    if (!rc && (rows == 0 || nnz == 0)) {
-        set_error("lctr_upload_batch_keys: empty batch (%lld rows, %lld entries) on a multi-GPU context", (long long)rows,
-                  (long long)nnz);
+        set_error("lctr_upload_batch_keys: insert = 0 is single-GPU (a sharded context predicts on slots uploaded with "
+                  "insert = 1; unseen keys of a test set need a world-1 load)");
         rc = 1;
     }
     if (!rc && std::min<int64_t>(nnz, (int64_t)c->F) > (int64_t)std::min<uint64_t>(c->cfg.max_nnz ? c->cfg.max_nnz : c->F, c->F)) {
@@ -586,7 +587,7 @@ static int upload_batch_keys_dist(lctr_ctx* c, int slot, int64_t rows, int64_t n
              cudaStreamSynchronize(c->stream) != cudaSuccess;
         if (rc && g_err.empty()) set_error("lctr_upload_batch_keys: slot buffers could not be reserved");
     }
-    if (!rc) rc = dist_keys_dedupe(c, s, key, nnz);
+    if (!rc && nnz > 0) rc = dist_keys_dedupe(c, s, key, nnz);  // an empty share posts empty lists (upload_batch_on)
     if (!rc) rc = upload_batch_on(c, c->stream, slot, rows, nnz, row_ptr, nullptr, field, val, label, true);
     std::string own;
     if (rc) {
@@ -657,6 +658,8 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
                "train_step: multi-GPU contexts need cfg.minibatch_size = the GLOBAL batch (the updater's divisor)");
     const uint64_t step = c->step;
     int rc = 0;
+    if (c->cfg.world > 1 && re == rb)  // an empty share: no forward publishes this step's statistics
+        LCTR_CUDA(cudaMemsetAsync(c->stats + 2 * (step % kStatRing), 0, 2 * sizeof(double), c->stream));
     if (c->csc_in_step && c->cfg.deterministic == 2 && c->cfg.world == 1 && rb == 0 && re == s.rows && s.nnz > 0) {
         // bench mode: the grouping of the batch (count / scan / fill) is part of the timed step instead of the upload
         ProfScope prof(c, PROF_CSC_BUILD);
@@ -911,6 +914,35 @@ int lctr_wait(lctr_ctx* c, uint64_t ticket, float* loss_sum, float* acc_cnt) {
     return 0;
 }
 
+// world > 1, FM / FFM: a collective pull-only round on the slot (dist.cu): the owners serve its rows from their shards into
+// the batch-compact cache, the single-GPU forward runs on that cache, and the cache is released to the owners.  No push,
+// merge or updater; the step counter does not advance.  Refused before anything is launched, alike on every rank that
+// passes the same arguments.
+static int predict_dist(lctr_ctx* c, Slot& s, int slot, int quirk_sumvx_slot, float* pctr) {
+    if (c->cfg.model == LCTR_MODEL_NFM) {
+        set_error("lctr_predict: the reference ships no NFM predictor (main.cpp:230-233)");
+        return 1;
+    }
+    LCTR_CHECK(quirk_sumvx_slot < 0, "lctr_predict: quirk_sumvx_slot is single-GPU: the quirk predictor reads another slot's "
+                                     "sumVX, which a sharded context does not keep for the rows of this slot (world %d)",
+               c->cfg.world);
+    const bool fm_tree = c->cfg.model == LCTR_MODEL_FM && fused_kernels_ok(c);
+    // the order-free FM forward waits for the owners' rows in-kernel; FFM and the other FM kernels behind a wait kernel
+    if (dist_pre_step(c, s, slot, fm_tree, false)) return 1;
+    int rc;
+    if (c->cfg.model == LCTR_MODEL_FFM) rc = launch_ffm_forward(c, s, 0, s.rows, false);
+    else if (fm_tree) rc = launch_fm_forward_tree(c, s, 0, s.rows, false);
+    else rc = launch_fm_forward(c, s, 0, s.rows, false, false);
+    if (dist_release(c)) return 1;  // also after a failed forward: the owners' next serve waits for it
+    if (rc) return 1;
+    if (dist_check_overflow(c)) return 1;  // a truncated key list gives no prediction
+    if (pctr && s.rows > 0) {
+        LCTR_CUDA(cudaMemcpyAsync(pctr, s.pred, (size_t)s.rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    }
+    return 0;
+}
+
 int lctr_predict(lctr_ctx* c, int slot, int quirk_sumvx_slot, float* pctr) {
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
@@ -919,22 +951,24 @@ int lctr_predict(lctr_ctx* c, int slot, int quirk_sumvx_slot, float* pctr) {
     LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "lctr_predict: slot %d is stale: lctr_evict_keys or a keyed checkpoint load "
                                                "renumbered rows after it was uploaded; upload it again", slot);
     int rc = 0;
+    if (c->cfg.world > 1 && c->cfg.model != LCTR_MODEL_WND) return predict_dist(c, s, slot, quirk_sumvx_slot, pctr);
     if (c->cfg.model == LCTR_MODEL_WND) {
         // Distributed_Algo_Abst::Predict (distributed_algo_abst.h:163-174): a forward pass over the slot; with several
-        // ranks a collective call (every rank serves the rows its peers need)
+        // ranks a collective pull-only round (every rank serves the rows its peers need, then releases its cache)
+        const bool multi = c->cfg.world > 1;
+        if (multi && dist_pre_step(c, s, slot, false, false)) return 1;
         const float* out = nullptr;
-        rc = (c->cfg.world > 1 && dist_pre_step(c, s, slot, false)) || mlp_reserve(c, s.rows) || wnd_reserve(c, s.rows) ||
-             launch_wnd_forward(c, s, 0, s.rows) || mlp_forward_only(c, s.rows, &out) || launch_wnd_pred(c, s, out, 0, s.rows);
+        rc = mlp_reserve(c, s.rows) || wnd_reserve(c, s.rows) || launch_wnd_forward(c, s, 0, s.rows) ||
+             (s.rows > 0 && (mlp_forward_only(c, s.rows, &out) || launch_wnd_pred(c, s, out, 0, s.rows)));
+        if (multi && dist_release(c)) return 1;
         if (rc) return 1;
+        if (multi && dist_check_overflow(c)) return 1;  // a truncated key list gives no prediction
         if (pctr) {
             LCTR_CUDA(cudaMemcpyAsync(pctr, s.pred, (size_t)s.rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
             LCTR_CUDA(cudaStreamSynchronize(c->stream));
         }
         return 0;
     }
-    // world > 1: the compute view only holds the rows pulled by the last train step, at their pre-update values
-    LCTR_CHECK(c->cfg.world == 1, "lctr_predict: multi-GPU contexts keep sharded tables; download the parameters "
-                                  "(lctr_download_params) into a single-GPU context to predict");
     if (c->cfg.model == LCTR_MODEL_FFM) {
         // parity mode: the reference's own pair loop order; otherwise the field-pair factorised forward
         rc = c->cfg.deterministic == 1 ? launch_ffm_predict_inorder(c, s) : launch_ffm_forward(c, s, 0, s.rows, false);

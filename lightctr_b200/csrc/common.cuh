@@ -371,7 +371,9 @@ int launch_ffm_predict_inorder(lctr_ctx* c, Slot& s);
 int dist_alloc(lctr_ctx* c);
 int dist_free(lctr_ctx* c);
 int dist_send_keys(lctr_ctx* c, Slot& s, int slot, cudaStream_t st);               // at upload: key lists -> the owners' inboxes
-int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait);           // owner-driven pull of the step's rows
+int dist_send_empty(lctr_ctx* c, int slot, cudaStream_t st);                      // at upload of an empty share: empty lists
+int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait, bool train = true);  // owner-driven pull of the step's rows
+int dist_release(lctr_ctx* c);                                                     // end of a pull-only round (train = false)
 int dist_post_step(lctr_ctx* c, Slot& s, int slot, int64_t rows_divisor);         // push gradients, owner-side merge + update
 int dist_check_overflow(lctr_ctx* c);
 // keyed contexts (collective upload): begin, requester dedupe into s.fid, refusal in place of the lists, owner translation

@@ -31,6 +31,18 @@
 // ids, the lists carry the keys, and each owner translates them into its shard's rows before the step (see "keyed upload").
 // Launches per step: 6; the barriers between the phases are flags written at the tail of one kernel and polled at the
 // head of the next -- no barrier launches, no host involvement.
+//
+// Pull-only rounds (lctr_predict: serve + forward, no push / merge / updater, no owner-side union build) and the cache
+// release.  Invariant: no owner writes into requester r's cache for epoch e+1 until r's kernels of epoch e have stopped
+// reading it.  In a training round this follows from the push: owner o serves e+1 only after its merge of e (stream order),
+// the merge waited for r's "pushes landed" flag, and r's push runs after r's compute has finished with the cache.  A
+// pull-only round has no push, so r ends it with release_cache_kernel, launched behind its forward (ordinary stream order:
+// every read of the cache has completed), which raises FLAG_RELEASED = e on every owner.  The next round's serve is
+// preceded by a wait for FLAG_RELEASED >= e from every requester -- only when the previous round was pull-only, which
+// every rank knows because rounds are collective.  Two training rounds in a row issue exactly the launches and waits they
+// did before pull-only rounds existed; a round after a pull-only one issues one extra (one-block) wait launch.
+// Empty shares: a rank that uploads 0 rows (or 0 entries) still posts its key lists, empty, with the generation flag, so
+// its peers' serve never waits for lists that would not come; it then serves, predicts 0 rows and pushes no gradients.
 #include <stdlib.h>
 #include <string.h>
 
@@ -55,7 +67,8 @@ struct PeerTable { Peer p[kMaxWorld]; };
 
 // byte offsets inside the arena (identical on every rank)
 struct ArenaLayout {
-    size_t flags;        // u64 [3 + kNumSlots][kMaxWorld]: row 0 rows delivered, 1 pushes landed, 3 + s keys of slot s
+    size_t flags;        // u64 [4 + kNumSlots][kMaxWorld]: row 0 rows delivered, 1 pushes landed, 2 keyed statuses, 3 cache
+                         // released (pull-only rounds), 4 + s keys of slot s
     size_t key_inbox;    // [kNumSlots][2][world] regions (2: parity of the slot's upload generation -- a list may still be read
                          // by a slower owner's merge when its sender already uploads the slot's next batch):
                          // 64 B header {u32 count, u32 requester status (keyed)} + cap_pair x uint2 {row, requester slot}
@@ -68,7 +81,7 @@ struct ArenaLayout {
     size_t grad_region;  // bytes per region
     size_t total;
 };
-enum { FLAG_PULLED = 0, FLAG_PUSHED = 1, FLAG_XLATED = 2, FLAG_KEYS = 3 };
+enum { FLAG_PULLED = 0, FLAG_PUSHED = 1, FLAG_XLATED = 2, FLAG_RELEASED = 3, FLAG_KEYS = 4 };
 // statuses of a keyed upload (code << 8 | rank): raised by every owner on every requester in FLAG_XLATED as seq << 16 | status
 enum { XS_OK = 0, XS_REFUSED = 1, XS_INBOX = 2, XS_TIMEOUT = 3, XS_CAPACITY = 4, XS_TABLE_FULL = 5 };
 // bound of every wait of the keyed upload: ~4 s at the H100's boost clock (longer at lower clocks)
@@ -102,6 +115,7 @@ struct DistState {
     void* opened[kMaxWorld][kNumHandles] = {{nullptr}};
     bool imported = false;
     unsigned long long epoch = 0;
+    unsigned long long released = 0; // epoch of the last round when it was pull-only (its requesters release their caches), else 0
     unsigned long long gen[kNumSlots] = {0};
     size_t bytes = 0;                 // device memory this module allocated
     // keyed contexts (cfg.key_mode = LCTR_KEYS_HASHED): requester-side dedupe of a batch's keys into batch-local ids u,
@@ -490,6 +504,18 @@ __global__ void wait_flags_kernel(PeerTable P, ArenaLayout A, int me, int row, i
     wait_flags(P.p[me].arena, A, row, world, value);
 }
 
+// end of a pull-only round, launched behind the forward (its reads of my cache are complete): every owner may write my
+// cache again
+__global__ void release_cache_kernel(PeerTable P, ArenaLayout A, int me, int world, unsigned long long epoch) {
+    const int o = threadIdx.x;
+    if (o < world) {
+        __threadfence_system();
+        volatile unsigned long long* f = flag_ptr(P.p[o].arena, A, FLAG_RELEASED, me);
+        *f = epoch;
+        __threadfence_system();
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // step 3: push.  The gradient rows of owner o are rows [o * cap_pair, o * cap_pair + n_o) of my compact buffer, in the
 // order of the list o received: one contiguous stream of records [gV (rowlen) | gW | pad] into o's gradient inbox.
@@ -732,7 +758,7 @@ int dist_alloc(lctr_ctx* c) {
     d->recw = (int)((c->rowlen + 4 + 3) / 4 * 4);
     ArenaLayout& A = d->A;
     size_t off = 0;
-    A.flags = off; off = align_up(off + (size_t)(3 + kNumSlots) * kMaxWorld * sizeof(unsigned long long), 256);
+    A.flags = off; off = align_up(off + (size_t)(FLAG_KEYS + kNumSlots) * kMaxWorld * sizeof(unsigned long long), 256);
     A.key_keys = 64 + d->cap_pair * sizeof(uint2);
     A.key_region = align_up(A.key_keys + (d->keyed ? d->cap_pair * sizeof(unsigned long long) : 0), 256);
     A.key_inbox = off; off += A.key_region * kNumSlots * 2 * R;
@@ -860,6 +886,22 @@ int dist_send_keys(lctr_ctx* c, Slot& s, int slot, cudaStream_t st) {
     const unsigned rg = (unsigned)std::max<int64_t>(1, std::min<int64_t>((s.nnz + 255) / 256, (int64_t)c->sm_count * 8));
     remap_entries_kernel<<<rg, 256, 0, st>>>(nullptr, s.nnz, opos, s.ent_pslot, s.ent_slot, hot_p ? s.hot_of : nullptr, s.n_uniq, hot_p);
     c->launches += 3;
+    LCTR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// an empty share (0 rows or 0 entries): empty key lists and the generation flag on every owner, status OK -- the peers'
+// serve / translation of this upload then finds my lists like any other
+int dist_send_empty(lctr_ctx* c, int slot, cudaStream_t st) {
+    DistState* d = c->dist;
+    LCTR_CHECK(d->imported, "multi-GPU upload before lctr_ipc_import");
+    d->gen[slot]++;
+    const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
+    if (d->keyed) LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), st));
+    send_keys_finish_kernel<<<1, 32, 0, st>>>(d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair, d->send_cnt,
+                                              d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow : nullptr, 0);
+    d->posted = d->keyed;
+    c->launches++;
     LCTR_CUDA(cudaGetLastError());
     return 0;
 }
@@ -992,12 +1034,13 @@ int dist_check_overflow(lctr_ctx* c) {
     return 0;
 }
 
-int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait) {
+// train = false: a pull-only round (no owner-side union: only the merge reads it); end it with dist_release
+int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait, bool train) {
     DistState* d = c->dist;
     LCTR_CHECK(d->imported, "multi-GPU step before lctr_ipc_import");
     LCTR_CHECK(s.fused_valid, "multi-GPU step on a slot without its key set");
     d->epoch++;
-    if (d->own_uniq && d->own_gen[slot] != d->gen[slot]) {  // first step on this upload of the slot: the owner-side union
+    if (train && d->own_uniq && d->own_gen[slot] != d->gen[slot]) {  // first step on this upload of the slot: the owner-side union
         const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
         const unsigned g1 = (unsigned)std::max<int64_t>(8, std::min<int64_t>((int64_t)c->sm_count * 4, ((int64_t)d->cap_pair + 255) / 256));
         LCTR_CUDA(cudaMemsetAsync(d->n_own + slot, 0, sizeof(unsigned int), c->stream));
@@ -1010,10 +1053,17 @@ int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait) {
         c->launches += 3;
         d->own_gen[slot] = d->gen[slot];
     }
+    if (d->released) {  // the previous round was pull-only: its requesters' kernels may still read their caches
+        wait_flags_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, FLAG_RELEASED, d->world, d->released);
+        c->launches++;
+        d->released = 0;
+    }
     { ProfScope prof(c, PROF_DIST_PULL);
-    // rows this rank serves ~ the union of what R requesters ask of it ~ (keys of a batch): one warp iteration = 32 rows (FM)
+    // rows this rank serves ~ the union of what R requesters ask of it ~ (keys of a batch): one warp iteration = 32 rows (FM).
+    // A rank with an empty share has no batch of its own to size by: it sizes for a full list (cap_pair)
+    const int64_t serve_keys = s.nnz > 0 ? std::min<int64_t>(s.nnz, (int64_t)c->F) : (int64_t)d->cap_pair;
     const unsigned pull_grid = (unsigned)std::max<int64_t>(8, std::min<int64_t>((int64_t)c->sm_count * 4,
-        (std::min<int64_t>(s.nnz, (int64_t)c->F) * (int64_t)std::max<size_t>(1, c->rowlen / 16) + 255) / 256));
+        (serve_keys * (int64_t)std::max<size_t>(1, c->rowlen / 16) + 255) / 256));
     serve_pull_kernel<<<pull_grid, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot * 2 + (int)(d->gen[slot] & 1), slot,
                                                              d->gen[slot], d->epoch, (int)c->rowlen, (unsigned)d->cap_pair, c->W, c->V,
                                                              d->done_ctr + 0); }
@@ -1023,6 +1073,16 @@ int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait) {
         wait_flags_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, FLAG_PULLED, d->world, d->epoch);
         c->launches++;
     }
+    LCTR_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// end of a pull-only round (behind its forward): my cache is released to every owner for the next round
+int dist_release(lctr_ctx* c) {
+    DistState* d = c->dist;
+    release_cache_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, d->epoch);
+    c->launches++;
+    d->released = d->epoch;
     LCTR_CUDA(cudaGetLastError());
     return 0;
 }

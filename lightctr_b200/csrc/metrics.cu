@@ -13,6 +13,7 @@
 // Integer work is bit-exact; AUC is bit-identical to the reference for the same pCTR array (tests/test_parity_gpu.py);
 // the logloss differs from glibc only through logf/log (<= 1 ulp per term).
 #include <algorithm>
+#include <vector>
 
 #include "common.cuh"
 
@@ -134,28 +135,20 @@ struct AucScratch {
     uint2* list = nullptr;
     size_t list_cap = 0;
     float* out = nullptr;
+    float *in_pred = nullptr, *in_label = nullptr;  // lctr_eval_pred: the caller's arrays on the device
+    size_t in_cap = 0;
 };
 
 void metrics_free(lctr_ctx* c) {
     AucScratch* a = (AucScratch*)c->auc_scratch;
     if (!a) return;
     cudaFree(a->pos); cudaFree(a->neg); cudaFree(a->tile_cnt); cudaFree(a->tile_off); cudaFree(a->total);
-    cudaFree(a->list); cudaFree(a->out);
+    cudaFree(a->list); cudaFree(a->out); cudaFree(a->in_pred); cudaFree(a->in_label);
     delete a;
     c->auc_scratch = nullptr;
 }
 
-}  // namespace lctr
-
-using namespace lctr;
-
-extern "C" {
-
-int lctr_eval(lctr_ctx* c, int slot, float* loss_sum, int64_t* correct, float* auc) {
-    LCTR_CHECK(c, "null ctx");
-    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
-    Slot& s = c->slots[slot];
-    LCTR_CHECK(s.rows > 0, "lctr_eval: slot %d is empty", slot);
+static int auc_scratch(lctr_ctx* c, AucScratch** out) {
     AucScratch* a = (AucScratch*)c->auc_scratch;
     if (!a) {
         a = new AucScratch();
@@ -170,17 +163,27 @@ int lctr_eval(lctr_ctx* c, int slot, float* loss_sum, int64_t* correct, float* a
         LCTR_CUDA(cudaMalloc((void**)&a->total, sizeof(unsigned int)));
         LCTR_CUDA(cudaMalloc((void**)&a->out, 4 * sizeof(float)));
     }
-    if ((size_t)s.rows > a->list_cap) {
+    *out = a;
+    return 0;
+}
+
+// the three metrics of n device-resident (pCTR, label) pairs, in row order: histogram, compaction of the non-empty buckets,
+// and the two fp32 chains (five launches)
+static int eval_device(lctr_ctx* c, AucScratch* a, const float* pred, const float* label, int64_t n, float* loss_sum,
+                       int64_t* correct, float* auc) {
+    if ((size_t)n > a->list_cap) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
         if (a->list) cudaFree(a->list);
-        LCTR_CUDA(cudaMalloc((void**)&a->list, (size_t)(s.rows + 32) * sizeof(uint2)));
-        a->list_cap = (size_t)s.rows;
+        a->list = nullptr;
+        a->list_cap = 0;
+        LCTR_CUDA(cudaMalloc((void**)&a->list, (size_t)(n + 32) * sizeof(uint2)));
+        a->list_cap = (size_t)n;
     }
-    auc_hist_kernel<<<(unsigned)((s.rows + 255) / 256), 256, 0, c->stream>>>(s.pred, s.label, s.rows, a->pos, a->neg);
+    auc_hist_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(pred, label, n, a->pos, a->neg);
     auc_tile_count_kernel<<<kAucTiles / 8, 256, 0, c->stream>>>(a->pos, a->neg, a->tile_cnt);
     auc_tile_scan_kernel<<<1, 1024, 0, c->stream>>>(a->tile_cnt, a->tile_off, a->total);
     auc_tile_write_kernel<<<kAucTiles / 8, 256, 0, c->stream>>>(a->pos, a->neg, a->tile_cnt, a->tile_off, a->list);
-    auc_chain_kernel<<<1, 32, 0, c->stream>>>(a->list, a->total, s.pred, s.label, s.rows, a->out);
+    auc_chain_kernel<<<1, 32, 0, c->stream>>>(a->list, a->total, pred, label, n, a->out);
     c->launches += 5;
     LCTR_CUDA(cudaGetLastError());
     float h[3];
@@ -190,6 +193,45 @@ int lctr_eval(lctr_ctx* c, int slot, float* loss_sum, int64_t* correct, float* a
     if (correct) *correct = (int64_t)h[1];
     if (auc) *auc = h[2];
     return 0;
+}
+
+}  // namespace lctr
+
+using namespace lctr;
+
+extern "C" {
+
+int lctr_eval(lctr_ctx* c, int slot, float* loss_sum, int64_t* correct, float* auc) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
+    Slot& s = c->slots[slot];
+    LCTR_CHECK(s.rows > 0, "lctr_eval: slot %d is empty", slot);
+    AucScratch* a = nullptr;
+    if (auc_scratch(c, &a)) return 1;
+    return eval_device(c, a, s.pred, s.label, s.rows, loss_sum, correct, auc);
+}
+
+// lctr_eval's metrics over host arrays (a whole test set gathered from the ranks of a sharded trainer, for one)
+int lctr_eval_pred(lctr_ctx* c, int64_t n, const float* pctr, const int32_t* label, float* loss_sum, int64_t* correct,
+                   float* auc) {
+    LCTR_CHECK(c && pctr && label, "null argument");
+    LCTR_CHECK(n > 0, "lctr_eval_pred: no rows (n = %lld)", (long long)n);
+    AucScratch* a = nullptr;
+    if (auc_scratch(c, &a)) return 1;
+    if ((size_t)n > a->in_cap) {
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
+        cudaFree(a->in_pred); cudaFree(a->in_label);
+        a->in_pred = a->in_label = nullptr;
+        a->in_cap = 0;
+        LCTR_CUDA(cudaMalloc((void**)&a->in_pred, (size_t)n * sizeof(float)));
+        LCTR_CUDA(cudaMalloc((void**)&a->in_label, (size_t)n * sizeof(float)));
+        a->in_cap = (size_t)n;
+    }
+    std::vector<float> y((size_t)n);  // as upload_batch widens them: (float) of the int32 label
+    for (int64_t i = 0; i < n; i++) y[(size_t)i] = (float)label[i];
+    LCTR_CUDA(cudaMemcpyAsync(a->in_pred, pctr, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    LCTR_CUDA(cudaMemcpyAsync(a->in_label, y.data(), (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    return eval_device(c, a, a->in_pred, a->in_label, n, loss_sum, correct, auc);  // (synchronises before y goes)
 }
 
 // test hook: overwrite the slot's pCTR array (lctr_eval then evaluates exactly these values)

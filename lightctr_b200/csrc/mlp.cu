@@ -266,14 +266,18 @@ int launch_nfm_mlp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_di
     if (c->cfg.mlp_precision == LCTR_MLP_BF16) return launch_nfm_mlp_bf16(c, s, rb, re, rows_divisor);
     LCTR_CHECK(c->cfg.mlp_precision == LCTR_MLP_FP32, "mlp_precision=%d unknown", c->cfg.mlp_precision);
     ProfScope prof(c, PROF_MLP);
-    mlp_forward_dev(c, B);
-    // ---- loss, delta of the output layer
-    double* out_slot = c->stats + 2 * (c->step % kStatRing);
-    MlpLayer& last = c->layers[nl - 1];
-    nfm_loss_kernel<<<mlp_blocks(B), 256, 0, c->stream>>>(s.wide, last.act, s.label, s.pred, last.delta, rb, B,
-                                                          c->stat_partial, c->stat_done, out_slot);
-    c->launches++;
-    mlp_backward_dev(c, B);
+    // B == 0 (a rank's empty share on several GPUs): no rows, no gradient (the buffer is zero between steps); the rank
+    // still joins the all-reduce and the replicated updater, so the collective stays matched and the layers stay equal
+    if (B > 0) {
+        mlp_forward_dev(c, B);
+        // ---- loss, delta of the output layer
+        double* out_slot = c->stats + 2 * (c->step % kStatRing);
+        MlpLayer& last = c->layers[nl - 1];
+        nfm_loss_kernel<<<mlp_blocks(B), 256, 0, c->stream>>>(s.wide, last.act, s.label, s.pred, last.delta, rb, B,
+                                                              c->stat_partial, c->stat_done, out_slot);
+        c->launches++;
+        mlp_backward_dev(c, B);
+    }
     if (mlp_sync_dense_grad(c)) return 1;
     if (!c->mlp_skip_update) mlp_apply_dev(c, c->cfg.minibatch_size ? c->cfg.minibatch_size : (uint64_t)rows_divisor);
     LCTR_CUDA(cudaGetLastError());

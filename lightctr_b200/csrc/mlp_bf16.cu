@@ -451,15 +451,19 @@ int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t ro
     P.w32_last = c->layers[nh].w;
     double* out_slot = c->stats + 2 * (c->step % kStatRing);
     const unsigned grid = (unsigned)((B + c->mlp_tm - 1) / c->mlp_tm);
-    if (c->mlp_umma && !c->mlp_has_mask) {  // wgmma kernel (mlp_umma.cu); dropout masks stay on the mma.sync kernel
-        if (launch_mlp_umma(c, s, rb, B, out_slot)) return 1;
-    } else if (c->mlp_tm == 128)
-        nfm_mlp_fused_kernel<128><<<grid, 256, c->mlp_smem, c->stream>>>(P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
-                                                                        c->stat_partial, c->stat_done, out_slot);
-    else
-        nfm_mlp_fused_kernel<64><<<grid, 128, c->mlp_smem, c->stream>>>(P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
-                                                                       c->stat_partial, c->stat_done, out_slot);
-    if (!(c->mlp_umma && !c->mlp_has_mask)) c->launches++;
+    // B == 0 (a rank's empty share on several GPUs): no rows, no gradient; the rank still joins the all-reduce and the
+    // replicated updater below
+    if (B > 0) {
+        if (c->mlp_umma && !c->mlp_has_mask) {  // wgmma kernel (mlp_umma.cu); dropout masks stay on the mma.sync kernel
+            if (launch_mlp_umma(c, s, rb, B, out_slot)) return 1;
+        } else if (c->mlp_tm == 128)
+            nfm_mlp_fused_kernel<128><<<grid, 256, c->mlp_smem, c->stream>>>(P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
+                                                                            c->stat_partial, c->stat_done, out_slot);
+        else
+            nfm_mlp_fused_kernel<64><<<grid, 128, c->mlp_smem, c->stream>>>(P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
+                                                                           c->stat_partial, c->stat_done, out_slot);
+        if (!(c->mlp_umma && !c->mlp_has_mask)) c->launches++;
+    }
     LCTR_CUDA(cudaGetLastError());
     if (mlp_sync_dense_grad(c)) return 1;
     if (!c->mlp_skip_update) {

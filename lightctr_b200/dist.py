@@ -73,6 +73,34 @@ def reduce_stats(loss, correct, group=None):
     return float(t[0]), float(t[1])
 
 
+def eval_global(ctx, slot, labels, group=None):
+    """(summed logloss, correct count, AUC) of the whole test set a sharded trainer just predicted (lctr_predict on `slot`,
+    collective): every rank passes the labels of its own rows.  This rank's pCTR is downloaded, (pCTR, labels) are
+    all-gathered in rank order and the concatenation is evaluated on every rank (lctr_eval_pred), so every rank returns the
+    same numbers, equal bit for bit to lctr_eval on one GPU holding the concatenated batch (rank 0's rows first) with the
+    same pCTR.  Shares may be uneven, or empty.  Host traffic per rank: R * n * 8 B, with n the largest share."""
+    import torch.distributed as dist
+    y = np.ascontiguousarray(labels, np.int32)
+    p = ctx.download_pred(slot)
+    world = dist.get_world_size(group)
+    # every rank's row and label counts first: a mismatch on any rank fails the call on every rank, none is left waiting
+    counts = np.frombuffer(exchange_blobs(np.array([len(p), len(y)], np.int64).tobytes(), group)[0], np.int64).reshape(world, 2)
+    bad = [r for r in range(world) if counts[r, 0] != counts[r, 1]]
+    if bad:
+        raise ValueError("eval_global: slot %d: pCTR rows and labels differ on rank(s) %s (%s)" %
+                         (slot, bad, ", ".join("%d vs %d" % tuple(counts[r]) for r in bad)))
+    counts = counts[:, 0]
+    n_max = int(counts.max())
+    blob = np.zeros(2 * n_max, np.float32)
+    blob[:len(p)] = p
+    blob.view(np.int32)[n_max:n_max + len(y)] = y
+    allb, per = exchange_blobs(blob.tobytes(), group)
+    parts = [np.frombuffer(allb[r * per:(r + 1) * per], np.float32) for r in range(world)]
+    pctr = np.concatenate([b[:counts[r]] for r, b in enumerate(parts)])
+    lab = np.concatenate([b.view(np.int32)[n_max:n_max + counts[r]] for r, b in enumerate(parts)])
+    return ctx.eval_pred(pctr, lab)
+
+
 def merge_shards(parts, world, n_rows):
     """Combine per-rank full-size arrays whose only valid rows are the owned ones (lctr_download_params, world > 1)."""
     rowlen = len(parts[0]) // n_rows
