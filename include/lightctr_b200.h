@@ -257,12 +257,19 @@ int lctr_mlp_download_grad(lctr_ctx* ctx, int layer, float* dweight, float* dbia
 
 /* ---- multi-GPU (replaces distribut/ring_collect.h + pull.h/push.h; see DESIGN.md) ------------ */
 /* Exchange of CUDA IPC handles is done by the caller's process group (torch.distributed / MPI):
- * export this rank's table handles, gather them, import all peers'. */
+ * export this rank's handle, gather them, import all peers'.  A rank shares one buffer, its exchange arena (flags, key
+ * inboxes, parameter cache, gradient inboxes), so the blob is one cudaIpcMemHandle_t (64 B); size it with
+ * lctr_ipc_export(ctx, NULL, 0, &n).  Import refuses a bytes_per_rank other than that size. */
 int lctr_ipc_export(lctr_ctx* ctx, void* handles_out, size_t cap, size_t* bytes);
 int lctr_ipc_import(lctr_ctx* ctx, const void* all_handles, size_t bytes_per_rank);
-/* device memory of the context in bytes: table shard + updater state (+ the key table in keyed mode, + 8 B per row of
- * stamps with key_evict = 1; per-call scratch is not counted), and (world > 1) the exchange arena, caches and
- * inboxes -- owner-sharding keeps the second number O(keys of a batch), not O(feature_cnt) */
+/* device memory of the context in bytes.  shard_bytes: the table shard W, V and the updater state s1 (+ s2 for the
+ * two-state updaters), Fl (k + 1) floats each for FM / NFM, Fl (Fc k + 1) for FFM; + update_g of the same size on the
+ * dense gradient path (FFM with deterministic 0 or 1, Wide&Deep, FM / NFM with deterministic = 0 and k outside
+ * {4, 8, 16, 32}, NFM with deterministic = 2) and for the grouped FFM backward (deterministic = 2); + the touched map,
+ * 1 B per row, on the dense path only; + the key table in keyed mode and 8 B per row of stamps with key_evict = 1.  The
+ * compact (FM / NFM, deterministic = 0, k in {4, 8, 16, 32}) and the other feature-major paths hold no gradient per row.
+ * Per-call scratch is not counted.  exchange_bytes (world > 1): the exchange arena, caches and inboxes -- owner-sharding
+ * keeps it O(keys of a batch), not O(feature_cnt) */
 int lctr_device_bytes(lctr_ctx* ctx, uint64_t* shard_bytes, uint64_t* exchange_bytes);
 /* Data-parallel dense layers (world > 1, NFM): the per-rank weightDelta / biasDelta of the batch must be summed over
  * the ranks before the updater runs -- Worker_RingReduce::syncGradient (distribut/ring_collect.h:48-72) on the

@@ -179,6 +179,15 @@ static int build_csc(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz, const int6
     s.csc_block = block; s.n_blocks = nblocks; s.n_segs = nseg;
     return 0;
 }
+// the one place that says where a context's sparse gradient goes (GradPath, common.cuh)
+static GradPath grad_path_of(const lctr_cfg& cf) {
+    const int k = (int)cf.factor_cnt;
+    const bool fm = cf.model == LCTR_MODEL_FM, nfm = cf.model == LCTR_MODEL_NFM;
+    if ((fm || nfm) && cf.deterministic == 0 && (k == 4 || k == 8 || k == 16 || k == 32)) return GRAD_COMPACT;
+    if ((fm && cf.deterministic != 0) || (nfm && cf.deterministic == 1) || (cf.model == LCTR_MODEL_FFM && cf.deterministic == 2))
+        return GRAD_FEATURE_MAJOR;
+    return GRAD_DENSE;
+}
 }  // namespace lctr
 
 using namespace lctr;
@@ -239,6 +248,9 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
     LCTR_CHECK(c->cfg.world == 1 || !cfg->deterministic, "lctr_create: deterministic modes are single-GPU only");
     LCTR_CHECK(cfg->deterministic >= 0 && cfg->deterministic <= 2, "lctr_create: deterministic must be 0, 1 or 2");
     c->rowlen = cfg->model == LCTR_MODEL_FFM ? (size_t)cfg->field_cnt * cfg->factor_cnt : cfg->factor_cnt;
+    c->grad_path = grad_path_of(c->cfg);
+    const bool dense = c->grad_path == GRAD_DENSE;
+    const bool update_g = dense || (cfg->model == LCTR_MODEL_FFM && c->grad_path == GRAD_FEATURE_MAJOR);
     cudaDeviceProp prop;
     LCTR_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
     c->sm_count = prop.multiProcessorCount;
@@ -249,29 +261,35 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
                      cfg->optimizer == LCTR_OPT_PS_DCASGD || cfg->optimizer == LCTR_OPT_PS_DCASGDA;
     int rc = 0;
     rc |= dalloc(&c->W, FL); rc |= dalloc(&c->V, nv);
-    rc |= dalloc(&c->gW, FL); rc |= dalloc(&c->gV, nv);
+    if (update_g) { rc |= dalloc(&c->gW, FL); rc |= dalloc(&c->gV, nv); }
     rc |= dalloc(&c->s1W, FL); rc |= dalloc(&c->s1V, nv);
     if (two) { rc |= dalloc(&c->s2W, FL); rc |= dalloc(&c->s2V, nv); }
-    rc |= dalloc(&c->touched, FL + 512);
-    rc |= dalloc(&c->touch_list, FL + 32);
-    rc |= dalloc(&c->n_touch, 1);
-    rc |= dalloc(&c->apply_done, 1);
+    if (dense) {  // the sparse apply of opt.cu: touched map, its compacted list and counters
+        rc |= dalloc(&c->touched, FL + 512);
+        rc |= dalloc(&c->touch_list, FL + 32);
+        rc |= dalloc(&c->n_touch, 1);
+        rc |= dalloc(&c->apply_done, 1);
+    }
     rc |= dalloc(&c->stats, (size_t)2 * kStatRing);
     rc |= dalloc(&c->stat_partial, 2);
     rc |= dalloc(&c->stat_done, 1);
     if (rc) { lctr_destroy(c); return 1; }
     LCTR_CUDA(cudaMallocHost((void**)&c->h_stats, 2 * sizeof(double)));
     if (reset_table_rows(c)) { lctr_destroy(c); return 1; }
-    LCTR_CUDA(cudaMemsetAsync(c->gW, 0, FL * sizeof(float), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(c->gV, 0, nv * sizeof(float), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(c->touched, 0, FL + 512, c->stream));
+    if (update_g) {
+        LCTR_CUDA(cudaMemsetAsync(c->gW, 0, FL * sizeof(float), c->stream));
+        LCTR_CUDA(cudaMemsetAsync(c->gV, 0, nv * sizeof(float), c->stream));
+    }
+    if (dense) {
+        LCTR_CUDA(cudaMemsetAsync(c->touched, 0, FL + 512, c->stream));
+        LCTR_CUDA(cudaMemsetAsync(c->n_touch, 0, sizeof(unsigned int), c->stream));
+        LCTR_CUDA(cudaMemsetAsync(c->apply_done, 0, sizeof(unsigned int), c->stream));
+    }
     if (c->cfg.world > 1) {
         if (dist_alloc(c)) { lctr_destroy(c); return 1; }
     } else {
         c->cW = c->W; c->cV = c->V; c->cgW = c->gW; c->cgV = c->gV;
     }
-    LCTR_CUDA(cudaMemsetAsync(c->n_touch, 0, sizeof(unsigned int), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(c->apply_done, 0, sizeof(unsigned int), c->stream));
     LCTR_CUDA(cudaMemsetAsync(c->stats, 0, sizeof(double) * 2 * kStatRing, c->stream));
     LCTR_CUDA(cudaMemsetAsync(c->stat_partial, 0, sizeof(double) * 2, c->stream));
     LCTR_CUDA(cudaMemsetAsync(c->stat_done, 0, sizeof(unsigned int), c->stream));
@@ -496,17 +514,14 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
     }
     s.fused_valid = false;
     s.key_state = SLOT_KEYS_OK;
-    if ((fused_supported(c) || c->cfg.world > 1) && rows > 0 && nnz > 0) {  // fused_supported: FM and NFM, one GPU
-        // slot map of the batch: the gradient rows of the order-free fused step; on several GPUs also the key set of the
-        // pull / push exchange, whose per-owner lists go out right away (posted stores, overlapping the previous step)
+    if (c->grad_path == GRAD_COMPACT || c->cfg.world > 1) {
+        // slot map of the batch: the gradient rows of the compact path; on several GPUs also the key set of the pull / push
+        // exchange, whose per-owner lists go out right away (posted stores, overlapping the previous step).  An empty batch
+        // (0 rows or 0 entries) gets an empty map, and the compact gradient buffers are reserved all the same (a train step
+        // reads them).  On several GPUs it still posts its (empty) key lists: the peers' serve waits for every rank's lists
+        const bool empty = rows == 0 || nnz == 0;
         if (fused_reserve(c, s, nnz) || fused_build_slot(c, s, st, nullptr, rows, nnz)) return 1;
-        if (c->cfg.world > 1 && dist_send_keys(c, s, slot, st)) return 1;
-    } else if (c->cfg.world > 1) {
-        // an empty share still posts its (empty) key lists: the peers' serve waits for every rank's lists.  The slot then
-        // takes part in predict (0 rows) and in train steps (no gradients; the push still reads the fused FM / NFM gradient
-        // buffers, which a rank whose every share was empty has not reserved yet)
-        if (fused_reserve(c, s, 0) || dist_send_empty(c, slot, st)) return 1;
-        s.fused_valid = true;
+        if (c->cfg.world > 1 && (empty ? dist_send_empty(c, slot, st) : dist_send_keys(c, s, slot, st))) return 1;
     }
     s.csc_block = 0;
     s.dev_csc = false;
@@ -657,73 +672,54 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
     LCTR_CHECK(c->cfg.world == 1 || c->cfg.minibatch_size > 0,
                "train_step: multi-GPU contexts need cfg.minibatch_size = the GLOBAL batch (the updater's divisor)");
     const uint64_t step = c->step;
+    const bool multi = c->cfg.world > 1;
+    const int64_t rows = re - rb;
     int rc = 0;
-    if (c->cfg.world > 1 && re == rb)  // an empty share: no forward publishes this step's statistics
+    if (rows == 0)  // no forward publishes this step's statistics
         LCTR_CUDA(cudaMemsetAsync(c->stats + 2 * (step % kStatRing), 0, 2 * sizeof(double), c->stream));
     if (c->csc_in_step && c->cfg.deterministic == 2 && c->cfg.world == 1 && rb == 0 && re == s.rows && s.nnz > 0) {
         // bench mode: the grouping of the batch (count / scan / fill) is part of the timed step instead of the upload
         ProfScope prof(c, PROF_CSC_BUILD);
         if (csc_build_device(c, s, c->stream, nullptr, nullptr, s.rows, s.nnz)) return 1;
     }
-    switch (c->cfg.model) {
-        case LCTR_MODEL_FM:
-            if (c->cfg.world > 1 && fused_kernels_ok(c))
-                rc = dist_pre_step(c, s, slot, true) || launch_fm_fused(c, s, rb, re, true, nullptr, nullptr) ||
-                     dist_post_step(c, s, slot, re - rb);
-            else if (c->cfg.world > 1)
-                rc = dist_pre_step(c, s, slot, false) || launch_fm_forward(c, s, rb, re, false, true) ||
-                     launch_fm_backward(c, s, rb, re, false) || dist_post_step(c, s, slot, re - rb);
-            else if (c->cfg.deterministic == 2)
-                rc = launch_fm_forward(c, s, rb, re, false, true) || launch_fm_backward_devcsc(c, s, rb, re);
-            else if (c->cfg.deterministic)
-                rc = launch_fm_forward(c, s, rb, re, false, true) || launch_fm_backward_csc(c, s, rb, re, false);
-            else if (s.fused_valid)  // order-free: one gather, RED scatter into the batch-compact buffer, compact updater
-                rc = launch_fm_fused(c, s, rb, re, true, nullptr, nullptr) || launch_apply_compact(c, s, re - rb, nullptr, nullptr);
-            else
-                rc = launch_fm_forward(c, s, rb, re, false, true) || launch_fm_backward(c, s, rb, re, false) ||
-                     launch_apply(c, re - rb);
+    // Several GPUs: the rows come from the owners' shards into the batch-compact cache (dist_pre_step) and the gradient rows
+    // go back to their owners, who merge and update (dist_post_step).  NFM / Wide&Deep: dense layers replicated, their
+    // gradients all-reduced (launch_nfm_mlp).
+    const bool fm = c->cfg.model == LCTR_MODEL_FM;
+    switch (c->grad_path) {
+        case GRAD_COMPACT:  // FM / NFM: one gather, RED scatter into the batch-compact buffer (fm_fused.cu), compact updater
+            if (!multi && rows == 0) break;  // nothing to update; on several GPUs the rank still joins the exchange
+            rc = (multi && dist_pre_step(c, s, slot, true)) ||
+                 (fm ? launch_fm_fused(c, s, rb, re, true, nullptr, nullptr)
+                     : mlp_reserve(c, rows) || launch_nfm_forward_fused(c, s, rb, re) || launch_nfm_mlp(c, s, rb, re, rows) ||
+                           launch_nfm_backward_fused(c, s, rb, re)) ||
+                 (multi ? dist_post_step(c, s, slot, rows) : launch_apply_compact(c, s, rows, nullptr, nullptr));
             break;
-        case LCTR_MODEL_FFM:
-            if (c->cfg.world > 1)
-                rc = dist_pre_step(c, s, slot, false) || launch_ffm_forward(c, s, rb, re, true) || dist_post_step(c, s, slot, re - rb);
-            else if (c->cfg.deterministic == 2)
-                rc = ffm_grouped_reserve(c, s.rows) || launch_ffm_forward_tiles(c, s, rb, re) ||
-                     launch_ffm_backward_grouped(c, s, rb, re);
+        case GRAD_FEATURE_MAJOR:  // one GPU: the updater runs inside the backward
+            if (c->cfg.model == LCTR_MODEL_FFM)
+                rc = ffm_grouped_reserve(c, s.rows) || launch_ffm_forward_tiles(c, s, rb, re) || launch_ffm_backward_grouped(c, s, rb, re);
+            else if (fm)
+                rc = launch_fm_forward(c, s, rb, re, false, true) ||
+                     (c->cfg.deterministic == 2 ? launch_fm_backward_devcsc(c, s, rb, re) : launch_fm_backward_csc(c, s, rb, re, false));
             else
-                rc = launch_ffm_forward(c, s, rb, re, true) || launch_ffm_backward(c, s, rb, re) || launch_apply(c, re - rb);
+                rc = mlp_reserve(c, rows) || launch_fm_forward(c, s, rb, re, true, false) || launch_nfm_mlp(c, s, rb, re, rows) ||
+                     launch_fm_backward_csc(c, s, rb, re, true);
             break;
-        case LCTR_MODEL_WND:
-            if (c->cfg.world > 1)  // rows from the owners' shards into the batch-compact cache, gradients back to the owners
-                rc = dist_pre_step(c, s, slot, false) || mlp_reserve(c, re - rb) || wnd_reserve(c, re - rb) ||
-                     launch_wnd_forward(c, s, rb, re) || launch_nfm_mlp(c, s, rb, re, re - rb) || launch_wnd_backward(c, s, rb, re) ||
-                     dist_post_step(c, s, slot, re - rb);
-            else
-                rc = mlp_reserve(c, re - rb) || wnd_reserve(c, re - rb) || launch_wnd_forward(c, s, rb, re) ||
-                     launch_nfm_mlp(c, s, rb, re, re - rb) || launch_wnd_backward(c, s, rb, re) || launch_apply(c, re - rb);
-            break;
-        case LCTR_MODEL_NFM:
-            if (fused_kernels_ok(c) && s.fused_valid) {
-                // order-free embedding side (fm_fused.cu) around the dense layers; on several GPUs the rows come from the
-                // batch-compact cache and the gradient rows go to their owners (dist.cu)
-                const bool multi = c->cfg.world > 1;
-                rc = (multi && dist_pre_step(c, s, slot, true)) || mlp_reserve(c, re - rb) || launch_nfm_forward_fused(c, s, rb, re) ||
-                     launch_nfm_mlp(c, s, rb, re, re - rb) || launch_nfm_backward_fused(c, s, rb, re) ||
-                     (multi ? dist_post_step(c, s, slot, re - rb) : launch_apply_compact(c, s, re - rb, nullptr, nullptr));
-                break;
+        case GRAD_DENSE:  // REDs into update_g (one GPU) or the exchange's gradient rows (several), then the sparse apply
+            if (multi && dist_pre_step(c, s, slot, false)) return 1;
+            switch (c->cfg.model) {
+                case LCTR_MODEL_FM: rc = launch_fm_forward(c, s, rb, re, false, true) || launch_fm_backward(c, s, rb, re, false); break;
+                case LCTR_MODEL_FFM: rc = launch_ffm_forward(c, s, rb, re, true); break;
+                case LCTR_MODEL_WND:
+                    rc = mlp_reserve(c, rows) || wnd_reserve(c, rows) || launch_wnd_forward(c, s, rb, re) ||
+                         launch_nfm_mlp(c, s, rb, re, rows) || launch_wnd_backward(c, s, rb, re);
+                    break;
+                case LCTR_MODEL_NFM:
+                    rc = mlp_reserve(c, rows) || launch_fm_forward(c, s, rb, re, true, false) || launch_nfm_mlp(c, s, rb, re, rows) ||
+                         launch_fm_backward(c, s, rb, re, true);
+                    break;
             }
-            if (c->cfg.world > 1) {
-                // embeddings: owner-sharded pull / push like FM; dense layers: replicated, gradients all-reduced
-                rc = dist_pre_step(c, s, slot, false) || mlp_reserve(c, re - rb) || launch_fm_forward(c, s, rb, re, true, false) ||
-                     launch_nfm_mlp(c, s, rb, re, re - rb) || launch_fm_backward(c, s, rb, re, true) ||
-                     dist_post_step(c, s, slot, re - rb);
-                break;
-            }
-            rc = mlp_reserve(c, re - rb) || launch_fm_forward(c, s, rb, re, true, false) ||
-                 launch_nfm_mlp(c, s, rb, re, re - rb);
-            if (!rc) {
-                if (c->cfg.deterministic == 1) rc = launch_fm_backward_csc(c, s, rb, re, true);
-                else rc = launch_fm_backward(c, s, rb, re, true) || launch_apply(c, re - rb);
-            }
+            rc = rc || (multi ? dist_post_step(c, s, slot, rows) : launch_apply(c, rows));
             break;
     }
     if (rc) return 1;
@@ -779,7 +775,7 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
         hp->opt = c->cfg.optimizer;
     }
     cudaGraph_t graph;
-    const bool fused = fused_supported(c);
+    const bool fused = c->grad_path == GRAD_COMPACT;  // else device grouping (GRAD_FEATURE_MAJOR)
     // ---- build graph (copy stream)
     LCTR_CUDA(cudaStreamBeginCapture(c->copy_stream, cudaStreamCaptureModeThreadLocal));
     int rc = cudaMemcpyAsync(g.d_hdr, g.h_hdr, 2 * sizeof(int64_t), cudaMemcpyHostToDevice, c->copy_stream) != cudaSuccess;
@@ -824,6 +820,7 @@ static int train_batch_async_graph(lctr_ctx* c, int64_t rows, int64_t nnz, const
     const int slot = kNumSlots - kPipe + p;
     Slot& s = c->slots[slot];
     PipeGraph& g = c->pipe_graph[p];
+    const bool fused = c->grad_path == GRAD_COMPACT;
     if (rows > s.cap_rows || nnz > s.cap_nnz || !g.build || g.has_val != (val != nullptr) || g.cap_rows != s.cap_rows ||
         g.cap_nnz != s.cap_nnz) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -831,7 +828,7 @@ static int train_batch_async_graph(lctr_ctx* c, int64_t rows, int64_t nnz, const
         LCTR_CUDA(cudaStreamSynchronize(c->build_stream));
         if (rows > s.cap_rows || nnz > s.cap_nnz)  // head-room so that slightly larger batches do not re-capture
             if (slot_reserve(c, s, std::max(rows, s.cap_rows) + rows / 8 + 64, std::max(nnz, s.cap_nnz) + nnz / 8 + 1024)) return 1;
-        if (fused_supported(c) ? fused_reserve(c, s, s.cap_nnz) : csc_reserve(c, s, s.cap_nnz)) return 1;
+        if (fused ? fused_reserve(c, s, s.cap_nnz) : csc_reserve(c, s, s.cap_nnz)) return 1;
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
         if (pipe_graph_capture(c, p, val != nullptr)) return 1;
     }
@@ -849,7 +846,6 @@ static int train_batch_async_graph(lctr_ctx* c, int64_t rows, int64_t nnz, const
     LCTR_CUDA(cudaGraphLaunch(g.build, c->build_stream));
     LCTR_CUDA(cudaEventRecord(c->ev_copied[p], c->build_stream));
     LCTR_CUDA(cudaStreamWaitEvent(c->stream, c->ev_copied[p], 0));
-    const bool fused = fused_supported(c);
     if (fused) fused_opt_params(c, rows, g.h_opt); else csc_opt_params(c, rows, g.h_opt);
     LCTR_CUDA(cudaGraphLaunch(g.step, c->stream));
     LCTR_CUDA(cudaEventRecord(c->ev_computed[p], c->stream));
@@ -869,8 +865,7 @@ int lctr_train_batch_async(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t
     LCTR_CHECK(c->cfg.deterministic != 1, "streamed batches need cfg.deterministic 0 (RED scatter) or 2 (device grouping)");
     if (pipe_init(c)) return 1;
     LCTR_CHECK(c->pipe_issued - c->pipe_waited < (uint64_t)kPipe, "more than %d streamed batches outstanding: call lctr_wait first", kPipe);
-    if ((c->cfg.deterministic == 2 || fused_supported(c)) && c->cfg.world == 1 && c->cfg.model == LCTR_MODEL_FM && !c->profiling &&
-        rows > 0 && nnz > 0)
+    if (c->cfg.model == LCTR_MODEL_FM && c->grad_path != GRAD_DENSE && c->cfg.world == 1 && !c->profiling && rows > 0 && nnz > 0)
         return train_batch_async_graph(c, rows, nnz, row_ptr, fid, val, label, ticket);
     const int p = (int)(c->pipe_issued % kPipe);
     const int slot = kNumSlots - kPipe + p;
@@ -926,7 +921,7 @@ static int predict_dist(lctr_ctx* c, Slot& s, int slot, int quirk_sumvx_slot, fl
     LCTR_CHECK(quirk_sumvx_slot < 0, "lctr_predict: quirk_sumvx_slot is single-GPU: the quirk predictor reads another slot's "
                                      "sumVX, which a sharded context does not keep for the rows of this slot (world %d)",
                c->cfg.world);
-    const bool fm_tree = c->cfg.model == LCTR_MODEL_FM && fused_kernels_ok(c);
+    const bool fm_tree = c->cfg.model == LCTR_MODEL_FM && c->grad_path == GRAD_COMPACT;
     // the order-free FM forward waits for the owners' rows in-kernel; FFM and the other FM kernels behind a wait kernel
     if (dist_pre_step(c, s, slot, fm_tree, false)) return 1;
     int rc;
@@ -978,7 +973,7 @@ int lctr_predict(lctr_ctx* c, int slot, int quirk_sumvx_slot, float* pctr) {
             rc = launch_predict_quirk(c, s, c->slots[quirk_sumvx_slot]);
         } else {
             // order-free contexts predict with the shuffle-tree forward; parity contexts with the in-order one
-            rc = fused_supported(c) ? launch_fm_forward_tree(c, s, 0, s.rows, false) : launch_fm_forward(c, s, 0, s.rows, false, false);
+            rc = c->grad_path == GRAD_COMPACT ? launch_fm_forward_tree(c, s, 0, s.rows, false) : launch_fm_forward(c, s, 0, s.rows, false, false);
         }
     } else {
         set_error("lctr_predict: the reference ships no NFM predictor (main.cpp:230-233)");

@@ -6,9 +6,10 @@
 // Differences we state rather than reproduce (SURVEY.md 8e): synchronous instead of SSP-async, fp32 instead of
 // fp16 on the wire, no |g| thresholding of pushes, owner = fid mod R instead of the murmur DHT ring.
 //
-// Tables are owner-sharded: row f lives on rank f % R at shard-local index f / R.  Every rank maps every peer's
-// W / V / update_g shards, touched map and ONE arena (flags, key inboxes, parameter cache, gradient inboxes) through
-// CUDA IPC.  Per-rank memory is the shard plus O(keys of a batch): the compute kernels work on a BATCH-COMPACT cache
+// Tables are owner-sharded: row f lives on rank f % R at shard-local index f / R.  Every rank maps ONE buffer of every
+// peer through CUDA IPC, its arena (flags, key inboxes, parameter cache, gradient inboxes): owners write rows into their
+// requesters' caches and requesters push gradient rows into their owners' inboxes, so no rank reads or writes a peer's
+// table shard.  Per-rank memory is the shard plus O(keys of a batch): the compute kernels work on a BATCH-COMPACT cache
 // (row = slot of the batch's key set, fm_fused.cu's slot map) instead of full-size copies of the tables.
 //
 //   upload (depends only on the batch; on the upload stream, overlaps the previous step)
@@ -56,12 +57,9 @@ namespace lctr {
 
 constexpr int kMaxWorld = 8;
 constexpr int kHotRepD = kHotRep, kHotMaxD = kHotMax;
-constexpr int kNumHandles = 6;  // W, V, gW, gV, touched, arena
 
 struct Peer {
-    float *W, *V, *gW, *gV;
-    uint8_t* touched;
-    unsigned char* arena;
+    unsigned char* arena;  // the only buffer ranks share (lctr_ipc_export)
 };
 struct PeerTable { Peer p[kMaxWorld]; };
 
@@ -112,7 +110,7 @@ struct DistState {
     uint8_t* own_mark = nullptr;      // permuted byte map over the shard (128 * own_T)
     size_t cap_own = 0, own_T = 0;
     unsigned long long own_gen[kNumSlots] = {0};
-    void* opened[kMaxWorld][kNumHandles] = {{nullptr}};
+    void* opened[kMaxWorld] = {nullptr};  // peers' arenas mapped by lctr_ipc_import
     bool imported = false;
     unsigned long long epoch = 0;
     unsigned long long released = 0; // epoch of the last round when it was pull-only (its requesters release their caches), else 0
@@ -780,7 +778,7 @@ int dist_alloc(lctr_ctx* c) {
     LCTR_CUDA(cudaMemsetAsync(d->done_ctr, 0, 4 * sizeof(unsigned int), c->stream));
     LCTR_CUDA(cudaMalloc((void**)&d->overflow, sizeof(int)));
     LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), c->stream));
-    if (fused_kernels_ok(c)) {  // the fused FM / NFM kernels keep their gradients in fm_fused.cu's G / Ghot (rows p)
+    if (c->grad_path == GRAD_COMPACT) {  // the fused FM / NFM kernels keep their gradients in fm_fused.cu's G / Ghot (rows p)
         LCTR_CUDA(cudaMalloc((void**)&d->hot_p, (size_t)kNumSlots * d->rows_x * sizeof(uint32_t)));
         LCTR_CUDA(cudaMemsetAsync(d->hot_p, 0xff, (size_t)kNumSlots * d->rows_x * sizeof(uint32_t), c->stream));
         d->bytes += (size_t)kNumSlots * d->rows_x * sizeof(uint32_t);
@@ -825,8 +823,7 @@ int dist_alloc(lctr_ctx* c) {
     c->cgW = d->cgW;
     c->cgV = d->cgV;
     memset(&d->peers, 0, sizeof(d->peers));
-    Peer& me = d->peers.p[d->rank];
-    me.W = c->W; me.V = c->V; me.gW = c->gW; me.gV = c->gV; me.touched = c->touched; me.arena = d->arena;
+    d->peers.p[d->rank].arena = d->arena;
     return 0;
 }
 
@@ -834,8 +831,7 @@ int dist_free(lctr_ctx* c) {
     DistState* d = c->dist;
     if (!d) return 0;
     for (int r = 0; r < d->world; r++)
-        for (int j = 0; j < kNumHandles; j++)
-            if (d->opened[r][j]) cudaIpcCloseMemHandle(d->opened[r][j]);
+        if (d->opened[r]) cudaIpcCloseMemHandle(d->opened[r]);
     cudaFree(d->arena); cudaFree(d->send_cnt); cudaFree(d->seg_cnt); cudaFree(d->opos); cudaFree(d->done_ctr); cudaFree(d->overflow);
     if (d->hot_p) cudaFree(d->hot_p);
     if (d->own_uniq) { cudaFree(d->own_uniq); cudaFree(d->own_pos); cudaFree(d->n_own); cudaFree(d->posmap); cudaFree(d->own_mark); }
@@ -1040,7 +1036,7 @@ int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait, bool trai
     LCTR_CHECK(d->imported, "multi-GPU step before lctr_ipc_import");
     LCTR_CHECK(s.fused_valid, "multi-GPU step on a slot without its key set");
     d->epoch++;
-    if (train && d->own_uniq && d->own_gen[slot] != d->gen[slot]) {  // first step on this upload of the slot: the owner-side union
+    if (train && c->grad_path == GRAD_COMPACT && d->own_gen[slot] != d->gen[slot]) {  // first step on this upload of the slot: the owner-side union
         const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
         const unsigned g1 = (unsigned)std::max<int64_t>(8, std::min<int64_t>((int64_t)c->sm_count * 4, ((int64_t)d->cap_pair + 255) / 256));
         LCTR_CUDA(cudaMemsetAsync(d->n_own + slot, 0, sizeof(unsigned int), c->stream));
@@ -1092,24 +1088,20 @@ int dist_post_step(lctr_ctx* c, Slot& s, int slot, int64_t rows_divisor) {
     const unsigned xgrid = (unsigned)std::max<int64_t>(8, std::min<int64_t>((int64_t)c->sm_count * 4,
         (std::min<int64_t>(s.nnz, (int64_t)c->F) * (int64_t)std::max<size_t>(1, c->rowlen / 16) + 255) / 256));
     const unsigned int* seg = d->seg_cnt + (size_t)slot * kMaxWorld;
-    { ProfScope prof(c, PROF_DIST_PUSH);
-    if (fused_kernels_ok(c)) {
-        FusedState* f = c->fused;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(xgrid); cfg.blockDim = dim3(256); cfg.stream = c->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;  // behind the gradient kernel
-        cudaLaunchKernelEx(&cfg, push_rows_kernel, seg, f->G, f->GS, f->G + c->rowlen, f->GS,
-                           (const uint32_t*)(d->hot_p + (size_t)slot * d->rows_x), f->Ghot, f->GS, (int)c->rowlen, d->recw,
-                           (unsigned)d->cap_pair, d->peers, d->A, d->rank, d->world, d->epoch, d->done_ctr + 1);
-    } else {
-        push_rows_kernel<<<xgrid, 256, 0, c->stream>>>(seg, d->cgV, (int)c->rowlen, d->cgW, 1, nullptr, nullptr, 0, (int)c->rowlen,
-                                                                 d->recw, (unsigned)d->cap_pair, d->peers, d->A, d->rank, d->world, d->epoch,
-                                                                 d->done_ctr + 1);
-    } }
-    if (d->own_uniq) {  // fused FM / NFM: merge + updater in one kernel over the owner-side union of the key lists
+    if (c->grad_path == GRAD_COMPACT) {  // push from G / Ghot, then merge + updater in one kernel over the owner-side union
+        {
+            ProfScope prof(c, PROF_DIST_PUSH);
+            FusedState* f = c->fused;
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3(xgrid); cfg.blockDim = dim3(256); cfg.stream = c->stream;
+            cudaLaunchAttribute at[1];
+            at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+            at[0].val.programmaticStreamSerializationAllowed = 1;
+            cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;  // behind the gradient kernel
+            cudaLaunchKernelEx(&cfg, push_rows_kernel, seg, f->G, f->GS, f->G + c->rowlen, f->GS,
+                               (const uint32_t*)(d->hot_p + (size_t)slot * d->rows_x), f->Ghot, f->GS, (int)c->rowlen, d->recw,
+                               (unsigned)d->cap_pair, d->peers, d->A, d->rank, d->world, d->epoch, d->done_ctr + 1);
+        }
         ProfScope prof(c, PROF_DIST_MERGE);
         const OptParams Pp = make_opt_params(c, rows_divisor);
         const unsigned mgrid = (unsigned)c->sm_count * 4;
@@ -1123,6 +1115,10 @@ int dist_post_step(lctr_ctx* c, Slot& s, int slot, int64_t rows_divisor) {
         LCTR_CUDA(cudaGetLastError());
         return 0;
     }
+    { ProfScope prof(c, PROF_DIST_PUSH);
+    push_rows_kernel<<<xgrid, 256, 0, c->stream>>>(seg, d->cgV, (int)c->rowlen, d->cgW, 1, nullptr, nullptr, 0, (int)c->rowlen,
+                                                   d->recw, (unsigned)d->cap_pair, d->peers, d->A, d->rank, d->world, d->epoch,
+                                                   d->done_ctr + 1); }
     { ProfScope prof(c, PROF_DIST_MERGE);
     merge_kernel<<<xgrid, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot * 2 + (int)(d->gen[slot] & 1), d->epoch,
                                                          (int)c->rowlen, d->recw, c->gW, c->gV, c->touched); }
@@ -1137,57 +1133,48 @@ using namespace lctr;
 
 extern "C" {
 
-// handles exported per rank, in this order: W, V shards, update_g W, V shards, touched map, arena
+// one handle per rank: its arena, the only buffer a peer reads or writes
 int lctr_ipc_export(lctr_ctx* c, void* handles_out, size_t cap, size_t* bytes) {
     LCTR_CHECK(c && bytes, "null argument");
     LCTR_CHECK(c->dist, "lctr_ipc_export: ctx was created with world == 1");
-    const size_t need = kNumHandles * sizeof(cudaIpcMemHandle_t);
+    const size_t need = sizeof(cudaIpcMemHandle_t);
     *bytes = need;
     if (!handles_out) return 0;
     LCTR_CHECK(cap >= need, "lctr_ipc_export: need %zu bytes", need);
-    cudaIpcMemHandle_t* h = reinterpret_cast<cudaIpcMemHandle_t*>(handles_out);
+    cudaIpcMemHandle_t h;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    LCTR_CUDA(cudaIpcGetMemHandle(&h[0], c->W));
-    LCTR_CUDA(cudaIpcGetMemHandle(&h[1], c->V));
-    LCTR_CUDA(cudaIpcGetMemHandle(&h[2], c->gW));
-    LCTR_CUDA(cudaIpcGetMemHandle(&h[3], c->gV));
-    LCTR_CUDA(cudaIpcGetMemHandle(&h[4], c->touched));
-    LCTR_CUDA(cudaIpcGetMemHandle(&h[5], c->dist->arena));
+    LCTR_CUDA(cudaIpcGetMemHandle(&h, c->dist->arena));
+    memcpy(handles_out, &h, sizeof(h));
     return 0;
 }
 
 int lctr_ipc_import(lctr_ctx* c, const void* all_handles, size_t bytes_per_rank) {
     LCTR_CHECK(c && all_handles, "null argument");
     LCTR_CHECK(c->dist, "lctr_ipc_import: ctx was created with world == 1");
-    LCTR_CHECK(bytes_per_rank == kNumHandles * sizeof(cudaIpcMemHandle_t), "lctr_ipc_import: bytes_per_rank %zu", bytes_per_rank);
+    LCTR_CHECK(bytes_per_rank == sizeof(cudaIpcMemHandle_t),
+               "lctr_ipc_import: bytes_per_rank %zu, this build exports %zu (size the blob with lctr_ipc_export(ctx, NULL, 0, &n))",
+               bytes_per_rank, sizeof(cudaIpcMemHandle_t));
     DistState* d = c->dist;
     const unsigned char* base = reinterpret_cast<const unsigned char*>(all_handles);
     for (int r = 0; r < d->world; r++) {
         if (r == d->rank) continue;
-        const cudaIpcMemHandle_t* h = reinterpret_cast<const cudaIpcMemHandle_t*>(base + (size_t)r * bytes_per_rank);
-        for (int j = 0; j < kNumHandles; j++) {
-            cudaIpcMemHandle_t hh;
-            memcpy(&hh, &h[j], sizeof(hh));
-            LCTR_CUDA(cudaIpcOpenMemHandle(&d->opened[r][j], hh, cudaIpcMemLazyEnablePeerAccess));
-        }
-        Peer& p = d->peers.p[r];
-        p.W = (float*)d->opened[r][0];
-        p.V = (float*)d->opened[r][1];
-        p.gW = (float*)d->opened[r][2];
-        p.gV = (float*)d->opened[r][3];
-        p.touched = (uint8_t*)d->opened[r][4];
-        p.arena = (unsigned char*)d->opened[r][5];
+        cudaIpcMemHandle_t h;
+        memcpy(&h, base + (size_t)r * bytes_per_rank, sizeof(h));
+        LCTR_CUDA(cudaIpcOpenMemHandle(&d->opened[r], h, cudaIpcMemLazyEnablePeerAccess));
+        d->peers.p[r].arena = (unsigned char*)d->opened[r];
     }
     d->imported = true;
     return 0;
 }
 
-/* device memory of this context in bytes: table shard + updater state (+ the key table in keyed mode) + multi-GPU arena /
- * caches (DESIGN.md 6) */
+/* device memory of this context in bytes: the shard figure is W, V and the updater state (s1, and s2 for two-state
+ * updaters), plus update_g (gW / gV, the size of W and V) on the dense path and for the grouped FFM backward, plus the
+ * touched map (1 B per row) on the dense path, plus the key table in keyed mode; the exchange figure is the multi-GPU
+ * arena, caches and index buffers (DESIGN.md 6) */
 int lctr_device_bytes(lctr_ctx* c, uint64_t* shard_bytes, uint64_t* exchange_bytes) {
     LCTR_CHECK(c, "null ctx");
-    const bool two = c->s2W != nullptr;
-    if (shard_bytes) *shard_bytes = (uint64_t)(c->Fl * (c->rowlen + 1) * sizeof(float) * (two ? 4 : 3) + c->Fl + keys_bytes(c));
+    const size_t tables = 2 + (c->s2W ? 1 : 0) + (c->gW ? 1 : 0);  // [W | V] blocks: parameters, s1, s2, update_g
+    if (shard_bytes) *shard_bytes = (uint64_t)(c->Fl * (c->rowlen + 1) * sizeof(float) * tables + (c->touched ? c->Fl : 0) + keys_bytes(c));
     if (exchange_bytes) *exchange_bytes = (uint64_t)dist_bytes(c);
     return 0;
 }

@@ -592,11 +592,10 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
     return 0;
 }
 
-// forward+backward are one fused kernel; launch_ffm_backward is therefore a no-op kept for symmetry
+// forward + backward are one fused kernel (stats: a train step; otherwise forward only)
 int launch_ffm_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
     return ffm_launch(c, s, rb, re, /*train=*/stats, stats);
 }
-int launch_ffm_backward(lctr_ctx*, Slot&, int64_t, int64_t) { return 0; }
 // forward half of the feature-grouped step: predictions, loss, and the T tiles for ffm_grouped.cu
 int launch_ffm_forward_tiles(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     return ffm_launch(c, s, rb, re, true, true, true);

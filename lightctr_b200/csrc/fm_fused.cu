@@ -10,15 +10,6 @@
 
 namespace lctr {
 
-// the fused kernels exist for FM and NFM (embedding side) with K in {4, 8, 16, 32}, order-free mode; on one GPU they read the tables directly,
-// on several (dist.cu) the batch-compact cache of the pulled rows
-bool fused_kernels_ok(const lctr_ctx* c) {
-    const int k = (int)c->cfg.factor_cnt;
-    return (c->cfg.model == LCTR_MODEL_FM || c->cfg.model == LCTR_MODEL_NFM) && c->cfg.deterministic == 0 &&
-           (k == 4 || k == 8 || k == 16 || k == 32);
-}
-bool fused_supported(const lctr_ctx* c) { return c->cfg.world == 1 && fused_kernels_ok(c); }
-
 void fused_free(lctr_ctx* c) {
     FusedState* f = c->fused;
     if (!f) return;
@@ -32,11 +23,11 @@ static int fused_init(lctr_ctx* c) {
     FusedState* f = new FusedState();
     c->fused = f;
     f->T = mark_rows(c->F);
-    f->GS = fused_kernels_ok(c) ? grad_stride((int)c->cfg.factor_cnt) : 0;  // other models: slot map only
     LCTR_CUDA(cudaMalloc((void**)&f->mark, 128 * f->T + 512));
     LCTR_CUDA(cudaMemsetAsync(f->mark, 0, 128 * f->T + 512, c->stream));
     LCTR_CUDA(cudaMalloc((void**)&f->slot_of, c->F * sizeof(uint32_t)));
-    if (f->GS) {
+    if (c->grad_path == GRAD_COMPACT) {
+        f->GS = grad_stride((int)c->cfg.factor_cnt);
         LCTR_CUDA(cudaMalloc((void**)&f->Ghot, (size_t)kHotMax * kHotRep * f->GS * sizeof(float)));
         LCTR_CUDA(cudaMemsetAsync(f->Ghot, 0, (size_t)kHotMax * kHotRep * f->GS * sizeof(float), c->stream));
     }
@@ -82,7 +73,7 @@ int fused_reserve(lctr_ctx* c, Slot& s, int64_t nnz) {
     }
     // gradient rows: one per slot; on several GPUs one per exchange row (dist.cu re-indexes the entries)
     const size_t g_rows = c->cfg.world > 1 ? c->dist_rows : (size_t)s.cap_uniq;
-    if (f->GS && g_rows > f->G_rows) {
+    if (c->grad_path == GRAD_COMPACT && g_rows > f->G_rows) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
         if (f->G) cudaFree(f->G);
         LCTR_CUDA(cudaMalloc((void**)&f->G, (g_rows + 64) * f->GS * sizeof(float)));
@@ -93,20 +84,24 @@ int fused_reserve(lctr_ctx* c, Slot& s, int64_t nnz) {
 }
 
 // slot map of the batch held by slot s, on stream st.  hdr != nullptr (graph capture): {rows, nnz} are read from device
-// memory and the grids are sized for the slot's capacities.
+// memory and the grids are sized for the slot's capacities.  An empty batch (0 rows or 0 entries) gets an empty map and no
+// kernel.
 int fused_build_slot(lctr_ctx* c, Slot& s, cudaStream_t st, const int64_t* hdr, int64_t rows_cap, int64_t nnz_cap) {
     FusedState* f = c->fused;
     s.fused_valid = false;
-    if (rows_cap <= 0 || nnz_cap <= 0) return 0;
     const int SM = c->sm_count;
     LCTR_CUDA(cudaMemsetAsync(s.n_uniq, 0, sizeof(unsigned int), st));
     LCTR_CUDA(cudaMemsetAsync(s.n_hot, 0, sizeof(unsigned int), st));
+    if (rows_cap <= 0 || nnz_cap <= 0) {
+        s.fused_valid = true;
+        return 0;
+    }
     const unsigned mkg = (unsigned)std::max<int64_t>(1, std::min<int64_t>((nnz_cap + 2047) / 2048, (int64_t)SM * 4));
     slotmap_mark_kernel<<<mkg, 256, 0, st>>>(s.fid, hdr, nnz_cap, f->mark, f->T);
     const size_t ntiles = (128 * f->T + 511) / 512;
     const unsigned cg = (unsigned)std::max<size_t>(1, std::min<size_t>((ntiles + 7) / 8, (size_t)SM * 8));
     slotmap_compact_kernel<<<cg, 256, 0, st>>>(f->mark, f->T, s.uniq, s.n_uniq, f->slot_of);
-    const bool hot = f->GS != 0;  // replica rows only exist for the fused FM kernels
+    const bool hot = c->grad_path == GRAD_COMPACT;  // replica rows only exist for the fused FM / NFM kernels
     if (hot) {
         const unsigned sg = (unsigned)std::min<int64_t>(((int64_t)kHotSampleRows * 128 + 255) / 256, (int64_t)SM * 8);
         slotmap_sample_kernel<<<sg, 256, 0, st>>>(s.row_ptr, s.fid, hdr, rows_cap, f->slot_of, f->cnt);

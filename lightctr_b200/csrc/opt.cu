@@ -23,16 +23,7 @@ namespace lctr {
 // space are dense (every mark set) while the tail is ~5 % dense.
 __global__ void __launch_bounds__(256)
 compact_touched_kernel(uint8_t* __restrict__ touched, size_t F, uint32_t* __restrict__ list,
-                       unsigned int* __restrict__ n_list, const unsigned long long* wait_flags, int n_wait,
-                       unsigned long long wait_epoch) {
-    if (wait_flags) {  // multi-GPU owner: every requester's gradient pushes of this step have landed (dist.cu)
-        if ((int)threadIdx.x < n_wait) {
-            const volatile unsigned long long* f = wait_flags + threadIdx.x;
-            while (*f < wait_epoch) __nanosleep(40);
-            __threadfence();
-        }
-        __syncthreads();
-    }
+                       unsigned int* __restrict__ n_list) {
     const int lane = threadIdx.x & 31;
     const size_t warp = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const size_t nwarps = (size_t)gridDim.x * (blockDim.x >> 5);
@@ -202,8 +193,7 @@ int launch_apply(lctr_ctx* c, int64_t rows_in_step) {
     if (grid_a == 0) grid_a = 1;
     const unsigned grid = (unsigned)c->sm_count * 2;
     ProfScope prof(c, PROF_APPLY);
-    compact_touched_kernel<<<grid_a, 256, 0, c->stream>>>(c->touched, c->Fl, c->touch_list, c->n_touch, c->apply_wait_flags,
-                                                          c->apply_wait_n, c->apply_wait_epoch);
+    compact_touched_kernel<<<grid_a, 256, 0, c->stream>>>(c->touched, c->Fl, c->touch_list, c->n_touch);
     c->launches++;
 #define APPLY_ARGS c->touch_list, c->n_touch, c->apply_done, rowlen, c->W, c->V, c->gW, c->gV, c->s1W, c->s1V, c->s2W, c->s2V, P
 #define APPLY_GO(L, VV, S, UU, OO) apply_kernel<L, VV, S, UU, OO><<<grid, 256, 0, c->stream>>>(APPLY_ARGS)
