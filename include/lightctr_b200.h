@@ -89,7 +89,14 @@ typedef struct lctr_cfg {
     /* keyed mode only: 1 = every row records the insert-upload that last met it (8 B per row), which lctr_evict_keys
      * needs; 0 = no record (refused on a dense context when non-zero, and with world > 1) */
     int32_t key_evict;
-    uint32_t reserved[2];
+    union {
+        /* keyed mode only: capacity in rows of the host tier that keeps evicted rows (see lctr_evict_keys); 0 = no tier.
+         * Needs key_mode = LCTR_KEYS_HASHED, key_evict = 1 and world = 1.  Takes (16 + 4 (rowlen + 1) (1 + states)) bytes
+         * of pinned host memory per row, states = 2 for the two-state updaters (FTRL, Adam, Adadelta, DCASGD, DCASGDA)
+         * and 1 otherwise, and an index of T = 2^m >= 2 key_host_rows slots of 12 B in device memory. */
+        uint32_t key_host_rows;
+        uint32_t reserved[2]; /* reserved[1] must stay 0 */
+    };
 } lctr_cfg;
 
 const char* lctr_last_error(void);
@@ -162,11 +169,37 @@ int lctr_set_key_init(lctr_ctx* ctx, uint64_t seed, float scale);
  * (ascending), carrying W, V, the optimizer state and its stamp bit for bit.  Rows [n_live, rows in use) return to the
  * state lctr_create gives and the table is rebuilt from the survivors, so keys stored without a row after a capacity
  * overflow are forgotten.  When a row was freed, every resident keyed slot becomes stale: train_step and predict refuse
- * it until it is uploaded again.  An evicted key that comes back is a new key: lazy-init values (which depend on the key
- * only) and fresh optimizer state; re-uploading exported rows with lctr_upload_keyed_params restores W and V, also with
- * fresh optimizer state.  Refused on a dense context and on a keyed context created with key_evict = 0. */
+ * it until it is uploaded again.  Without a host tier, an evicted key that comes back is a new key: lazy-init values
+ * (which depend on the key only) and fresh optimizer state; re-uploading exported rows with lctr_upload_keyed_params
+ * restores W and V, also with fresh optimizer state.  With a host tier (cfg.key_host_rows, below) the evicted rows are
+ * kept there and come back whole.  Refused on a dense context and on a keyed context created with key_evict = 0. */
 int lctr_evict_keys(lctr_ctx* ctx, uint64_t max_idle, uint64_t max_rows, uint64_t* keys_out, float* W_out, float* V_out,
                     uint64_t cap_out, uint64_t* n_evicted);
+/* Host tier (cfg.key_host_rows > 0; keyed, key_evict = 1, one GPU), so that the model can outgrow device memory.
+ * THE RULE: on a tiered context the model is the device rows plus the tier rows.  A key lives in at most one of them,
+ * and no call except lctr_evict_host_tier loses one.  A tier row holds the key, its stamp, W, V and the optimizer state.
+ *   lctr_evict_keys: the same rule, renumbering and export as without a tier, but the evicted rows are appended to the tier
+ *     (in export order) instead of being dropped; without room in the tier for all of them the call fails before
+ *     anything changes, naming the tier's capacity and its free rows.
+ *   lctr_upload_batch_keys, insert = 1: a key absent from the device but held in the tier gets a device row as a new key
+ *     does, then its W, V and optimizer state from the tier bit for bit (in place of the lazy init), and the new clock as
+ *     any row the upload meets; it leaves the tier.  A key the capacity check refuses stays in the tier unchanged.
+ *   lctr_upload_batch_keys, insert = 0: keys held in the tier are brought back the same way and keep their tier stamp;
+ *     the clock does not advance; keys in neither table map to the null row.  Restoring past the device capacity fails
+ *     with the capacity message, as an insert-upload does.
+ *   lctr_upload_keyed_params: a key held in the tier counts as present: it gets its device row by the rule for absent
+ *     keys, its optimizer state from the tier, then the call's W / V.
+ *   lctr_lookup_keys, lctr_download_keys, the parameter and the opt-state transfers see the device rows only.
+ *   Checkpoints carry the tier (a tiered file and an untiered context refuse each other, as files of another key_evict).
+ * Cost: restored and spilled rows cross PCIe as zero-copy 16-byte accesses (scalar when rowlen % 4 != 0); keys that miss
+ * the tier cost one probe of its device-side index per new row. */
+/* the tier's rows in tier order: keys [n], W [n], V [n * rowlen]; keys = W = V = NULL queries *n_rows, otherwise each
+ * non-NULL array must hold cap >= *n_rows rows.  The only view of the part of the model held in the tier. */
+int lctr_download_host_tier(lctr_ctx* ctx, uint64_t* keys, float* W, float* V, uint64_t cap, uint64_t* n_rows);
+/* lctr_evict_keys's rule, tie handling, export order (ascending tier row) and cap_out contract, applied to the tier's
+ * stamps against the same clock.  The rows it frees leave the model; the rest are renumbered by the same rule. */
+int lctr_evict_host_tier(lctr_ctx* ctx, uint64_t max_idle, uint64_t max_rows, uint64_t* keys_out, float* W_out, float* V_out,
+                         uint64_t cap_out, uint64_t* n_evicted);
 /* Keyed mode on several GPUs (world > 1; the reference's parameter servers key by size_t and create on first touch,
  * distribut/paramserver.h:315-339).
  * Owner rule: key k lives on rank fmix64(k) >> (64 - log2 world) (the top bits of MurmurHash3's 64-bit finaliser); the
@@ -266,7 +299,8 @@ int lctr_ipc_import(lctr_ctx* ctx, const void* all_handles, size_t bytes_per_ran
  * two-state updaters), Fl (k + 1) floats each for FM / NFM, Fl (Fc k + 1) for FFM; + update_g of the same size on the
  * dense gradient path (FFM with deterministic 0 or 1, Wide&Deep, FM / NFM with deterministic = 0 and k outside
  * {4, 8, 16, 32}, NFM with deterministic = 2) and for the grouped FFM backward (deterministic = 2); + the touched map,
- * 1 B per row, on the dense path only; + the key table in keyed mode and 8 B per row of stamps with key_evict = 1.  The
+ * 1 B per row, on the dense path only; + the key table in keyed mode and 8 B per row of stamps with key_evict = 1; + the
+ * host tier's index (12 B per slot) with cfg.key_host_rows > 0 (its rows are in host memory and not counted).  The
  * compact (FM / NFM, deterministic = 0, k in {4, 8, 16, 32}) and the other feature-major paths hold no gradient per row.
  * Per-call scratch is not counted.  exchange_bytes (world > 1): the exchange arena, caches and inboxes -- owner-sharding
  * keeps it O(keys of a batch), not O(feature_cnt) */

@@ -33,6 +33,7 @@ SYMBOLS = [
     "lctr_dense_grad_buffer", "lctr_device_bytes", "lctr_load_libffm", "lctr_free_dataset", "lctr_launch_count", "lctr_stream", "lctr_profile", "lctr_profile_read",
     "lctr_upload_batch_keys", "lctr_lookup_keys", "lctr_download_keys", "lctr_upload_keyed_params", "lctr_set_key_init",
     "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys", "lctr_load_checkpoint_shards", "lctr_eval_pred",
+    "lctr_download_host_tier", "lctr_evict_host_tier",
 ]
 NO_LIMIT = (1 << 64) - 1  # lctr_evict_keys: UINT64_MAX = no limit
 
@@ -48,6 +49,9 @@ class Cfg(C.Structure):
                 ("world", C.c_int32), ("deterministic", C.c_int32), ("key_mode", C.c_int32),
                 ("csc_row_block", C.c_uint64), ("ema_rate", C.c_float), ("key_evict", C.c_int32),
                 ("reserved", C.c_uint32 * 2)]
+
+    # cfg.key_host_rows shares its word with reserved[0] (a union in the header)
+    key_host_rows = property(lambda self: self.reserved[0], lambda self, v: self.reserved.__setitem__(0, v))
 
 
 class DatasetC(C.Structure):
@@ -127,6 +131,8 @@ def load_library():
     L.lctr_load_libffm_keys.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.POINTER(KeyedDatasetC))]
     L.lctr_free_keyed_dataset.argtypes = [C.POINTER(KeyedDatasetC)]
     L.lctr_evict_keys.argtypes = [vp, C.c_uint64, C.c_uint64, vp, f32p, f32p, C.c_uint64, C.POINTER(C.c_uint64)]
+    L.lctr_evict_host_tier.argtypes = [vp, C.c_uint64, C.c_uint64, vp, f32p, f32p, C.c_uint64, C.POINTER(C.c_uint64)]
+    L.lctr_download_host_tier.argtypes = [vp, vp, f32p, f32p, C.c_uint64, C.POINTER(C.c_uint64)]
     _lib = L
     return L
 
@@ -244,9 +250,11 @@ class Context:
     def __init__(self, model, feature_cnt, factor_cnt, field_cnt=0, optimizer=OPT_ADAGRAD, lr=0.05, l2=0.001,
                  minibatch_size=0, momentum=0.8, momentum_adam2=0.999, hidden=(), activation=ACT_SIGMOID,
                  mlp_precision=MLP_FP32, device=0, rank=0, world=1, deterministic=0, csc_row_block=0, max_rows=0,
-                 max_nnz=0, ema_rate=0.99, key_mode=KEYS_DENSE, key_evict=False):
+                 max_nnz=0, ema_rate=0.99, key_mode=KEYS_DENSE, key_evict=False, key_host_rows=0):
         """key_mode=KEYS_HASHED: batches carry uint64 keys (upload_batch_keys) and feature_cnt is the row capacity.
-        key_evict=True (keyed only): rows record the insert-upload that last met them, for evict_keys."""
+        key_evict=True (keyed only): rows record the insert-upload that last met them, for evict_keys.
+        key_host_rows > 0 (with key_evict=True): evicted rows go to a host-memory tier of that many rows and come back
+        when their keys do."""
         L = load_library()
         cfg = Cfg()
         cfg.abi_version = ABI_VERSION
@@ -264,6 +272,7 @@ class Context:
         cfg.max_rows, cfg.max_nnz = max_rows, max_nnz
         cfg.key_mode = key_mode
         cfg.key_evict = 1 if key_evict else 0
+        cfg.key_host_rows = key_host_rows
         self.cfg = cfg
         self.h = C.c_void_p()
         _chk(L.lctr_create(C.byref(cfg), C.byref(self.h)))
@@ -370,6 +379,33 @@ class Context:
         W = np.empty(max(cap, 1), np.float32)
         V = np.empty(max(cap, 1) * self.rowlen, np.float32)
         _chk(self.L.lctr_evict_keys(self.h, idle, rows, _p(keys), _p(W), _p(V), cap, C.byref(n)))
+        m = n.value
+        return keys[:m].copy(), W[:m].copy(), V[:m * self.rowlen].copy()
+
+    def download_host_tier(self):
+        """(keys, W, V) of the host tier's rows in tier order (V flat, rowlen floats per key)"""
+        n = C.c_uint64()
+        _chk(self.L.lctr_download_host_tier(self.h, None, None, None, 0, C.byref(n)))
+        m = n.value
+        keys, W, V = np.empty(max(m, 1), np.uint64), np.empty(max(m, 1), np.float32), np.empty(max(m, 1) * self.rowlen, np.float32)
+        _chk(self.L.lctr_download_host_tier(self.h, _p(keys), _p(W), _p(V), m, C.byref(n)))
+        return keys[:m].copy(), W[:m].copy(), V[:m * self.rowlen].copy()
+
+    def evict_host_tier(self, max_idle=None, max_rows=None, export=False):
+        """evict_keys's rule on the host tier's rows; the rows it frees leave the model.  Returns the number freed, or
+        with export=True (keys, W, V) of the freed rows in ascending order of their tier row."""
+        idle = NO_LIMIT if max_idle is None else int(max_idle)
+        rows = NO_LIMIT if max_rows is None else int(max_rows)
+        n = C.c_uint64()
+        if not export:
+            _chk(self.L.lctr_evict_host_tier(self.h, idle, rows, None, None, None, 0, C.byref(n)))
+            return n.value
+        _chk(self.L.lctr_download_host_tier(self.h, None, None, None, 0, C.byref(n)))
+        cap = n.value
+        keys = np.empty(max(cap, 1), np.uint64)
+        W = np.empty(max(cap, 1), np.float32)
+        V = np.empty(max(cap, 1) * self.rowlen, np.float32)
+        _chk(self.L.lctr_evict_host_tier(self.h, idle, rows, _p(keys), _p(W), _p(V), cap, C.byref(n)))
         m = n.value
         return keys[:m].copy(), W[:m].copy(), V[:m * self.rowlen].copy()
 

@@ -205,6 +205,9 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
     LCTR_CHECK(cfg->optimizer >= LCTR_OPT_ADAGRAD && cfg->optimizer <= LCTR_OPT_PS_DCASGDA, "lctr_create: bad optimizer %d",
                cfg->optimizer);
     LCTR_CHECK(cfg->key_mode == LCTR_KEYS_DENSE || cfg->key_mode == LCTR_KEYS_HASHED, "lctr_create: bad key_mode %d", cfg->key_mode);
+    LCTR_CHECK(cfg->key_host_rows == 0 || (cfg->key_mode == LCTR_KEYS_HASHED && cfg->key_evict == 1 && cfg->world <= 1),
+               "lctr_create: key_host_rows = %u (a host tier) needs key_mode = LCTR_KEYS_HASHED, key_evict = 1 and world = 1 "
+               "(got key_mode %d, key_evict %d, world %d)", cfg->key_host_rows, cfg->key_mode, cfg->key_evict, cfg->world);
     if (cfg->key_mode == LCTR_KEYS_HASHED) {
         // exact-order modes build their feature-major view on the host from host ids, which a keyed upload does not have;
         // on several GPUs an eviction would renumber rows across the shards, which needs a collective of its own

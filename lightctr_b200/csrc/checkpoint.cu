@@ -14,6 +14,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <memory>
 #include <string>
 #include <vector>
@@ -35,8 +36,11 @@ struct CkptShard {
 };
 static_assert(sizeof(CkptHeader) == 136 && sizeof(CkptShard) == 24, "checkpoint headers are a file format");
 
-// cfg.key_mode in the low byte, cfg.key_evict in bit 8: dense and untracked keyed files keep the value they always had
-static int32_t key_word(const lctr_cfg& cfg) { return cfg.key_mode | (cfg.key_evict ? 0x100 : 0); }
+// cfg.key_mode in the low byte, cfg.key_evict in bit 8, a host tier (cfg.key_host_rows > 0) in bit 9: dense, untracked and
+// untiered keyed files keep the value they always had
+static int32_t key_word(const lctr_cfg& cfg) {
+    return cfg.key_mode | (cfg.key_evict ? 0x100 : 0) | (cfg.key_host_rows ? 0x200 : 0);
+}
 
 static bool put(FILE* f, const void* p, size_t n) { return n == 0 || fwrite(p, 1, n, f) == n; }
 static bool get(FILE* f, void* p, size_t n) { return n == 0 || fread(p, 1, n, f) == n; }
@@ -72,8 +76,9 @@ static bool same_trainer(const lctr_ctx* c, const CkptHeader& h) {
 }
 
 // The sections of a file after its header(s), in file order: the row sections over the file's rows, the parts of every
-// layer, then for keyed tables the row count and the key of every row, and for key_evict = 1 the upload clock and the
-// stamp of every row.  Everything that walks the format takes the first two from these helpers.
+// layer, then for keyed tables the row count and the key of every row, for key_evict = 1 the upload clock and the stamp
+// of every row, and for a host tier its row count n, the key and the stamp of each of its rows, then the row sections over
+// those n rows.  Everything that walks the format takes the row sections and the layer parts from these helpers.
 
 // W, V, s1W, s1V[, s2W, s2V] of this rank's shard
 struct RowSections {
@@ -84,6 +89,12 @@ struct RowSections {
 };
 static RowSections row_sections(const lctr_ctx* c) {
     return {{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V}, c->s2W ? 6 : 4, c->rowlen};
+}
+// the same sections over the host tier's arrays (pinned host memory)
+static RowSections tier_sections(const lctr_ctx* c, const TierRows& tr) {
+    RowSections rs = row_sections(c);
+    for (int a = 0; a < 6; a++) rs.p[a] = tr.p[a];
+    return rs;
 }
 
 // w, b, acc_w, acc_b, mask of one dense layer and their sizes in floats
@@ -144,6 +155,8 @@ struct CkptFile {
     std::vector<uint64_t> keys;
     uint64_t clock = 0;
     std::vector<uint64_t> stamps;
+    std::vector<uint64_t> tier_keys, tier_stamps;  // host tier (cfg.key_host_rows > 0)
+    long tier_rows_at = 0;                         // offset of its row sections
     CkptFile() = default;
     CkptFile(const CkptFile&) = delete;
     CkptFile& operator=(const CkptFile&) = delete;
@@ -159,7 +172,7 @@ static int ckpt_open(lctr_ctx* c, const char* path, CkptFile& cf) {
     const bool shard = ok && memcmp(cf.h.magic, "LCTRCKS1", 8) == 0;
     LCTR_CHECK(shard || (ok && memcmp(cf.h.magic, "LCTRCKP1", 8) == 0), "%s is not a lightctr_b200 checkpoint", path);
     LCTR_CHECK(same_trainer(c, cf.h), "checkpoint %s was written by a different trainer (model/optimizer/feature_cnt/field_cnt/"
-                                      "factor_cnt/layers/key_mode/key_evict)", path);
+                                      "factor_cnt/layers/key_mode/key_evict/key_host_rows)", path);
     const uint64_t rows = api_rows(c);
     if (shard) {
         LCTR_CHECK(get(cf.f, &cf.s, sizeof(cf.s)), "checkpoint %s: short shard header", path);
@@ -190,6 +203,24 @@ static int ckpt_open(lctr_ctx* c, const char* path, CkptFile& cf) {
             LCTR_CHECK(get(cf.f, &cf.clock, sizeof(cf.clock)) && get(cf.f, cf.stamps.data(), n * sizeof(uint64_t)),
                        "checkpoint %s: short read of the row stamps", path);
             end += (long)((1 + n) * sizeof(uint64_t));
+        }
+        TierRows tr;
+        if (keys_tier(c, &tr)) {
+            uint64_t nt = 0;
+            LCTR_CHECK(get(cf.f, &nt, sizeof(nt)) && nt <= tr.cap,
+                       "checkpoint %s: missing host-tier section, or more rows than cfg.key_host_rows = %zu", path, tr.cap);
+            cf.tier_keys.resize(nt);
+            cf.tier_stamps.resize(nt);
+            LCTR_CHECK(get(cf.f, cf.tier_keys.data(), nt * sizeof(uint64_t)) && get(cf.f, cf.tier_stamps.data(), nt * sizeof(uint64_t)),
+                       "checkpoint %s: short read of the host tier's keys", path);
+            // a key lives in at most one of the two tables
+            std::vector<uint64_t> all(cf.keys);
+            all.insert(all.end(), cf.tier_keys.begin(), cf.tier_keys.end());
+            std::sort(all.begin(), all.end());
+            LCTR_CHECK(std::adjacent_find(all.begin(), all.end()) == all.end() && (all.empty() || all.back() != kEmptyKey),
+                       "checkpoint %s: a host-tier key is reserved or held twice", path);
+            cf.tier_rows_at = end + (long)((1 + 2 * nt) * sizeof(uint64_t));
+            end = cf.tier_rows_at + (long)(nt * row_floats(c) * sizeof(float));
         }
     }
     long len = -1;
@@ -292,6 +323,17 @@ static int load_shard_in_place(lctr_ctx* c, CkptFile& cf) {
         mark_slots_stale(c);
         if (keys_restore(c, cf.keys.data(), cf.keys.size())) return 1;
         if (keys_tracked(c) && keys_restore_stamps(c, cf.stamps.data(), cf.stamps.size(), cf.clock)) return 1;
+        TierRows tr;
+        if (keys_tier(c, &tr)) {  // straight into the pinned arrays, then a fresh index
+            const size_t nt = cf.tier_keys.size();
+            memcpy(tr.key, cf.tier_keys.data(), nt * sizeof(uint64_t));
+            memcpy(tr.stamp, cf.tier_stamps.data(), nt * sizeof(uint64_t));
+            const RowSections ts = tier_sections(c, tr);
+            LCTR_CHECK(fseek(cf.f, cf.tier_rows_at, SEEK_SET) == 0, "checkpoint %s: seek failed", cf.path.c_str());
+            for (int a = 0; a < ts.n; a++)
+                LCTR_CHECK(get(cf.f, ts.p[a], nt * ts.width(a) * sizeof(float)), "checkpoint %s: short read of the host tier", cf.path.c_str());
+            if (keys_tier_restore(c, nt)) return 1;
+        }
     }
     return finish_load(c, cf.h);
 }
@@ -338,6 +380,13 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
             uint64_t clock = 0;
             rc = keys_download_stamps(c, n, stamps, &clock);
             if (!rc) rc = !(put(f, &clock, sizeof(clock)) && put(f, stamps.data(), n * sizeof(uint64_t)));
+        }
+        TierRows tr;
+        if (!rc && keys_tier(c, &tr)) {  // host tier: row count, keys, stamps, then its row sections
+            const uint64_t nt = tr.n;
+            const RowSections ts = tier_sections(c, tr);
+            rc = !(put(f, &nt, sizeof(nt)) && put(f, tr.key, nt * sizeof(uint64_t)) && put(f, tr.stamp, nt * sizeof(uint64_t)));
+            for (int a = 0; a < ts.n && !rc; a++) rc = !put(f, ts.p[a], nt * ts.width(a) * sizeof(float));
         }
     }
     if (fclose(f) != 0) rc = 1;

@@ -431,6 +431,15 @@ int keys_download(lctr_ctx* c, std::vector<uint64_t>& out);
 bool keys_tracked(const lctr_ctx* c);
 int keys_download_stamps(lctr_ctx* c, uint64_t n, std::vector<uint64_t>& stamps, uint64_t* clock);
 int keys_restore_stamps(lctr_ctx* c, const uint64_t* stamps, uint64_t n, uint64_t clock);
+// cfg.key_host_rows > 0: the host tier's arrays (pinned host memory, rows [0, n) live), p[] in the order of the row
+// sections (W, V, s1W, s1V, s2W, s2V); false without a tier.  keys_tier_restore: the arrays hold n rows, rebuild the index
+struct TierRows {
+    unsigned long long *key, *stamp;
+    float* p[6];
+    size_t n, cap;
+};
+bool keys_tier(const lctr_ctx* c, TierRows* out);
+int keys_tier_restore(lctr_ctx* c, uint64_t n);
 // rows of the row-indexed parameter / optimizer-state transfers: F, or the capacity in keyed mode (the null row stays out)
 inline size_t api_rows(const lctr_ctx* c) { return c->keys ? c->F - 1 : c->F; }
 // global rows < rows that rank holds when global row g lives on rank g % world (at local row g / world); rank < world

@@ -59,6 +59,14 @@
 //   rebuild    table emptied and rows [0, n_live) re-inserted with row = index (key_insert_fixed_kernel).
 // The per-row arrays that do not move: gW / gV and `touched` are zero between steps, fused->slot_of and touch_list are
 // scratch written by each step before it reads them.  Slots hold row ids of the old numbering and become stale.
+//
+// Host tier (cfg.key_host_rows > 0, HostTier below): the evicted rows are first appended to the tier (tier_spill_kernel,
+// after the export, before the move).  Uploads give a device row to a key the tier holds as to a new key (insert = 0:
+// key_lookup_restore_kernel, for tier keys only); key_restore_init_kernel then copies its row back in place of the lazy
+// init and lists the tier row it released, and tier_compact closes the holes with evict_move_kernel.  The compaction is
+// planned on the host from that list alone (the holes below the new end, sorted, and the scan of the window
+// [n_live, n) above it), so its cost scales with the rows restored, never with the tier's size.  lctr_evict_host_tier
+// runs the whole eviction on the tier's arrays, with scratch of the tier's size allocated for the call.
 #include <algorithm>
 #include <vector>
 
@@ -68,6 +76,29 @@ namespace lctr {
 
 constexpr int kEvTile = 1024;  // rows per block of the eviction count / index kernels
 constexpr int kEvBins = 1 << 16;  // radix-select digit
+
+// the per-row arrays that move with a row
+struct RowArrays {
+    float *W, *V, *s1W, *s1V, *s2W, *s2V;
+    unsigned long long *row_key, *last_seen;
+};
+
+// Host tier (cfg.key_host_rows > 0): rows of evicted keys in pinned, device-mapped host memory, live rows [0, n), and an
+// index key -> tier row in HBM with the key table's layout.  Index slots go from empty to a key only; a restored key keeps
+// its slot with kNoRow, so `used` (slots holding a key) counts live and dead slots, and the index is rebuilt from
+// row_key[0, n) once it passes T / 2.
+struct HostTier {
+    RowArrays a{};                          // device-mapped host arrays of `cap` rows
+    unsigned long long* key = nullptr;      // [T] index slot keys (HBM)
+    uint32_t* row = nullptr;                // [T] tier row of the slot's key, kNoRow once restored
+    unsigned int* flags = nullptr;          // [0] rows restored, [1] index full, [2] slots claimed by a spill
+    unsigned int* h_flags = nullptr;        // pinned mirror
+    size_t T = 0, cap = 0, n = 0, used = 0;
+    // scratch of the compaction after a restore, sized with the key table's per-call scratch (at most one entry per new row)
+    uint32_t* rel = nullptr;                // tier rows released by the current call, in no order
+    uint32_t* wscan = nullptr;              // [m + 1] released rows in [n_live, n_live + i)
+    uint32_t* holes = nullptr;              // released rows below n_live, ascending
+};
 
 struct KeyTable {
     unsigned long long* key = nullptr;      // [T] slot keys, kEmptyKey = free
@@ -93,10 +124,15 @@ struct KeyTable {
     unsigned int* ev_hist = nullptr;          // [65536] digit histogram of the radix select
     unsigned long long* ev_res = nullptr;     // [4] counters read back by the host
     unsigned long long* h_res = nullptr;      // pinned mirror
+    HostTier* tier = nullptr;                 // cfg.key_host_rows > 0
 };
 
 static KeyView view(const KeyTable* t) {
     return KeyView{t->key, t->row, t->row_key, t->count, t->flags, t->new_rows, t->T / kGroup, t->cap};
+}
+// the tier's index: row_key is the tier's (host) row -> key map; no row counter and no new-row list
+static KeyView view(const HostTier* h) {
+    return KeyView{h->key, h->row, h->a.row_key, nullptr, h->flags, nullptr, h->T / kGroup, h->cap};
 }
 
 // 1. claim a slot and a row for every key not yet in the table (one 16-lane tile per key)
@@ -137,6 +173,25 @@ __device__ __forceinline__ float key_gauss(unsigned long long hk, size_t rowlen,
     return scale * sqrtf(-2.0f * logf(u1)) * cosf(6.2831853f * u2);
 }
 
+// lazy init of row r of key `key` by one warp: W = 0, V from the key, the optimizer state lctr_create gives
+__device__ __forceinline__ void warp_lazy_init(float* __restrict__ W, float* __restrict__ V, float* __restrict__ s1W,
+                                               float* __restrict__ s1V, float* __restrict__ s2W, float* __restrict__ s2V, uint32_t r,
+                                               unsigned long long key, size_t rowlen, float s1_init, unsigned long long seed,
+                                               float scale, int lane) {
+    const unsigned long long hk = fmix64(key);
+    const size_t o = (size_t)r * rowlen;
+    for (size_t j = lane; j < rowlen; j += 32) {
+        V[o + j] = key_gauss(hk, rowlen, j, seed, scale);
+        s1V[o + j] = s1_init;
+        if (s2V) s2V[o + j] = 0.f;
+    }
+    if (lane == 0) {
+        W[r] = 0.f;
+        s1W[r] = s1_init;
+        if (s2W) s2W[r] = 0.f;
+    }
+}
+
 // 2. lazy init of the rows created by this upload: one warp per row
 __global__ void __launch_bounds__(256) key_init_kernel(KeyView t, float* __restrict__ W, float* __restrict__ V, float* __restrict__ s1W,
                                                        float* __restrict__ s1V, float* __restrict__ s2W, float* __restrict__ s2V,
@@ -146,17 +201,119 @@ __global__ void __launch_bounds__(256) key_init_kernel(KeyView t, float* __restr
     const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
     for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n; w += nwarps) {
         const uint32_t r = t.new_rows[w];
-        const unsigned long long hk = fmix64(t.row_key[r]);
-        const size_t o = (size_t)r * rowlen;
-        for (size_t j = lane; j < rowlen; j += 32) {
-            V[o + j] = key_gauss(hk, rowlen, j, seed, scale);
-            s1V[o + j] = s1_init;
-            if (s2V) s2V[o + j] = 0.f;
+        warp_lazy_init(W, V, s1W, s1V, s2W, s2V, r, t.row_key[r], rowlen, s1_init, seed, scale, lane);
+    }
+}
+
+// copy of one rowlen-float row by a warp, dst row d <- src row s, 16-byte accesses when rowlen % 4 == 0 (rows are then
+// 16-byte aligned); either side may be device-mapped host memory
+template <bool VEC4>
+__device__ __forceinline__ void warp_copy_row(float* __restrict__ dst, size_t d, const float* __restrict__ src, size_t s,
+                                              size_t rowlen, int lane) {
+    if (VEC4) {
+        float4* d4 = reinterpret_cast<float4*>(dst + d * rowlen);
+        const float4* s4 = reinterpret_cast<const float4*>(src + s * rowlen);
+        for (size_t j = lane; j < rowlen / 4; j += 32) d4[j] = s4[j];
+    } else {
+        for (size_t j = lane; j < rowlen; j += 32) dst[d * rowlen + j] = src[s * rowlen + j];
+    }
+}
+
+// every array of row s of `from` into row d of `to` (one warp)
+template <bool VEC4>
+__device__ __forceinline__ void warp_copy_all(const RowArrays& to, size_t d, const RowArrays& from, size_t s, size_t rowlen, int lane) {
+    warp_copy_row<VEC4>(to.V, d, from.V, s, rowlen, lane);
+    warp_copy_row<VEC4>(to.s1V, d, from.s1V, s, rowlen, lane);
+    if (to.s2V) warp_copy_row<VEC4>(to.s2V, d, from.s2V, s, rowlen, lane);
+    if (lane == 0) {
+        to.W[d] = from.W[s];
+        to.s1W[d] = from.s1W[s];
+        if (to.s2W) to.s2W[d] = from.s2W[s];
+        to.row_key[d] = from.row_key[s];
+        to.last_seen[d] = from.last_seen[s];
+    }
+}
+
+// 2'. tiered twin of key_init_kernel (one warp per new row): a key found in the tier index takes its row from host memory
+//     bit for bit (stamp included), its index slot turns kNoRow and its tier row joins the released list; any other key
+//     gets the lazy init of key_init_kernel
+template <bool VEC4>
+__global__ void __launch_bounds__(256) key_restore_init_kernel(KeyView t, KeyView h, RowArrays dev, RowArrays tier, size_t rowlen,
+                                                               uint32_t* __restrict__ rel, float s1_init,
+                                                               unsigned long long seed, float scale) {
+    const unsigned n = t.flags[2];
+    const int lane = threadIdx.x & 31;
+    const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
+    for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n; w += nwarps) {
+        const uint32_t r = t.new_rows[w];
+        const unsigned long long key = t.row_key[r];
+        long long pos = -1;
+        if (lane < kGroup) pos = tile_find(h, key, lane, 0xffffu);
+        uint32_t tr = kNoRow;  // read by lane 0 alone, which later overwrites the word
+        if (lane == 0 && pos >= 0) tr = h.row[pos];
+        pos = __shfl_sync(~0u, pos, 0);
+        tr = __shfl_sync(~0u, tr, 0);
+        if (tr == kNoRow) {
+            warp_lazy_init(dev.W, dev.V, dev.s1W, dev.s1V, dev.s2W, dev.s2V, r, key, rowlen, s1_init, seed, scale, lane);
+            continue;
         }
+        warp_copy_all<VEC4>(dev, r, tier, tr, rowlen, lane);
         if (lane == 0) {
-            W[r] = 0.f;
-            s1W[r] = s1_init;
-            if (s2W) s2W[r] = 0.f;
+            h.row[pos] = kNoRow;
+            rel[atomicAdd(&h.flags[0], 1u)] = tr;
+        }
+    }
+}
+
+// 3'. lookup-only restore (one 16-lane tile per key): a key found live in the tier index claims a device row (the key
+//     table's insert: new rows recorded for key_restore_init_kernel, capacity flag past the capacity); others are left
+__global__ void __launch_bounds__(256) key_lookup_restore_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t, KeyView h) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const unsigned long long key = keys[i];
+    const long long pos = tile_find(h, key, sub, gmask);
+    if (pos < 0 || __ldg(h.row + pos) == kNoRow) return;  // whole tiles leave together
+    tile_insert(t, key, sub, gmask);
+}
+
+// insert = 0, after the restore: a key still live in the tier whose device slot holds kNoRow was refused by the capacity,
+// in this upload or an earlier one, and raises the capacity flag (an insert-upload's key_find_kernel raises it itself).
+// A separate launch, so that no tile reads the row of a slot another tile of the same launch has just claimed.
+__global__ void __launch_bounds__(256) key_tier_refused_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t, KeyView h) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const unsigned long long key = keys[i];
+    const long long pos = tile_find(t, key, sub, gmask);
+    if (pos < 0 || __ldg(t.row + pos) != kNoRow) return;  // whole tiles leave together
+    const long long hp = tile_find(h, key, sub, gmask);
+    if (sub == 0 && hp >= 0 && h.row[hp] != kNoRow) t.flags[0] = 1u;
+}
+
+// spill of evicted device rows into tier rows base + i (warp per row, ascending old row, before anything moves), then the
+// claim of each key's index slot; a dead slot of the same key is taken again
+template <bool VEC4>
+__global__ void __launch_bounds__(256) tier_spill_kernel(const uint32_t* __restrict__ ev_rows, size_t m, RowArrays dev, RowArrays tier,
+                                                         size_t base, size_t rowlen, KeyView h) {
+    const int lane = threadIdx.x & 31;
+    const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
+    for (size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; i < m; i += nwarps) {
+        const size_t r = ev_rows[i], d = base + i;
+        warp_copy_all<VEC4>(tier, d, dev, r, rowlen, lane);
+        if (lane < kGroup) {
+            bool claimed;
+            const long long pos = tile_claim(h, dev.row_key[r], lane, 0xffffu, &claimed);
+            if (lane == 0) {
+                if (pos < 0) {
+                    h.flags[1] = 1u;
+                } else {
+                    h.row[pos] = (uint32_t)d;
+                    if (claimed) atomicAdd(&h.flags[2], 1u);
+                }
+            }
         }
     }
 }
@@ -216,11 +373,6 @@ __device__ __forceinline__ bool row_evicted(const EvictRule& e, unsigned long lo
     return age > e.max_idle || (e.limit && age >= e.cut);
 }
 
-// the per-row arrays that move with a row
-struct RowArrays {
-    float *W, *V, *s1W, *s1V, *s2W, *s2V;
-    unsigned long long *row_key, *last_seen;
-};
 
 // res[0] += rows with age <= max_idle, res[1] = max(res[1], their largest age)
 __global__ void __launch_bounds__(256) evict_survey_kernel(const unsigned long long* __restrict__ last_seen, size_t n,
@@ -373,17 +525,6 @@ __global__ void __launch_bounds__(256) evict_export_kernel(const uint32_t* __res
     }
 }
 
-// copy of one rowlen-float row by a warp, 16-byte accesses when rowlen % 4 == 0 (rows are then 16-byte aligned)
-template <bool VEC4>
-__device__ __forceinline__ void warp_copy_row(float* __restrict__ a, size_t d, size_t s, size_t rowlen, int lane) {
-    if (VEC4) {
-        float4* dst = reinterpret_cast<float4*>(a + d * rowlen);
-        const float4* src = reinterpret_cast<const float4*>(a + s * rowlen);
-        for (size_t j = lane; j < rowlen / 4; j += 32) dst[j] = src[j];
-    } else {
-        for (size_t j = lane; j < rowlen; j += 32) a[d * rowlen + j] = a[s * rowlen + j];
-    }
-}
 template <bool VEC4>
 __device__ __forceinline__ void warp_fill_row(float* __restrict__ a, size_t d, size_t rowlen, float v, int lane) {
     if (VEC4) {
@@ -394,29 +535,36 @@ __device__ __forceinline__ void warp_fill_row(float* __restrict__ a, size_t d, s
     }
 }
 
-// survivors at or above n_live into the holes below it (warp per row of [n_live, n); evicted rows there skip)
+// survivors at or above n_live into the holes below it (warp per row of [n_live, n); evicted rows there skip).  wscan[i]
+// = E(n_live + i) for i in [0, n - n_live]: the window of the scan above n_live; holes = the rows that leave, ascending
+// (only those below n_live are read)
 template <bool VEC4>
 __global__ void __launch_bounds__(256) evict_move_kernel(RowArrays a, size_t rowlen, size_t n_live, size_t n,
-                                                         const uint32_t* __restrict__ scan, const uint32_t* __restrict__ ev_rows) {
+                                                         const uint32_t* __restrict__ wscan, const uint32_t* __restrict__ holes) {
     const int lane = threadIdx.x & 31;
     const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
-    const uint32_t e_live = scan[n_live];
+    const uint32_t e_live = wscan[0];
     for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n - n_live; w += nwarps) {
         const size_t r = n_live + w;
-        const uint32_t E = scan[r];
-        if (scan[r + 1] != E) continue;  // evicted
-        const size_t d = ev_rows[(r - n_live) - (E - e_live)];
-        warp_copy_row<VEC4>(a.V, d, r, rowlen, lane);
-        warp_copy_row<VEC4>(a.s1V, d, r, rowlen, lane);
-        if (a.s2V) warp_copy_row<VEC4>(a.s2V, d, r, rowlen, lane);
-        if (lane == 0) {
-            a.W[d] = a.W[r];
-            a.s1W[d] = a.s1W[r];
-            if (a.s2W) a.s2W[d] = a.s2W[r];
-            a.row_key[d] = a.row_key[r];
-            a.last_seen[d] = a.last_seen[r];
-        }
+        const uint32_t E = wscan[w];
+        if (wscan[w + 1] != E) continue;  // evicted
+        const size_t d = holes[w - (E - e_live)];
+        warp_copy_all<VEC4>(a, d, a, r, rowlen, lane);
     }
+}
+
+// after a tier move: the index slot of every moved row names its new row (one 16-lane tile per row of [n_live, n))
+__global__ void __launch_bounds__(256) tier_reindex_kernel(KeyView h, size_t n_live, size_t n, const uint32_t* __restrict__ wscan,
+                                                           const uint32_t* __restrict__ holes) {
+    const size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (w >= n - n_live) return;
+    const size_t r = n_live + w;
+    const uint32_t E = wscan[w];
+    if (wscan[w + 1] != E) return;  // left the tier
+    const size_t d = holes[w - (E - wscan[0])];
+    const int sub = threadIdx.x & (kGroup - 1);
+    const long long pos = tile_find(h, h.row_key[r], sub, 0xffffu << (threadIdx.x & 16));
+    if (sub == 0 && pos >= 0) h.row[pos] = (uint32_t)d;
 }
 
 // rows [lo, hi) back to the state lctr_create gives (warp per row)
@@ -450,23 +598,51 @@ static int scratch_reserve(lctr_ctx* c, size_t n) {
     LCTR_CUDA(cudaMalloc((void**)&t->d_keys, cap * sizeof(unsigned long long)));
     LCTR_CUDA(cudaMalloc((void**)&t->d_rows, cap * sizeof(int64_t)));
     LCTR_CUDA(cudaMalloc((void**)&t->new_rows, cap * sizeof(uint32_t)));
+    if (HostTier* h = t->tier) {  // a call restores at most one tier row per new row
+        cudaFree(h->rel); cudaFree(h->wscan); cudaFree(h->holes);
+        h->rel = h->wscan = h->holes = nullptr;
+        LCTR_CUDA(cudaMalloc((void**)&h->rel, cap * sizeof(uint32_t)));
+        LCTR_CUDA(cudaMalloc((void**)&h->wscan, (cap + 1) * sizeof(uint32_t)));
+        LCTR_CUDA(cudaMalloc((void**)&h->holes, cap * sizeof(uint32_t)));
+    }
     t->cap_scratch = cap;
     return 0;
 }
 
+static RowArrays device_rows(lctr_ctx* c) {
+    return RowArrays{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, c->keys->row_key, c->keys->last_seen};
+}
+
+// tiered contexts whose tier holds rows restore the keys it holds instead of initialising them
+static bool tier_live(const KeyTable* t) { return t->tier && t->tier->n > 0; }
+
 static int init_new_rows(lctr_ctx* c, int64_t max_new) {
     KeyTable* t = c->keys;
     const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((max_new + 7) / 8, (int64_t)c->sm_count * 16));
-    key_init_kernel<<<grid, 256, 0, c->stream>>>(view(t), c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, c->rowlen,
-                                                 initial_s1(c->cfg), t->seed, t->scale);
+    if (tier_live(t)) {
+        HostTier* h = t->tier;
+        const RowArrays dev = device_rows(c);
+        if ((c->rowlen & 3) == 0)
+            key_restore_init_kernel<true><<<grid, 256, 0, c->stream>>>(view(t), view(h), dev, h->a, c->rowlen, h->rel,
+                                                                      initial_s1(c->cfg), t->seed, t->scale);
+        else
+            key_restore_init_kernel<false><<<grid, 256, 0, c->stream>>>(view(t), view(h), dev, h->a, c->rowlen, h->rel,
+                                                                       initial_s1(c->cfg), t->seed, t->scale);
+    } else {
+        key_init_kernel<<<grid, 256, 0, c->stream>>>(view(t), c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, c->rowlen,
+                                                     initial_s1(c->cfg), t->seed, t->scale);
+    }
     c->launches++;
     LCTR_CUDA(cudaGetLastError());
     return 0;
 }
 
+// the key table's flags and, on a tiered context, the tier's, with one synchronisation
 static int read_flags(lctr_ctx* c) {
     KeyTable* t = c->keys;
     LCTR_CUDA(cudaMemcpyAsync(t->h_flags, t->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    if (t->tier)
+        LCTR_CUDA(cudaMemcpyAsync(t->tier->h_flags, t->tier->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }
@@ -509,12 +685,48 @@ int keys_alloc(lctr_ctx* c) {
         LCTR_CUDA(cudaMalloc((void**)&t->last_seen, t->cap * sizeof(unsigned long long)));
         LCTR_CUDA(cudaMemsetAsync(t->last_seen, 0, t->cap * sizeof(unsigned long long), c->stream));
     }
+    if (c->cfg.key_host_rows) {
+        HostTier* h = new HostTier();
+        t->tier = h;
+        h->cap = c->cfg.key_host_rows;
+        size_t TT = kGroup;
+        while (TT < 2 * h->cap) TT <<= 1;
+        h->T = TT;
+        LCTR_CUDA(cudaMalloc((void**)&h->key, TT * sizeof(unsigned long long)));
+        LCTR_CUDA(cudaMalloc((void**)&h->row, TT * sizeof(uint32_t)));
+        LCTR_CUDA(cudaMalloc((void**)&h->flags, 3 * sizeof(unsigned int)));
+        LCTR_CUDA(cudaMallocHost((void**)&h->h_flags, 3 * sizeof(unsigned int)));
+        LCTR_CUDA(cudaMemsetAsync(h->key, 0xff, TT * sizeof(unsigned long long), c->stream));
+        LCTR_CUDA(cudaMemsetAsync(h->row, 0xff, TT * sizeof(uint32_t), c->stream));
+        LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
+        // rows in pinned host memory mapped into the device address space: kernels read and write them over PCIe
+        auto host = [&](void** p, size_t bytes) {
+            return cudaHostAlloc(p, bytes, cudaHostAllocMapped) == cudaSuccess && (memset(*p, 0, bytes), true);
+        };
+        const size_t R = h->cap, nv = R * c->rowlen;
+        bool ok = host((void**)&h->a.row_key, R * 8) && host((void**)&h->a.last_seen, R * 8) && host((void**)&h->a.W, R * 4) &&
+                  host((void**)&h->a.V, nv * 4) && host((void**)&h->a.s1W, R * 4) && host((void**)&h->a.s1V, nv * 4);
+        if (ok && c->s2W) ok = host((void**)&h->a.s2W, R * 4) && host((void**)&h->a.s2V, nv * 4);
+        LCTR_CHECK(ok, "lctr_create: cannot allocate %llu rows of pinned host memory (cfg.key_host_rows)",
+                   (unsigned long long)h->cap);
+    }
     return 0;
+}
+
+static void tier_free(HostTier* h) {
+    cudaFree(h->key); cudaFree(h->row); cudaFree(h->flags);
+    cudaFree(h->rel); cudaFree(h->wscan); cudaFree(h->holes);
+    if (h->h_flags) cudaFreeHost(h->h_flags);
+    for (void* p : {(void*)h->a.row_key, (void*)h->a.last_seen, (void*)h->a.W, (void*)h->a.V, (void*)h->a.s1W, (void*)h->a.s1V,
+                    (void*)h->a.s2W, (void*)h->a.s2V})
+        if (p) cudaFreeHost(p);
+    delete h;
 }
 
 void keys_free(lctr_ctx* c) {
     KeyTable* t = c->keys;
     if (!t) return;
+    if (t->tier) tier_free(t->tier);
     cudaFree(t->key); cudaFree(t->row); cudaFree(t->row_key); cudaFree(t->count); cudaFree(t->flags);
     cudaFree(t->new_rows); cudaFree(t->d_keys); cudaFree(t->d_rows);
     cudaFree(t->last_seen); cudaFree(t->ev_scan); cudaFree(t->ev_rows); cudaFree(t->ev_tiles); cudaFree(t->ev_hist);
@@ -527,6 +739,22 @@ void keys_free(lctr_ctx* c) {
 
 bool keys_tracked(const lctr_ctx* c) { return c->keys && c->keys->last_seen; }
 
+static int tier_rebuild(lctr_ctx* c);
+
+bool keys_tier(const lctr_ctx* c, TierRows* out) {
+    if (!c->keys || !c->keys->tier) return false;
+    const HostTier* h = c->keys->tier;
+    *out = TierRows{h->a.row_key, h->a.last_seen, {h->a.W, h->a.V, h->a.s1W, h->a.s1V, h->a.s2W, h->a.s2V}, h->n, h->cap};
+    return true;
+}
+
+int keys_tier_restore(lctr_ctx* c, uint64_t n) {
+    HostTier* h = c->keys->tier;
+    LCTR_CHECK(n <= h->cap, "checkpoint: %llu host-tier rows exceed cfg.key_host_rows = %zu", (unsigned long long)n, h->cap);
+    h->n = (size_t)n;
+    return tier_rebuild(c);
+}
+
 KeyView keys_view(lctr_ctx* c) { return view(c->keys); }
 int keys_reserve_new_rows(lctr_ctx* c, size_t n) { return scratch_reserve(c, n); }
 int keys_init_new_rows(lctr_ctx* c, int64_t max_new) { return init_new_rows(c, max_new); }
@@ -536,10 +764,93 @@ size_t keys_bytes(const lctr_ctx* c) {
     const KeyTable* t = c->keys;
     if (!t) return 0;
     return t->T * (sizeof(unsigned long long) + sizeof(uint32_t)) + t->cap * sizeof(unsigned long long) +
-           (t->last_seen ? t->cap * sizeof(unsigned long long) : 0);
+           (t->last_seen ? t->cap * sizeof(unsigned long long) : 0) +
+           (t->tier ? t->tier->T * (sizeof(unsigned long long) + sizeof(uint32_t)) : 0);
 }
 
-// keys of one upload -> rows in fid (device, n entries); insert: create and initialise rows for new keys first
+#define LCTR_LAUNCHED()                  \
+    do {                                 \
+        c->launches++;                   \
+        LCTR_CUDA(cudaGetLastError());   \
+    } while (0)
+
+// the tier index emptied and rows [0, n) re-inserted with row = index
+static int tier_rebuild(lctr_ctx* c) {
+    HostTier* h = c->keys->tier;
+    LCTR_CUDA(cudaMemsetAsync(h->key, 0xff, h->T * sizeof(unsigned long long), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(h->row, 0xff, h->T * sizeof(uint32_t), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    if (h->n) {
+        key_insert_fixed_kernel<<<tile_grid((int64_t)h->n), 256, 0, c->stream>>>(h->a.row_key, nullptr, (int64_t)h->n, view(h), 0);
+        LCTR_LAUNCHED();
+    }
+    LCTR_CUDA(cudaMemcpyAsync(h->h_flags, h->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    LCTR_CHECK(!h->h_flags[1], "host tier: index full while re-inserting %zu keys", h->n);
+    h->used = h->n;
+    return 0;
+}
+
+// survivors at or above n_live into the holes below it, for the rows of one table (wscan, holes: evict_move_kernel)
+static int launch_move(lctr_ctx* c, const RowArrays& a, size_t n_live, size_t n, const uint32_t* wscan, const uint32_t* holes) {
+    const size_t m = n - n_live;
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
+    if ((c->rowlen & 3) == 0) evict_move_kernel<true><<<grid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, wscan, holes);
+    else evict_move_kernel<false><<<grid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, wscan, holes);
+    LCTR_LAUNCHED();
+    return 0;
+}
+
+// ascending order of distinct values below 2^32: LSD radix sort, three passes of 11 bits
+static void radix_sort_u32(std::vector<uint32_t>& v) {
+    std::vector<uint32_t> tmp(v.size());
+    for (int shift = 0; shift < 32; shift += 11) {
+        size_t cnt[2049] = {0};
+        for (uint32_t x : v) cnt[((x >> shift) & 2047) + 1]++;
+        for (int b = 0; b < 2048; b++) cnt[b + 1] += cnt[b];
+        for (uint32_t x : v) tmp[cnt[(x >> shift) & 2047]++] = x;
+        v.swap(tmp);
+    }
+}
+
+// after an upload that restored rows (tier flags read back): the m released rows leave the tier, and the survivors of the
+// window [n_live, n) fill the holes below n_live by eviction's rule (the j-th survivor, ascending, into the j-th hole,
+// ascending).  Planned on the host from the released list: O(m) copies and work (the sort is a radix sort), then one
+// move and one reindex launch over the window; nothing reads the rest of the tier.
+static int tier_compact(lctr_ctx* c) {
+    HostTier* h = c->keys->tier;
+    if (!h || !h->h_flags[0]) return 0;
+    const size_t m = h->h_flags[0], n = h->n, n_live = n - m;
+    std::vector<uint32_t> rel(m), holes;
+    LCTR_CUDA(cudaMemcpyAsync(rel.data(), h->rel, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    std::vector<uint32_t> wscan(m + 1, 0);  // first as flags of the window, then its exclusive scan
+    for (uint32_t r : rel) {
+        if (r >= n_live) wscan[r - n_live] = 1;
+        else holes.push_back(r);
+    }
+    radix_sort_u32(holes);
+    uint32_t e = 0;
+    for (size_t i = 0; i <= m; i++) {
+        const uint32_t f = wscan[i];
+        wscan[i] = e;
+        e += f;
+    }
+    LCTR_CUDA(cudaMemcpyAsync(h->wscan, wscan.data(), (m + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    if (!holes.empty())
+        LCTR_CUDA(cudaMemcpyAsync(h->holes, holes.data(), holes.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    if (launch_move(c, h->a, n_live, n, h->wscan, h->holes)) return 1;
+    tier_reindex_kernel<<<tile_grid((int64_t)m), 256, 0, c->stream>>>(view(h), n_live, n, h->wscan, h->holes);
+    LCTR_LAUNCHED();
+    LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    h->h_flags[0] = 0;
+    h->n = n_live;
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the host vectors above are the copies' sources
+    return 0;
+}
+
+// keys of one upload -> rows in fid (device, n entries); insert: create and initialise rows for new keys first.  Tiered:
+// new keys the tier holds are restored from it; insert = 0 gives rows to the keys the tier holds, and to no other.
 int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid) {
     KeyTable* t = c->keys;
     if (insert) t->clock++;  // the clock counts insert-uploads, empty ones included
@@ -547,13 +858,20 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, h_keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
     LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    const bool restoring = tier_live(t);
     {
         ProfScope prof(c, PROF_KEYS);
-        if (insert) {
-            key_insert_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t));
+        if (insert || restoring) {
+            if (insert) key_insert_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t));
+            else key_lookup_restore_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), view(t->tier));
             c->launches++;
             LCTR_CUDA(cudaGetLastError());
             if (init_new_rows(c, std::min<int64_t>(n, (int64_t)t->cap))) return 1;
+            if (!insert) {
+                key_tier_refused_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), view(t->tier));
+                c->launches++;
+                LCTR_CUDA(cudaGetLastError());
+            }
         }
         key_find_kernel<0><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0,
                                                                 insert ? t->last_seen : nullptr, t->clock);
@@ -561,6 +879,7 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
         LCTR_CUDA(cudaGetLastError());
     }
     if (read_flags(c)) return 1;
+    if (restoring && tier_compact(c)) return 1;  // before any failure below: restored rows have left the tier either way
     LCTR_CHECK(!t->h_flags[1], "key table: no free slot on a probe path (%zu slots for capacity %zu)", t->T, t->cap);
     LCTR_CHECK(!t->h_flags[0], "key table: capacity of %zu rows (cfg.feature_cnt) exhausted; the batch's new keys do not fit",
                t->cap);
@@ -649,15 +968,9 @@ static int read_res(lctr_ctx* c, int n) {
     return 0;
 }
 
-#define LCTR_LAUNCHED()                  \
-    do {                                 \
-        c->launches++;                   \
-        LCTR_CUDA(cudaGetLastError());   \
-    } while (0)
-
 // the age of rank `rank` (0-based, ascending) among the rows of age <= max_idle, of which the largest is max_age
-static int radix_select_age(lctr_ctx* c, size_t n, unsigned long long max_idle, unsigned long long max_age,
-                            unsigned long long rank, unsigned long long* out) {
+static int radix_select_age(lctr_ctx* c, const unsigned long long* last_seen, size_t n, unsigned long long max_idle,
+                            unsigned long long max_age, unsigned long long rank, unsigned long long* out) {
     KeyTable* t = c->keys;
     const int bits = std::max(1, 64 - __builtin_clzll(max_age | 1ull));
     const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
@@ -667,7 +980,7 @@ static int radix_select_age(lctr_ctx* c, size_t n, unsigned long long max_idle, 
         const int width = std::min(16, shift);
         shift -= width;
         LCTR_CUDA(cudaMemsetAsync(t->ev_hist, 0, ((size_t)1 << width) * sizeof(unsigned int), c->stream));
-        evict_hist_kernel<<<grid, 256, 0, c->stream>>>(t->last_seen, n, t->clock, max_idle, shift, width, pshift, prefix, t->ev_hist);
+        evict_hist_kernel<<<grid, 256, 0, c->stream>>>(last_seen, n, t->clock, max_idle, shift, width, pshift, prefix, t->ev_hist);
         LCTR_LAUNCHED();
         evict_pick_kernel<<<1, 1024, 0, c->stream>>>(t->ev_hist, 1 << width, rank, t->ev_res);
         LCTR_LAUNCHED();
@@ -677,6 +990,86 @@ static int radix_select_age(lctr_ctx* c, size_t n, unsigned long long max_idle, 
         pshift = shift;
     }
     *out = prefix;
+    return 0;
+}
+
+// one table as the eviction sees it: the device table or the host tier (rows [0, n), scratch sized for its capacity)
+struct EvTable {
+    RowArrays a;
+    size_t n;
+    uint32_t *scan, *rows, *tiles;
+};
+
+// survey, select, count and scan of the stamp rule against the upload clock: *m rows of the table leave by rule *l
+static int evict_plan(lctr_ctx* c, const EvTable& tb, uint64_t max_idle, uint64_t max_rows, EvictRule* e, size_t* m) {
+    KeyTable* t = c->keys;
+    const size_t n = tb.n;
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
+    // 1 + 2: the rule
+    LCTR_CUDA(cudaMemsetAsync(t->ev_res, 0, 2 * sizeof(unsigned long long), c->stream));
+    evict_survey_kernel<<<grid, 256, 0, c->stream>>>(tb.a.last_seen, n, t->clock, max_idle, t->ev_res);
+    LCTR_LAUNCHED();
+    if (read_res(c, 2)) return 1;
+    const unsigned long long survivors = t->h_res[0], max_age = t->h_res[1];
+    *e = EvictRule{t->clock, max_idle, 0ull, 0};
+    if (survivors > max_rows) {
+        if (radix_select_age(c, tb.a.last_seen, n, max_idle, max_age, max_rows, &e->cut)) return 1;
+        e->limit = 1;
+    }
+    // count and scan
+    const size_t ntiles = n / kEvTile + 1;  // tiles cover [0, n]: E(n) is needed too
+    evict_count_kernel<<<(unsigned)ntiles, kEvTile, 0, c->stream>>>(tb.a.last_seen, n, *e, tb.tiles);
+    LCTR_LAUNCHED();
+    evict_scan_tiles_kernel<<<1, 1024, 0, c->stream>>>(tb.tiles, ntiles, t->ev_res);
+    LCTR_LAUNCHED();
+    if (read_res(c, 1)) return 1;
+    *m = (size_t)t->h_res[0];
+    return 0;
+}
+
+// E(r) and the list of the m rows that leave, then their key, W and V into the caller's buffers (each may be null)
+static int evict_index_export(lctr_ctx* c, const EvTable& tb, const EvictRule& e, size_t m, uint64_t* keys_out, float* W_out,
+                              float* V_out) {
+    evict_index_kernel<<<(unsigned)(tb.n / kEvTile + 1), kEvTile, 0, c->stream>>>(tb.a.last_seen, tb.n, e, tb.tiles, tb.scan, tb.rows);
+    LCTR_LAUNCHED();
+    if (!(keys_out || W_out || V_out)) return 0;
+    const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
+    unsigned long long* dK = nullptr;
+    float *dW = nullptr, *dV = nullptr;
+    cudaError_t err = cudaSuccess;
+    if (keys_out && err == cudaSuccess) err = cudaMalloc((void**)&dK, m * sizeof(unsigned long long));
+    if (W_out && err == cudaSuccess) err = cudaMalloc((void**)&dW, m * sizeof(float));
+    if (V_out && err == cudaSuccess) err = cudaMalloc((void**)&dV, m * c->rowlen * sizeof(float));
+    if (err == cudaSuccess) {
+        evict_export_kernel<<<mgrid, 256, 0, c->stream>>>(tb.rows, m, tb.a.row_key, tb.a.W, tb.a.V, c->rowlen, dK, dW, dV);
+        c->launches++;
+        err = cudaGetLastError();
+    }
+    if (err == cudaSuccess && dK) err = cudaMemcpyAsync(keys_out, dK, m * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
+    if (err == cudaSuccess && dW) err = cudaMemcpyAsync(W_out, dW, m * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
+    if (err == cudaSuccess && dV) err = cudaMemcpyAsync(V_out, dV, m * c->rowlen * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
+    const cudaError_t es = cudaStreamSynchronize(c->stream);
+    cudaFree(dK); cudaFree(dW); cudaFree(dV);
+    LCTR_CUDA(err);
+    LCTR_CUDA(es);
+    return 0;
+}
+
+// the m rows of the device table's eviction list appended to the tier at rows [n, n + m), keys claimed in its index
+static int tier_spill(lctr_ctx* c, const EvTable& dev, size_t m) {
+    HostTier* h = c->keys->tier;
+    LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
+    if ((c->rowlen & 3) == 0) tier_spill_kernel<true><<<mgrid, 256, 0, c->stream>>>(dev.rows, m, dev.a, h->a, h->n, c->rowlen, view(h));
+    else tier_spill_kernel<false><<<mgrid, 256, 0, c->stream>>>(dev.rows, m, dev.a, h->a, h->n, c->rowlen, view(h));
+    LCTR_LAUNCHED();
+    LCTR_CUDA(cudaMemcpyAsync(h->h_flags, h->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    h->n += m;
+    h->used += h->h_flags[2];
+    LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    // a full probe path (never expected below T / 2 used slots) or more than T / 2 slots in use: a fresh index
+    if (h->h_flags[1] || 2 * h->used > h->T) return tier_rebuild(c);
     return 0;
 }
 
@@ -776,10 +1169,12 @@ static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* key
         key_insert_fixed_kernel<<<tile_grid(m), 256, 0, c->stream>>>(t->d_keys, t->d_rows, m, view(t), 1);
         c->launches++;
         LCTR_CUDA(cudaGetLastError());
+        const bool restoring = tier_live(t);  // tier keys bring their optimizer state back
         if (init_new_rows(c, m)) return 1;
         const unsigned long long cnt = used + (uint64_t)m;
         LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
         if (read_flags(c)) return 1;
+        if (restoring && tier_compact(c)) return 1;
         LCTR_CHECK(!t->h_flags[1], "lctr_upload_keyed_params: key table full");
     }
     if (t->last_seen || W || V)
@@ -833,64 +1228,26 @@ int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t*
     if (rc) return 1;
     if (n == 0) return 0;
     if (evict_scratch(c)) return 1;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
-
-    // 1 + 2: the rule
-    LCTR_CUDA(cudaMemsetAsync(t->ev_res, 0, 2 * sizeof(unsigned long long), c->stream));
-    evict_survey_kernel<<<grid, 256, 0, c->stream>>>(t->last_seen, n, t->clock, max_idle, t->ev_res);
-    LCTR_LAUNCHED();
-    if (read_res(c, 2)) return 1;
-    const unsigned long long survivors = t->h_res[0], max_age = t->h_res[1];
-    EvictRule e{t->clock, max_idle, 0ull, 0};
-    if (survivors > max_rows) {
-        if (radix_select_age(c, n, max_idle, max_age, max_rows, &e.cut)) return 1;
-        e.limit = 1;
-    }
-
-    // count and scan
-    const size_t ntiles = n / kEvTile + 1;  // tiles cover [0, n]: E(n) is needed too
-    evict_count_kernel<<<(unsigned)ntiles, kEvTile, 0, c->stream>>>(t->last_seen, n, e, t->ev_tiles);
-    LCTR_LAUNCHED();
-    evict_scan_tiles_kernel<<<1, 1024, 0, c->stream>>>(t->ev_tiles, ntiles, t->ev_res);
-    LCTR_LAUNCHED();
-    if (read_res(c, 1)) return 1;
-    const size_t m = (size_t)t->h_res[0];
+    const EvTable tb{device_rows(c), n, t->ev_scan, t->ev_rows, t->ev_tiles};
+    EvictRule e;
+    size_t m = 0;
+    if (evict_plan(c, tb, max_idle, max_rows, &e, &m)) return 1;
     if (m == 0) return 0;  // nothing leaves: the table, its rows and the slots stay as they are
     const bool exporting = keys_out || W_out || V_out;
     LCTR_CHECK(!exporting || cap_out >= m, "lctr_evict_keys: room for %llu evicted rows, %zu would leave (nothing was changed)",
                (unsigned long long)cap_out, m);
+    HostTier* h = t->tier;
+    LCTR_CHECK(!h || h->n + m <= h->cap, "lctr_evict_keys: %zu rows would leave for the host tier, which holds %zu rows "
+               "(cfg.key_host_rows) with %zu free (nothing was changed)", m, h ? h->cap : 0, h ? h->cap - h->n : 0);
     const size_t n_live = n - m;
-    evict_index_kernel<<<(unsigned)ntiles, kEvTile, 0, c->stream>>>(t->last_seen, n, e, t->ev_tiles, t->ev_scan, t->ev_rows);
-    LCTR_LAUNCHED();
-
-    const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
-    if (exporting) {  // gathered before anything moves
-        unsigned long long* dK = nullptr;
-        float *dW = nullptr, *dV = nullptr;
-        cudaError_t err = cudaSuccess;
-        if (keys_out && err == cudaSuccess) err = cudaMalloc((void**)&dK, m * sizeof(unsigned long long));
-        if (W_out && err == cudaSuccess) err = cudaMalloc((void**)&dW, m * sizeof(float));
-        if (V_out && err == cudaSuccess) err = cudaMalloc((void**)&dV, m * c->rowlen * sizeof(float));
-        if (err == cudaSuccess) {
-            evict_export_kernel<<<mgrid, 256, 0, c->stream>>>(t->ev_rows, m, t->row_key, c->W, c->V, c->rowlen, dK, dW, dV);
-            c->launches++;
-            err = cudaGetLastError();
-        }
-        if (err == cudaSuccess && dK) err = cudaMemcpyAsync(keys_out, dK, m * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
-        if (err == cudaSuccess && dW) err = cudaMemcpyAsync(W_out, dW, m * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
-        if (err == cudaSuccess && dV) err = cudaMemcpyAsync(V_out, dV, m * c->rowlen * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
-        const cudaError_t es = cudaStreamSynchronize(c->stream);
-        cudaFree(dK); cudaFree(dW); cudaFree(dV);
-        LCTR_CUDA(err);
-        LCTR_CUDA(es);
-    }
+    if (evict_index_export(c, tb, e, m, keys_out, W_out, V_out)) return 1;  // gathered before anything moves
+    if (h && tier_spill(c, tb, m)) return 1;
 
     // move, reset, rebuild
-    const RowArrays a{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, t->row_key, t->last_seen};
+    const RowArrays& a = tb.a;
     const bool vec4 = (c->rowlen & 3) == 0;  // 16-byte rows: FM / NFM k % 4 == 0, FFM Fc * k % 4 == 0
-    if (vec4) evict_move_kernel<true><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, t->ev_scan, t->ev_rows);
-    else evict_move_kernel<false><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, t->ev_scan, t->ev_rows);
-    LCTR_LAUNCHED();
+    if (launch_move(c, a, n_live, n, t->ev_scan + n_live, t->ev_rows)) return 1;
+    const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
     if (vec4) evict_reset_kernel<true><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, initial_s1(c->cfg));
     else evict_reset_kernel<false><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, initial_s1(c->cfg));
     LCTR_LAUNCHED();
@@ -908,6 +1265,53 @@ int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t*
     for (int s = 0; s < kNumSlots; s++)  // their row ids belong to the old numbering
         if (c->slots[s].key_state != SLOT_KEYS_INVALID) c->slots[s].key_state = SLOT_KEYS_STALE;
     *n_evicted = m;
+    return 0;
+}
+
+int lctr_evict_host_tier(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t* keys_out, float* W_out, float* V_out,
+                         uint64_t cap_out, uint64_t* n_evicted) {
+    LCTR_CHECK(c && n_evicted, "null argument");
+    LCTR_CHECK(c->keys && c->keys->tier, "lctr_evict_host_tier: the context was not created with a host tier (cfg.key_host_rows)");
+    HostTier* h = c->keys->tier;
+    *n_evicted = 0;
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    const size_t n = h->n;
+    if (n == 0) return 0;
+    if (evict_scratch(c)) return 1;
+    // scratch of the tier's size for this call only: a tier eviction reads every tier row anyway
+    struct Scratch {
+        uint32_t *scan = nullptr, *rows = nullptr, *tiles = nullptr;
+        ~Scratch() { cudaFree(scan); cudaFree(rows); cudaFree(tiles); }
+    } sc;
+    LCTR_CUDA(cudaMalloc((void**)&sc.scan, (n + 1) * sizeof(uint32_t)));
+    LCTR_CUDA(cudaMalloc((void**)&sc.rows, n * sizeof(uint32_t)));
+    LCTR_CUDA(cudaMalloc((void**)&sc.tiles, (n / kEvTile + 1) * sizeof(uint32_t)));
+    const EvTable tb{h->a, n, sc.scan, sc.rows, sc.tiles};
+    EvictRule e;
+    size_t m = 0;
+    if (evict_plan(c, tb, max_idle, max_rows, &e, &m)) return 1;
+    if (m == 0) return 0;
+    LCTR_CHECK(!(keys_out || W_out || V_out) || cap_out >= m,
+               "lctr_evict_host_tier: room for %llu evicted rows, %zu would leave (nothing was changed)", (unsigned long long)cap_out, m);
+    if (evict_index_export(c, tb, e, m, keys_out, W_out, V_out)) return 1;
+    if (launch_move(c, h->a, n - m, n, sc.scan + (n - m), sc.rows)) return 1;
+    h->n = n - m;
+    if (tier_rebuild(c)) return 1;
+    *n_evicted = m;
+    return 0;
+}
+
+int lctr_download_host_tier(lctr_ctx* c, uint64_t* keys, float* W, float* V, uint64_t cap, uint64_t* n_rows) {
+    LCTR_CHECK(c && n_rows, "null argument");
+    LCTR_CHECK(c->keys && c->keys->tier, "lctr_download_host_tier: the context was not created with a host tier (cfg.key_host_rows)");
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the tier's rows change only on the ctx stream
+    const HostTier* h = c->keys->tier;
+    *n_rows = h->n;
+    if (!keys && !W && !V) return 0;
+    LCTR_CHECK(cap >= h->n, "lctr_download_host_tier: room for %llu rows, the tier holds %zu", (unsigned long long)cap, h->n);
+    if (keys) memcpy(keys, h->a.row_key, h->n * sizeof(uint64_t));
+    if (W) memcpy(W, h->a.W, h->n * sizeof(float));
+    if (V) memcpy(V, h->a.V, h->n * c->rowlen * sizeof(float));
     return 0;
 }
 
