@@ -200,6 +200,42 @@ int lctr_download_host_tier(lctr_ctx* ctx, uint64_t* keys, float* W, float* V, u
  * stamps against the same clock.  The rows it frees leave the model; the rest are renumbered by the same rule. */
 int lctr_evict_host_tier(lctr_ctx* ctx, uint64_t max_idle, uint64_t max_rows, uint64_t* keys_out, float* W_out, float* V_out,
                          uint64_t cap_out, uint64_t* n_evicted);
+/* Frequency admission (keyed, world = 1, FM / FFM / NFM), so that keys met once and never again get no row: a new key
+ * gets a row only once it has been met min_count times.  The counts live in a count-min sketch in device memory: 4 rows
+ * of 2^log2_width u32 counters (16 * 2^log2_width bytes, counted by lctr_device_bytes), log2_width in [10, 28]; counter i
+ * (0..3) of key x is
+ *     fmix64(x ^ ((i + 1) * 0x9E3779B97F4A7C15)) >> (64 - log2_width)      (arithmetic mod 2^64)
+ * with fmix64 the MurmurHash3 finaliser of the owner rule below.  The count of a key is the smallest of its 4 counters.
+ * A key is PRESENT when the key table holds it (with a row, or without one after a capacity overflow) or the host tier
+ * holds it.  One lctr_upload_batch_keys with insert = 1:
+ *   1. every entry whose key is not present adds 1 to the key's 4 counters (entries, not distinct keys: the counts do not
+ *      depend on order);
+ *   2. then a key that is not present is admitted when its count is >= min_count, and gets a row as a new key does (lazy
+ *      init, capacity check and failure message unchanged);
+ *   3. every entry of a key that is not admitted is removed from the batch: kept entries keep their order within their
+ *      row, with their field / val.  Rows are never removed: labels, the row count and the per-row outputs
+ *      (lctr_predict, lctr_download_pred) stay aligned with the caller's rows, and a row that lost every entry trains as
+ *      a row without entries does;
+ *   4. key_evict = 1: the clock advances as always; only rows that kept entries are stamped.
+ * Present keys (tier keys restored by the upload included) are never counted or dropped; insert = 0 uploads count and
+ * drop nothing; lctr_upload_keyed_params creates the keys it names whatever their count.  Eviction leaves the counters as
+ * they are, so an evicted key is admitted again at its next occurrence unless the sketch was decayed or reset since.
+ * Checkpoints carry the settings and the sketch (header flag bit 10): lctr_load_checkpoint requires the same settings on
+ * both sides (off = off) and refuses otherwise before writing anything, naming both; lctr_load_checkpoint_shards into a
+ * context with admission off ignores the section, into one with other settings it refuses.  Files saved with admission off
+ * keep their bytes.
+ *
+ * lctr_set_key_admission sets min_count and zeroes the sketch, at any time.  min_count <= 1 turns admission off and frees
+ * the sketch (log2_width is then ignored): the context behaves, and launches, exactly as one that never called it.
+ * Refused on a dense context, with world > 1, on Wide&Deep (it reads the first id of each field, which dropping entries
+ * would change) and with log2_width outside [10, 28].
+ * lctr_decay_key_admission shifts every counter right by shift, in [1, 32] (32 clears the sketch), so that admission can
+ * age with a drifting stream: without it collisions fill a finite sketch and eventually admit everything.
+ * lctr_key_admission_stats gives the entries the last insert-upload dropped and the keys it admitted (0 and 0 when
+ * admission is off); either pointer may be NULL. */
+int lctr_set_key_admission(lctr_ctx* ctx, uint32_t min_count, uint32_t log2_width);
+int lctr_decay_key_admission(lctr_ctx* ctx, uint32_t shift);
+int lctr_key_admission_stats(lctr_ctx* ctx, uint64_t* dropped_entries, uint64_t* admitted_keys);
 /* Keyed mode on several GPUs (world > 1; the reference's parameter servers key by size_t and create on first touch,
  * distribut/paramserver.h:315-339).
  * Owner rule: key k lives on rank fmix64(k) >> (64 - log2 world) (the top bits of MurmurHash3's 64-bit finaliser); the
@@ -300,7 +336,8 @@ int lctr_ipc_import(lctr_ctx* ctx, const void* all_handles, size_t bytes_per_ran
  * dense gradient path (FFM with deterministic 0 or 1, Wide&Deep, FM / NFM with deterministic = 0 and k outside
  * {4, 8, 16, 32}, NFM with deterministic = 2) and for the grouped FFM backward (deterministic = 2); + the touched map,
  * 1 B per row, on the dense path only; + the key table in keyed mode and 8 B per row of stamps with key_evict = 1; + the
- * host tier's index (12 B per slot) with cfg.key_host_rows > 0 (its rows are in host memory and not counted).  The
+ * host tier's index (12 B per slot) with cfg.key_host_rows > 0 (its rows are in host memory and not counted); + the key
+ * admission sketch (16 * 2^log2_width B) while admission is on (lctr_set_key_admission).  The
  * compact (FM / NFM, deterministic = 0, k in {4, 8, 16, 32}) and the other feature-major paths hold no gradient per row.
  * Per-call scratch is not counted.  exchange_bytes (world > 1): the exchange arena, caches and inboxes -- owner-sharding
  * keeps it O(keys of a batch), not O(feature_cnt) */

@@ -33,7 +33,8 @@ SYMBOLS = [
     "lctr_dense_grad_buffer", "lctr_device_bytes", "lctr_load_libffm", "lctr_free_dataset", "lctr_launch_count", "lctr_stream", "lctr_profile", "lctr_profile_read",
     "lctr_upload_batch_keys", "lctr_lookup_keys", "lctr_download_keys", "lctr_upload_keyed_params", "lctr_set_key_init",
     "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys", "lctr_load_checkpoint_shards", "lctr_eval_pred",
-    "lctr_download_host_tier", "lctr_evict_host_tier",
+    "lctr_download_host_tier", "lctr_evict_host_tier", "lctr_set_key_admission", "lctr_decay_key_admission",
+    "lctr_key_admission_stats",
 ]
 NO_LIMIT = (1 << 64) - 1  # lctr_evict_keys: UINT64_MAX = no limit
 
@@ -133,6 +134,9 @@ def load_library():
     L.lctr_evict_keys.argtypes = [vp, C.c_uint64, C.c_uint64, vp, f32p, f32p, C.c_uint64, C.POINTER(C.c_uint64)]
     L.lctr_evict_host_tier.argtypes = [vp, C.c_uint64, C.c_uint64, vp, f32p, f32p, C.c_uint64, C.POINTER(C.c_uint64)]
     L.lctr_download_host_tier.argtypes = [vp, vp, f32p, f32p, C.c_uint64, C.POINTER(C.c_uint64)]
+    L.lctr_set_key_admission.argtypes = [vp, C.c_uint32, C.c_uint32]
+    L.lctr_decay_key_admission.argtypes = [vp, C.c_uint32]
+    L.lctr_key_admission_stats.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     _lib = L
     return L
 
@@ -408,6 +412,22 @@ class Context:
         _chk(self.L.lctr_evict_host_tier(self.h, idle, rows, _p(keys), _p(W), _p(V), cap, C.byref(n)))
         m = n.value
         return keys[:m].copy(), W[:m].copy(), V[:m * self.rowlen].copy()
+
+    def set_key_admission(self, min_count, log2_width=20):
+        """Give a new key a row only once insert-uploads have met it min_count times, counted in a count-min sketch of
+        4 x 2^log2_width counters (zeroed by this call); min_count <= 1 turns admission off.  Entries of keys not admitted
+        are dropped from the batch, rows stay."""
+        _chk(self.L.lctr_set_key_admission(self.h, int(min_count), int(log2_width)))
+
+    def decay_key_admission(self, shift):
+        """every counter of the admission sketch >>= shift (1..32)"""
+        _chk(self.L.lctr_decay_key_admission(self.h, int(shift)))
+
+    def key_admission_stats(self):
+        """(entries dropped, keys admitted) by the last insert-upload"""
+        d, a = C.c_uint64(), C.c_uint64()
+        _chk(self.L.lctr_key_admission_stats(self.h, C.byref(d), C.byref(a)))
+        return d.value, a.value
 
     def upload_dataset(self, slot, ds, all_ones_as_null=True):
         val = ds.val

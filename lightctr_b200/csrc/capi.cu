@@ -504,6 +504,10 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
         if (field) LCTR_CUDA(cudaMemcpyAsync(s.field, field, (size_t)nnz * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
         if (val) LCTR_CUDA(cudaMemcpyAsync(s.val, val, (size_t)nnz * sizeof(float), cudaMemcpyHostToDevice, st));
     }
+    if (fid_resident && c->keys) {  // key admission dropped entries: the slot holds the kept ones, before the slot map
+        if (keys_admission_compact(c, s, st, rows, &nnz)) return 1;
+        s.nnz = nnz;
+    }
     const bool grouped = c->cfg.deterministic == 2 && rows > 0 && nnz > 0 && c->cfg.world == 1;
     int32_t* tmp = reinterpret_cast<int32_t*>(s.pred);  // pred is overwritten by the next forward anyway
     if (rows) {

@@ -41,6 +41,9 @@ static_assert(sizeof(CkptHeader) == 136 && sizeof(CkptShard) == 24, "checkpoint 
 static int32_t key_word(const lctr_cfg& cfg) {
     return cfg.key_mode | (cfg.key_evict ? 0x100 : 0) | (cfg.key_host_rows ? 0x200 : 0);
 }
+// bit 10: key admission was on (lctr_set_key_admission), and the file ends with its section.  Not part of the cfg, so it
+// is compared apart from the other bits
+constexpr int32_t kAdmissionBit = 0x400;
 
 static bool put(FILE* f, const void* p, size_t n) { return n == 0 || fwrite(p, 1, n, f) == n; }
 static bool get(FILE* f, void* p, size_t n) { return n == 0 || fread(p, 1, n, f) == n; }
@@ -70,7 +73,7 @@ static int file_to_dev(lctr_ctx* c, FILE* f, float* dev, size_t n) {
 static bool same_trainer(const lctr_ctx* c, const CkptHeader& h) {
     bool same = h.model == c->cfg.model && h.optimizer == c->cfg.optimizer && h.n_layers == c->n_layers &&
                 h.feature_cnt == c->F && h.field_cnt == c->cfg.field_cnt && h.factor_cnt == c->cfg.factor_cnt &&
-                h.reserved == key_word(c->cfg);
+                (h.reserved & ~kAdmissionBit) == key_word(c->cfg);
     for (int l = 0; l < c->n_layers && same; l++) same = h.in[l] == c->layers[l].in && h.out[l] == c->layers[l].out;
     return same;
 }
@@ -78,7 +81,8 @@ static bool same_trainer(const lctr_ctx* c, const CkptHeader& h) {
 // The sections of a file after its header(s), in file order: the row sections over the file's rows, the parts of every
 // layer, then for keyed tables the row count and the key of every row, for key_evict = 1 the upload clock and the stamp
 // of every row, and for a host tier its row count n, the key and the stamp of each of its rows, then the row sections over
-// those n rows.  Everything that walks the format takes the row sections and the layer parts from these helpers.
+// those n rows, and with key admission (header bit 10) u32 min_count, u32 log2_width and the 4 * 2^log2_width u32
+// counters of the sketch.  Everything that walks the format takes the row sections and the layer parts from these helpers.
 
 // W, V, s1W, s1V[, s2W, s2V] of this rank's shard
 struct RowSections {
@@ -157,6 +161,9 @@ struct CkptFile {
     std::vector<uint64_t> stamps;
     std::vector<uint64_t> tier_keys, tier_stamps;  // host tier (cfg.key_host_rows > 0)
     long tier_rows_at = 0;                         // offset of its row sections
+    bool adm = false;                              // key admission section (header bit 10)
+    uint32_t adm_min = 0, adm_lw = 0;
+    long adm_at = 0;                               // offset of its counters
     CkptFile() = default;
     CkptFile(const CkptFile&) = delete;
     CkptFile& operator=(const CkptFile&) = delete;
@@ -221,6 +228,16 @@ static int ckpt_open(lctr_ctx* c, const char* path, CkptFile& cf) {
                        "checkpoint %s: a host-tier key is reserved or held twice", path);
             cf.tier_rows_at = end + (long)((1 + 2 * nt) * sizeof(uint64_t));
             end = cf.tier_rows_at + (long)(nt * row_floats(c) * sizeof(float));
+        }
+        if (cf.h.reserved & kAdmissionBit) {
+            uint32_t s[2] = {0, 0};
+            LCTR_CHECK(fseek(cf.f, end, SEEK_SET) == 0 && get(cf.f, s, sizeof(s)) && s[0] > 1 && s[1] >= 10 && s[1] <= 28,
+                       "checkpoint %s: missing or inconsistent key admission section", path);
+            cf.adm = true;
+            cf.adm_min = s[0];
+            cf.adm_lw = s[1];
+            cf.adm_at = end + (long)sizeof(s);
+            end = cf.adm_at + (long)(((size_t)4 << s[1]) * sizeof(uint32_t));
         }
     }
     long len = -1;
@@ -306,6 +323,21 @@ static int scatter_section(lctr_ctx* c, Stage& st, FILE* f, float* dst, size_t n
     return 0;
 }
 
+// the key admission settings of a file against the context's: they must be equal (off = off), except that a context with
+// admission off may be told to ignore the file's section (skip_when_off)
+static int check_admission(const lctr_ctx* c, const CkptFile& cf, bool skip_when_off) {
+    uint32_t mc = 0, lw = 0;
+    const bool on = keys_admission(c, &mc, &lw);
+    if (!on && skip_when_off) return 0;
+    if (on == cf.adm && mc == cf.adm_min && lw == cf.adm_lw) return 0;
+    char mine[64] = "off", theirs[64] = "off";
+    if (on) snprintf(mine, sizeof(mine), "min_count %u, log2_width %u", mc, lw);
+    if (cf.adm) snprintf(theirs, sizeof(theirs), "min_count %u, log2_width %u", cf.adm_min, cf.adm_lw);
+    set_error("checkpoint %s was saved with key admission %s, this context has %s (lctr_set_key_admission must match; nothing "
+              "was changed)", cf.path.c_str(), theirs, mine);
+    return 1;
+}
+
 // a file ckpt_open checked, written by this rank of this world: the sections land where they were read
 static int load_shard_in_place(lctr_ctx* c, CkptFile& cf) {
     LCTR_CHECK(!c->keys || cf.keys.size() <= keys_capacity(c), "checkpoint %s: %zu keyed rows exceed the shard's capacity %zu",
@@ -334,6 +366,13 @@ static int load_shard_in_place(lctr_ctx* c, CkptFile& cf) {
                 LCTR_CHECK(get(cf.f, ts.p[a], nt * ts.width(a) * sizeof(float)), "checkpoint %s: short read of the host tier", cf.path.c_str());
             if (keys_tier_restore(c, nt)) return 1;
         }
+        uint32_t mc, lw;
+        if (cf.adm && keys_admission(c, &mc, &lw)) {  // check_admission made the settings equal
+            std::vector<uint32_t> sketch((size_t)4 << lw);
+            LCTR_CHECK(fseek(cf.f, cf.adm_at, SEEK_SET) == 0 && get(cf.f, sketch.data(), sketch.size() * sizeof(uint32_t)),
+                       "checkpoint %s: short read of the key admission sketch", cf.path.c_str());
+            if (keys_admission_restore(c, sketch.data())) return 1;
+        }
     }
     return finish_load(c, cf.h);
 }
@@ -357,7 +396,9 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
     h.model = c->cfg.model; h.optimizer = c->cfg.optimizer; h.n_layers = c->n_layers;
     h.feature_cnt = c->F; h.field_cnt = c->cfg.field_cnt; h.factor_cnt = c->cfg.factor_cnt;
     h.adam_iter = c->adam_iter; h.step = c->step;
-    h.reserved = key_word(c->cfg);
+    uint32_t adm[2];
+    const bool admission = keys_admission(c, &adm[0], &adm[1]);
+    h.reserved = key_word(c->cfg) | (admission ? kAdmissionBit : 0);
     for (int l = 0; l < c->n_layers; l++) { h.in[l] = c->layers[l].in; h.out[l] = c->layers[l].out; }
     int rc = put(f, &h, sizeof(h)) ? 0 : 1;
     if (!rc && shard) {
@@ -388,6 +429,11 @@ int lctr_save_checkpoint(lctr_ctx* c, const char* path) {
             rc = !(put(f, &nt, sizeof(nt)) && put(f, tr.key, nt * sizeof(uint64_t)) && put(f, tr.stamp, nt * sizeof(uint64_t)));
             for (int a = 0; a < ts.n && !rc; a++) rc = !put(f, ts.p[a], nt * ts.width(a) * sizeof(float));
         }
+        if (!rc && admission) {  // key admission: min_count, log2_width, the sketch
+            std::vector<uint32_t> sketch;
+            rc = keys_admission_download(c, sketch);
+            if (!rc) rc = !(put(f, adm, sizeof(adm)) && put(f, sketch.data(), sketch.size() * sizeof(uint32_t)));
+        }
     }
     if (fclose(f) != 0) rc = 1;
     if (rc) {
@@ -411,6 +457,7 @@ int lctr_load_checkpoint(lctr_ctx* c, const char* path) {
     LCTR_CHECK(cf.s.world == c->cfg.world && cf.s.rank == c->cfg.rank,
                "checkpoint %s was written by rank %d of world %d, this context is rank %d of world %d (a save of another "
                "world loads through lctr_load_checkpoint_shards)", path, cf.s.rank, cf.s.world, c->cfg.rank, c->cfg.world);
+    if (check_admission(c, cf, false)) return 1;
     return load_shard_in_place(c, cf);
 }
 
@@ -424,6 +471,7 @@ int lctr_load_checkpoint_shards(lctr_ctx* c, int n, const char* const* paths) {
         LCTR_CHECK(paths[i], "lctr_load_checkpoint_shards: null path %d", i);
         fs[i].reset(new CkptFile());
         if (ckpt_open(c, paths[i], *fs[i])) return 1;
+        if (check_admission(c, *fs[i], true)) return 1;  // a context with admission off skips the section
     }
     std::vector<CkptFile*> by_rank(n, nullptr);  // the files in rank order: the source order of keyed rows
     for (int i = 0; i < n; i++) {

@@ -440,6 +440,12 @@ struct TierRows {
 };
 bool keys_tier(const lctr_ctx* c, TierRows* out);
 int keys_tier_restore(lctr_ctx* c, uint64_t n);
+// frequency admission (lctr_set_key_admission): the compaction of the slot after an insert-upload that dropped entries
+// (*nnz in: the entries uploaded, out: those kept); the settings (false when off) and the sketch for checkpoints
+int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, int64_t* nnz);
+bool keys_admission(const lctr_ctx* c, uint32_t* min_count, uint32_t* log2_width);
+int keys_admission_download(lctr_ctx* c, std::vector<uint32_t>& sketch);
+int keys_admission_restore(lctr_ctx* c, const uint32_t* sketch);
 // rows of the row-indexed parameter / optimizer-state transfers: F, or the capacity in keyed mode (the null row stays out)
 inline size_t api_rows(const lctr_ctx* c) { return c->keys ? c->F - 1 : c->F; }
 // global rows < rows that rank holds when global row g lives on rank g % world (at local row g / world); rank < world

@@ -67,8 +67,28 @@
 // planned on the host from that list alone (the holes below the new end, sorted, and the scan of the window
 // [n_live, n) above it), so its cost scales with the rows restored, never with the tier's size.  lctr_evict_host_tier
 // runs the whole eviction on the tier's arrays, with scratch of the tier's size allocated for the call.
+//
+// Frequency admission (lctr_set_key_admission, one GPU, FM / FFM / NFM): a new key gets a row only once it has been met
+// min_count times, counted in a count-min sketch of 4 rows of 2^w u32 counters in HBM, counter i of key x at
+//     fmix64(x ^ ((i + 1) * 0x9E3779B97F4A7C15)) >> (64 - w)
+// (the XOR keeps the cell independent of the table's low bits and the owner's top bits of fmix64(x)).  A key is present
+// when the table holds it (with a row, or without one after a capacity overflow) or the tier holds it live.  An
+// insert-upload then runs, in place of key_insert_kernel:
+//   count   key_count_kernel: every entry of a key that is not present adds 1 to its 4 counters (entries, not distinct
+//           keys, so the counts do not depend on order);
+//   admit   key_admit_kernel: keys the tier holds, and keys whose smallest counter has reached min_count, go through
+//           tile_insert (present keys find their slot and stop there); init / restore follow unchanged;
+// and key_find_kernel<0> writes kNoRow, the drop marker, for a key still absent, counting dropped entries with one
+// warp-aggregated atomic.  The host reads the count at the synchronise of read_flags.  When entries were dropped,
+// keys_admission_compact (called by the upload once row_ptr / field / val are on the device, before the slot map) closes the
+// gaps: D(i) = dropped entries below i by the eviction's count / scan / index kernels over the drop flags, then entry i
+// moves to i - D(i) in scratch (copied back into the slot) and row_ptr[r] -= D(row_ptr[r]) in place.  Rows are never
+// removed.  Counters are never cleared by eviction: an evicted key is admitted again at its next occurrence unless
+// lctr_decay_key_admission (counter >>= shift, one grid-stride launch) or a new lctr_set_key_admission lowered its count.
 #include <algorithm>
 #include <vector>
+
+#include <cooperative_groups.h>
 
 #include "keys.cuh"
 
@@ -100,6 +120,22 @@ struct HostTier {
     uint32_t* holes = nullptr;              // released rows below n_live, ascending
 };
 
+// frequency admission (lctr_set_key_admission): the sketch, the counters of the last insert-upload, compaction scratch
+constexpr int kSketchDepth = 4;
+struct Admission {
+    uint32_t* sketch = nullptr;             // [kSketchDepth << lw] counters
+    uint32_t min_count = 0, lw = 0;
+    unsigned long long* cnt = nullptr;      // [3] dropped entries, admitted keys of the current upload, scan total (device)
+    unsigned long long* h_cnt = nullptr;    // pinned mirror of [0, 2)
+    uint64_t dropped = 0, admitted = 0;     // of the last insert-upload
+    uint64_t pending = 0;                   // entries of the upload in flight that keys_admission_compact removes
+    // compaction scratch, grown on demand (per-call scratch: not counted by lctr_device_bytes)
+    size_t cap = 0;
+    uint32_t *scan = nullptr, *tiles = nullptr, *fid = nullptr;
+    uint16_t* field = nullptr;
+    float* val = nullptr;
+};
+
 struct KeyTable {
     unsigned long long* key = nullptr;      // [T] slot keys, kEmptyKey = free
     uint32_t* row = nullptr;                // [T] row of the slot's key, kNoRow when the capacity was exhausted
@@ -125,6 +161,7 @@ struct KeyTable {
     unsigned long long* ev_res = nullptr;     // [4] counters read back by the host
     unsigned long long* h_res = nullptr;      // pinned mirror
     HostTier* tier = nullptr;                 // cfg.key_host_rows > 0
+    Admission* adm = nullptr;                 // lctr_set_key_admission with min_count > 1
 };
 
 static KeyView view(const KeyTable* t) {
@@ -319,12 +356,14 @@ __global__ void __launch_bounds__(256) tier_spill_kernel(const uint32_t* __restr
 }
 
 // 3. translation: MODE 0 -> u32 row per entry into a slot (absent: the null row; kNoRow: capacity flag + null row), and
-//    with a stamp array (tracked context, insert-upload) last_seen[row] = clock;
+//    with a stamp array (tracked context, insert-upload) last_seen[row] = clock; with a drop counter (admission on,
+//    insert-upload) an absent key was not admitted: its entries get the drop marker kNoRow and are counted;
 //    MODE 1 -> int64 row per key, -1 when absent or without a row
 template <int MODE>
 __global__ void __launch_bounds__(256) key_find_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t,
                                                        uint32_t* __restrict__ fid, int64_t* __restrict__ rows, int insert,
-                                                       unsigned long long* __restrict__ last_seen, unsigned long long clock) {
+                                                       unsigned long long* __restrict__ last_seen, unsigned long long clock,
+                                                       unsigned long long* __restrict__ dropped) {
     const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
     if (i >= n) return;
     const int sub = threadIdx.x & (kGroup - 1);
@@ -333,6 +372,13 @@ __global__ void __launch_bounds__(256) key_find_kernel(const unsigned long long*
     if (sub != 0) return;
     const uint32_t r = pos >= 0 ? __ldg(t.row + pos) : kNoRow;
     if (MODE == 0) {
+        if (dropped && pos < 0) {
+            namespace cg = cooperative_groups;
+            const cg::coalesced_group g = cg::coalesced_threads();
+            if (g.thread_rank() == 0) atomicAdd(dropped, (unsigned long long)g.size());
+            fid[i] = kNoRow;
+            return;
+        }
         if (r == kNoRow && insert) t.flags[pos >= 0 ? 0 : 1] = 1u;
         // hot rows appear in many entries of a batch: entries that find the stamp already written skip the store
         if (last_seen && r != kNoRow && __ldcg(last_seen + r) != clock) last_seen[r] = clock;
@@ -360,6 +406,81 @@ __global__ void __launch_bounds__(256) key_stamp_rows_kernel(const int64_t* __re
                                                              unsigned long long* __restrict__ last_seen, unsigned long long clock) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
         last_seen[rows[i]] = clock;
+}
+
+// ---- frequency admission ----------------------------------------------------------------------------------------------
+// counter i of a key: row i of the sketch, column from the top lw bits of a hash independent of the table's
+__device__ __forceinline__ size_t sketch_cell(unsigned long long key, int i, unsigned lw) {
+    return ((size_t)i << lw) + (size_t)(fmix64(key ^ ((unsigned long long)(i + 1) * 0x9E3779B97F4A7C15ull)) >> (64 - lw));
+}
+
+// the tier holds the key live (all lanes of the tile)
+__device__ __forceinline__ bool tier_holds(const KeyView& h, unsigned long long key, int sub, unsigned gmask) {
+    const long long hp = tile_find(h, key, sub, gmask);
+    return hp >= 0 && __ldg(h.row + hp) != kNoRow;
+}
+
+// count: every entry of a key that is not present adds 1 to its kSketchDepth counters (lanes 0..3 of its tile)
+__global__ void __launch_bounds__(256) key_count_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t, KeyView h,
+                                                        int tiered, uint32_t* __restrict__ sketch, unsigned lw) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const unsigned long long key = keys[i];
+    if (tile_find(t, key, sub, gmask) >= 0) return;  // whole tiles leave together
+    if (tiered && tier_holds(h, key, sub, gmask)) return;
+    if (sub < kSketchDepth) atomicAdd(sketch + sketch_cell(key, sub, lw), 1u);
+}
+
+// admit + insert: keys the tier holds, and keys whose smallest counter reached min_count, go through tile_insert (a present
+// key finds its slot and stops there); admitted counts the slots claimed for keys the tier did not hold
+__global__ void __launch_bounds__(256) key_admit_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t, KeyView h,
+                                                        int tiered, const uint32_t* __restrict__ sketch, unsigned lw,
+                                                        unsigned min_count, unsigned long long* __restrict__ admitted) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
+    if (i >= n) return;
+    const int sub = threadIdx.x & (kGroup - 1);
+    const unsigned gmask = 0xffffu << (threadIdx.x & 16);
+    const unsigned long long key = keys[i];
+    const bool restore = tiered && tier_holds(h, key, sub, gmask);
+    if (!restore) {
+        unsigned v = sub < kSketchDepth ? __ldg(sketch + sketch_cell(key, sub, lw)) : ~0u;
+        for (int o = kGroup / 2; o; o >>= 1) v = min(v, __shfl_xor_sync(gmask, v, o));
+        if (v < min_count) return;  // whole tiles leave together
+    }
+    if (tile_insert(t, key, sub, gmask) && !restore && sub == 0) atomicAdd(admitted, 1ull);
+}
+
+// every counter >>= shift (shift in [1, 32]); n % 4 == 0
+__global__ void __launch_bounds__(256) sketch_decay_kernel(uint4* __restrict__ sketch, size_t n4, unsigned shift) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+        uint4 v = sketch[i];
+        if (shift >= 32) v = make_uint4(0u, 0u, 0u, 0u);
+        else v = make_uint4(v.x >> shift, v.y >> shift, v.z >> shift, v.w >> shift);
+        sketch[i] = v;
+    }
+}
+
+// the kept entries into their dense positions i - D(i) of the scratch arrays (field / val may be null), and
+// row_ptr[r] -= D(row_ptr[r]) in place; scan[i] = D(i), entries dropped below i, for i in [0, n]
+__global__ void __launch_bounds__(256) admit_compact_kernel(const uint32_t* __restrict__ fid, const uint16_t* __restrict__ field,
+                                                            const float* __restrict__ val, size_t n, const uint32_t* __restrict__ scan,
+                                                            int64_t* __restrict__ row_ptr, size_t rows, uint32_t* __restrict__ fid2,
+                                                            uint16_t* __restrict__ field2, float* __restrict__ val2) {
+    const size_t m = n > rows + 1 ? n : rows + 1;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (size_t)gridDim.x * blockDim.x) {
+        if (i < n) {
+            const uint32_t f = fid[i];
+            if (f != kNoRow) {
+                const size_t d = i - scan[i];
+                fid2[d] = f;
+                if (field) field2[d] = field[i];
+                if (val) val2[d] = val[i];
+            }
+        }
+        if (i <= rows) row_ptr[i] -= (int64_t)scan[row_ptr[i]];
+    }
 }
 
 // ---- eviction ----------------------------------------------------------------------------------------------------------
@@ -471,11 +592,22 @@ __device__ __forceinline__ unsigned block_scan_incl(unsigned v, unsigned* ws, un
     return out;
 }
 
-// evicted rows per tile of kEvTile rows (tiles cover [0, n])
-__global__ void __launch_bounds__(kEvTile) evict_count_kernel(const unsigned long long* __restrict__ last_seen, size_t n,
-                                                              EvictRule e, uint32_t* __restrict__ tiles) {
+// the flag the count / scan / index kernels below act on: a row the eviction rule frees, or an entry admission dropped
+struct EvictFlag {
+    const unsigned long long* last_seen;
+    EvictRule e;
+    __device__ __forceinline__ bool operator()(size_t r) const { return row_evicted(e, last_seen[r]); }
+};
+struct DropFlag {
+    const uint32_t* fid;
+    __device__ __forceinline__ bool operator()(size_t i) const { return fid[i] == kNoRow; }
+};
+
+// flagged positions per tile of kEvTile (tiles cover [0, n])
+template <class Flag>
+__global__ void __launch_bounds__(kEvTile) evict_count_kernel(Flag flag, size_t n, uint32_t* __restrict__ tiles) {
     const size_t r = (size_t)blockIdx.x * kEvTile + threadIdx.x;
-    const int cnt = __syncthreads_count(r < n && row_evicted(e, last_seen[r]));
+    const int cnt = __syncthreads_count(r < n && flag(r));
     if (threadIdx.x == 0) tiles[blockIdx.x] = (uint32_t)cnt;
 }
 
@@ -495,17 +627,17 @@ __global__ void __launch_bounds__(1024) evict_scan_tiles_kernel(uint32_t* __rest
     if (threadIdx.x == 0) res[0] = carry;
 }
 
-// E(r) for r in [0, n] and the evicted-row list ev_rows[E(r)] = r
-__global__ void __launch_bounds__(kEvTile) evict_index_kernel(const unsigned long long* __restrict__ last_seen, size_t n,
-                                                              EvictRule e, const uint32_t* __restrict__ tiles,
+// E(r) = flagged positions below r, for r in [0, n], and (ev_rows non-null) the list ev_rows[E(r)] = r of the flagged ones
+template <class Flag>
+__global__ void __launch_bounds__(kEvTile) evict_index_kernel(Flag flag, size_t n, const uint32_t* __restrict__ tiles,
                                                               uint32_t* __restrict__ scan, uint32_t* __restrict__ ev_rows) {
     __shared__ unsigned ws[32];
     const size_t r = (size_t)blockIdx.x * kEvTile + threadIdx.x;
-    const unsigned f = r < n && row_evicted(e, last_seen[r]);
+    const unsigned f = r < n && flag(r);
     unsigned tot;
     const unsigned E = tiles[blockIdx.x] + block_scan_incl(f, ws, &tot) - f;
     if (r <= n) scan[r] = E;
-    if (f) ev_rows[E] = (uint32_t)r;
+    if (f && ev_rows) ev_rows[E] = (uint32_t)r;
 }
 
 // export of the evicted rows (warp per row): key, W, V into dense device buffers, each may be null
@@ -637,12 +769,15 @@ static int init_new_rows(lctr_ctx* c, int64_t max_new) {
     return 0;
 }
 
-// the key table's flags and, on a tiered context, the tier's, with one synchronisation
-static int read_flags(lctr_ctx* c) {
+// the key table's flags and, on a tiered context, the tier's, with one synchronisation; admission: also the counters of
+// an insert-upload
+static int read_flags(lctr_ctx* c, bool admission = false) {
     KeyTable* t = c->keys;
     LCTR_CUDA(cudaMemcpyAsync(t->h_flags, t->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     if (t->tier)
         LCTR_CUDA(cudaMemcpyAsync(t->tier->h_flags, t->tier->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    if (admission)
+        LCTR_CUDA(cudaMemcpyAsync(t->adm->h_cnt, t->adm->cnt, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }
@@ -713,6 +848,16 @@ int keys_alloc(lctr_ctx* c) {
     return 0;
 }
 
+static void admission_free(KeyTable* t) {
+    Admission* a = t->adm;
+    if (!a) return;
+    cudaFree(a->sketch); cudaFree(a->cnt);
+    cudaFree(a->scan); cudaFree(a->tiles); cudaFree(a->fid); cudaFree(a->field); cudaFree(a->val);
+    if (a->h_cnt) cudaFreeHost(a->h_cnt);
+    delete a;
+    t->adm = nullptr;
+}
+
 static void tier_free(HostTier* h) {
     cudaFree(h->key); cudaFree(h->row); cudaFree(h->flags);
     cudaFree(h->rel); cudaFree(h->wscan); cudaFree(h->holes);
@@ -727,6 +872,7 @@ void keys_free(lctr_ctx* c) {
     KeyTable* t = c->keys;
     if (!t) return;
     if (t->tier) tier_free(t->tier);
+    admission_free(t);
     cudaFree(t->key); cudaFree(t->row); cudaFree(t->row_key); cudaFree(t->count); cudaFree(t->flags);
     cudaFree(t->new_rows); cudaFree(t->d_keys); cudaFree(t->d_rows);
     cudaFree(t->last_seen); cudaFree(t->ev_scan); cudaFree(t->ev_rows); cudaFree(t->ev_tiles); cudaFree(t->ev_hist);
@@ -765,7 +911,8 @@ size_t keys_bytes(const lctr_ctx* c) {
     if (!t) return 0;
     return t->T * (sizeof(unsigned long long) + sizeof(uint32_t)) + t->cap * sizeof(unsigned long long) +
            (t->last_seen ? t->cap * sizeof(unsigned long long) : 0) +
-           (t->tier ? t->tier->T * (sizeof(unsigned long long) + sizeof(uint32_t)) : 0);
+           (t->tier ? t->tier->T * (sizeof(unsigned long long) + sizeof(uint32_t)) : 0) +
+           (t->adm ? ((size_t)kSketchDepth << t->adm->lw) * sizeof(uint32_t) : 0);
 }
 
 #define LCTR_LAUNCHED()                  \
@@ -851,19 +998,34 @@ static int tier_compact(lctr_ctx* c) {
 
 // keys of one upload -> rows in fid (device, n entries); insert: create and initialise rows for new keys first.  Tiered:
 // new keys the tier holds are restored from it; insert = 0 gives rows to the keys the tier holds, and to no other.
+// Admission on, insert = 1: count + admit replace the insert, entries of keys not admitted get the drop marker, and the
+// dropped count is left for keys_admission_compact.
 int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid) {
     KeyTable* t = c->keys;
+    Admission* adm = insert ? t->adm : nullptr;
     if (insert) t->clock++;  // the clock counts insert-uploads, empty ones included
+    if (t->adm) t->adm->pending = 0;
+    if (adm) adm->dropped = adm->admitted = 0;
     if (n == 0) return 0;
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, h_keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
     LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    if (adm) LCTR_CUDA(cudaMemsetAsync(adm->cnt, 0, 2 * sizeof(unsigned long long), c->stream));
     const bool restoring = tier_live(t);
     {
         ProfScope prof(c, PROF_KEYS);
         if (insert || restoring) {
-            if (insert) key_insert_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t));
-            else key_lookup_restore_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), view(t->tier));
+            if (adm) {
+                const KeyView hv = restoring ? view(t->tier) : KeyView{};
+                key_count_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), hv, restoring, adm->sketch, adm->lw);
+                LCTR_LAUNCHED();
+                key_admit_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), hv, restoring, adm->sketch, adm->lw,
+                                                                      adm->min_count, adm->cnt + 1);
+            } else if (insert) {
+                key_insert_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t));
+            } else {
+                key_lookup_restore_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), view(t->tier));
+            }
             c->launches++;
             LCTR_CUDA(cudaGetLastError());
             if (init_new_rows(c, std::min<int64_t>(n, (int64_t)t->cap))) return 1;
@@ -874,11 +1036,16 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
             }
         }
         key_find_kernel<0><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0,
-                                                                insert ? t->last_seen : nullptr, t->clock);
+                                                                insert ? t->last_seen : nullptr, t->clock,
+                                                                adm ? adm->cnt : nullptr);
         c->launches++;
         LCTR_CUDA(cudaGetLastError());
     }
-    if (read_flags(c)) return 1;
+    if (read_flags(c, adm != nullptr)) return 1;
+    if (adm) {
+        adm->dropped = adm->pending = adm->h_cnt[0];
+        adm->admitted = adm->h_cnt[1];
+    }
     if (restoring && tier_compact(c)) return 1;  // before any failure below: restored rows have left the tier either way
     LCTR_CHECK(!t->h_flags[1], "key table: no free slot on a probe path (%zu slots for capacity %zu)", t->T, t->cap);
     LCTR_CHECK(!t->h_flags[0], "key table: capacity of %zu rows (cfg.feature_cnt) exhausted; the batch's new keys do not fit",
@@ -886,11 +1053,56 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
     return 0;
 }
 
+// after keys_translate dropped entries of the slot's batch (row_ptr, fid, field, val on the device): the kept entries in
+// order, the new row_ptr, *nnz = the kept count.  Nothing runs when no entry was dropped.
+int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, int64_t* nnz) {
+    Admission* a = c->keys ? c->keys->adm : nullptr;
+    if (!a || !a->pending) return 0;
+    const size_t n = (size_t)*nnz, kept = n - a->pending;
+    a->pending = 0;
+    if (n > a->cap) {
+        LCTR_CUDA(cudaStreamSynchronize(st));
+        const size_t cap = std::max(n, a->cap + a->cap / 2);
+        cudaFree(a->scan); cudaFree(a->tiles); cudaFree(a->fid); cudaFree(a->field); cudaFree(a->val);
+        a->scan = a->tiles = a->fid = nullptr; a->field = nullptr; a->val = nullptr; a->cap = 0;
+        LCTR_CUDA(cudaMalloc((void**)&a->scan, (cap + 1) * sizeof(uint32_t)));
+        LCTR_CUDA(cudaMalloc((void**)&a->tiles, (cap / kEvTile + 1) * sizeof(uint32_t)));
+        LCTR_CUDA(cudaMalloc((void**)&a->fid, cap * sizeof(uint32_t)));
+        LCTR_CUDA(cudaMalloc((void**)&a->field, cap * sizeof(uint16_t)));
+        LCTR_CUDA(cudaMalloc((void**)&a->val, cap * sizeof(float)));
+        a->cap = cap;
+    }
+    const uint16_t* field = s.has_field ? s.field : nullptr;
+    const float* val = s.has_val ? s.val : nullptr;
+    {
+        ProfScope prof(c, PROF_KEYS);
+        const size_t ntiles = n / kEvTile + 1;  // tiles cover [0, n]: D(n) is read for row_ptr[rows] = n
+        evict_count_kernel<<<(unsigned)ntiles, kEvTile, 0, st>>>(DropFlag{s.fid}, n, a->tiles);
+        LCTR_LAUNCHED();
+        evict_scan_tiles_kernel<<<1, 1024, 0, st>>>(a->tiles, ntiles, a->cnt + 2);
+        LCTR_LAUNCHED();
+        evict_index_kernel<<<(unsigned)ntiles, kEvTile, 0, st>>>(DropFlag{s.fid}, n, a->tiles, a->scan, nullptr);
+        LCTR_LAUNCHED();
+        const size_t m = std::max(n, (size_t)rows + 1);
+        const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 255) / 256, (size_t)c->sm_count * 8));
+        admit_compact_kernel<<<grid, 256, 0, st>>>(s.fid, field, val, n, a->scan, s.row_ptr, (size_t)rows, a->fid,
+                                                   field ? a->field : nullptr, val ? a->val : nullptr);
+        LCTR_LAUNCHED();
+    }
+    if (kept) {
+        LCTR_CUDA(cudaMemcpyAsync(s.fid, a->fid, kept * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+        if (field) LCTR_CUDA(cudaMemcpyAsync(s.field, a->field, kept * sizeof(uint16_t), cudaMemcpyDeviceToDevice, st));
+        if (val) LCTR_CUDA(cudaMemcpyAsync(s.val, a->val, kept * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    }
+    *nnz = (int64_t)kept;
+    return 0;
+}
+
 static int lookup_dev(lctr_ctx* c, const uint64_t* keys, int64_t n) {
     KeyTable* t = c->keys;
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
-    key_find_kernel<1><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), nullptr, t->d_rows, 0, nullptr, 0);
+    key_find_kernel<1><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), nullptr, t->d_rows, 0, nullptr, 0, nullptr);
     c->launches++;
     LCTR_CUDA(cudaGetLastError());
     return 0;
@@ -1018,7 +1230,7 @@ static int evict_plan(lctr_ctx* c, const EvTable& tb, uint64_t max_idle, uint64_
     }
     // count and scan
     const size_t ntiles = n / kEvTile + 1;  // tiles cover [0, n]: E(n) is needed too
-    evict_count_kernel<<<(unsigned)ntiles, kEvTile, 0, c->stream>>>(tb.a.last_seen, n, *e, tb.tiles);
+    evict_count_kernel<<<(unsigned)ntiles, kEvTile, 0, c->stream>>>(EvictFlag{tb.a.last_seen, *e}, n, tb.tiles);
     LCTR_LAUNCHED();
     evict_scan_tiles_kernel<<<1, 1024, 0, c->stream>>>(tb.tiles, ntiles, t->ev_res);
     LCTR_LAUNCHED();
@@ -1030,7 +1242,8 @@ static int evict_plan(lctr_ctx* c, const EvTable& tb, uint64_t max_idle, uint64_
 // E(r) and the list of the m rows that leave, then their key, W and V into the caller's buffers (each may be null)
 static int evict_index_export(lctr_ctx* c, const EvTable& tb, const EvictRule& e, size_t m, uint64_t* keys_out, float* W_out,
                               float* V_out) {
-    evict_index_kernel<<<(unsigned)(tb.n / kEvTile + 1), kEvTile, 0, c->stream>>>(tb.a.last_seen, tb.n, e, tb.tiles, tb.scan, tb.rows);
+    evict_index_kernel<<<(unsigned)(tb.n / kEvTile + 1), kEvTile, 0, c->stream>>>(EvictFlag{tb.a.last_seen, e}, tb.n, tb.tiles,
+                                                                                  tb.scan, tb.rows);
     LCTR_LAUNCHED();
     if (!(keys_out || W_out || V_out)) return 0;
     const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
@@ -1052,6 +1265,29 @@ static int evict_index_export(lctr_ctx* c, const EvTable& tb, const EvictRule& e
     cudaFree(dK); cudaFree(dW); cudaFree(dV);
     LCTR_CUDA(err);
     LCTR_CUDA(es);
+    return 0;
+}
+
+bool keys_admission(const lctr_ctx* c, uint32_t* min_count, uint32_t* log2_width) {
+    const Admission* a = c->keys ? c->keys->adm : nullptr;
+    *min_count = a ? a->min_count : 0;
+    *log2_width = a ? a->lw : 0;
+    return a != nullptr;
+}
+
+int keys_admission_download(lctr_ctx* c, std::vector<uint32_t>& sketch) {
+    const Admission* a = c->keys->adm;
+    sketch.resize((size_t)kSketchDepth << a->lw);
+    LCTR_CUDA(cudaMemcpyAsync(sketch.data(), a->sketch, sketch.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int keys_admission_restore(lctr_ctx* c, const uint32_t* sketch) {
+    Admission* a = c->keys->adm;
+    LCTR_CUDA(cudaMemcpyAsync(a->sketch, sketch, ((size_t)kSketchDepth << a->lw) * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    a->dropped = a->admitted = a->pending = 0;
     return 0;
 }
 
@@ -1212,6 +1448,66 @@ int lctr_set_key_init(lctr_ctx* c, uint64_t seed, float scale) {
     LCTR_CHECK(c->keys, "lctr_set_key_init: the context was not created with key_mode = LCTR_KEYS_HASHED");
     c->keys->seed = seed;
     c->keys->scale = scale;
+    return 0;
+}
+
+int lctr_set_key_admission(lctr_ctx* c, uint32_t min_count, uint32_t log2_width) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(c->keys, "lctr_set_key_admission: the context was not created with key_mode = LCTR_KEYS_HASHED (a dense context "
+                        "has no keys to admit)");
+    LCTR_CHECK(c->cfg.world <= 1, "lctr_set_key_admission: world = %d: admission is single-GPU (the requester's slot map is "
+                                  "built before the owners translate, so it cannot drop entries)", c->cfg.world);
+    LCTR_CHECK(c->cfg.model != LCTR_MODEL_WND, "lctr_set_key_admission: Wide&Deep reads the first id of each field, and dropping "
+                                               "entries would change which id that is");
+    KeyTable* t = c->keys;
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    if (min_count <= 1) {  // off: the context behaves and launches as one that never set it
+        admission_free(t);
+        return 0;
+    }
+    LCTR_CHECK(log2_width >= 10 && log2_width <= 28, "lctr_set_key_admission: log2_width = %u outside [10, 28]", log2_width);
+    if (!t->adm || t->adm->lw != log2_width) {
+        admission_free(t);
+        Admission* a = new Admission();
+        t->adm = a;
+        a->lw = log2_width;
+        const cudaError_t e1 = cudaMalloc((void**)&a->sketch, ((size_t)kSketchDepth << log2_width) * sizeof(uint32_t));
+        const cudaError_t e2 = cudaMalloc((void**)&a->cnt, 3 * sizeof(unsigned long long));
+        const cudaError_t e3 = cudaMallocHost((void**)&a->h_cnt, 2 * sizeof(unsigned long long));
+        if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess) {
+            admission_free(t);
+            LCTR_CHECK(false, "lctr_set_key_admission: cannot allocate a sketch of %llu bytes (admission is off)",
+                       (unsigned long long)(((size_t)kSketchDepth << log2_width) * sizeof(uint32_t)));
+        }
+    }
+    Admission* a = t->adm;
+    a->min_count = min_count;
+    a->dropped = a->admitted = a->pending = 0;
+    LCTR_CUDA(cudaMemsetAsync(a->sketch, 0, ((size_t)kSketchDepth << a->lw) * sizeof(uint32_t), c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int lctr_decay_key_admission(lctr_ctx* c, uint32_t shift) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(c->keys && c->keys->adm, "lctr_decay_key_admission: admission is off (lctr_set_key_admission with min_count > 1 "
+                                        "turns it on)");
+    LCTR_CHECK(shift >= 1 && shift <= 32, "lctr_decay_key_admission: shift = %u outside [1, 32]", shift);
+    const Admission* a = c->keys->adm;
+    const size_t n4 = ((size_t)kSketchDepth << a->lw) / 4;
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n4 + 255) / 256, (size_t)c->sm_count * 8));
+    sketch_decay_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<uint4*>(a->sketch), n4, shift);
+    LCTR_LAUNCHED();
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int lctr_key_admission_stats(lctr_ctx* c, uint64_t* dropped_entries, uint64_t* admitted_keys) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(c->keys, "lctr_key_admission_stats: the context was not created with key_mode = LCTR_KEYS_HASHED");
+    const Admission* a = c->keys->adm;
+    if (dropped_entries) *dropped_entries = a ? a->dropped : 0;
+    if (admitted_keys) *admitted_keys = a ? a->admitted : 0;
     return 0;
 }
 

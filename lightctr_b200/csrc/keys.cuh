@@ -73,12 +73,13 @@ __device__ __forceinline__ long long tile_find(const KeyView& t, unsigned long l
 // one key of an insert (a whole 16-lane tile calls it): a tile that finds no match claims the first empty slot of the
 // group; the winner takes a row from the counter and records it in the list of new rows, or stores kNoRow and raises the
 // capacity flag when the counter has passed the capacity.  flags: [0] capacity exhausted, [1] table full, [2] new rows.
-__device__ __forceinline__ void tile_insert(const KeyView& t, unsigned long long key, int sub, unsigned gmask) {
+// Returns whether this tile claimed the key's slot (all lanes).
+__device__ __forceinline__ bool tile_insert(const KeyView& t, unsigned long long key, int sub, unsigned gmask) {
     bool claimed;
     const long long pos = tile_claim(t, key, sub, gmask, &claimed);
-    if (sub != 0) return;
-    if (pos < 0) { t.flags[1] = 1u; return; }
-    if (!claimed) return;
+    if (sub != 0) return claimed;
+    if (pos < 0) { t.flags[1] = 1u; return false; }
+    if (!claimed) return false;
     const unsigned long long r = atomicAdd(t.count, 1ull);
     if (r < t.cap) {
         t.row[pos] = (uint32_t)r;
@@ -88,6 +89,7 @@ __device__ __forceinline__ void tile_insert(const KeyView& t, unsigned long long
         t.row[pos] = kNoRow;
         t.flags[0] = 1u;
     }
+    return true;
 }
 
 // host side of keys.cu used by dist.cu: the context's key table as a view, room for `n` new rows in its scratch, and the

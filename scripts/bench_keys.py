@@ -2,7 +2,7 @@
 """Keyed mode against dense mode on one GPU: the same workload and batches, ids fed as 64-bit keys fmix64(fid) into a keyed
 context of capacity F (cfg.key_mode = LCTR_KEYS_HASHED), alternated with the dense context in one process.
 
-    python scripts/bench_keys.py [--workload fm_c2|ffm_c3|nfm_c4] [--steps K] [--warmup W] [--rounds R] [--evict]
+    python scripts/bench_keys.py [--workload fm_c2|ffm_c3|nfm_c4] [--steps K] [--warmup W] [--rounds R] [--evict | --admit]
 
 Prints ONE JSON line:
   keyed_ms_per_step / dense_ms_per_step   device-timed step (one CUDA-event pair per step, L2 flushed before each step,
@@ -22,6 +22,15 @@ instead holds, per round:
                                           table of 1M rows whose ages are spread uniformly over 0..99, evicting 10 %, 25 %
                                           and 50 % of them through max_rows, with and without export of keys, W and V;
   rows_moved                              survivors renumbered by each of those calls.
+With --admit (frequency admission, lctr_set_key_admission; workload fm_c2, capacity 1M, sketch 4 x 2^22) the line holds,
+for admission off and at min_count 2 and 4, contexts alternated within each round:
+  translate_us_per_batch                  device time of the upload-side key launches (count, admit, init, translate and
+                                          the compaction of dropped entries) per batch, over a first and a second pass of
+                                          the same batches ("pass1", "pass2");
+  upload_ms_per_batch                     host clock around lctr_upload_batch_keys (it ends in a stream synchronise);
+  rows_created                            rows held after each pass (exact), and "model": the same counts from a numpy
+                                          restatement of the sketch and the admission rule;
+  dropped_entries                         entries dropped over each pass.
 Writes nothing to the tree (the full table is restored from a checkpoint in a temporary directory).
 """
 import argparse
@@ -192,6 +201,85 @@ def main_evict(args):
     return 0
 
 
+ADMIT_LW = 22
+
+
+def admit_model(key_batches, passes, min_count, lw=ADMIT_LW):
+    """rows held after each pass of the stream: numpy restatement of the sketch (include/lightctr_b200.h) and the rule"""
+    gold = 0x9E3779B97F4A7C15
+
+    def cells(keys):
+        return [(fmix64(keys ^ np.uint64(((i + 1) * gold) % (1 << 64))) >> np.uint64(64 - lw)).astype(np.int64) for i in range(4)]
+
+    sk = np.zeros((4, 1 << lw), np.int64)
+    present = np.zeros(0, np.uint64)
+    out = []
+    for _ in range(passes):
+        for keys in key_batches:
+            absent = keys[~np.isin(keys, present)]
+            for i, c in enumerate(cells(absent)):
+                sk[i] += np.bincount(c, minlength=1 << lw)
+            new = np.unique(absent)
+            cnt = np.min(np.stack([sk[i][c] for i, c in enumerate(cells(new))]), axis=0) if len(new) else np.zeros(0)
+            present = np.union1d(present, new[cnt >= min_count])
+        out.append(int(len(present)))
+    return out
+
+
+def admit_run(wl, batches, keys, min_count):
+    from lightctr_b200 import capi
+    ctx = capi.Context(capi.MODEL_FM, wl["F"], wl["k"], optimizer=capi.OPT_ADAGRAD, max_nnz=wl["batch"] * 100,
+                       key_mode=capi.KEYS_HASHED)
+    ctx.set_key_init(1234, float(1.0 / np.sqrt(wl["k"])))
+    ctx.set_key_admission(min_count, ADMIT_LW)
+    out = {"translate_us_per_batch": {}, "upload_ms_per_batch": {}, "rows_created": [], "dropped_entries": []}
+    ctx.profile(True)
+    for p in ("pass1", "pass2"):
+        dev, host, dropped = [], [], 0
+        for i, (rp, fid, fld, lab) in enumerate(batches):
+            ctx.profile_read(reset=True)
+            t0 = time.perf_counter()
+            rc = ctx.L.lctr_upload_batch_keys(ctx.h, i, len(rp) - 1, len(keys[i]), rp.ctypes.data, keys[i].ctypes.data, None,
+                                              None, lab.ctypes.data, 1)
+            host.append(1e3 * (time.perf_counter() - t0))
+            if rc:
+                raise RuntimeError(capi.load_library().lctr_last_error().decode())
+            dev.append(1e3 * ctx.profile_read(reset=True)["keys_translate"][0])
+            dropped += ctx.key_admission_stats()[0]
+        out["translate_us_per_batch"][p] = float(np.mean(dev))
+        out["upload_ms_per_batch"][p] = float(np.mean(host))
+        out["rows_created"].append(int(len(ctx.download_keys())))
+        out["dropped_entries"].append(int(dropped))
+    ctx.profile(False)
+    ctx.close()
+    return out
+
+
+def main_admit(args):
+    wl = dict(WORKLOADS["fm_c2"])
+    batches = make_batches(wl, wl.get("nb", 8))
+    batches = [(np.ascontiguousarray(rp, np.int64), fid, fld, np.ascontiguousarray(lab, np.int32)) for rp, fid, fld, lab in batches]
+    keys = [fmix64(b[1]) for b in batches]
+    line = {"workload": wl["desc"] + ", keyed capacity 1M", "keys": "key = fmix64(fid)", "gpu": gpu_info(),
+            "sketch": "4 x 2^%d u32" % ADMIT_LW, "batches": len(batches), "entries": int(sum(len(k) for k in keys)),
+            "min_count": {}}
+    names = [1, 2, 4]
+    for r in range(args.rounds):
+        for mc in (names if r % 2 == 0 else names[::-1]):
+            o = admit_run(wl, batches, keys, mc)
+            d = line["min_count"].setdefault(str(mc), {"translate_us_per_batch": {"pass1": [], "pass2": []},
+                                                       "upload_ms_per_batch": {"pass1": [], "pass2": []}})
+            for p in ("pass1", "pass2"):
+                d["translate_us_per_batch"][p].append(o["translate_us_per_batch"][p])
+                d["upload_ms_per_batch"][p].append(o["upload_ms_per_batch"][p])
+            d["rows_created"], d["dropped_entries"] = o["rows_created"], o["dropped_entries"]
+    for mc in names:
+        line["min_count"][str(mc)]["rows_created"] = {"gpu": line["min_count"][str(mc)]["rows_created"],
+                                                      "model": admit_model(keys, 2, mc)}
+    print(json.dumps(line))
+    return 0
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="fm_c2", choices=["fm_c2", "ffm_c3", "nfm_c4"])
@@ -199,6 +287,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=2, help="dense / keyed alternations")
     ap.add_argument("--evict", action="store_true", help="row eviction (key_evict) instead: see the module docstring")
+    ap.add_argument("--admit", action="store_true", help="frequency admission instead: see the module docstring")
     args = ap.parse_args()
     import torch
     from lightctr_b200 import build as lbuild
@@ -207,6 +296,8 @@ def main():
         raise SystemExit("bench_keys.py: no CUDA device (the product has no CPU path)")
     if args.evict:
         return main_evict(args)
+    if args.admit:
+        return main_admit(args)
     wl = dict(WORKLOADS[args.workload])
     batches = make_batches(wl, wl.get("nb", 8))
     line = {"workload": wl["desc"], "keys": "key = fmix64(fid), keyed context of capacity F", "gpu": gpu_info(),
