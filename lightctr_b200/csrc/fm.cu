@@ -285,7 +285,7 @@ fm_forward_coalesced_kernel(const int64_t* __restrict__ row_ptr, const uint32_t*
                             const int64_t* __restrict__ hdr, const float* __restrict__ quirk_sumvx, int64_t quirk_rows) {
     static_assert(K % 8 == 0 && K <= 32, "coalesced forward: K in {8, 16, 24, 32}");
     const int64_t re = hdr ? hdr[0] : re_arg;
-    constexpr int LPR = K / 4 >= 8 ? 8 : (K / 4 >= 4 ? 4 : 2);  // lanes per row (power of two >= K/4 for K=24 -> 8)
+    constexpr int LPR = K / 4 > 4 ? 8 : K / 4;  // lanes per row: K/4, or 8 for K=24 (power of two >= K/4)
     constexpr int G = 32 / LPR;         // rows per gather instruction
     constexpr int NB = 64;              // features per pass
     constexpr int NIT = NB / G;         // gather iterations per pass
@@ -410,10 +410,17 @@ static int fwd_go(lctr_ctx* c, Slot& s, bool nfm, int64_t rb, int64_t re, double
     const int wpb = co ? 4 : 8;
     const unsigned grid = (unsigned)((re - rb + wpb - 1) / wpb);
     const size_t smem = co ? (size_t)wpb * (K + 2) * 68 * sizeof(float) : (size_t)wpb * 64 * (K + 4) * sizeof(float);
+    // past 48 KB of static + dynamic shared memory a launch needs the opt-in; the FM kernels' static part is publish_stats's
+    // scratch (K = 20: 48 KB of tile + that scratch).  `co` is fixed per process, so each site sees one kernel.
 #define FWD_GO(HV, NF)                                                                                         \
     do {                                                                                                       \
         auto kern = co ? fm_forward_coalesced_kernel<kCoalesced ? K : 8, HV, NF> : fm_forward_kernel<K, HV, NF>; \
-        if (smem > 48 * 1024) LCTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        static const size_t static_smem = [&] {                                                                \
+            cudaFuncAttributes a;                                                                              \
+            return cudaFuncGetAttributes(&a, kern) == cudaSuccess ? a.sharedSizeBytes : (size_t)48 * 1024;     \
+        }();                                                                                                   \
+        if (smem + static_smem > 48 * 1024)                                                                    \
+            LCTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));     \
         kern<<<grid, wpb * 32, smem, c->stream>>>(s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val, s.label, c->cW, c->cV, s.pred, s.sumvx, c->z, \
                                              s.wide, rb, re, c->stat_partial, c->stat_done, out_slot, stats, hdr,   \
                                              c->fwd_quirk_sumvx, c->fwd_quirk_rows);                               \
