@@ -19,19 +19,6 @@ void set_error(const char* fmt, ...) {
     g_err = buf;
 }
 
-template <typename T>
-static int dalloc(T** p, size_t n) {
-    *p = nullptr;
-    if (n == 0) return 0;
-    LCTR_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
-    return 0;
-}
-template <typename T>
-static void dfree(T*& p) {
-    if (p) cudaFree(p);
-    p = nullptr;
-}
-
 static int slot_reserve(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz) {
     const size_t k = c->cfg.factor_cnt;
     if (rows > s.cap_rows) {
@@ -543,6 +530,20 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
     return 0;
 }
 
+// the CSR structure of an upload (`who` prefixes the messages): row_ptr from 0 to nnz, never decreasing, and the fields
+// below field_cnt where the model reads them
+static int check_csr(const lctr_ctx* c, const char* who, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint16_t* field) {
+    LCTR_CHECK(row_ptr[0] == 0 && row_ptr[rows] == nnz, "%s: row_ptr must run from 0 to nnz (%lld .. %lld, nnz %lld)", who,
+               (long long)row_ptr[0], (long long)row_ptr[rows], (long long)nnz);
+    for (int64_t r = 0; r < rows; r++)
+        LCTR_CHECK(row_ptr[r] <= row_ptr[r + 1], "%s: row_ptr decreases at row %lld", who, (long long)r);
+    if ((c->cfg.model == LCTR_MODEL_FFM || c->cfg.model == LCTR_MODEL_WND) && field)
+        for (int64_t i = 0; i < nnz; i++)
+            LCTR_CHECK(field[i] < c->cfg.field_cnt, "%s: field %u at entry %lld >= field_cnt %u", who, (unsigned)field[i],
+                       (long long)i, c->cfg.field_cnt);
+    return 0;
+}
+
 int lctr_upload_batch(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
                       const uint16_t* field, const float* val, const int32_t* label) {
     LCTR_CHECK(c, "null ctx");
@@ -551,16 +552,9 @@ int lctr_upload_batch(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const in
     // address inside a gather (the reference indexes W / V unchecked too, fm_algo_abst.h:146-151, but there feature_cnt
     // is derived from the same file).  The streamed entry points (lctr_train_batch[_async]) trust their caller.
     LCTR_CHECK(rows >= 0 && nnz >= 0 && row_ptr && (nnz == 0 || fid), "upload_batch: null input");
-    LCTR_CHECK(row_ptr[0] == 0 && row_ptr[rows] == nnz, "upload_batch: row_ptr must run from 0 to nnz (%lld .. %lld, nnz %lld)",
-               (long long)row_ptr[0], (long long)row_ptr[rows], (long long)nnz);
-    for (int64_t r = 0; r < rows; r++)
-        LCTR_CHECK(row_ptr[r] <= row_ptr[r + 1], "upload_batch: row_ptr decreases at row %lld", (long long)r);
+    if (check_csr(c, "upload_batch", rows, nnz, row_ptr, field)) return 1;
     for (int64_t i = 0; i < nnz; i++)
         LCTR_CHECK(fid[i] < c->F, "upload_batch: fid %u at entry %lld >= feature_cnt %zu", fid[i], (long long)i, c->F);
-    if ((c->cfg.model == LCTR_MODEL_FFM || c->cfg.model == LCTR_MODEL_WND) && field)
-        for (int64_t i = 0; i < nnz; i++)
-            LCTR_CHECK(field[i] < c->cfg.field_cnt, "upload_batch: field %u at entry %lld >= field_cnt %u", (unsigned)field[i],
-                       (long long)i, c->cfg.field_cnt);
     return upload_batch_on(c, c->stream, slot, rows, nnz, row_ptr, fid, field, val, label);
 }
 
@@ -568,17 +562,8 @@ int lctr_upload_batch(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, const in
 static int check_batch_keys(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint64_t* key,
                             const uint16_t* field, const int32_t* label) {
     LCTR_CHECK(rows >= 0 && nnz >= 0 && row_ptr && (nnz == 0 || key) && (rows == 0 || label), "upload_batch_keys: null input");
-    LCTR_CHECK(row_ptr[0] == 0 && row_ptr[rows] == nnz, "upload_batch_keys: row_ptr must run from 0 to nnz (%lld .. %lld, nnz %lld)",
-               (long long)row_ptr[0], (long long)row_ptr[rows], (long long)nnz);
-    for (int64_t r = 0; r < rows; r++)
-        LCTR_CHECK(row_ptr[r] <= row_ptr[r + 1], "upload_batch_keys: row_ptr decreases at row %lld", (long long)r);
-    for (int64_t i = 0; i < nnz; i++)
-        LCTR_CHECK(key[i] != ~0ull, "upload_batch_keys: key %llu at entry %lld is reserved (the empty marker of the key table)",
-                   (unsigned long long)key[i], (long long)i);
-    if ((c->cfg.model == LCTR_MODEL_FFM || c->cfg.model == LCTR_MODEL_WND) && field)
-        for (int64_t i = 0; i < nnz; i++)
-            LCTR_CHECK(field[i] < c->cfg.field_cnt, "upload_batch_keys: field %u at entry %lld >= field_cnt %u", (unsigned)field[i],
-                       (long long)i, c->cfg.field_cnt);
+    if (check_csr(c, "upload_batch_keys", rows, nnz, row_ptr, field)) return 1;
+    if (check_keys_reserved(key, nnz, "upload_batch_keys")) return 1;
     LCTR_CHECK((c->cfg.model != LCTR_MODEL_FFM && c->cfg.model != LCTR_MODEL_WND) || field || nnz == 0,
                "upload_batch_keys: FFM / Wide&Deep need the field array");
     return 0;

@@ -30,6 +30,20 @@ void set_error(const char* fmt, ...);
         }                                      \
     } while (0)
 
+// device array of n elements (n == 0: nullptr); dfree frees and clears a pointer, null or not
+template <typename T>
+inline int dalloc(T** p, size_t n) {
+    *p = nullptr;
+    if (n == 0) return 0;
+    LCTR_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
+    return 0;
+}
+template <typename T>
+inline void dfree(T*& p) {
+    if (p) cudaFree(p);
+    p = nullptr;
+}
+
 constexpr int kNumSlots = 8;
 constexpr int kPipe = LCTR_PIPE_DEPTH;  // streamed pipeline: batches in flight (the last kPipe slots are its buffers)
 constexpr int kNumProf = 17;  // per-kernel timing buckets
@@ -425,6 +439,8 @@ int keys_alloc(lctr_ctx* c);
 void keys_free(lctr_ctx* c);
 size_t keys_bytes(const lctr_ctx* c);
 int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid);
+// fails naming `who` when one of the n keys is ~0, the empty marker of the key table
+int check_keys_reserved(const uint64_t* keys, int64_t n, const char* who);
 int keys_restore(lctr_ctx* c, const uint64_t* row_key, uint64_t n);
 int keys_download(lctr_ctx* c, std::vector<uint64_t>& out);
 // key_evict = 1: the upload clock and the stamps of rows [0, n) (checkpoints)

@@ -969,7 +969,7 @@ int dist_keys_translate(lctr_ctx* c, int slot) {
     d->posted = false;
     d->xseq++;
     KeyView t = keys_view(c);
-    if (keys_reserve_new_rows(c, std::min(d->rows_x, keys_capacity(c)))) return 1;
+    if (scratch_reserve(c, std::min(d->rows_x, keys_capacity(c)))) return 1;
     t = keys_view(c);  // the scratch may have moved
     LCTR_CUDA(cudaMemsetAsync(t.flags, 0, 3 * sizeof(unsigned int), c->stream));
     const unsigned tg = (unsigned)std::max<int64_t>(1, std::min<int64_t>(((int64_t)d->rows_x * kGroup + 255) / 256,
@@ -980,7 +980,7 @@ int dist_keys_translate(lctr_ctx* c, int slot) {
         xlate_keys_kernel<0><<<tg, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, d->xstat, t);
         c->launches += 2;
         LCTR_CUDA(cudaGetLastError());
-        if (keys_init_new_rows(c, (int64_t)std::min(d->rows_x, keys_capacity(c)))) return 1;
+        if (init_new_rows(c, (int64_t)std::min(d->rows_x, keys_capacity(c)))) return 1;
         xlate_keys_kernel<1><<<tg, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, d->xstat, t);
         xlate_finish_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, d->xseq, d->xstat, t.flags, d->xres);
         c->launches += 2;

@@ -16,8 +16,8 @@
 //      winner takes a row from an atomicAdd counter and records it in the list of new rows.  A key met again in the same
 //      batch finds the claimed slot with a plain load once the CAS has landed, so batch-local duplicates cost atomics only
 //      while their first claim is in flight, and keys already in the table cost none.
-//   2. key_init_kernel: one warp per new row (FFM rows are Fc * k floats) writes W = 0, V, and the optimizer state
-//      lctr_create gives (s1 = initial_s1, s2 = 0).
+//   2. key_init_kernel<TIERED = false>: one warp per new row (FFM rows are Fc * k floats) writes W = 0, V, and the
+//      optimizer state lctr_create gives (s1 = initial_s1, s2 = 0).
 //   3. key_find_kernel: the translated row of every entry into the slot's fid array -- a second launch, so no tile ever
 //      waits on another tile's row inside a kernel.
 // Lookup-only uploads (insert = 0) run step 3 alone: absent keys map to the null row (index capacity), all zeros and
@@ -62,8 +62,8 @@
 //
 // Host tier (cfg.key_host_rows > 0, HostTier below): the evicted rows are first appended to the tier (tier_spill_kernel,
 // after the export, before the move).  Uploads give a device row to a key the tier holds as to a new key (insert = 0:
-// key_lookup_restore_kernel, for tier keys only); key_restore_init_kernel then copies its row back in place of the lazy
-// init and lists the tier row it released, and tier_compact closes the holes with evict_move_kernel.  The compaction is
+// key_lookup_restore_kernel, for tier keys only); key_init_kernel<TIERED = true> then copies its row back in place of the
+// lazy init and lists the tier row it released, and tier_compact closes the holes with evict_move_kernel.  The compaction is
 // planned on the host from that list alone (the holes below the new end, sorted, and the scan of the window
 // [n_live, n) above it), so its cost scales with the rows restored, never with the tier's size.  lctr_evict_host_tier
 // runs the whole eviction on the tier's arrays, with scratch of the tier's size allocated for the call.
@@ -97,23 +97,72 @@ namespace lctr {
 constexpr int kEvTile = 1024;  // rows per block of the eviction count / index kernels
 constexpr int kEvBins = 1 << 16;  // radix-select digit
 
+#define LCTR_LAUNCHED()                  \
+    do {                                 \
+        c->launches++;                   \
+        LCTR_CUDA(cudaGetLastError());   \
+    } while (0)
+
+// grid of a warp-per-item kernel over m items (8 warps a block), and of a grid-stride kernel of one thread per item
+static unsigned warp_grid(const lctr_ctx* c, size_t m) {
+    return (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
+}
+static unsigned stride_grid(const lctr_ctx* c, size_t n) {
+    return (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
+}
+// the instance of a row kernel for the context's rows: 16-byte accesses when rowlen % 4 == 0 (FM / NFM k % 4 == 0,
+// FFM Fc * k % 4 == 0), scalar ones otherwise
+template <class K>
+static K by_rowlen(const lctr_ctx* c, K vec4, K scalar) {
+    return (c->rowlen & 3) == 0 ? vec4 : scalar;
+}
+
 // the per-row arrays that move with a row
 struct RowArrays {
     float *W, *V, *s1W, *s1V, *s2W, *s2V;
     unsigned long long *row_key, *last_seen;
 };
 
+// Hash index key -> row: open addressing over T = 2^m >= 2 * capacity slots of a u64 key (kEmptyKey = free) and a u32
+// row, with three flag words whose meaning is the owner's ([1] is "full" for both) and their pinned mirror.  Both the
+// key table and the host tier index their rows with one.
+struct KeyIndex {
+    unsigned long long* key = nullptr;
+    uint32_t* row = nullptr;
+    unsigned int* flags = nullptr;
+    unsigned int* h_flags = nullptr;
+    size_t T = 0;
+
+    int clear(cudaStream_t st) {
+        LCTR_CUDA(cudaMemsetAsync(key, 0xff, T * sizeof(unsigned long long), st));
+        LCTR_CUDA(cudaMemsetAsync(row, 0xff, T * sizeof(uint32_t), st));
+        LCTR_CUDA(cudaMemsetAsync(flags, 0, 3 * sizeof(unsigned int), st));
+        return 0;
+    }
+    int alloc(size_t cap, cudaStream_t st) {
+        T = kGroup;
+        while (T < 2 * cap) T <<= 1;
+        if (dalloc(&key, T) || dalloc(&row, T) || dalloc(&flags, 3)) return 1;
+        LCTR_CUDA(cudaMallocHost((void**)&h_flags, 3 * sizeof(unsigned int)));
+        return clear(st);
+    }
+    void free() {
+        dfree(key); dfree(row); dfree(flags);
+        if (h_flags) cudaFreeHost(h_flags);
+        h_flags = nullptr;
+    }
+    // emptied, then key row_key[i] re-inserted with row i for i < n (v: this index's view); fails naming `what` when full
+    int rebuild(lctr_ctx* c, const KeyView& v, const unsigned long long* row_key, size_t n, const char* what);
+};
+
 // Host tier (cfg.key_host_rows > 0): rows of evicted keys in pinned, device-mapped host memory, live rows [0, n), and an
-// index key -> tier row in HBM with the key table's layout.  Index slots go from empty to a key only; a restored key keeps
-// its slot with kNoRow, so `used` (slots holding a key) counts live and dead slots, and the index is rebuilt from
-// row_key[0, n) once it passes T / 2.
+// index key -> tier row in HBM (flags: [0] rows restored, [1] index full, [2] slots claimed by a spill).  Index slots go
+// from empty to a key only; a restored key keeps its slot with kNoRow, so `used` (slots holding a key) counts live and
+// dead slots, and the index is rebuilt from row_key[0, n) once it passes T / 2.
 struct HostTier {
     RowArrays a{};                          // device-mapped host arrays of `cap` rows
-    unsigned long long* key = nullptr;      // [T] index slot keys (HBM)
-    uint32_t* row = nullptr;                // [T] tier row of the slot's key, kNoRow once restored
-    unsigned int* flags = nullptr;          // [0] rows restored, [1] index full, [2] slots claimed by a spill
-    unsigned int* h_flags = nullptr;        // pinned mirror
-    size_t T = 0, cap = 0, n = 0, used = 0;
+    KeyIndex ix;
+    size_t cap = 0, n = 0, used = 0;
     // scratch of the compaction after a restore, sized with the key table's per-call scratch (at most one entry per new row)
     uint32_t* rel = nullptr;                // tier rows released by the current call, in no order
     uint32_t* wscan = nullptr;              // [m + 1] released rows in [n_live, n_live + i)
@@ -137,17 +186,15 @@ struct Admission {
 };
 
 struct KeyTable {
-    unsigned long long* key = nullptr;      // [T] slot keys, kEmptyKey = free
-    uint32_t* row = nullptr;                // [T] row of the slot's key, kNoRow when the capacity was exhausted
+    KeyIndex ix;                            // row kNoRow when the capacity was exhausted; flags: [0] capacity exhausted,
+                                            // [1] table full, [2] new rows of this upload
     unsigned long long* row_key = nullptr;  // [capacity] key of each row
     unsigned long long* count = nullptr;    // rows claimed (may pass capacity: claims that got no row)
-    unsigned int* flags = nullptr;          // [0] capacity exhausted, [1] table full, [2] new rows of this upload
-    unsigned int* h_flags = nullptr;        // pinned mirror of flags
     uint32_t* new_rows = nullptr;           // rows created by this upload
     unsigned long long* d_keys = nullptr;   // staging of the keys of one call
     int64_t* d_rows = nullptr;              // lookup results / fixed rows of one call
     size_t cap_scratch = 0;
-    size_t T = 0, cap = 0;
+    size_t cap = 0;
     unsigned long long seed = 0;
     float scale = 1.f;
     // key_evict = 1
@@ -165,11 +212,11 @@ struct KeyTable {
 };
 
 static KeyView view(const KeyTable* t) {
-    return KeyView{t->key, t->row, t->row_key, t->count, t->flags, t->new_rows, t->T / kGroup, t->cap};
+    return KeyView{t->ix.key, t->ix.row, t->row_key, t->count, t->ix.flags, t->new_rows, t->ix.T / kGroup, t->cap};
 }
 // the tier's index: row_key is the tier's (host) row -> key map; no row counter and no new-row list
 static KeyView view(const HostTier* h) {
-    return KeyView{h->key, h->row, h->a.row_key, nullptr, h->flags, nullptr, h->T / kGroup, h->cap};
+    return KeyView{h->ix.key, h->ix.row, h->a.row_key, nullptr, h->ix.flags, nullptr, h->ix.T / kGroup, h->cap};
 }
 
 // 1. claim a slot and a row for every key not yet in the table (one 16-lane tile per key)
@@ -181,9 +228,9 @@ __global__ void __launch_bounds__(256) key_insert_kernel(const unsigned long lon
     tile_insert(t, keys[i], sub, gmask);
 }
 
-// keys with caller-chosen rows (lctr_upload_keyed_params, checkpoint restore): every key gets rows[i]; `record` appends the
-// row to the new-row list for key_init_kernel.  rows == nullptr: key i gets row i and keys is the row -> key map itself
-// (the rebuild after an eviction), which is then left as it is.
+// keys with caller-chosen rows (lctr_upload_keyed_params): every key gets rows[i]; `record` appends the row to the new-row
+// list for key_init_kernel.  rows == nullptr: key i gets row i and keys is the row -> key map itself (KeyIndex::rebuild),
+// which is then left as it is.
 __global__ void __launch_bounds__(256) key_insert_fixed_kernel(const unsigned long long* keys, const int64_t* __restrict__ rows,
                                                                int64_t n, KeyView t, int record) {
     const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
@@ -211,34 +258,19 @@ __device__ __forceinline__ float key_gauss(unsigned long long hk, size_t rowlen,
 }
 
 // lazy init of row r of key `key` by one warp: W = 0, V from the key, the optimizer state lctr_create gives
-__device__ __forceinline__ void warp_lazy_init(float* __restrict__ W, float* __restrict__ V, float* __restrict__ s1W,
-                                               float* __restrict__ s1V, float* __restrict__ s2W, float* __restrict__ s2V, uint32_t r,
-                                               unsigned long long key, size_t rowlen, float s1_init, unsigned long long seed,
-                                               float scale, int lane) {
+__device__ __forceinline__ void warp_lazy_init(const RowArrays& a, uint32_t r, unsigned long long key, size_t rowlen, float s1_init,
+                                               unsigned long long seed, float scale, int lane) {
     const unsigned long long hk = fmix64(key);
     const size_t o = (size_t)r * rowlen;
     for (size_t j = lane; j < rowlen; j += 32) {
-        V[o + j] = key_gauss(hk, rowlen, j, seed, scale);
-        s1V[o + j] = s1_init;
-        if (s2V) s2V[o + j] = 0.f;
+        a.V[o + j] = key_gauss(hk, rowlen, j, seed, scale);
+        a.s1V[o + j] = s1_init;
+        if (a.s2V) a.s2V[o + j] = 0.f;
     }
     if (lane == 0) {
-        W[r] = 0.f;
-        s1W[r] = s1_init;
-        if (s2W) s2W[r] = 0.f;
-    }
-}
-
-// 2. lazy init of the rows created by this upload: one warp per row
-__global__ void __launch_bounds__(256) key_init_kernel(KeyView t, float* __restrict__ W, float* __restrict__ V, float* __restrict__ s1W,
-                                                       float* __restrict__ s1V, float* __restrict__ s2W, float* __restrict__ s2V,
-                                                       size_t rowlen, float s1_init, unsigned long long seed, float scale) {
-    const unsigned n = t.flags[2];
-    const int lane = threadIdx.x & 31;
-    const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
-    for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n; w += nwarps) {
-        const uint32_t r = t.new_rows[w];
-        warp_lazy_init(W, V, s1W, s1V, s2W, s2V, r, t.row_key[r], rowlen, s1_init, seed, scale, lane);
+        a.W[r] = 0.f;
+        a.s1W[r] = s1_init;
+        if (a.s2W) a.s2W[r] = 0.f;
     }
 }
 
@@ -271,39 +303,41 @@ __device__ __forceinline__ void warp_copy_all(const RowArrays& to, size_t d, con
     }
 }
 
-// 2'. tiered twin of key_init_kernel (one warp per new row): a key found in the tier index takes its row from host memory
-//     bit for bit (stamp included), its index slot turns kNoRow and its tier row joins the released list; any other key
-//     gets the lazy init of key_init_kernel
-template <bool VEC4>
-__global__ void __launch_bounds__(256) key_restore_init_kernel(KeyView t, KeyView h, RowArrays dev, RowArrays tier, size_t rowlen,
-                                                               uint32_t* __restrict__ rel, float s1_init,
-                                                               unsigned long long seed, float scale) {
+// 2. the rows created by this upload, one warp per row: the lazy init.  TIERED (the tier holds rows): a key found in the
+//    tier index takes its row from host memory bit for bit (stamp included) instead, its index slot turns kNoRow and its
+//    tier row joins the released list.
+template <bool TIERED, bool VEC4>
+__global__ void __launch_bounds__(256) key_init_kernel(KeyView t, KeyView h, RowArrays dev, RowArrays tier, size_t rowlen,
+                                                       uint32_t* __restrict__ rel, float s1_init, unsigned long long seed,
+                                                       float scale) {
     const unsigned n = t.flags[2];
     const int lane = threadIdx.x & 31;
     const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
     for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n; w += nwarps) {
         const uint32_t r = t.new_rows[w];
         const unsigned long long key = t.row_key[r];
-        long long pos = -1;
-        if (lane < kGroup) pos = tile_find(h, key, lane, 0xffffu);
-        uint32_t tr = kNoRow;  // read by lane 0 alone, which later overwrites the word
-        if (lane == 0 && pos >= 0) tr = h.row[pos];
-        pos = __shfl_sync(~0u, pos, 0);
-        tr = __shfl_sync(~0u, tr, 0);
-        if (tr == kNoRow) {
-            warp_lazy_init(dev.W, dev.V, dev.s1W, dev.s1V, dev.s2W, dev.s2V, r, key, rowlen, s1_init, seed, scale, lane);
-            continue;
+        if constexpr (TIERED) {
+            long long pos = -1;
+            if (lane < kGroup) pos = tile_find(h, key, lane, 0xffffu);
+            uint32_t tr = kNoRow;  // read by lane 0 alone, which later overwrites the word
+            if (lane == 0 && pos >= 0) tr = h.row[pos];
+            pos = __shfl_sync(~0u, pos, 0);
+            tr = __shfl_sync(~0u, tr, 0);
+            if (tr != kNoRow) {
+                warp_copy_all<VEC4>(dev, r, tier, tr, rowlen, lane);
+                if (lane == 0) {
+                    h.row[pos] = kNoRow;
+                    rel[atomicAdd(&h.flags[0], 1u)] = tr;
+                }
+                continue;
+            }
         }
-        warp_copy_all<VEC4>(dev, r, tier, tr, rowlen, lane);
-        if (lane == 0) {
-            h.row[pos] = kNoRow;
-            rel[atomicAdd(&h.flags[0], 1u)] = tr;
-        }
+        warp_lazy_init(dev, r, key, rowlen, s1_init, seed, scale, lane);
     }
 }
 
 // 3'. lookup-only restore (one 16-lane tile per key): a key found live in the tier index claims a device row (the key
-//     table's insert: new rows recorded for key_restore_init_kernel, capacity flag past the capacity); others are left
+//     table's insert: new rows recorded for key_init_kernel, capacity flag past the capacity); others are left
 __global__ void __launch_bounds__(256) key_lookup_restore_kernel(const unsigned long long* __restrict__ keys, int64_t n, KeyView t, KeyView h) {
     const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kGroup;
     if (i >= n) return;
@@ -396,7 +430,7 @@ __global__ void __launch_bounds__(256) key_scatter_params_kernel(const int64_t* 
     const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x / 32);
     for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; i < n; i += nwarps) {
         const size_t r = (size_t)rows[i];
-        if (Vin) for (size_t j = lane; j < rowlen; j += 32) V[r * rowlen + j] = Vin[(size_t)i * rowlen + j];
+        if (Vin) warp_copy_row<false>(V, r, Vin, (size_t)i, rowlen, lane);
         if (Win && lane == 0) W[r] = Win[i];
     }
 }
@@ -649,7 +683,7 @@ __global__ void __launch_bounds__(256) evict_export_kernel(const uint32_t* __res
     const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
     for (size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; i < m; i += nwarps) {
         const size_t r = ev_rows[i];
-        if (V_out) for (size_t j = lane; j < rowlen; j += 32) V_out[i * rowlen + j] = V[r * rowlen + j];
+        if (V_out) warp_copy_row<false>(V_out, i, V, r, rowlen, lane);
         if (lane == 0) {
             if (keys_out) keys_out[i] = row_key[r];
             if (W_out) W_out[i] = W[r];
@@ -720,24 +754,61 @@ __global__ void __launch_bounds__(256) evict_reset_kernel(RowArrays a, size_t ro
 
 static unsigned tile_grid(int64_t n) { return (unsigned)std::max<int64_t>(1, (n * kGroup + 255) / 256); }
 
-static int scratch_reserve(lctr_ctx* c, size_t n) {
+int KeyIndex::rebuild(lctr_ctx* c, const KeyView& v, const unsigned long long* row_key, size_t n, const char* what) {
+    if (clear(c->stream)) return 1;
+    if (n) {
+        key_insert_fixed_kernel<<<tile_grid((int64_t)n), 256, 0, c->stream>>>(row_key, nullptr, (int64_t)n, v, 0);
+        LCTR_LAUNCHED();
+    }
+    LCTR_CUDA(cudaMemcpyAsync(h_flags, flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    LCTR_CHECK(!h_flags[1], "%s %zu keys", what, n);
+    return 0;
+}
+
+// the per-call scratch of the key table and of the tier compaction for `cap` keys (0: freed)
+static int key_scratch(KeyTable* t, size_t cap) {
+    HostTier* h = t->tier;
+    dfree(t->d_keys); dfree(t->d_rows); dfree(t->new_rows);
+    if (h) { dfree(h->rel); dfree(h->wscan); dfree(h->holes); }
+    t->cap_scratch = 0;
+    if (!cap) return 0;
+    if (dalloc(&t->d_keys, cap) || dalloc(&t->d_rows, cap) || dalloc(&t->new_rows, cap)) return 1;
+    if (h && (dalloc(&h->rel, cap) || dalloc(&h->wscan, cap + 1) || dalloc(&h->holes, cap))) return 1;  // a call restores
+    t->cap_scratch = cap;                                                                              // <= 1 row per new row
+    return 0;
+}
+
+// room for n keys in the per-call scratch, grown by half at least
+int scratch_reserve(lctr_ctx* c, size_t n) {
     KeyTable* t = c->keys;
     if (n <= t->cap_scratch) return 0;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    const size_t cap = std::max(n, t->cap_scratch + t->cap_scratch / 2);
-    cudaFree(t->d_keys); cudaFree(t->d_rows); cudaFree(t->new_rows);
-    t->d_keys = nullptr; t->d_rows = nullptr; t->new_rows = nullptr; t->cap_scratch = 0;
-    LCTR_CUDA(cudaMalloc((void**)&t->d_keys, cap * sizeof(unsigned long long)));
-    LCTR_CUDA(cudaMalloc((void**)&t->d_rows, cap * sizeof(int64_t)));
-    LCTR_CUDA(cudaMalloc((void**)&t->new_rows, cap * sizeof(uint32_t)));
-    if (HostTier* h = t->tier) {  // a call restores at most one tier row per new row
-        cudaFree(h->rel); cudaFree(h->wscan); cudaFree(h->holes);
-        h->rel = h->wscan = h->holes = nullptr;
-        LCTR_CUDA(cudaMalloc((void**)&h->rel, cap * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&h->wscan, (cap + 1) * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&h->holes, cap * sizeof(uint32_t)));
-    }
-    t->cap_scratch = cap;
+    return key_scratch(t, std::max(n, t->cap_scratch + t->cap_scratch / 2));
+}
+
+// the compaction scratch of admission for n entries (0: freed)
+static int admission_scratch(Admission* a, size_t cap) {
+    dfree(a->scan); dfree(a->tiles); dfree(a->fid); dfree(a->field); dfree(a->val);
+    a->cap = 0;
+    if (!cap) return 0;
+    if (dalloc(&a->scan, cap + 1) || dalloc(&a->tiles, cap / kEvTile + 1) || dalloc(&a->fid, cap) || dalloc(&a->field, cap) ||
+        dalloc(&a->val, cap))
+        return 1;
+    a->cap = cap;
+    return 0;
+}
+
+// the scratch of lctr_evict_keys for a table of cap rows (0: freed); h_res, allocated last, marks it complete
+static int evict_scratch(KeyTable* t, size_t cap) {
+    dfree(t->ev_scan); dfree(t->ev_rows); dfree(t->ev_tiles); dfree(t->ev_hist); dfree(t->ev_res);
+    if (t->h_res) cudaFreeHost(t->h_res);
+    t->h_res = nullptr;
+    if (!cap) return 0;
+    if (dalloc(&t->ev_scan, cap + 1) || dalloc(&t->ev_rows, cap) || dalloc(&t->ev_tiles, cap / kEvTile + 1) ||
+        dalloc(&t->ev_hist, (size_t)kEvBins) || dalloc(&t->ev_res, 4))
+        return 1;
+    LCTR_CUDA(cudaMallocHost((void**)&t->h_res, 4 * sizeof(unsigned long long)));
     return 0;
 }
 
@@ -748,24 +819,15 @@ static RowArrays device_rows(lctr_ctx* c) {
 // tiered contexts whose tier holds rows restore the keys it holds instead of initialising them
 static bool tier_live(const KeyTable* t) { return t->tier && t->tier->n > 0; }
 
-static int init_new_rows(lctr_ctx* c, int64_t max_new) {
+// the rows the last insert recorded (at most max_new), initialised or restored from the tier
+int init_new_rows(lctr_ctx* c, int64_t max_new) {
     KeyTable* t = c->keys;
-    const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((max_new + 7) / 8, (int64_t)c->sm_count * 16));
-    if (tier_live(t)) {
-        HostTier* h = t->tier;
-        const RowArrays dev = device_rows(c);
-        if ((c->rowlen & 3) == 0)
-            key_restore_init_kernel<true><<<grid, 256, 0, c->stream>>>(view(t), view(h), dev, h->a, c->rowlen, h->rel,
-                                                                      initial_s1(c->cfg), t->seed, t->scale);
-        else
-            key_restore_init_kernel<false><<<grid, 256, 0, c->stream>>>(view(t), view(h), dev, h->a, c->rowlen, h->rel,
-                                                                       initial_s1(c->cfg), t->seed, t->scale);
-    } else {
-        key_init_kernel<<<grid, 256, 0, c->stream>>>(view(t), c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, c->rowlen,
-                                                     initial_s1(c->cfg), t->seed, t->scale);
-    }
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
+    const bool tiered = tier_live(t);
+    const auto kernel = tiered ? by_rowlen(c, key_init_kernel<true, true>, key_init_kernel<true, false>) : key_init_kernel<false, false>;
+    HostTier* h = tiered ? t->tier : nullptr;
+    kernel<<<warp_grid(c, (size_t)max_new), 256, 0, c->stream>>>(view(t), h ? view(h) : KeyView{}, device_rows(c), h ? h->a : RowArrays{},
+                                                                 c->rowlen, h ? h->rel : nullptr, initial_s1(c->cfg), t->seed, t->scale);
+    LCTR_LAUNCHED();
     return 0;
 }
 
@@ -773,9 +835,9 @@ static int init_new_rows(lctr_ctx* c, int64_t max_new) {
 // an insert-upload
 static int read_flags(lctr_ctx* c, bool admission = false) {
     KeyTable* t = c->keys;
-    LCTR_CUDA(cudaMemcpyAsync(t->h_flags, t->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaMemcpyAsync(t->ix.h_flags, t->ix.flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     if (t->tier)
-        LCTR_CUDA(cudaMemcpyAsync(t->tier->h_flags, t->tier->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+        LCTR_CUDA(cudaMemcpyAsync(t->tier->ix.h_flags, t->tier->ix.flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     if (admission)
         LCTR_CUDA(cudaMemcpyAsync(t->adm->h_cnt, t->adm->cnt, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -790,7 +852,7 @@ static uint64_t rows_in_use(lctr_ctx* c, int* rc) {
     return std::min<uint64_t>(n, c->keys->cap);
 }
 
-static int check_keys_host(const uint64_t* keys, int64_t n, const char* who) {
+int check_keys_reserved(const uint64_t* keys, int64_t n, const char* who) {
     for (int64_t i = 0; i < n; i++)
         LCTR_CHECK(keys[i] != kEmptyKey, "%s: key %llu at entry %lld is reserved (the empty marker of the key table)", who,
                    (unsigned long long)keys[i], (long long)i);
@@ -802,38 +864,18 @@ int keys_alloc(lctr_ctx* c) {
     c->keys = t;
     // several GPUs: this rank's shard holds the global rows l * world + rank below feature_cnt (dist.cu: placement)
     t->cap = owned_rows(c->F - 1, c->cfg.world, c->cfg.rank);
-    size_t T = kGroup;
-    while (T < 2 * t->cap) T <<= 1;
-    t->T = T;
     t->scale = (float)(1.0 / sqrt((double)c->cfg.factor_cnt));
-    LCTR_CUDA(cudaMalloc((void**)&t->key, T * sizeof(unsigned long long)));
-    LCTR_CUDA(cudaMalloc((void**)&t->row, T * sizeof(uint32_t)));
-    LCTR_CUDA(cudaMalloc((void**)&t->row_key, t->cap * sizeof(unsigned long long)));
-    LCTR_CUDA(cudaMalloc((void**)&t->count, sizeof(unsigned long long)));
-    LCTR_CUDA(cudaMalloc((void**)&t->flags, 3 * sizeof(unsigned int)));
-    LCTR_CUDA(cudaMallocHost((void**)&t->h_flags, 3 * sizeof(unsigned int)));
-    LCTR_CUDA(cudaMemsetAsync(t->key, 0xff, T * sizeof(unsigned long long), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(t->row, 0xff, T * sizeof(uint32_t), c->stream));
+    if (t->ix.alloc(t->cap, c->stream) || dalloc(&t->row_key, t->cap) || dalloc(&t->count, 1)) return 1;
     LCTR_CUDA(cudaMemsetAsync(t->count, 0, sizeof(unsigned long long), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
     if (c->cfg.key_evict) {
-        LCTR_CUDA(cudaMalloc((void**)&t->last_seen, t->cap * sizeof(unsigned long long)));
+        if (dalloc(&t->last_seen, t->cap)) return 1;
         LCTR_CUDA(cudaMemsetAsync(t->last_seen, 0, t->cap * sizeof(unsigned long long), c->stream));
     }
     if (c->cfg.key_host_rows) {
         HostTier* h = new HostTier();
         t->tier = h;
         h->cap = c->cfg.key_host_rows;
-        size_t TT = kGroup;
-        while (TT < 2 * h->cap) TT <<= 1;
-        h->T = TT;
-        LCTR_CUDA(cudaMalloc((void**)&h->key, TT * sizeof(unsigned long long)));
-        LCTR_CUDA(cudaMalloc((void**)&h->row, TT * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&h->flags, 3 * sizeof(unsigned int)));
-        LCTR_CUDA(cudaMallocHost((void**)&h->h_flags, 3 * sizeof(unsigned int)));
-        LCTR_CUDA(cudaMemsetAsync(h->key, 0xff, TT * sizeof(unsigned long long), c->stream));
-        LCTR_CUDA(cudaMemsetAsync(h->row, 0xff, TT * sizeof(uint32_t), c->stream));
-        LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
+        if (h->ix.alloc(h->cap, c->stream)) return 1;
         // rows in pinned host memory mapped into the device address space: kernels read and write them over PCIe
         auto host = [&](void** p, size_t bytes) {
             return cudaHostAlloc(p, bytes, cudaHostAllocMapped) == cudaSuccess && (memset(*p, 0, bytes), true);
@@ -851,17 +893,15 @@ int keys_alloc(lctr_ctx* c) {
 static void admission_free(KeyTable* t) {
     Admission* a = t->adm;
     if (!a) return;
-    cudaFree(a->sketch); cudaFree(a->cnt);
-    cudaFree(a->scan); cudaFree(a->tiles); cudaFree(a->fid); cudaFree(a->field); cudaFree(a->val);
+    dfree(a->sketch); dfree(a->cnt);
+    admission_scratch(a, 0);
     if (a->h_cnt) cudaFreeHost(a->h_cnt);
     delete a;
     t->adm = nullptr;
 }
 
 static void tier_free(HostTier* h) {
-    cudaFree(h->key); cudaFree(h->row); cudaFree(h->flags);
-    cudaFree(h->rel); cudaFree(h->wscan); cudaFree(h->holes);
-    if (h->h_flags) cudaFreeHost(h->h_flags);
+    h->ix.free();
     for (void* p : {(void*)h->a.row_key, (void*)h->a.last_seen, (void*)h->a.W, (void*)h->a.V, (void*)h->a.s1W, (void*)h->a.s1V,
                     (void*)h->a.s2W, (void*)h->a.s2V})
         if (p) cudaFreeHost(p);
@@ -871,14 +911,12 @@ static void tier_free(HostTier* h) {
 void keys_free(lctr_ctx* c) {
     KeyTable* t = c->keys;
     if (!t) return;
+    key_scratch(t, 0);  // the tier's compaction scratch too: before the tier goes
+    evict_scratch(t, 0);
     if (t->tier) tier_free(t->tier);
     admission_free(t);
-    cudaFree(t->key); cudaFree(t->row); cudaFree(t->row_key); cudaFree(t->count); cudaFree(t->flags);
-    cudaFree(t->new_rows); cudaFree(t->d_keys); cudaFree(t->d_rows);
-    cudaFree(t->last_seen); cudaFree(t->ev_scan); cudaFree(t->ev_rows); cudaFree(t->ev_tiles); cudaFree(t->ev_hist);
-    cudaFree(t->ev_res);
-    if (t->h_flags) cudaFreeHost(t->h_flags);
-    if (t->h_res) cudaFreeHost(t->h_res);
+    t->ix.free();
+    dfree(t->row_key); dfree(t->count); dfree(t->last_seen);
     delete t;
     c->keys = nullptr;
 }
@@ -902,48 +940,29 @@ int keys_tier_restore(lctr_ctx* c, uint64_t n) {
 }
 
 KeyView keys_view(lctr_ctx* c) { return view(c->keys); }
-int keys_reserve_new_rows(lctr_ctx* c, size_t n) { return scratch_reserve(c, n); }
-int keys_init_new_rows(lctr_ctx* c, int64_t max_new) { return init_new_rows(c, max_new); }
 size_t keys_capacity(const lctr_ctx* c) { return c->keys->cap; }
 
 size_t keys_bytes(const lctr_ctx* c) {
     const KeyTable* t = c->keys;
     if (!t) return 0;
-    return t->T * (sizeof(unsigned long long) + sizeof(uint32_t)) + t->cap * sizeof(unsigned long long) +
+    return t->ix.T * (sizeof(unsigned long long) + sizeof(uint32_t)) + t->cap * sizeof(unsigned long long) +
            (t->last_seen ? t->cap * sizeof(unsigned long long) : 0) +
-           (t->tier ? t->tier->T * (sizeof(unsigned long long) + sizeof(uint32_t)) : 0) +
+           (t->tier ? t->tier->ix.T * (sizeof(unsigned long long) + sizeof(uint32_t)) : 0) +
            (t->adm ? ((size_t)kSketchDepth << t->adm->lw) * sizeof(uint32_t) : 0);
 }
-
-#define LCTR_LAUNCHED()                  \
-    do {                                 \
-        c->launches++;                   \
-        LCTR_CUDA(cudaGetLastError());   \
-    } while (0)
 
 // the tier index emptied and rows [0, n) re-inserted with row = index
 static int tier_rebuild(lctr_ctx* c) {
     HostTier* h = c->keys->tier;
-    LCTR_CUDA(cudaMemsetAsync(h->key, 0xff, h->T * sizeof(unsigned long long), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(h->row, 0xff, h->T * sizeof(uint32_t), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
-    if (h->n) {
-        key_insert_fixed_kernel<<<tile_grid((int64_t)h->n), 256, 0, c->stream>>>(h->a.row_key, nullptr, (int64_t)h->n, view(h), 0);
-        LCTR_LAUNCHED();
-    }
-    LCTR_CUDA(cudaMemcpyAsync(h->h_flags, h->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
-    LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    LCTR_CHECK(!h->h_flags[1], "host tier: index full while re-inserting %zu keys", h->n);
+    if (h->ix.rebuild(c, view(h), h->a.row_key, h->n, "host tier: index full while re-inserting")) return 1;
     h->used = h->n;
     return 0;
 }
 
 // survivors at or above n_live into the holes below it, for the rows of one table (wscan, holes: evict_move_kernel)
 static int launch_move(lctr_ctx* c, const RowArrays& a, size_t n_live, size_t n, const uint32_t* wscan, const uint32_t* holes) {
-    const size_t m = n - n_live;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
-    if ((c->rowlen & 3) == 0) evict_move_kernel<true><<<grid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, wscan, holes);
-    else evict_move_kernel<false><<<grid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, wscan, holes);
+    by_rowlen(c, evict_move_kernel<true>, evict_move_kernel<false>)<<<warp_grid(c, n - n_live), 256, 0, c->stream>>>(
+        a, c->rowlen, n_live, n, wscan, holes);
     LCTR_LAUNCHED();
     return 0;
 }
@@ -966,8 +985,8 @@ static void radix_sort_u32(std::vector<uint32_t>& v) {
 // move and one reindex launch over the window; nothing reads the rest of the tier.
 static int tier_compact(lctr_ctx* c) {
     HostTier* h = c->keys->tier;
-    if (!h || !h->h_flags[0]) return 0;
-    const size_t m = h->h_flags[0], n = h->n, n_live = n - m;
+    if (!h || !h->ix.h_flags[0]) return 0;
+    const size_t m = h->ix.h_flags[0], n = h->n, n_live = n - m;
     std::vector<uint32_t> rel(m), holes;
     LCTR_CUDA(cudaMemcpyAsync(rel.data(), h->rel, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -989,8 +1008,8 @@ static int tier_compact(lctr_ctx* c) {
     if (launch_move(c, h->a, n_live, n, h->wscan, h->holes)) return 1;
     tier_reindex_kernel<<<tile_grid((int64_t)m), 256, 0, c->stream>>>(view(h), n_live, n, h->wscan, h->holes);
     LCTR_LAUNCHED();
-    LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
-    h->h_flags[0] = 0;
+    LCTR_CUDA(cudaMemsetAsync(h->ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
+    h->ix.h_flags[0] = 0;
     h->n = n_live;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the host vectors above are the copies' sources
     return 0;
@@ -1009,7 +1028,7 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
     if (n == 0) return 0;
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, h_keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
-    LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    LCTR_CUDA(cudaMemsetAsync(t->ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
     if (adm) LCTR_CUDA(cudaMemsetAsync(adm->cnt, 0, 2 * sizeof(unsigned long long), c->stream));
     const bool restoring = tier_live(t);
     {
@@ -1026,20 +1045,17 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
             } else {
                 key_lookup_restore_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), view(t->tier));
             }
-            c->launches++;
-            LCTR_CUDA(cudaGetLastError());
+            LCTR_LAUNCHED();
             if (init_new_rows(c, std::min<int64_t>(n, (int64_t)t->cap))) return 1;
             if (!insert) {
                 key_tier_refused_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), view(t->tier));
-                c->launches++;
-                LCTR_CUDA(cudaGetLastError());
+                LCTR_LAUNCHED();
             }
         }
         key_find_kernel<0><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0,
                                                                 insert ? t->last_seen : nullptr, t->clock,
                                                                 adm ? adm->cnt : nullptr);
-        c->launches++;
-        LCTR_CUDA(cudaGetLastError());
+        LCTR_LAUNCHED();
     }
     if (read_flags(c, adm != nullptr)) return 1;
     if (adm) {
@@ -1047,8 +1063,8 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
         adm->admitted = adm->h_cnt[1];
     }
     if (restoring && tier_compact(c)) return 1;  // before any failure below: restored rows have left the tier either way
-    LCTR_CHECK(!t->h_flags[1], "key table: no free slot on a probe path (%zu slots for capacity %zu)", t->T, t->cap);
-    LCTR_CHECK(!t->h_flags[0], "key table: capacity of %zu rows (cfg.feature_cnt) exhausted; the batch's new keys do not fit",
+    LCTR_CHECK(!t->ix.h_flags[1], "key table: no free slot on a probe path (%zu slots for capacity %zu)", t->ix.T, t->cap);
+    LCTR_CHECK(!t->ix.h_flags[0], "key table: capacity of %zu rows (cfg.feature_cnt) exhausted; the batch's new keys do not fit",
                t->cap);
     return 0;
 }
@@ -1062,15 +1078,7 @@ int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, 
     a->pending = 0;
     if (n > a->cap) {
         LCTR_CUDA(cudaStreamSynchronize(st));
-        const size_t cap = std::max(n, a->cap + a->cap / 2);
-        cudaFree(a->scan); cudaFree(a->tiles); cudaFree(a->fid); cudaFree(a->field); cudaFree(a->val);
-        a->scan = a->tiles = a->fid = nullptr; a->field = nullptr; a->val = nullptr; a->cap = 0;
-        LCTR_CUDA(cudaMalloc((void**)&a->scan, (cap + 1) * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&a->tiles, (cap / kEvTile + 1) * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&a->fid, cap * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&a->field, cap * sizeof(uint16_t)));
-        LCTR_CUDA(cudaMalloc((void**)&a->val, cap * sizeof(float)));
-        a->cap = cap;
+        if (admission_scratch(a, std::max(n, a->cap + a->cap / 2))) return 1;
     }
     const uint16_t* field = s.has_field ? s.field : nullptr;
     const float* val = s.has_val ? s.val : nullptr;
@@ -1083,9 +1091,7 @@ int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, 
         LCTR_LAUNCHED();
         evict_index_kernel<<<(unsigned)ntiles, kEvTile, 0, st>>>(DropFlag{s.fid}, n, a->tiles, a->scan, nullptr);
         LCTR_LAUNCHED();
-        const size_t m = std::max(n, (size_t)rows + 1);
-        const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 255) / 256, (size_t)c->sm_count * 8));
-        admit_compact_kernel<<<grid, 256, 0, st>>>(s.fid, field, val, n, a->scan, s.row_ptr, (size_t)rows, a->fid,
+        admit_compact_kernel<<<stride_grid(c, std::max(n, (size_t)rows + 1)), 256, 0, st>>>(s.fid, field, val, n, a->scan, s.row_ptr, (size_t)rows, a->fid,
                                                    field ? a->field : nullptr, val ? a->val : nullptr);
         LCTR_LAUNCHED();
     }
@@ -1103,8 +1109,7 @@ static int lookup_dev(lctr_ctx* c, const uint64_t* keys, int64_t n) {
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
     key_find_kernel<1><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), nullptr, t->d_rows, 0, nullptr, 0, nullptr);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
+    LCTR_LAUNCHED();
     return 0;
 }
 
@@ -1112,24 +1117,10 @@ static int lookup_dev(lctr_ctx* c, const uint64_t* keys, int64_t n) {
 int keys_restore(lctr_ctx* c, const uint64_t* row_key, uint64_t n) {
     KeyTable* t = c->keys;
     LCTR_CHECK(n <= t->cap, "checkpoint: %llu keyed rows exceed the capacity %zu", (unsigned long long)n, t->cap);
-    LCTR_CUDA(cudaMemsetAsync(t->key, 0xff, t->T * sizeof(unsigned long long), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(t->row, 0xff, t->T * sizeof(uint32_t), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
     const unsigned long long cnt = n;
     LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
-    if (n) {
-        if (scratch_reserve(c, (size_t)n)) return 1;
-        std::vector<int64_t> rows(n);
-        for (uint64_t i = 0; i < n; i++) rows[i] = (int64_t)i;
-        LCTR_CUDA(cudaMemcpyAsync(t->d_keys, row_key, n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
-        LCTR_CUDA(cudaMemcpyAsync(t->d_rows, rows.data(), n * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
-        key_insert_fixed_kernel<<<tile_grid((int64_t)n), 256, 0, c->stream>>>(t->d_keys, t->d_rows, (int64_t)n, view(t), 0);
-        c->launches++;
-        LCTR_CUDA(cudaGetLastError());
-    }
-    if (read_flags(c)) return 1;
-    LCTR_CHECK(!t->h_flags[1], "checkpoint: key table full while restoring %llu keys", (unsigned long long)n);
-    return 0;
+    if (n) LCTR_CUDA(cudaMemcpyAsync(t->row_key, row_key, n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
+    return t->ix.rebuild(c, view(t), t->row_key, (size_t)n, "checkpoint: key table full while restoring");
 }
 
 int keys_download(lctr_ctx* c, std::vector<uint64_t>& out) {
@@ -1161,18 +1152,6 @@ int keys_restore_stamps(lctr_ctx* c, const uint64_t* stamps, uint64_t n, uint64_
     return 0;
 }
 
-static int evict_scratch(lctr_ctx* c) {
-    KeyTable* t = c->keys;
-    if (t->ev_scan) return 0;
-    LCTR_CUDA(cudaMalloc((void**)&t->ev_scan, (t->cap + 1) * sizeof(uint32_t)));
-    LCTR_CUDA(cudaMalloc((void**)&t->ev_rows, t->cap * sizeof(uint32_t)));
-    LCTR_CUDA(cudaMalloc((void**)&t->ev_tiles, (t->cap / kEvTile + 1) * sizeof(uint32_t)));
-    LCTR_CUDA(cudaMalloc((void**)&t->ev_hist, kEvBins * sizeof(unsigned int)));
-    LCTR_CUDA(cudaMalloc((void**)&t->ev_res, 4 * sizeof(unsigned long long)));
-    LCTR_CUDA(cudaMallocHost((void**)&t->h_res, 4 * sizeof(unsigned long long)));
-    return 0;
-}
-
 static int read_res(lctr_ctx* c, int n) {
     KeyTable* t = c->keys;
     LCTR_CUDA(cudaMemcpyAsync(t->h_res, t->ev_res, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
@@ -1185,7 +1164,7 @@ static int radix_select_age(lctr_ctx* c, const unsigned long long* last_seen, si
                             unsigned long long max_age, unsigned long long rank, unsigned long long* out) {
     KeyTable* t = c->keys;
     const int bits = std::max(1, 64 - __builtin_clzll(max_age | 1ull));
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
+    const unsigned grid = stride_grid(c, n);
     unsigned long long prefix = 0;
     int pshift = 64, shift = bits;  // bits above `bits` are zero for every survivor: no prefix condition on the first pass
     while (shift > 0) {
@@ -1216,10 +1195,9 @@ struct EvTable {
 static int evict_plan(lctr_ctx* c, const EvTable& tb, uint64_t max_idle, uint64_t max_rows, EvictRule* e, size_t* m) {
     KeyTable* t = c->keys;
     const size_t n = tb.n;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
     // 1 + 2: the rule
     LCTR_CUDA(cudaMemsetAsync(t->ev_res, 0, 2 * sizeof(unsigned long long), c->stream));
-    evict_survey_kernel<<<grid, 256, 0, c->stream>>>(tb.a.last_seen, n, t->clock, max_idle, t->ev_res);
+    evict_survey_kernel<<<stride_grid(c, n), 256, 0, c->stream>>>(tb.a.last_seen, n, t->clock, max_idle, t->ev_res);
     LCTR_LAUNCHED();
     if (read_res(c, 2)) return 1;
     const unsigned long long survivors = t->h_res[0], max_age = t->h_res[1];
@@ -1246,7 +1224,6 @@ static int evict_index_export(lctr_ctx* c, const EvTable& tb, const EvictRule& e
                                                                                   tb.scan, tb.rows);
     LCTR_LAUNCHED();
     if (!(keys_out || W_out || V_out)) return 0;
-    const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
     unsigned long long* dK = nullptr;
     float *dW = nullptr, *dV = nullptr;
     cudaError_t err = cudaSuccess;
@@ -1254,7 +1231,7 @@ static int evict_index_export(lctr_ctx* c, const EvTable& tb, const EvictRule& e
     if (W_out && err == cudaSuccess) err = cudaMalloc((void**)&dW, m * sizeof(float));
     if (V_out && err == cudaSuccess) err = cudaMalloc((void**)&dV, m * c->rowlen * sizeof(float));
     if (err == cudaSuccess) {
-        evict_export_kernel<<<mgrid, 256, 0, c->stream>>>(tb.rows, m, tb.a.row_key, tb.a.W, tb.a.V, c->rowlen, dK, dW, dV);
+        evict_export_kernel<<<warp_grid(c, m), 256, 0, c->stream>>>(tb.rows, m, tb.a.row_key, tb.a.W, tb.a.V, c->rowlen, dK, dW, dV);
         c->launches++;
         err = cudaGetLastError();
     }
@@ -1294,18 +1271,18 @@ int keys_admission_restore(lctr_ctx* c, const uint32_t* sketch) {
 // the m rows of the device table's eviction list appended to the tier at rows [n, n + m), keys claimed in its index
 static int tier_spill(lctr_ctx* c, const EvTable& dev, size_t m) {
     HostTier* h = c->keys->tier;
-    LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
-    const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
-    if ((c->rowlen & 3) == 0) tier_spill_kernel<true><<<mgrid, 256, 0, c->stream>>>(dev.rows, m, dev.a, h->a, h->n, c->rowlen, view(h));
-    else tier_spill_kernel<false><<<mgrid, 256, 0, c->stream>>>(dev.rows, m, dev.a, h->a, h->n, c->rowlen, view(h));
+    KeyIndex& ix = h->ix;
+    LCTR_CUDA(cudaMemsetAsync(ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
+    by_rowlen(c, tier_spill_kernel<true>, tier_spill_kernel<false>)<<<warp_grid(c, m), 256, 0, c->stream>>>(
+        dev.rows, m, dev.a, h->a, h->n, c->rowlen, view(h));
     LCTR_LAUNCHED();
-    LCTR_CUDA(cudaMemcpyAsync(h->h_flags, h->flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaMemcpyAsync(ix.h_flags, ix.flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     h->n += m;
-    h->used += h->h_flags[2];
-    LCTR_CUDA(cudaMemsetAsync(h->flags, 0, 3 * sizeof(unsigned int), c->stream));
+    h->used += ix.h_flags[2];
+    LCTR_CUDA(cudaMemsetAsync(ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
     // a full probe path (never expected below T / 2 used slots) or more than T / 2 slots in use: a fresh index
-    if (h->h_flags[1] || 2 * h->used > h->T) return tier_rebuild(c);
+    if (ix.h_flags[1] || 2 * h->used > ix.T) return tier_rebuild(c);
     return 0;
 }
 
@@ -1352,7 +1329,7 @@ int lctr_upload_keyed_params(lctr_ctx* c, int64_t n, const uint64_t* keys, const
     LCTR_CHECK(c->keys, "lctr_upload_keyed_params: the context was not created with key_mode = LCTR_KEYS_HASHED");
     LCTR_CHECK(n >= 0 && (n == 0 || keys), "lctr_upload_keyed_params: null argument");
     if (n == 0) return 0;
-    if (check_keys_host(keys, n, "lctr_upload_keyed_params")) return 1;
+    if (check_keys_reserved(keys, n, "lctr_upload_keyed_params")) return 1;
     {
         std::vector<uint64_t> sorted(keys, keys + n);
         std::sort(sorted.begin(), sorted.end());
@@ -1399,44 +1376,40 @@ static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* key
                new_keys.size(), t->cap, (unsigned long long)used);
     const int64_t m = (int64_t)new_keys.size();
     if (m) {
-        LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
+        LCTR_CUDA(cudaMemsetAsync(t->ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
         LCTR_CUDA(cudaMemcpyAsync(t->d_keys, new_keys.data(), (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
         LCTR_CUDA(cudaMemcpyAsync(t->d_rows, new_rows.data(), (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
         key_insert_fixed_kernel<<<tile_grid(m), 256, 0, c->stream>>>(t->d_keys, t->d_rows, m, view(t), 1);
-        c->launches++;
-        LCTR_CUDA(cudaGetLastError());
+        LCTR_LAUNCHED();
         const bool restoring = tier_live(t);  // tier keys bring their optimizer state back
         if (init_new_rows(c, m)) return 1;
         const unsigned long long cnt = used + (uint64_t)m;
         LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
         if (read_flags(c)) return 1;
         if (restoring && tier_compact(c)) return 1;
-        LCTR_CHECK(!t->h_flags[1], "lctr_upload_keyed_params: key table full");
+        LCTR_CHECK(!t->ix.h_flags[1], "lctr_upload_keyed_params: key table full");
     }
     if (t->last_seen || W || V)
         LCTR_CUDA(cudaMemcpyAsync(t->d_rows, rows.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
     if (t->last_seen) {  // every named row counts as met at the current clock
-        const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)c->sm_count * 8));
-        key_stamp_rows_kernel<<<grid, 256, 0, c->stream>>>(t->d_rows, n, t->last_seen, t->clock);
-        c->launches++;
-        LCTR_CUDA(cudaGetLastError());
+        key_stamp_rows_kernel<<<stride_grid(c, (size_t)n), 256, 0, c->stream>>>(t->d_rows, n, t->last_seen, t->clock);
+        LCTR_LAUNCHED();
     }
     if (W || V) {
         float *dW = nullptr, *dV = nullptr;
         if (W) {
-            LCTR_CUDA(cudaMalloc((void**)&dW, (size_t)n * sizeof(float)));
+            if (dalloc(&dW, (size_t)n)) return 1;
             LCTR_CUDA(cudaMemcpyAsync(dW, W, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
         }
         if (V) {
-            LCTR_CUDA(cudaMalloc((void**)&dV, (size_t)n * c->rowlen * sizeof(float)));
+            if (dalloc(&dV, (size_t)n * c->rowlen)) return 1;
             LCTR_CUDA(cudaMemcpyAsync(dV, V, (size_t)n * c->rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
         }
-        const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 7) / 8, (int64_t)c->sm_count * 16));
-        key_scatter_params_kernel<<<grid, 256, 0, c->stream>>>(t->d_rows, n, dW, dV, c->W, c->V, c->rowlen);
-        c->launches++;
+        key_scatter_params_kernel<<<warp_grid(c, (size_t)n), 256, 0, c->stream>>>(t->d_rows, n, dW, dV, c->W, c->V, c->rowlen);
+        c->launches++;  // as LCTR_LAUNCHED, with the staging freed before an error returns
         const cudaError_t e = cudaGetLastError();
         cudaStreamSynchronize(c->stream);
-        cudaFree(dW); cudaFree(dV);
+        dfree(dW); dfree(dV);
         LCTR_CUDA(e);
     }
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -1471,10 +1444,8 @@ int lctr_set_key_admission(lctr_ctx* c, uint32_t min_count, uint32_t log2_width)
         Admission* a = new Admission();
         t->adm = a;
         a->lw = log2_width;
-        const cudaError_t e1 = cudaMalloc((void**)&a->sketch, ((size_t)kSketchDepth << log2_width) * sizeof(uint32_t));
-        const cudaError_t e2 = cudaMalloc((void**)&a->cnt, 3 * sizeof(unsigned long long));
-        const cudaError_t e3 = cudaMallocHost((void**)&a->h_cnt, 2 * sizeof(unsigned long long));
-        if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess) {
+        if (dalloc(&a->sketch, (size_t)kSketchDepth << log2_width) || dalloc(&a->cnt, 3) ||
+            cudaMallocHost((void**)&a->h_cnt, 2 * sizeof(unsigned long long)) != cudaSuccess) {
             admission_free(t);
             LCTR_CHECK(false, "lctr_set_key_admission: cannot allocate a sketch of %llu bytes (admission is off)",
                        (unsigned long long)(((size_t)kSketchDepth << log2_width) * sizeof(uint32_t)));
@@ -1495,8 +1466,7 @@ int lctr_decay_key_admission(lctr_ctx* c, uint32_t shift) {
     LCTR_CHECK(shift >= 1 && shift <= 32, "lctr_decay_key_admission: shift = %u outside [1, 32]", shift);
     const Admission* a = c->keys->adm;
     const size_t n4 = ((size_t)kSketchDepth << a->lw) / 4;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n4 + 255) / 256, (size_t)c->sm_count * 8));
-    sketch_decay_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<uint4*>(a->sketch), n4, shift);
+    sketch_decay_kernel<<<stride_grid(c, n4), 256, 0, c->stream>>>(reinterpret_cast<uint4*>(a->sketch), n4, shift);
     LCTR_LAUNCHED();
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
@@ -1523,7 +1493,7 @@ int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t*
     const size_t n = rows_in_use(c, &rc);
     if (rc) return 1;
     if (n == 0) return 0;
-    if (evict_scratch(c)) return 1;
+    if (!t->h_res && evict_scratch(t, t->cap)) return 1;
     const EvTable tb{device_rows(c), n, t->ev_scan, t->ev_rows, t->ev_tiles};
     EvictRule e;
     size_t m = 0;
@@ -1540,24 +1510,13 @@ int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t*
     if (h && tier_spill(c, tb, m)) return 1;
 
     // move, reset, rebuild
-    const RowArrays& a = tb.a;
-    const bool vec4 = (c->rowlen & 3) == 0;  // 16-byte rows: FM / NFM k % 4 == 0, FFM Fc * k % 4 == 0
-    if (launch_move(c, a, n_live, n, t->ev_scan + n_live, t->ev_rows)) return 1;
-    const unsigned mgrid = (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
-    if (vec4) evict_reset_kernel<true><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, initial_s1(c->cfg));
-    else evict_reset_kernel<false><<<mgrid, 256, 0, c->stream>>>(a, c->rowlen, n_live, n, initial_s1(c->cfg));
+    if (launch_move(c, tb.a, n_live, n, t->ev_scan + n_live, t->ev_rows)) return 1;
+    by_rowlen(c, evict_reset_kernel<true>, evict_reset_kernel<false>)<<<warp_grid(c, m), 256, 0, c->stream>>>(
+        tb.a, c->rowlen, n_live, n, initial_s1(c->cfg));
     LCTR_LAUNCHED();
-    LCTR_CUDA(cudaMemsetAsync(t->key, 0xff, t->T * sizeof(unsigned long long), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(t->row, 0xff, t->T * sizeof(uint32_t), c->stream));
-    LCTR_CUDA(cudaMemsetAsync(t->flags, 0, 3 * sizeof(unsigned int), c->stream));
-    if (n_live) {
-        key_insert_fixed_kernel<<<tile_grid((int64_t)n_live), 256, 0, c->stream>>>(t->row_key, nullptr, (int64_t)n_live, view(t), 0);
-        LCTR_LAUNCHED();
-    }
     const unsigned long long cnt = n_live;
     LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
-    if (read_flags(c)) return 1;
-    LCTR_CHECK(!t->h_flags[1], "lctr_evict_keys: key table full while re-inserting %zu keys", n_live);
+    if (t->ix.rebuild(c, view(t), t->row_key, n_live, "lctr_evict_keys: key table full while re-inserting")) return 1;
     for (int s = 0; s < kNumSlots; s++)  // their row ids belong to the old numbering
         if (c->slots[s].key_state != SLOT_KEYS_INVALID) c->slots[s].key_state = SLOT_KEYS_STALE;
     *n_evicted = m;
@@ -1573,15 +1532,13 @@ int lctr_evict_host_tier(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     const size_t n = h->n;
     if (n == 0) return 0;
-    if (evict_scratch(c)) return 1;
+    if (!c->keys->h_res && evict_scratch(c->keys, c->keys->cap)) return 1;
     // scratch of the tier's size for this call only: a tier eviction reads every tier row anyway
     struct Scratch {
         uint32_t *scan = nullptr, *rows = nullptr, *tiles = nullptr;
         ~Scratch() { cudaFree(scan); cudaFree(rows); cudaFree(tiles); }
     } sc;
-    LCTR_CUDA(cudaMalloc((void**)&sc.scan, (n + 1) * sizeof(uint32_t)));
-    LCTR_CUDA(cudaMalloc((void**)&sc.rows, n * sizeof(uint32_t)));
-    LCTR_CUDA(cudaMalloc((void**)&sc.tiles, (n / kEvTile + 1) * sizeof(uint32_t)));
+    if (dalloc(&sc.scan, n + 1) || dalloc(&sc.rows, n) || dalloc(&sc.tiles, n / kEvTile + 1)) return 1;
     const EvTable tb{h->a, n, sc.scan, sc.rows, sc.tiles};
     EvictRule e;
     size_t m = 0;

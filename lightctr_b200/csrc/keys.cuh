@@ -92,11 +92,11 @@ __device__ __forceinline__ bool tile_insert(const KeyView& t, unsigned long long
     return true;
 }
 
-// host side of keys.cu used by dist.cu: the context's key table as a view, room for `n` new rows in its scratch, and the
-// lazy init of the rows the last insert recorded (one launch)
+// host side of keys.cu used by dist.cu: the context's key table as a view, room for `n` keys (and new rows) in its
+// scratch, and the lazy init of the rows the last insert recorded (one launch)
 KeyView keys_view(lctr_ctx* c);
-int keys_reserve_new_rows(lctr_ctx* c, size_t n);
-int keys_init_new_rows(lctr_ctx* c, int64_t max_new);
+int scratch_reserve(lctr_ctx* c, size_t n);
+int init_new_rows(lctr_ctx* c, int64_t max_new);
 size_t keys_capacity(const lctr_ctx* c);
 
 }  // namespace lctr

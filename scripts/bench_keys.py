@@ -48,18 +48,7 @@ sys.dont_write_bytecode = True  # the tree may be read-only
 import numpy as np  # noqa: E402
 
 from bench import N_FIELDS, WORKLOADS, make_batches  # noqa: E402
-
-
-def fmix64(x):
-    """MurmurHash3's 64-bit finaliser (a bijection of uint64)"""
-    k = np.asarray(x, np.uint64).copy()
-    with np.errstate(over="ignore"):
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xff51afd7ed558ccd)
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xc4ceb9fe1a85ec53)
-        k ^= k >> np.uint64(33)
-    return k
+from lightctr_b200.dist import fmix64  # noqa: E402
 
 
 def gpu_info():

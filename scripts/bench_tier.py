@@ -34,18 +34,9 @@ sys.dont_write_bytecode = True  # the tree may be read-only
 
 import numpy as np  # noqa: E402
 
+from lightctr_b200.dist import fmix64  # noqa: E402
+
 CAP, K, ROWS, PER, TIER = 1_000_000, 16, 4096, 39, 500_000
-
-
-def fmix64(x):
-    k = np.asarray(x, np.uint64).copy()
-    with np.errstate(over="ignore"):
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xff51afd7ed558ccd)
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xc4ceb9fe1a85ec53)
-        k ^= k >> np.uint64(33)
-    return k
 
 
 def gpu_info():

@@ -7,29 +7,13 @@ import math
 import numpy as np
 import pytest
 
+from keyed_model import cells
+from lightctr_b200.dist import fmix64
+
 pytestmark = pytest.mark.gpu
 
-GOLD = 0x9E3779B97F4A7C15
 FC = 39  # fields of the FFM cases, as the C2 stream has
 CAP = 50000
-
-
-def fmix64(x):
-    """MurmurHash3's 64-bit finaliser, mod 2^64 (keys.cuh: fmix64)"""
-    k = np.asarray(x, np.uint64).copy()
-    with np.errstate(over="ignore"):
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xff51afd7ed558ccd)
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xc4ceb9fe1a85ec53)
-        k ^= k >> np.uint64(33)
-    return k
-
-
-def cells(keys, lw):
-    """counter i of each key: fmix64(x ^ ((i + 1) * 0x9E3779B97F4A7C15)) >> (64 - log2_width), i = 0..3"""
-    keys = np.asarray(keys, np.uint64)
-    return [(fmix64(keys ^ np.uint64(((i + 1) * GOLD) % (1 << 64))) >> np.uint64(64 - lw)).astype(np.int64) for i in range(4)]
 
 
 class Admit:

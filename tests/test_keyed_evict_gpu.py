@@ -9,37 +9,13 @@ import os
 import numpy as np
 import pytest
 
+from keyed_model import OPTS, Batch, Clock, bits, history, init_v, model_evict, replay
+from keyed_model import rows as _rows
+from lightctr_b200.dist import fmix64
+
 pytestmark = pytest.mark.gpu
 
 K_FM, K_NFM, K_FFM, FC_FFM = 8, 16, 3, 5  # FFM rows of 15 floats take the scalar path of the row move
-
-
-def fmix64(x):
-    """MurmurHash3's 64-bit finaliser, mod 2^64 (keys.cu: fmix64)"""
-    k = np.asarray(x, np.uint64).copy()
-    with np.errstate(over="ignore"):
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xff51afd7ed558ccd)
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xc4ceb9fe1a85ec53)
-        k ^= k >> np.uint64(33)
-    return k
-
-
-def init_v(keys, rowlen, seed, scale):
-    """the lazy-init generator of include/lightctr_b200.h / keys.cu: [len(keys), rowlen] float32"""
-    hk = fmix64(keys)[:, None]
-    j = np.arange(rowlen, dtype=np.uint64)[None, :]
-    with np.errstate(over="ignore"):
-        g = hk * np.uint64(rowlen) + j
-        h = fmix64(g * np.uint64(0x9E3779B97F4A7C15) + np.uint64(seed))
-    u1 = ((h & np.uint64(0x7fffff)).astype(np.float32) + np.float32(0.5)) * np.float32(2.0 ** -23)
-    u2 = ((h >> np.uint64(24)) & np.uint64(0xffffff)).astype(np.float32) * np.float32(2.0 ** -24)
-    r = np.sqrt(np.float32(-2.0) * np.log(u1))
-    return (np.float32(scale) * r * np.cos(np.float32(6.2831853) * u2)).astype(np.float32)
-
-
-OPTS = {"adagrad": 0, "ftrl": 1, "ps_adagrad": 6}
 
 
 def _ctx(model, cap, opt=0, key_evict=True, rows=100):
@@ -52,82 +28,14 @@ def _ctx(model, cap, opt=0, key_evict=True, rows=100):
                         key_mode=capi.KEYS_HASHED, key_evict=key_evict)
 
 
-class Batch:
-    def __init__(self, keys, per, rng):
-        self.keys = np.ascontiguousarray(keys, np.uint64)
-        rows = len(keys) // per
-        self.rp = np.arange(0, rows * per + 1, per, dtype=np.int64)
-        self.fld = (np.arange(len(keys)) % FC_FFM).astype(np.uint16)
-        self.lab = (rng.random(rows) < 0.3).astype(np.int32)
-
-    def upload(self, ctx, slot, insert=True):
-        ctx.upload_batch_keys(slot, self.rp, self.keys, self.fld if ctx.Fc else None, None, self.lab, insert=insert)
-
-
-def _history(seed, n_up=12, universe=3000, rows=100, per=6):
-    """n_up batches over a sliding window of the key universe: keys fall out of use as the window moves on"""
-    rng = np.random.default_rng(seed)
-    pool = fmix64(np.arange(universe, dtype=np.uint64) + np.uint64(1 << 33))
-    out = []
-    for i in range(n_up):
-        lo = i * universe // (2 * n_up)
-        out.append(Batch(pool[rng.integers(lo, lo + universe // 2, rows * per)], per, rng))
-    return out
-
-
-class Clock:
-    """numpy model of the stamps: key -> clock of the insert-upload that last met it"""
-
-    def __init__(self):
-        self.clock, self.stamp = 0, {}
-
-    def insert(self, keys):
-        self.clock += 1
-        for k in np.unique(keys).tolist():
-            self.stamp[k] = self.clock
-
-    def ages(self, table):
-        return np.array([self.clock - self.stamp[k] for k in table.tolist()], np.int64)
-
-
-def model_evict(table, ages, max_idle, max_rows):
-    """evicted mask over the old rows and the renumbered row -> key map (include/lightctr_b200.h)"""
-    ev = np.zeros(len(table), bool)
-    if max_idle is not None:
-        ev |= ages > max_idle
-    if max_rows is not None and (~ev).sum() > max_rows:
-        cut = np.sort(ages[~ev])[max_rows]  # a*: rows younger than the age of rank max_rows stay
-        ev |= ages >= cut
-    n_live = len(table) - int(ev.sum())
-    holes = np.nonzero(ev[:n_live])[0]
-    movers = n_live + np.nonzero(~ev[n_live:])[0]
-    assert len(holes) == len(movers)
-    new = table.copy()
-    new[holes] = table[movers]
-    return ev, new[:n_live]
-
-
-def _replay(ctx, batches, clock=None, train=False):
-    for i, b in enumerate(batches):
-        b.upload(ctx, i % 8)
-        if clock is not None:
-            clock.insert(b.keys)
-        if train:
-            ctx.train_step(i % 8)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
-
-
 # ---- 1. policy -----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("model", ["fm", "ffm", "nfm"])
 @pytest.mark.parametrize("rule", ["idle", "rows", "both"])
 def test_policy_matches_the_model_of_the_upload_history(model, rule):
-    batches = _history(11)
+    batches = history(11, 12)
     ctx = _ctx(model, 4000)
     clk = Clock()
-    _replay(ctx, batches, clk)
+    replay(ctx, batches, clk)
     table = ctx.download_keys()
     ages = clk.ages(table)
     n = len(table)
@@ -150,7 +58,7 @@ def test_ties_at_the_cutoff_leave_together():
     pool = fmix64(np.arange(300, dtype=np.uint64) + np.uint64(99))
     batches = [Batch(pool[100 * i:100 * (i + 1)], 4, rng) for i in range(3)]  # ages 2, 1, 0 for 100 rows each
     ctx = _ctx("fm", 1000)
-    _replay(ctx, batches)
+    replay(ctx, batches)
     # max_rows = 150 falls inside the age-1 group: the whole group leaves with the age-2 group
     assert ctx.evict_keys(max_rows=150) == 200
     assert np.array_equal(np.sort(ctx.download_keys()), np.sort(pool[200:]))
@@ -161,20 +69,12 @@ def test_ties_at_the_cutoff_leave_together():
 
 
 # ---- 2. state ------------------------------------------------------------------------------------------------------
-def _rows(ctx):
-    """per-row arrays W [F], V [F, rowlen], s1W, s1V, s2W, s2V (s2 zero when the rule has none)"""
-    F, r = ctx.F, ctx.rowlen
-    W, V = ctx.download_params()
-    s1, s2 = ctx.download_opt_state()
-    return [W, V.reshape(F, r), s1[:F], s1[F:].reshape(F, r), s2[:F], s2[F:].reshape(F, r)]
-
-
 @pytest.mark.parametrize("opt", ["adagrad", "ftrl", "ps_adagrad"])
 def test_survivors_keep_their_state_bit_for_bit(opt):
     cap = 4000
-    batches = _history(5, n_up=8)
+    batches = history(5, n_up=8)
     ctx = _ctx("fm", cap, OPTS[opt])
-    _replay(ctx, batches, train=True)
+    replay(ctx, batches, train=True)
     table = ctx.download_keys()
     n = len(table)
     before = _rows(ctx)
@@ -186,13 +86,13 @@ def test_survivors_keep_their_state_bit_for_bit(opt):
     old = np.array([pos[k] for k in new.tolist()])
     after = _rows(ctx)
     for a, b in zip(before, after):  # survivors by key
-        assert np.array_equal(_bits(b[:n_live]), _bits(a[old]))
+        assert np.array_equal(bits(b[:n_live]), bits(a[old]))
     ev = np.array([pos[k] for k in keys.tolist()])
-    assert np.array_equal(_bits(We), _bits(before[0][ev]))
-    assert np.array_equal(_bits(Ve), _bits(before[1][ev].ravel()))
+    assert np.array_equal(bits(We), bits(before[0][ev]))
+    assert np.array_equal(bits(Ve), bits(before[1][ev].ravel()))
     fresh = _ctx("fm", cap, OPTS[opt])
     for a, b in zip(after, _rows(fresh)):  # vacated rows as lctr_create leaves them
-        assert np.array_equal(_bits(a[n_live:]), _bits(b[n_live:]))
+        assert np.array_equal(bits(a[n_live:]), bits(b[n_live:]))
     ctx.close(); fresh.close()
 
 
@@ -201,9 +101,9 @@ def test_survivors_keep_their_state_bit_for_bit(opt):
 def test_training_after_eviction_matches_a_context_seeded_with_the_survivors(opt):
     from lightctr_b200 import capi
     cap, k = 4000, K_FM
-    batches = _history(8, n_up=8)
+    batches = history(8, n_up=8)
     a = _ctx("fm", cap, OPTS[opt])
-    _replay(a, batches, train=True)
+    replay(a, batches, train=True)
     n = len(a.download_keys())
     gone, We, Ve = a.evict_keys(max_rows=n // 2, export=True)
     live = a.download_keys()
@@ -244,17 +144,17 @@ def test_training_after_eviction_matches_a_context_seeded_with_the_survivors(opt
     a.upload_keyed_params(gone, We, Ve)
     rg = a.lookup_keys(gone)
     Wa, Va = a.download_params()
-    assert np.array_equal(_bits(Wa[rg]), _bits(We))
-    assert np.array_equal(_bits(Va.reshape(cap, k)[rg].ravel()), _bits(Ve))
+    assert np.array_equal(bits(Wa[rg]), bits(We))
+    assert np.array_equal(bits(Va.reshape(cap, k)[rg].ravel()), bits(Ve))
     a.close(); b.close()
 
 
 # ---- 4. staleness --------------------------------------------------------------------------------------------------
 def test_resident_slots_go_stale_only_when_rows_were_freed():
     from lightctr_b200 import capi
-    batches = _history(4, n_up=4)
+    batches = history(4, n_up=4)
     ctx = _ctx("fm", 4000)
-    _replay(ctx, batches)
+    replay(ctx, batches)
     assert ctx.evict_keys(max_idle=100) == 0  # nothing freed: every slot stays usable
     ctx.train_step(3)
     ctx.predict(2)
@@ -335,9 +235,9 @@ def test_one_eviction_clears_the_keys_left_without_a_row():
 def test_checkpoint_keeps_clock_and_stamps(tmp_path):
     from lightctr_b200 import capi
     cap = 4000
-    batches = _history(21, n_up=7)
+    batches = history(21, n_up=7)
     a = _ctx("fm", cap, OPTS["ftrl"])
-    _replay(a, batches, train=True)
+    replay(a, batches, train=True)
     path = str(tmp_path / "tracked.ckpt")
     a.save_checkpoint(path)
     b = _ctx("fm", cap, OPTS["ftrl"])
@@ -345,10 +245,10 @@ def test_checkpoint_keeps_clock_and_stamps(tmp_path):
     ka, Wa, Va = a.evict_keys(max_idle=2, export=True)
     kb, Wb, Vb = b.evict_keys(max_idle=2, export=True)
     assert len(ka) > 0
-    assert np.array_equal(ka, kb) and np.array_equal(_bits(Wa), _bits(Wb)) and np.array_equal(_bits(Va), _bits(Vb))
+    assert np.array_equal(ka, kb) and np.array_equal(bits(Wa), bits(Wb)) and np.array_equal(bits(Va), bits(Vb))
     assert np.array_equal(a.download_keys(), b.download_keys())
     for x, y in zip(_rows(a), _rows(b)):
-        assert np.array_equal(_bits(x), _bits(y))
+        assert np.array_equal(bits(x), bits(y))
     # the clock goes on from the restored value
     for c in (a, b):
         batches[0].upload(c, 0)
@@ -359,7 +259,7 @@ def test_checkpoint_keeps_clock_and_stamps(tmp_path):
     b.save_checkpoint(path)
     # an untracked keyed checkpoint has exactly the layout it had before key_evict existed
     u = _ctx("fm", cap, OPTS["ftrl"], key_evict=False)
-    _replay(u, batches, train=True)
+    replay(u, batches, train=True)
     upath = str(tmp_path / "untracked.ckpt")
     u.save_checkpoint(upath)
     F, r, nu = cap + 1, K_FM, len(u.download_keys())
@@ -394,9 +294,9 @@ def test_rejections_and_device_bytes():
 
 def test_too_small_export_changes_nothing():
     from lightctr_b200 import capi
-    batches = _history(31, n_up=4)
+    batches = history(31, n_up=4)
     ctx = _ctx("fm", 4000)
-    _replay(ctx, batches, train=True)
+    replay(ctx, batches, train=True)
     table = ctx.download_keys()
     before = _rows(ctx)
     keys = np.zeros(1, np.uint64)
@@ -405,7 +305,7 @@ def test_too_small_export_changes_nothing():
     assert rc != 0 and "room for 1" in capi.load_library().lctr_last_error().decode()
     assert np.array_equal(ctx.download_keys(), table)
     for x, y in zip(before, _rows(ctx)):
-        assert np.array_equal(_bits(x), _bits(y))
+        assert np.array_equal(bits(x), bits(y))
     ctx.train_step(3)  # slots stay usable
     assert ctx.evict_keys(max_idle=0) > 0
     ctx.close()

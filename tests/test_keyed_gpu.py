@@ -6,31 +6,10 @@ keys, checkpoints and refused calls behave as include/lightctr_b200.h states."""
 import numpy as np
 import pytest
 
+from keyed_model import OPTS, init_v
+from lightctr_b200.dist import fmix64
+
 pytestmark = pytest.mark.gpu
-
-def fmix64(x):
-    """MurmurHash3's 64-bit finaliser, mod 2^64 (keys.cu: fmix64)"""
-    k = np.asarray(x, np.uint64).copy()
-    with np.errstate(over="ignore"):
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xff51afd7ed558ccd)
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xc4ceb9fe1a85ec53)
-        k ^= k >> np.uint64(33)
-    return k
-
-
-def init_v(keys, rowlen, seed, scale):
-    """numpy restatement of the lazy-init generator of include/lightctr_b200.h / keys.cu: [len(keys), rowlen] float32"""
-    hk = fmix64(keys)[:, None]
-    j = np.arange(rowlen, dtype=np.uint64)[None, :]
-    with np.errstate(over="ignore"):
-        g = hk * np.uint64(rowlen) + j
-        h = fmix64(g * np.uint64(0x9E3779B97F4A7C15) + np.uint64(seed))
-    u1 = ((h & np.uint64(0x7fffff)).astype(np.float32) + np.float32(0.5)) * np.float32(2.0 ** -23)
-    u2 = ((h >> np.uint64(24)) & np.uint64(0xffffff)).astype(np.float32) * np.float32(2.0 ** -24)
-    r = np.sqrt(np.float32(-2.0) * np.log(u1))
-    return (np.float32(scale) * r * np.cos(np.float32(6.2831853) * u2)).astype(np.float32)
 
 
 def _rel(a, b):
@@ -47,9 +26,6 @@ def _params_close(got, want, tol, threshold_updater):
     if not threshold_updater:
         return float(d.max()) < tol
     return float(np.mean(d > tol)) <= 1e-5 and float(d.max()) < 1e-2
-
-
-OPTS = {"adagrad": 0, "ftrl": 1, "ps_adagrad": 6}
 
 
 @pytest.mark.parametrize("opt", ["adagrad", "ftrl", "ps_adagrad"])

@@ -5,66 +5,13 @@ in at most one of them, and only lctr_evict_host_tier drops one."""
 import numpy as np
 import pytest
 
+from keyed_model import OPTS, Batch, Clock, bits, history, init_v, model_evict, replay
+from keyed_model import rows as _rows
+from lightctr_b200.dist import fmix64
+
 pytestmark = pytest.mark.gpu
 
 K_FM, K_NFM, K_FFM, FC_FFM = 8, 16, 3, 5  # FFM rows of 15 floats take the scalar copies
-OPTS = {"adagrad": 0, "ftrl": 1, "ps_adagrad": 6}
-
-
-def fmix64(x):
-    """MurmurHash3's 64-bit finaliser, mod 2^64 (keys.cu: fmix64)"""
-    k = np.asarray(x, np.uint64).copy()
-    with np.errstate(over="ignore"):
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xff51afd7ed558ccd)
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xc4ceb9fe1a85ec53)
-        k ^= k >> np.uint64(33)
-    return k
-
-
-def init_v(keys, rowlen, seed, scale):
-    """the lazy-init generator of include/lightctr_b200.h / keys.cu: [len(keys), rowlen] float32"""
-    hk = fmix64(keys)[:, None]
-    j = np.arange(rowlen, dtype=np.uint64)[None, :]
-    with np.errstate(over="ignore"):
-        g = hk * np.uint64(rowlen) + j
-        h = fmix64(g * np.uint64(0x9E3779B97F4A7C15) + np.uint64(seed))
-    u1 = ((h & np.uint64(0x7fffff)).astype(np.float32) + np.float32(0.5)) * np.float32(2.0 ** -23)
-    u2 = ((h >> np.uint64(24)) & np.uint64(0xffffff)).astype(np.float32) * np.float32(2.0 ** -24)
-    r = np.sqrt(np.float32(-2.0) * np.log(u1))
-    return (np.float32(scale) * r * np.cos(np.float32(6.2831853) * u2)).astype(np.float32)
-
-
-class Clock:
-    """numpy model of the stamps: key -> clock of the insert-upload that last met it"""
-
-    def __init__(self):
-        self.clock, self.stamp = 0, {}
-
-    def insert(self, keys):
-        self.clock += 1
-        for k in np.unique(keys).tolist():
-            self.stamp[k] = self.clock
-
-    def ages(self, table):
-        return np.array([self.clock - self.stamp[k] for k in table.tolist()], np.int64)
-
-
-def model_evict(table, ages, max_idle, max_rows):
-    """evicted mask over the old rows and the renumbered row -> key map (include/lightctr_b200.h)"""
-    ev = np.zeros(len(table), bool)
-    if max_idle is not None:
-        ev |= ages > max_idle
-    if max_rows is not None and (~ev).sum() > max_rows:
-        cut = np.sort(ages[~ev])[max_rows]
-        ev |= ages >= cut
-    n_live = len(table) - int(ev.sum())
-    holes = np.nonzero(ev[:n_live])[0]
-    movers = n_live + np.nonzero(~ev[n_live:])[0]
-    new = table.copy()
-    new[holes] = table[movers]
-    return ev, new[:n_live]
 
 
 def _ctx(model, cap, opt=0, tier=0, key_evict=True, rows=100):
@@ -75,47 +22,6 @@ def _ctx(model, cap, opt=0, tier=0, key_evict=True, rows=100):
     if model == "ffm":
         return capi.Context(capi.MODEL_FFM, cap, K_FFM, FC_FFM, **kw)
     return capi.Context(capi.MODEL_NFM, cap, K_NFM, hidden=(32,), minibatch_size=rows, **kw)
-
-
-class Batch:
-    def __init__(self, keys, per, rng):
-        self.keys = np.ascontiguousarray(keys, np.uint64)
-        rows = len(keys) // per
-        self.rp = np.arange(0, rows * per + 1, per, dtype=np.int64)
-        self.fld = (np.arange(len(keys)) % FC_FFM).astype(np.uint16)
-        self.lab = (rng.random(rows) < 0.3).astype(np.int32)
-
-    def upload(self, ctx, slot, insert=True):
-        ctx.upload_batch_keys(slot, self.rp, self.keys, self.fld if ctx.Fc else None, None, self.lab, insert=insert)
-
-
-def _history(seed, n_up=8, universe=3000, rows=100, per=6):
-    """batches over a sliding window of the key universe: keys fall out of use as the window moves on"""
-    rng = np.random.default_rng(seed)
-    pool = fmix64(np.arange(universe, dtype=np.uint64) + np.uint64(1 << 33))
-    return [Batch(pool[rng.integers(i * universe // (2 * n_up), i * universe // (2 * n_up) + universe // 2, rows * per)], per, rng)
-            for i in range(n_up)]
-
-
-def _replay(ctx, batches, clock=None, train=False):
-    for i, b in enumerate(batches):
-        b.upload(ctx, i % 8)
-        if clock is not None:
-            clock.insert(b.keys)
-        if train:
-            ctx.train_step(i % 8)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
-
-
-def _rows(ctx):
-    """per-row arrays W [F], V [F, rowlen], s1W, s1V, s2W, s2V (s2 zero when the rule has none)"""
-    F, r = ctx.F, ctx.rowlen
-    W, V = ctx.download_params()
-    s1, s2 = ctx.download_opt_state()
-    return [W, V.reshape(F, r), s1[:F], s1[F:].reshape(F, r), s2[:F], s2[F:].reshape(F, r)]
 
 
 def _by_key(ctx):
@@ -132,9 +38,9 @@ def _tier(ctx):
 def _same_state(ctx, before):
     assert np.array_equal(ctx.download_keys(), before[0])
     for x, y in zip(before[1], _rows(ctx)):
-        assert np.array_equal(_bits(x), _bits(y))
+        assert np.array_equal(bits(x), bits(y))
     for x, y in zip(before[2], _tier(ctx)):
-        assert np.array_equal(_bits(x) if x.dtype != np.uint64 else x, _bits(y) if y.dtype != np.uint64 else y)
+        assert np.array_equal(bits(x) if x.dtype != np.uint64 else x, bits(y) if y.dtype != np.uint64 else y)
 
 
 def _state(ctx):
@@ -147,20 +53,20 @@ def _same_model(a, b):
     assert sorted(ka) == sorted(kb)
     for k, va in ka.items():
         for x, y in zip(va, kb[k]):
-            assert np.array_equal(_bits(np.atleast_1d(x)), _bits(np.atleast_1d(y)))
+            assert np.array_equal(bits(np.atleast_1d(x)), bits(np.atleast_1d(y)))
     ta, tb = _tier(a), _tier(b)
     ia, ib = np.argsort(ta[0]), np.argsort(tb[0])
     assert np.array_equal(ta[0][ia], tb[0][ib])
     for x, y in zip(ta[1:], tb[1:]):
-        assert np.array_equal(_bits(x[ia]), _bits(y[ib]))
+        assert np.array_equal(bits(x[ia]), bits(y[ib]))
 
 
 # ---- 1. spill ------------------------------------------------------------------------------------------------------
 def test_spill_leaves_the_device_as_an_untiered_eviction_and_keeps_the_rows():
-    batches = _history(5)
+    batches = history(5, 8)
     ctx = _ctx("fm", 4000, OPTS["ftrl"], tier=4000)
     clk = Clock()
-    _replay(ctx, batches, clk, train=True)
+    replay(ctx, batches, clk, train=True)
     table = ctx.download_keys()
     n = len(table)
     before = _rows(ctx)
@@ -171,11 +77,11 @@ def test_spill_leaves_the_device_as_an_untiered_eviction_and_keeps_the_rows():
     pos = {k: i for i, k in enumerate(table.tolist())}
     old = np.array([pos[k] for k in new.tolist()])
     for a, b in zip(before, _rows(ctx)):
-        assert np.array_equal(_bits(b[:len(new)]), _bits(a[old]))
+        assert np.array_equal(bits(b[:len(new)]), bits(a[old]))
     tk, tW, tV = _tier(ctx)
     assert np.array_equal(tk, keys)
-    assert np.array_equal(_bits(tW), _bits(We)) and np.array_equal(_bits(tV.ravel()), _bits(Ve))
-    assert np.array_equal(_bits(We), _bits(before[0][:n][ev])) and np.array_equal(_bits(Ve), _bits(before[1][:n][ev].ravel()))
+    assert np.array_equal(bits(tW), bits(We)) and np.array_equal(bits(tV.ravel()), bits(Ve))
+    assert np.array_equal(bits(We), bits(before[0][:n][ev])) and np.array_equal(bits(Ve), bits(before[1][:n][ev].ravel()))
     ctx.close()
 
 
@@ -184,8 +90,8 @@ def test_spill_leaves_the_device_as_an_untiered_eviction_and_keeps_the_rows():
 @pytest.mark.parametrize("opt", ["adagrad", "ftrl", "ps_adagrad"])
 def test_returning_keys_get_their_rows_back_bit_for_bit(model, opt):
     ctx = _ctx(model, 4000, OPTS[opt], tier=4000)
-    batches = _history(7)
-    _replay(ctx, batches, train=True)
+    batches = history(7, 8)
+    replay(ctx, batches, train=True)
     before = _by_key(ctx)
     n = len(before)
     gone, _, _ = ctx.evict_keys(max_rows=n // 2, export=True)
@@ -202,12 +108,12 @@ def test_returning_keys_get_their_rows_back_bit_for_bit(model, opt):
     assert np.all(rows >= 0)
     for k, r in zip(ret.tolist(), rows.tolist()):
         for a, b in zip(before[k], after):
-            assert np.array_equal(_bits(np.atleast_1d(a)), _bits(np.atleast_1d(b[r])))
+            assert np.array_equal(bits(np.atleast_1d(a)), bits(np.atleast_1d(b[r])))
     tk, tW, tV = _tier(ctx)
     assert np.array_equal(np.sort(tk), np.setdiff1d(gone, ret))
     p0 = {k: i for i, k in enumerate(tk0.tolist())}
     idx = np.array([p0[k] for k in tk.tolist()])
-    assert np.array_equal(_bits(tW), _bits(tW0[idx])) and np.array_equal(_bits(tV), _bits(tV0[idx]))
+    assert np.array_equal(bits(tW), bits(tW0[idx])) and np.array_equal(bits(tV), bits(tV0[idx]))
     assert np.isfinite(ctx.train_step(0)[0])
     ctx.close()
 
@@ -215,7 +121,7 @@ def test_returning_keys_get_their_rows_back_bit_for_bit(model, opt):
 # ---- 3. nothing is lost ------------------------------------------------------------------------------------------------
 def test_every_uploaded_key_stays_in_exactly_one_table():
     ctx = _ctx("fm", 1200, tier=20000)
-    batches = _history(3, n_up=16, universe=6000)
+    batches = history(3, n_up=16, universe=6000)
     seen = set()
     for i, b in enumerate(batches):
         if i % 3 == 2:
@@ -267,7 +173,7 @@ def test_tiered_training_matches_a_context_that_never_evicts(unique):
         want_W = Wb[np.concatenate([rd, rt])]
         want_V = Vb.reshape(-1, K_FM)[np.concatenate([rd, rt])]
         if unique:
-            assert np.array_equal(_bits(got_W), _bits(want_W)) and np.array_equal(_bits(got_V), _bits(want_V)), i
+            assert np.array_equal(bits(got_W), bits(want_W)) and np.array_equal(bits(got_V), bits(want_V)), i
         else:
             assert np.max(np.abs(got_W - want_W)) < 2e-5 and np.max(np.abs(got_V - want_V)) < 2e-5, i
     assert len(t.download_host_tier()[0]) > 0
@@ -279,8 +185,8 @@ def test_lookup_only_upload_restores_tier_keys_and_keeps_their_stamps():
     from lightctr_b200 import capi
     ctx = _ctx("fm", 4000, tier=4000)
     clk = Clock()
-    batches = _history(13)
-    _replay(ctx, batches, clk, train=True)
+    batches = history(13, 8)
+    replay(ctx, batches, clk, train=True)
     gone, _, _ = ctx.evict_keys(max_idle=3, export=True)
     assert len(gone) > 20
     rng = np.random.default_rng(4)
@@ -310,7 +216,7 @@ def test_spill_into_a_full_tier_changes_nothing():
     rng = np.random.default_rng(17)
     pool = fmix64(np.arange(400, dtype=np.uint64) + np.uint64(77))
     ctx = _ctx("fm", 4000, tier=150)
-    _replay(ctx, [Batch(pool[100 * i:100 * (i + 1)], 4, rng) for i in range(4)], train=True)  # ages 3, 2, 1, 0
+    replay(ctx, [Batch(pool[100 * i:100 * (i + 1)], 4, rng) for i in range(4)], train=True)  # ages 3, 2, 1, 0
     before = _state(ctx)
     with pytest.raises(capi.LctrError, match=r"150 rows \(cfg.key_host_rows\) with 150 free"):
         ctx.evict_keys(max_idle=0)
@@ -348,7 +254,7 @@ def test_restore_past_the_device_capacity_fails_and_keeps_the_keys_in_the_tier(i
     def tier_unchanged():  # every key left in the tier keeps its row bit for bit
         k, W, V = _tier(ctx)
         idx = np.array([at[x] for x in k.tolist()])
-        assert np.array_equal(_bits(W), _bits(W0[idx])) and np.array_equal(_bits(V), _bits(V0[idx]))
+        assert np.array_equal(bits(W), bits(W0[idx])) and np.array_equal(bits(V), bits(V0[idx]))
         return k
 
     tier_unchanged()
@@ -377,7 +283,7 @@ def test_spills_past_half_the_index_rebuild_it_and_lose_nothing():
         assert np.all(rows >= 0)
         for key, r in zip(keys.tolist(), rows.tolist()):
             for x, y in zip(before[key], after):
-                assert np.array_equal(_bits(np.atleast_1d(x)), _bits(np.atleast_1d(y[r])))
+                assert np.array_equal(bits(np.atleast_1d(x)), bits(np.atleast_1d(y[r])))
 
     assert ctx.evict_keys(max_idle=0) == 100  # A: 100 slots claimed
     assert np.array_equal(np.sort(ctx.download_host_tier()[0]), np.sort(A.keys))
@@ -397,7 +303,7 @@ def test_spills_past_half_the_index_rebuild_it_and_lose_nothing():
 def test_evict_host_tier_follows_the_rule_on_tier_stamps():
     ctx = _ctx("fm", 4000, tier=4000)
     clk = Clock()
-    batches = _history(19, n_up=10)
+    batches = history(19, n_up=10)
     for i, b in enumerate(batches):
         b.upload(ctx, 0)
         clk.insert(b.keys)
@@ -410,11 +316,11 @@ def test_evict_host_tier_follows_the_rule_on_tier_stamps():
     assert 0 < ev.sum() < len(tier)
     keys, W, V = ctx.evict_host_tier(7, int(len(tier) * 0.4), export=True)
     assert np.array_equal(keys, tier[ev])
-    assert np.array_equal(_bits(W), _bits(tW[ev])) and np.array_equal(_bits(V), _bits(tV[ev].ravel()))
+    assert np.array_equal(bits(W), bits(tW[ev])) and np.array_equal(bits(V), bits(tV[ev].ravel()))
     tk, tW2, _ = _tier(ctx)
     assert np.array_equal(tk, new)
     pos = {k: i for i, k in enumerate(tier.tolist())}
-    assert np.array_equal(_bits(tW2), _bits(tW[[pos[k] for k in new.tolist()]]))
+    assert np.array_equal(bits(tW2), bits(tW[[pos[k] for k in new.tolist()]]))
     # the freed keys left the model: they come back as new keys, the kept ones from the tier
     back = np.concatenate([keys[:5], new[:5]])
     Batch(back, 2, np.random.default_rng(0)).upload(ctx, 1)
@@ -422,16 +328,16 @@ def test_evict_host_tier_follows_the_rule_on_tier_stamps():
     r = ctx.lookup_keys(back)
     assert np.all(W_dev[r[:5]] == 0)
     assert np.max(np.abs(V_dev.reshape(-1, K_FM)[r[:5]] - init_v(keys[:5], K_FM, 0, 1 / np.sqrt(K_FM)))) < 1e-6
-    assert np.array_equal(_bits(W_dev[r[5:]]), _bits(tW2[:5]))
+    assert np.array_equal(bits(W_dev[r[5:]]), bits(tW2[:5]))
     ctx.close()
 
 
 # ---- 7. checkpoint -------------------------------------------------------------------------------------------------
 def test_checkpoint_round_trip_and_refusals(tmp_path):
     from lightctr_b200 import capi
-    batches = _history(23)
+    batches = history(23, 8)
     a = _ctx("fm", 4000, OPTS["ftrl"], tier=3000)
-    _replay(a, batches, train=True)
+    replay(a, batches, train=True)
     a.evict_keys(max_idle=2)
     path = str(tmp_path / "tiered.ckpt")
     a.save_checkpoint(path)
@@ -447,11 +353,11 @@ def test_checkpoint_round_trip_and_refusals(tmp_path):
     _same_model(a, b)
     # refused loads, each leaving the context as it was
     u = _ctx("fm", 4000, OPTS["ftrl"])
-    _replay(u, batches[:3], train=True)
+    replay(u, batches[:3], train=True)
     upath = str(tmp_path / "untiered.ckpt")
     u.save_checkpoint(upath)
     small = _ctx("fm", 4000, OPTS["ftrl"], tier=10)
-    _replay(small, batches[:2], train=True)
+    replay(small, batches[:2], train=True)
     for ctx, p, msg in [(u, path, "different trainer"), (b, upath, "different trainer"), (small, path, "key_host_rows = 10")]:
         before = _state(ctx) if ctx is not u else (ctx.download_keys(), _rows(ctx))
         with pytest.raises(capi.LctrError, match=msg):
@@ -459,7 +365,7 @@ def test_checkpoint_round_trip_and_refusals(tmp_path):
         if ctx is u:
             assert np.array_equal(ctx.download_keys(), before[0])
             for x, y in zip(before[1], _rows(ctx)):
-                assert np.array_equal(_bits(x), _bits(y))
+                assert np.array_equal(bits(x), bits(y))
         else:
             _same_state(ctx, before)
     a.close(); b.close(); u.close(); small.close()
