@@ -58,10 +58,8 @@ int reset_table_rows(lctr_ctx* c) {
         LCTR_CUDA(cudaMemsetAsync(c->s1W, 0, c->Fl * sizeof(float), c->stream));
         LCTR_CUDA(cudaMemsetAsync(c->s1V, 0, nv * sizeof(float), c->stream));
     } else {
-        fill_value_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(c->s1W, c->Fl, s1);
-        fill_value_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(c->s1V, nv, s1);
-        c->launches += 2;
-        LCTR_CUDA(cudaGetLastError());
+        const Launch l{(unsigned)c->sm_count * 4, 256, 0, c->stream};
+        if (launch(c, l, fill_value_kernel, c->s1W, c->Fl, s1) || launch(c, l, fill_value_kernel, c->s1V, nv, s1)) return 1;
     }
     if (c->s2W) {
         LCTR_CUDA(cudaMemsetAsync(c->s2W, 0, c->Fl * sizeof(float), c->stream));
@@ -389,10 +387,9 @@ int lctr_download_params(lctr_ctx* c, float* W, float* V) {
 }
 int lctr_fill_params(lctr_ctx* c, uint64_t seed, float scale) {
     LCTR_CHECK(c, "null ctx");
-    fill_params_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->W, c->V, c->Fl, c->rowlen, c->cfg.rank, c->cfg.world,
-                                                               (unsigned long long)seed, scale);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
+    if (launch(c, {(unsigned)c->sm_count * 8, 256, 0, c->stream}, fill_params_kernel, c->W, c->V, c->Fl, c->rowlen, c->cfg.rank,
+               c->cfg.world, (unsigned long long)seed, scale))
+        return 1;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }
@@ -500,11 +497,8 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
     if (rows) {
         // labels travel as int32 and are widened on device (the reference compares a `float target`)
         LCTR_CUDA(cudaMemcpyAsync(tmp, label, (size_t)rows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-        if (!grouped) {
-            label_to_float_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>(tmp, s.label, rows, nullptr);
-            c->launches++;
-            LCTR_CUDA(cudaGetLastError());
-        }
+        if (!grouped && launch(c, {(unsigned)((rows + 255) / 256), 256, 0, st}, label_to_float_kernel, tmp, s.label, rows, nullptr))
+            return 1;
     }
     s.fused_valid = false;
     s.key_state = SLOT_KEYS_OK;
@@ -747,6 +741,21 @@ static int pipe_init(lctr_ctx* c) {
 // forward, grouped backward + update, result copy, on the compute stream).  Kernels take the batch size from the
 // device-side slot header and the updater parameters from device memory, so the graphs are static: a streamed step
 // costs the host three cudaMemcpyAsync, two graph launches and four event calls instead of ~20 launches.
+// *n = the kernel nodes of a captured graph
+static int count_kernel_nodes(cudaGraph_t graph, int* n) {
+    *n = 0;
+    size_t count = 0;
+    LCTR_CUDA(cudaGraphGetNodes(graph, nullptr, &count));
+    std::vector<cudaGraphNode_t> nodes(count);
+    LCTR_CUDA(cudaGraphGetNodes(graph, nodes.data(), &count));
+    for (cudaGraphNode_t node : nodes) {
+        cudaGraphNodeType t;
+        LCTR_CUDA(cudaGraphNodeGetType(node, &t));
+        *n += t == cudaGraphNodeTypeKernel;
+    }
+    return 0;
+}
+
 static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
     PipeGraph& g = c->pipe_graph[p];
     Slot& s = c->slots[kNumSlots - kPipe + p];
@@ -773,16 +782,16 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
     int rc = cudaMemcpyAsync(g.d_hdr, g.h_hdr, 2 * sizeof(int64_t), cudaMemcpyHostToDevice, c->copy_stream) != cudaSuccess;
     if (!rc) {
         if (fused) {  // labels widened, then the slot map of the batch (fm_fused.cu)
-            label_to_float_kernel<<<(unsigned)((s.cap_rows + 255) / 256), 256, 0, c->copy_stream>>>(
-                reinterpret_cast<int32_t*>(s.pred), s.label, s.cap_rows, g.d_hdr);
-            c->launches++;
-            rc = fused_build_slot(c, s, c->copy_stream, g.d_hdr, s.cap_rows, s.cap_nnz);
+            rc = launch(c, {(unsigned)((s.cap_rows + 255) / 256), 256, 0, c->copy_stream}, label_to_float_kernel,
+                        reinterpret_cast<int32_t*>(s.pred), s.label, s.cap_rows, g.d_hdr) ||
+                 fused_build_slot(c, s, c->copy_stream, g.d_hdr, s.cap_rows, s.cap_nnz);
         } else {
             rc = csc_build_device(c, s, c->copy_stream, reinterpret_cast<int32_t*>(s.pred), g.d_hdr, s.cap_rows, s.cap_nnz);
         }
     }
     cudaError_t ce = cudaStreamEndCapture(c->copy_stream, &graph);  // always closes the capture, also on error paths
     if (rc || ce != cudaSuccess) { set_error("streamed pipeline: capture of the build graph failed (%s)", cudaGetErrorString(ce)); return 1; }
+    if (count_kernel_nodes(graph, &g.build_kernels)) return 1;
     LCTR_CUDA(cudaGraphInstantiate(&g.build, graph, 0));
     cudaGraphDestroy(graph);
     // ---- step graph (compute stream)
@@ -800,6 +809,7 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
     if (!rc) rc = cudaMemcpyAsync(g.h_stat, g.d_stat, 2 * sizeof(double), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess;
     ce = cudaStreamEndCapture(c->stream, &graph);
     if (rc || ce != cudaSuccess) { set_error("streamed pipeline: capture of the step graph failed (%s)", cudaGetErrorString(ce)); return 1; }
+    if (count_kernel_nodes(graph, &g.step_kernels)) return 1;
     LCTR_CUDA(cudaGraphInstantiate(&g.step, graph, 0));
     cudaGraphDestroy(graph);
     g.cap_rows = s.cap_rows; g.cap_nnz = s.cap_nnz; g.has_val = has_val;
@@ -835,15 +845,14 @@ static int train_batch_async_graph(lctr_ctx* c, int64_t rows, int64_t nnz, const
     // build kernels share scratch buffers, so they stay serialised among themselves -- on this one stream)
     LCTR_CUDA(cudaEventRecord(c->ev_h2d[p], c->copy_stream));
     LCTR_CUDA(cudaStreamWaitEvent(c->build_stream, c->ev_h2d[p], 0));
-    LCTR_CUDA(cudaGraphLaunch(g.build, c->build_stream));
+    if (launch_graph(c, g.build, g.build_kernels, c->build_stream)) return 1;
     LCTR_CUDA(cudaEventRecord(c->ev_copied[p], c->build_stream));
     LCTR_CUDA(cudaStreamWaitEvent(c->stream, c->ev_copied[p], 0));
     if (fused) fused_opt_params(c, rows, g.h_opt); else csc_opt_params(c, rows, g.h_opt);
-    LCTR_CUDA(cudaGraphLaunch(g.step, c->stream));
+    if (launch_graph(c, g.step, g.step_kernels, c->stream)) return 1;
     LCTR_CUDA(cudaEventRecord(c->ev_computed[p], c->stream));
     s.dev_csc = !fused;
     s.fused_valid = fused;
-    c->launches += 8;  // kernels inside the two graphs (6 + 2 on the fused path, 5 + 3 on the grouped one)
     g.ticket = c->step;
     *ticket = c->step++;
     c->pipe_issued++;

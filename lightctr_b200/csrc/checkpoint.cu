@@ -308,16 +308,12 @@ static int scatter_section(lctr_ctx* c, Stage& st, FILE* f, float* dst, size_t n
         if (map) LCTR_CUDA(cudaMemcpyAsync(st.dmap, map + l0, m * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
         rule.map = map ? st.dmap : nullptr;
         rule.l0 = l0;
-        if (rowlen == 1) {
-            reshard_scalars_kernel<<<(unsigned)std::max<size_t>(1, std::min((m + 255) / 256, grid_cap)), 256, 0, c->stream>>>(
-                st.d, dst, m, rule);
-        } else {
-            const unsigned grid = (unsigned)std::max<size_t>(1, std::min((m + 7) / 8, grid_cap));
-            if (rowlen % 4 == 0) reshard_rows_kernel<true><<<grid, 256, 0, c->stream>>>(st.d, dst, m, rowlen, rule);
-            else reshard_rows_kernel<false><<<grid, 256, 0, c->stream>>>(st.d, dst, m, rowlen, rule);
-        }
-        c->launches++;
-        LCTR_CUDA(cudaGetLastError());
+        const int rc = rowlen == 1
+            ? launch(c, {(unsigned)std::max<size_t>(1, std::min((m + 255) / 256, grid_cap)), 256, 0, c->stream},
+                     reshard_scalars_kernel, st.d, dst, m, rule)
+            : launch(c, {(unsigned)std::max<size_t>(1, std::min((m + 7) / 8, grid_cap)), 256, 0, c->stream},
+                     rowlen % 4 == 0 ? reshard_rows_kernel<true> : reshard_rows_kernel<false>, st.d, dst, m, rowlen, rule);
+        if (rc) return 1;
         LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the host chunk is refilled next
     }
     return 0;

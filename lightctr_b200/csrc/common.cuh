@@ -114,6 +114,7 @@ struct PipeGraph {
     void *d_opt = nullptr, *h_opt = nullptr;     // updater parameters of the step
     double *d_stat = nullptr, *h_stat = nullptr; // (loss, correct)
     uint64_t ticket = ~0ull;
+    int build_kernels = 0, step_kernels = 0;  // kernel nodes of each graph: the launches its replay counts
 };
 
 struct MlpLayer {
@@ -426,9 +427,8 @@ inline size_t mlp_in0(const lctr_cfg& cf) {
     return cf.model == LCTR_MODEL_WND ? (size_t)cf.field_cnt * cf.factor_cnt : (size_t)cf.factor_cnt;
 }
 int mlp_sync_dense_grad(lctr_ctx* c);
-bool pdl_on();  // LCTR_PDL != 0 (fm_fused.cu)
 // scan + clear of a permuted byte map (fm_fused.cuh): appends the ids of the set positions to uniq, counts in *n_uniq
-void launch_slotmap_compact(lctr_ctx* c, uint8_t* mark, size_t T, uint32_t* uniq, unsigned int* n_uniq, cudaStream_t st);
+int launch_slotmap_compact(lctr_ctx* c, uint8_t* mark, size_t T, uint32_t* uniq, unsigned int* n_uniq, cudaStream_t st);
 int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats);  // 0 launched, -1 shape not covered, 1 error
 int mlp_bf16_prepare(lctr_ctx* c);
 int mlp_bf16_refresh(lctr_ctx* c, int layer);
@@ -474,3 +474,5 @@ inline float initial_s1(const lctr_cfg& cf) {
 int reset_table_rows(lctr_ctx* c);
 
 }  // namespace lctr
+
+#include "launch.cuh"  // launch(): every kernel launch of the library

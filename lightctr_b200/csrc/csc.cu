@@ -474,18 +474,15 @@ int csc_build_device(lctr_ctx* c, Slot& s, cudaStream_t st, const int32_t* label
     if (!hdr && csc_reserve(c, s, nnz)) return 1;
     const unsigned g1 = (unsigned)std::min<int64_t>((nnz + 255) / 256, (int64_t)c->sm_count * 8);
     const unsigned gt = (unsigned)std::min<size_t>((sc->ntiles + 7) / 8, (size_t)c->sm_count * 8);
-    csc_count_kernel<<<std::max(g1, 1u), 256, 0, st>>>(s.fid, s.nnz, sc->cnt, label_i32, s.label, s.rows, hdr);
-    csc_tile_reduce_kernel<<<std::max(gt, 1u), 256, 0, st>>>(sc->cnt, c->F, sc->tile_sum);
-    csc_tile_scan_kernel<<<1, 1024, 0, st>>>(sc->tile_sum, sc->ntiles, sc->tile_off, s.csc_totals, s.seg_ptr);
-    csc_tile_write_kernel<<<std::max(gt, 1u), 256, 0, st>>>(sc->cnt, c->F, sc->tile_off, sc->off, s.seg_fid, s.seg_ptr,
-                                                           s.short_list, reinterpret_cast<uint2*>(s.long_list),
-                                                           s.csc_totals);
     const unsigned gf = (unsigned)std::min<int64_t>((rows + 7) / 8, (int64_t)c->sm_count * 8);
-    csc_fill_kernel<<<std::max(gf, 1u), 256, 0, st>>>(s.row_ptr, s.fid, s.has_val ? s.val : nullptr, s.rows, sc->off,
-                                                     sc->cnt, s.ent_row, s.ent_x, hdr,
-                                                     s.has_field ? s.field : nullptr, s.ent_field);
-    c->launches += 5;
-    LCTR_CUDA(cudaGetLastError());
+    if (launch(c, {std::max(g1, 1u), 256, 0, st}, csc_count_kernel, s.fid, s.nnz, sc->cnt, label_i32, s.label, s.rows, hdr) ||
+        launch(c, {std::max(gt, 1u), 256, 0, st}, csc_tile_reduce_kernel, sc->cnt, c->F, sc->tile_sum) ||
+        launch(c, {1, 1024, 0, st}, csc_tile_scan_kernel, sc->tile_sum, sc->ntiles, sc->tile_off, s.csc_totals, s.seg_ptr) ||
+        launch(c, {std::max(gt, 1u), 256, 0, st}, csc_tile_write_kernel, sc->cnt, c->F, sc->tile_off, sc->off, s.seg_fid, s.seg_ptr,
+               s.short_list, reinterpret_cast<uint2*>(s.long_list), s.csc_totals) ||
+        launch(c, {std::max(gf, 1u), 256, 0, st}, csc_fill_kernel, s.row_ptr, s.fid, s.has_val ? s.val : nullptr, s.rows, sc->off,
+               sc->cnt, s.ent_row, s.ent_x, hdr, s.has_field ? s.field : nullptr, s.ent_field))
+        return 1;
     s.dev_csc = true;
     s.csc_block = 0;
     return 0;
@@ -497,14 +494,10 @@ static int bwd_go(lctr_ctx* c, Slot& s, const OptParams& P, const OptParams* dP)
     const CscView C{s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, s.label, s.pred, s.sumvx};
     const ParamView T{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V};
     const uint2* longs = reinterpret_cast<const uint2*>(s.long_list);
-    if (s.has_val) {
-        csc_backward_long_kernel<K, true><<<grid, 256, 0, c->stream>>>(longs, s.csc_totals, C, T, s.csc_acc, s.csc_arrived, c->cfg.l2_reg, P, dP);
-        csc_backward_short_kernel<K, true><<<grid, 256, 0, c->stream>>>(s.short_list, s.csc_totals, C, T, c->cfg.l2_reg, P, dP);
-    } else {
-        csc_backward_long_kernel<K, false><<<grid, 256, 0, c->stream>>>(longs, s.csc_totals, C, T, s.csc_acc, s.csc_arrived, c->cfg.l2_reg, P, dP);
-        csc_backward_short_kernel<K, false><<<grid, 256, 0, c->stream>>>(s.short_list, s.csc_totals, C, T, c->cfg.l2_reg, P, dP);
-    }
-    return 0;
+    return launch(c, {grid, 256, 0, c->stream}, s.has_val ? csc_backward_long_kernel<K, true> : csc_backward_long_kernel<K, false>,
+                  longs, s.csc_totals, C, T, s.csc_acc, s.csc_arrived, c->cfg.l2_reg, P, dP) ||
+           launch(c, {grid, 256, 0, c->stream}, s.has_val ? csc_backward_short_kernel<K, true> : csc_backward_short_kernel<K, false>,
+                  s.short_list, s.csc_totals, C, T, c->cfg.l2_reg, P, dP);
 }
 
 // dP != nullptr (graph capture): the updater parameters are read from device memory at run time
@@ -518,17 +511,14 @@ int launch_fm_backward_devcsc_ex(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, c
     ProfScope prof(c, PROF_FM_BWD_CSC);
     const OptParams* d = reinterpret_cast<const OptParams*>(dP);
     switch (k) {
-        case 4: bwd_go<4>(c, s, P, d); break;
-        case 8: bwd_go<8>(c, s, P, d); break;
-        case 16: bwd_go<16>(c, s, P, d); break;
-        case 32: bwd_go<32>(c, s, P, d); break;
+        case 4: return bwd_go<4>(c, s, P, d);
+        case 8: return bwd_go<8>(c, s, P, d);
+        case 16: return bwd_go<16>(c, s, P, d);
+        case 32: return bwd_go<32>(c, s, P, d);
         default:
             set_error("device feature-major backward is built for k in {4, 8, 16, 32} (k=%d)", k);
             return 1;
     }
-    c->launches += 2;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
 }
 
 int launch_fm_backward_devcsc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {

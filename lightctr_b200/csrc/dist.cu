@@ -702,30 +702,8 @@ merge_apply_kernel(PeerTable P, ArenaLayout A, int me, int world, unsigned long 
 }
 
 template <int K>
-static void merge_apply_go(lctr_ctx* c, DistState* d, int slot, const OptParams& Pp, unsigned grid) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(256); cfg.stream = c->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;  // behind my push kernel
-#define MA_GO(OPTC)                                                                                                               \
-    cudaLaunchKernelEx(&cfg, merge_apply_kernel<K, OPTC>, d->peers, d->A, d->rank, d->world, d->epoch, d->recw,                    \
-        (const uint32_t*)(d->own_uniq + (size_t)slot * d->cap_own), (const unsigned int*)(d->n_own + slot),                        \
-        (const uint32_t*)(d->own_pos + (size_t)slot * d->world * d->cap_own), (unsigned)d->cap_own, c->W, c->V, c->s1W, c->s1V,   \
-        c->s2W, c->s2V, Pp)
-    switch (Pp.opt) {
-        case LCTR_OPT_ADAGRAD: MA_GO(LCTR_OPT_ADAGRAD); break;
-        case LCTR_OPT_FTRL: MA_GO(LCTR_OPT_FTRL); break;
-        case LCTR_OPT_ADAM: MA_GO(LCTR_OPT_ADAM); break;
-        case LCTR_OPT_RMSPROP: MA_GO(LCTR_OPT_RMSPROP); break;
-        case LCTR_OPT_ADADELTA: MA_GO(LCTR_OPT_ADADELTA); break;
-        case LCTR_OPT_PS_SGD: MA_GO(LCTR_OPT_PS_SGD); break;
-        case LCTR_OPT_PS_ADAGRAD: MA_GO(LCTR_OPT_PS_ADAGRAD); break;
-        case LCTR_OPT_PS_DCASGD: MA_GO(LCTR_OPT_PS_DCASGD); break;
-        default: MA_GO(LCTR_OPT_PS_DCASGDA); break;
-    }
-#undef MA_GO
+static auto merge_apply_instance(int opt) {
+    return by_opt(opt, [](auto o) { return merge_apply_kernel<K, o.value>; });
 }
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -868,22 +846,18 @@ int dist_send_keys(lctr_ctx* c, Slot& s, int slot, cudaStream_t st) {
     uint32_t* opos = d->opos + (size_t)slot * d->cap_keys;
     uint32_t* hot_p = d->hot_p ? d->hot_p + (size_t)slot * d->rows_x : nullptr;
     if (hot_p) LCTR_CUDA(cudaMemsetAsync(hot_p, 0xff, d->rows_x * sizeof(uint32_t), st));  // the previous batch's hot rows
-    if (d->keyed) {  // an overflow fails this upload only (reported through the owners' statuses)
-        LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), st));
-        send_keys_kernel<true><<<grid, 256, 0, st>>>(s.uniq, s.n_uniq, d->peers, d->A, d->rank, d->world, slot2, d->shift,
-                                                     (unsigned)d->cap_pair, d->send_cnt, opos, d->overflow, d->batch_key);
-    } else {
-        send_keys_kernel<false><<<grid, 256, 0, st>>>(s.uniq, s.n_uniq, d->peers, d->A, d->rank, d->world, slot2, d->shift,
-                                                      (unsigned)d->cap_pair, d->send_cnt, opos, d->overflow, nullptr);
-    }
-    send_keys_finish_kernel<<<1, 32, 0, st>>>(d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair, d->send_cnt,
-                                              d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow : nullptr, 0);
+    // keyed: an overflow fails this upload only (reported through the owners' statuses)
+    if (d->keyed) LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), st));
+    if (launch(c, {grid, 256, 0, st}, d->keyed ? send_keys_kernel<true> : send_keys_kernel<false>, s.uniq, s.n_uniq, d->peers, d->A,
+               d->rank, d->world, slot2, d->shift, (unsigned)d->cap_pair, d->send_cnt, opos, d->overflow,
+               d->keyed ? d->batch_key : nullptr) ||
+        launch(c, {1, 32, 0, st}, send_keys_finish_kernel, d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair,
+               d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow : nullptr, 0))
+        return 1;
     d->posted = d->keyed;
     const unsigned rg = (unsigned)std::max<int64_t>(1, std::min<int64_t>((s.nnz + 255) / 256, (int64_t)c->sm_count * 8));
-    remap_entries_kernel<<<rg, 256, 0, st>>>(nullptr, s.nnz, opos, s.ent_pslot, s.ent_slot, hot_p ? s.hot_of : nullptr, s.n_uniq, hot_p);
-    c->launches += 3;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return launch(c, {rg, 256, 0, st}, remap_entries_kernel, nullptr, s.nnz, opos, s.ent_pslot, s.ent_slot, hot_p ? s.hot_of : nullptr,
+                  s.n_uniq, hot_p);
 }
 
 // an empty share (0 rows or 0 entries): empty key lists and the generation flag on every owner, status OK -- the peers'
@@ -894,11 +868,10 @@ int dist_send_empty(lctr_ctx* c, int slot, cudaStream_t st) {
     d->gen[slot]++;
     const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
     if (d->keyed) LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), st));
-    send_keys_finish_kernel<<<1, 32, 0, st>>>(d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair, d->send_cnt,
-                                              d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow : nullptr, 0);
+    if (launch(c, {1, 32, 0, st}, send_keys_finish_kernel, d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair,
+               d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow : nullptr, 0))
+        return 1;
     d->posted = d->keyed;
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
     return 0;
 }
 
@@ -931,12 +904,11 @@ int dist_keys_dedupe(lctr_ctx* c, Slot& s, const uint64_t* h_keys, int64_t nnz) 
                                                                          (int64_t)c->sm_count * 8));
     {
         ProfScope prof(c, PROF_KEYS);
-        batch_insert_kernel<<<tg, 256, 0, c->stream>>>(d->bt_stage, nnz, bt, d->bt_claimed);
-        batch_find_kernel<<<tg, 256, 0, c->stream>>>(d->bt_stage, nnz, bt, s.fid);
-        batch_clear_kernel<<<cg, 256, 0, c->stream>>>(bt, d->bt_claimed, d->bt_T);
+        if (launch(c, {tg, 256, 0, c->stream}, batch_insert_kernel, d->bt_stage, nnz, bt, d->bt_claimed) ||
+            launch(c, {tg, 256, 0, c->stream}, batch_find_kernel, d->bt_stage, nnz, bt, s.fid) ||
+            launch(c, {cg, 256, 0, c->stream}, batch_clear_kernel, bt, d->bt_claimed, d->bt_T))
+            return 1;
     }
-    c->launches += 3;
-    LCTR_CUDA(cudaGetLastError());
     unsigned long long u = 0;
     unsigned int fl[3] = {0, 0, 0};
     LCTR_CUDA(cudaMemcpyAsync(&u, d->bt_cnt, sizeof(u), cudaMemcpyDeviceToHost, c->stream));
@@ -953,10 +925,9 @@ int dist_keys_refuse(lctr_ctx* c, int slot) {
     if (d->posted) return 0;
     d->gen[slot]++;
     const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
-    send_keys_finish_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair,
-                                                     d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->overflow, 1);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
+    if (launch(c, {1, 32, 0, c->stream}, send_keys_finish_kernel, d->peers, d->A, d->rank, d->world, slot2, slot,
+               (unsigned)d->cap_pair, d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->overflow, 1))
+        return 1;
     d->posted = true;
     return 0;
 }
@@ -976,15 +947,12 @@ int dist_keys_translate(lctr_ctx* c, int slot) {
                                                                          (int64_t)c->sm_count * 16));
     {
         ProfScope prof(c, PROF_KEYS);
-        xlate_wait_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, slot, d->gen[slot], d->xstat);
-        xlate_keys_kernel<0><<<tg, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, d->xstat, t);
-        c->launches += 2;
-        LCTR_CUDA(cudaGetLastError());
-        if (init_new_rows(c, (int64_t)std::min(d->rows_x, keys_capacity(c)))) return 1;
-        xlate_keys_kernel<1><<<tg, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, d->xstat, t);
-        xlate_finish_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, d->xseq, d->xstat, t.flags, d->xres);
-        c->launches += 2;
-        LCTR_CUDA(cudaGetLastError());
+        if (launch(c, {1, 32, 0, c->stream}, xlate_wait_kernel, d->peers, d->A, d->rank, d->world, slot2, slot, d->gen[slot], d->xstat) ||
+            launch(c, {tg, 256, 0, c->stream}, xlate_keys_kernel<0>, d->peers, d->A, d->rank, d->world, slot2, d->xstat, t) ||
+            init_new_rows(c, (int64_t)std::min(d->rows_x, keys_capacity(c))) ||
+            launch(c, {tg, 256, 0, c->stream}, xlate_keys_kernel<1>, d->peers, d->A, d->rank, d->world, slot2, d->xstat, t) ||
+            launch(c, {1, 32, 0, c->stream}, xlate_finish_kernel, d->peers, d->A, d->rank, d->world, d->xseq, d->xstat, t.flags, d->xres))
+            return 1;
     }
     unsigned long long res[kMaxWorld] = {0};
     LCTR_CUDA(cudaMemcpyAsync(res, d->xres, (size_t)d->world * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
@@ -1040,18 +1008,17 @@ int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait, bool trai
         const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
         const unsigned g1 = (unsigned)std::max<int64_t>(8, std::min<int64_t>((int64_t)c->sm_count * 4, ((int64_t)d->cap_pair + 255) / 256));
         LCTR_CUDA(cudaMemsetAsync(d->n_own + slot, 0, sizeof(unsigned int), c->stream));
-        own_mark_kernel<<<g1, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, slot, d->gen[slot], d->posmap, c->Fl,
-                                                   d->own_mark, d->own_T);
-        launch_slotmap_compact(c, d->own_mark, d->own_T, d->own_uniq + (size_t)slot * d->cap_own, d->n_own + slot, c->stream);
-        own_pos_kernel<<<g1, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot2, d->own_uniq + (size_t)slot * d->cap_own,
-                                                  d->n_own + slot, d->posmap, c->Fl, d->own_pos + (size_t)slot * d->world * d->cap_own,
-                                                  (unsigned)d->cap_own);
-        c->launches += 3;
+        if (launch(c, {g1, 256, 0, c->stream}, own_mark_kernel, d->peers, d->A, d->rank, d->world, slot2, slot, d->gen[slot], d->posmap,
+                   c->Fl, d->own_mark, d->own_T) ||
+            launch_slotmap_compact(c, d->own_mark, d->own_T, d->own_uniq + (size_t)slot * d->cap_own, d->n_own + slot, c->stream) ||
+            launch(c, {g1, 256, 0, c->stream}, own_pos_kernel, d->peers, d->A, d->rank, d->world, slot2,
+                   d->own_uniq + (size_t)slot * d->cap_own, d->n_own + slot, d->posmap, c->Fl,
+                   d->own_pos + (size_t)slot * d->world * d->cap_own, (unsigned)d->cap_own))
+            return 1;
         d->own_gen[slot] = d->gen[slot];
     }
     if (d->released) {  // the previous round was pull-only: its requesters' kernels may still read their caches
-        wait_flags_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, FLAG_RELEASED, d->world, d->released);
-        c->launches++;
+        if (launch(c, {1, 32, 0, c->stream}, wait_flags_kernel, d->peers, d->A, d->rank, FLAG_RELEASED, d->world, d->released)) return 1;
         d->released = 0;
     }
     { ProfScope prof(c, PROF_DIST_PULL);
@@ -1060,26 +1027,20 @@ int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait, bool trai
     const int64_t serve_keys = s.nnz > 0 ? std::min<int64_t>(s.nnz, (int64_t)c->F) : (int64_t)d->cap_pair;
     const unsigned pull_grid = (unsigned)std::max<int64_t>(8, std::min<int64_t>((int64_t)c->sm_count * 4,
         (serve_keys * (int64_t)std::max<size_t>(1, c->rowlen / 16) + 255) / 256));
-    serve_pull_kernel<<<pull_grid, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot * 2 + (int)(d->gen[slot] & 1), slot,
-                                                             d->gen[slot], d->epoch, (int)c->rowlen, (unsigned)d->cap_pair, c->W, c->V,
-                                                             d->done_ctr + 0); }
-    c->launches++;
-    if (!in_kernel_wait) {
-        ProfScope prof(c, PROF_DIST_BAR1);
-        wait_flags_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, FLAG_PULLED, d->world, d->epoch);
-        c->launches++;
-    }
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    if (launch(c, {pull_grid, 256, 0, c->stream}, serve_pull_kernel, d->peers, d->A, d->rank, d->world,
+               slot * 2 + (int)(d->gen[slot] & 1), slot, d->gen[slot], d->epoch, (int)c->rowlen, (unsigned)d->cap_pair, c->W, c->V,
+               d->done_ctr + 0))
+        return 1; }
+    if (in_kernel_wait) return 0;
+    ProfScope prof(c, PROF_DIST_BAR1);
+    return launch(c, {1, 32, 0, c->stream}, wait_flags_kernel, d->peers, d->A, d->rank, FLAG_PULLED, d->world, d->epoch);
 }
 
 // end of a pull-only round (behind its forward): my cache is released to every owner for the next round
 int dist_release(lctr_ctx* c) {
     DistState* d = c->dist;
-    release_cache_kernel<<<1, 32, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, d->epoch);
-    c->launches++;
+    if (launch(c, {1, 32, 0, c->stream}, release_cache_kernel, d->peers, d->A, d->rank, d->world, d->epoch)) return 1;
     d->released = d->epoch;
-    LCTR_CUDA(cudaGetLastError());
     return 0;
 }
 
@@ -1092,38 +1053,31 @@ int dist_post_step(lctr_ctx* c, Slot& s, int slot, int64_t rows_divisor) {
         {
             ProfScope prof(c, PROF_DIST_PUSH);
             FusedState* f = c->fused;
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(xgrid); cfg.blockDim = dim3(256); cfg.stream = c->stream;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            at[0].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;  // behind the gradient kernel
-            cudaLaunchKernelEx(&cfg, push_rows_kernel, seg, f->G, f->GS, f->G + c->rowlen, f->GS,
-                               (const uint32_t*)(d->hot_p + (size_t)slot * d->rows_x), f->Ghot, f->GS, (int)c->rowlen, d->recw,
-                               (unsigned)d->cap_pair, d->peers, d->A, d->rank, d->world, d->epoch, d->done_ctr + 1);
+            // dependent: behind the gradient kernel
+            if (launch(c, {xgrid, 256, 0, c->stream, true}, push_rows_kernel, seg, f->G, f->GS, f->G + c->rowlen, f->GS,
+                       d->hot_p + (size_t)slot * d->rows_x, f->Ghot, f->GS, (int)c->rowlen, d->recw, (unsigned)d->cap_pair, d->peers,
+                       d->A, d->rank, d->world, d->epoch, d->done_ctr + 1))
+                return 1;
         }
         ProfScope prof(c, PROF_DIST_MERGE);
         const OptParams Pp = make_opt_params(c, rows_divisor);
-        const unsigned mgrid = (unsigned)c->sm_count * 4;
-        switch ((int)c->cfg.factor_cnt) {
-            case 4: merge_apply_go<4>(c, d, slot, Pp, mgrid); break;
-            case 8: merge_apply_go<8>(c, d, slot, Pp, mgrid); break;
-            case 16: merge_apply_go<16>(c, d, slot, Pp, mgrid); break;
-            default: merge_apply_go<32>(c, d, slot, Pp, mgrid); break;
-        }
-        c->launches += 2;
-        LCTR_CUDA(cudaGetLastError());
-        return 0;
+        const int k = (int)c->cfg.factor_cnt;
+        auto kern = k == 4 ? merge_apply_instance<4>(Pp.opt) : k == 8 ? merge_apply_instance<8>(Pp.opt)
+                  : k == 16 ? merge_apply_instance<16>(Pp.opt) : merge_apply_instance<32>(Pp.opt);
+        // dependent: behind my push kernel
+        return launch(c, {(unsigned)c->sm_count * 4, 256, 0, c->stream, true}, kern, d->peers, d->A, d->rank, d->world,
+                      d->epoch, d->recw, d->own_uniq + (size_t)slot * d->cap_own, d->n_own + slot,
+                      d->own_pos + (size_t)slot * d->world * d->cap_own, (unsigned)d->cap_own, c->W, c->V, c->s1W, c->s1V, c->s2W,
+                      c->s2V, Pp);
     }
     { ProfScope prof(c, PROF_DIST_PUSH);
-    push_rows_kernel<<<xgrid, 256, 0, c->stream>>>(seg, d->cgV, (int)c->rowlen, d->cgW, 1, nullptr, nullptr, 0, (int)c->rowlen,
-                                                   d->recw, (unsigned)d->cap_pair, d->peers, d->A, d->rank, d->world, d->epoch,
-                                                   d->done_ctr + 1); }
+    if (launch(c, {xgrid, 256, 0, c->stream}, push_rows_kernel, seg, d->cgV, (int)c->rowlen, d->cgW, 1, nullptr, nullptr, 0,
+               (int)c->rowlen, d->recw, (unsigned)d->cap_pair, d->peers, d->A, d->rank, d->world, d->epoch, d->done_ctr + 1))
+        return 1; }
     { ProfScope prof(c, PROF_DIST_MERGE);
-    merge_kernel<<<xgrid, 256, 0, c->stream>>>(d->peers, d->A, d->rank, d->world, slot * 2 + (int)(d->gen[slot] & 1), d->epoch,
-                                                         (int)c->rowlen, d->recw, c->gW, c->gV, c->touched); }
-    c->launches += 2;
-    LCTR_CUDA(cudaGetLastError());
+    if (launch(c, {xgrid, 256, 0, c->stream}, merge_kernel, d->peers, d->A, d->rank, d->world, slot * 2 + (int)(d->gen[slot] & 1),
+               d->epoch, (int)c->rowlen, d->recw, c->gW, c->gV, c->touched))
+        return 1; }
     return launch_apply(c, rows_divisor);  // sparse updater on the shard (the merge waited for every requester's pushes)
 }
 

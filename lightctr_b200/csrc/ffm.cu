@@ -492,15 +492,19 @@ int launch_ffm_predict_inorder(lctr_ctx* c, Slot& s) {
     if (s.rows <= 0) return 0;
     LCTR_CHECK(s.has_field, "FFM batch uploaded without the field array");
     const unsigned grid = (unsigned)((s.rows + 7) / 8);
-    if (s.has_val)
-        ffm_predict_inorder_kernel<true><<<grid, 256, 0, c->stream>>>(s.row_ptr, s.fid, s.field, s.val, c->cW, c->cV,
-                                                                      (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt, s.pred, s.rows);
-    else
-        ffm_predict_inorder_kernel<false><<<grid, 256, 0, c->stream>>>(s.row_ptr, s.fid, s.field, s.val, c->cW, c->cV,
-                                                                       (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt, s.pred, s.rows);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return launch(c, {grid, 256, 0, c->stream}, s.has_val ? ffm_predict_inorder_kernel<true> : ffm_predict_inorder_kernel<false>,
+                  s.row_ptr, s.fid, s.field, s.val, c->cW, c->cV, (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt, s.pred, s.rows);
+}
+
+// the CTA-per-sample kernel's instance (bulk: the TMA bulk reduce-add of the gradient rows, 4-wide training rows only)
+template <int VEC, bool HV, bool TR>
+static auto ffm_kernel(bool bulk) {
+    return bulk ? ffm_fused_kernel<VEC, HV, TR, (VEC == 4) && TR> : ffm_fused_kernel<VEC, HV, TR, false>;
+}
+template <int VEC>
+static auto ffm_kernel(bool hv, bool train, bool bulk) {
+    return hv ? (train ? ffm_kernel<VEC, true, true>(bulk) : ffm_kernel<VEC, true, false>(bulk))
+              : (train ? ffm_kernel<VEC, false, true>(bulk) : ffm_kernel<VEC, false, false>(bulk));
 }
 
 static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, bool stats, bool grouped = false) {
@@ -523,16 +527,10 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
     ProfScope prof(c, PROF_FFM_FUSED);
     if (grouped) {
         LCTR_CHECK(train && vec == 4 && c->ffm_T && c->ffm_cnt, "grouped FFM step needs k %% 4 == 0 and the tile buffer");
-        auto go = [&](auto kern) {
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            kern<<<(unsigned)rows, tpb, smem, c->stream>>>(s.row_ptr, s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred,
-                                                           c->cgW, c->cgV, nullptr, c->cfg.l2_reg, rb, c->stat_partial,
-                                                           c->stat_done, out_slot, stats ? 1 : 0, c->ffm_T, c->ffm_cnt);
-        };
-        if (s.has_val) go(ffm_fused_kernel<4, true, true, false, true>); else go(ffm_fused_kernel<4, false, true, false, true>);
-        c->launches++;
-        LCTR_CUDA(cudaGetLastError());
-        return 0;
+        return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream},
+                      s.has_val ? ffm_fused_kernel<4, true, true, false, true> : ffm_fused_kernel<4, false, true, false, true>,
+                      s.row_ptr, s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, nullptr, c->cfg.l2_reg, rb,
+                      c->stat_partial, c->stat_done, out_slot, stats ? 1 : 0, c->ffm_T, c->ffm_cnt);
     }
     // LCTR_FFM_TMA=1 selects the TMA-staged kernel (cp.async.bulk rows + mbarrier).  It is parity-green but NOT the
     // default: both kernels are issue-bound rather than memory-bound, and staging whole rows in shared memory cuts the
@@ -552,44 +550,21 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
         LCTR_CHECK(CR >= 8, "FFM field-pair tile + row buffer do not fit 227 KB shared memory: Fc=%d k=%d", Fc, k);
         const size_t smem2 = (size_t)CR * (stage_bytes + 14) + fixed;
         const int tpb2 = std::max(64, (A + 31) / 32 * 32);
-        auto go = [&](auto kern) {
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
-            kern<<<(unsigned)rows, tpb2, smem2, c->stream>>>(s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label,
-                                                            c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV,
-                                                            c->cfg.world > 1 ? nullptr : c->touched, c->cfg.l2_reg, rb, c->stat_partial,
-                                                            c->stat_done, out_slot, stats ? 1 : 0, CR);
-        };
-        if (s.has_val) go(ffm_tma_kernel<true>); else go(ffm_tma_kernel<false>);
-        c->launches++;
-        LCTR_CUDA(cudaGetLastError());
-        return 0;
+        return launch(c, {(unsigned)rows, (unsigned)tpb2, smem2, c->stream}, s.has_val ? ffm_tma_kernel<true> : ffm_tma_kernel<false>,
+                      s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW,
+                      c->cgV, c->cfg.world > 1 ? nullptr : c->touched, c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot,
+                      stats ? 1 : 0, CR);
     }
     // default for k % 4 == 0: the warp-per-sample kernel of ffm_warp.cu (LCTR_FFM_WARP=0 keeps the CTA-per-sample kernel below)
     if (train && !bulk && vec == 4) {
         const int rc = launch_ffm_warp(c, s, rb, re, stats);
         if (rc >= 0) return rc;
     }
-#define FFM_GO(VECN, HV, TR)                                                                                          \
-    do {                                                                                                              \
-        auto kern = bulk ? ffm_fused_kernel<VECN, HV, TR, (VECN == 4) && TR> : ffm_fused_kernel<VECN, HV, TR, false>; \
-        LCTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                \
-        kern<<<(unsigned)rows, tpb, smem, c->stream>>>(s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, \
-                                                       s.pred, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched, c->cfg.l2_reg, rb, \
-                                                       c->stat_partial, c->stat_done, out_slot, stats ? 1 : 0, nullptr, nullptr); \
-    } while (0)
-#define FFM_GO2(VECN)                                                                \
-    do {                                                                             \
-        if (s.has_val) { if (train) FFM_GO(VECN, true, true); else FFM_GO(VECN, true, false); } \
-        else { if (train) FFM_GO(VECN, false, true); else FFM_GO(VECN, false, false); }          \
-    } while (0)
-    if (vec == 4) FFM_GO2(4);
-    else if (vec == 2) FFM_GO2(2);
-    else FFM_GO2(1);
-#undef FFM_GO2
-#undef FFM_GO
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, train, bulk) : vec == 2 ? ffm_kernel<2>(s.has_val, train, bulk)
+                                                                    : ffm_kernel<1>(s.has_val, train, bulk);
+    return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid,
+                  s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched,
+                  c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, stats ? 1 : 0, nullptr, nullptr);
 }
 
 // forward + backward are one fused kernel (stats: a train step; otherwise forward only)

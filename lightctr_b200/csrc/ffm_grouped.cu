@@ -253,16 +253,9 @@ int launch_ffm_backward_grouped(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     const unsigned grid = (unsigned)c->sm_count * 8;
     ProfScope prof(c, PROF_FM_BWD_CSC);
     LCTR_CHECK(NS >= 1 && NS <= 4, "grouped FFM backward: row of %d floats exceeds 512", Fc * k);
-    if (s.has_val) {
-        if (fuse) ffm_backward_grouped_kernel<true, true><<<grid, 128, 0, c->stream>>>(C, T, Fc, k, NS, c->cfg.l2_reg, P);
-        else ffm_backward_grouped_kernel<true, false><<<grid, 128, 0, c->stream>>>(C, T, Fc, k, NS, c->cfg.l2_reg, P);
-    } else {
-        if (fuse) ffm_backward_grouped_kernel<false, true><<<grid, 128, 0, c->stream>>>(C, T, Fc, k, NS, c->cfg.l2_reg, P);
-        else ffm_backward_grouped_kernel<false, false><<<grid, 128, 0, c->stream>>>(C, T, Fc, k, NS, c->cfg.l2_reg, P);
-    }
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    auto kern = s.has_val ? (fuse ? ffm_backward_grouped_kernel<true, true> : ffm_backward_grouped_kernel<true, false>)
+                          : (fuse ? ffm_backward_grouped_kernel<false, true> : ffm_backward_grouped_kernel<false, false>);
+    return launch(c, {grid, 128, 0, c->stream}, kern, C, T, Fc, k, NS, c->cfg.l2_reg, P);
 }
 
 }  // namespace lctr

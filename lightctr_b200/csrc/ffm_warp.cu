@@ -284,6 +284,9 @@ ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
 }  // namespace
 
 // returns 0 when launched, -1 when the shape is not covered (caller falls back to ffm.cu), 1 on error
+template <int PASSES>
+static auto warp_kernel(bool hv) { return hv ? ffm_warp_kernel<PASSES, true> : ffm_warp_kernel<PASSES, false>; }
+
 int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
     static const bool off = getenv("LCTR_FFM_WARP") && atoi(getenv("LCTR_FFM_WARP")) == 0;
     const int k = (int)c->cfg.factor_cnt, Fc = (int)c->cfg.field_cnt;
@@ -303,25 +306,11 @@ int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
     ProfScope prof(c, PROF_FFM_FUSED);
     const uint32_t* ids = c->cfg.world > 1 ? s.ent_pslot : s.fid;
     uint8_t* touched = c->cfg.world > 1 ? nullptr : c->touched;
-#define FFM_WARP_GO(P, HV)                                                                                                \
-    do {                                                                                                                   \
-        LCTR_CUDA(cudaFuncSetAttribute(ffm_warp_kernel<P, HV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
-        ffm_warp_kernel<P, HV><<<grid, warps * 32, smem, c->stream>>>(s.row_ptr, ids, s.field, s.val, s.label, c->cW, c->cV, Fc, k, \
-                                                                      s.pred, c->cgW, c->cgV, touched, c->cfg.l2_reg, rb, rows, (int)tile, \
-                                                                      c->stat_partial, c->stat_done, out_slot, stats ? 1 : 0);           \
-    } while (0)
-#define FFM_WARP_GO2(P) do { if (s.has_val) FFM_WARP_GO(P, true); else FFM_WARP_GO(P, false); } while (0)
-    switch (passes) {
-        case 1: FFM_WARP_GO2(1); break;
-        case 2: FFM_WARP_GO2(2); break;
-        case 3: FFM_WARP_GO2(3); break;
-        default: FFM_WARP_GO2(4); break;
-    }
-#undef FFM_WARP_GO2
-#undef FFM_WARP_GO
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    auto kern = passes == 1 ? warp_kernel<1>(s.has_val) : passes == 2 ? warp_kernel<2>(s.has_val)
+              : passes == 3 ? warp_kernel<3>(s.has_val) : warp_kernel<4>(s.has_val);
+    return launch(c, {grid, (unsigned)warps * 32, smem, c->stream}, kern, s.row_ptr, ids, s.field, s.val, s.label, c->cW, c->cV, Fc,
+                  k, s.pred, c->cgW, c->cgV, touched, c->cfg.l2_reg, rb, rows, (int)tile, c->stat_partial, c->stat_done, out_slot,
+                  stats ? 1 : 0);
 }
 
 }  // namespace lctr

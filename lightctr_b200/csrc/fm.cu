@@ -250,25 +250,23 @@ static bool pick_shape(int k, Shape& sh) {
     return false;
 }
 
-#define FM_DISPATCH_LPR(KERNEL, VECN, HV, NF, ...)                                     \
-    switch (sh.lpr) {                                                                  \
-        case 1: KERNEL<1, VECN, HV, NF><<<grid, 256, 0, c->stream>>>(__VA_ARGS__); break;   \
-        case 2: KERNEL<2, VECN, HV, NF><<<grid, 256, 0, c->stream>>>(__VA_ARGS__); break;   \
-        case 4: KERNEL<4, VECN, HV, NF><<<grid, 256, 0, c->stream>>>(__VA_ARGS__); break;   \
-        case 8: KERNEL<8, VECN, HV, NF><<<grid, 256, 0, c->stream>>>(__VA_ARGS__); break;   \
-        case 16: KERNEL<16, VECN, HV, NF><<<grid, 256, 0, c->stream>>>(__VA_ARGS__); break; \
-        case 32: KERNEL<32, VECN, HV, NF><<<grid, 256, 0, c->stream>>>(__VA_ARGS__); break; \
+// the instance of fm_backward_kernel for the row shape
+template <int VEC, bool HV, bool NF>
+static auto backward_lpr(int lpr) {
+    switch (lpr) {
+        case 1: return fm_backward_kernel<1, VEC, HV, NF>;
+        case 2: return fm_backward_kernel<2, VEC, HV, NF>;
+        case 4: return fm_backward_kernel<4, VEC, HV, NF>;
+        case 8: return fm_backward_kernel<8, VEC, HV, NF>;
+        case 16: return fm_backward_kernel<16, VEC, HV, NF>;
+        default: return fm_backward_kernel<32, VEC, HV, NF>;
     }
-#define FM_DISPATCH(KERNEL, ...)                                                        \
-    do {                                                                                \
-        if (sh.vec == 4) {                                                              \
-            if (s.has_val) { if (nfm) { FM_DISPATCH_LPR(KERNEL, 4, true, true, __VA_ARGS__) } else { FM_DISPATCH_LPR(KERNEL, 4, true, false, __VA_ARGS__) } } \
-            else { if (nfm) { FM_DISPATCH_LPR(KERNEL, 4, false, true, __VA_ARGS__) } else { FM_DISPATCH_LPR(KERNEL, 4, false, false, __VA_ARGS__) } } \
-        } else {                                                                        \
-            if (s.has_val) { if (nfm) { FM_DISPATCH_LPR(KERNEL, 1, true, true, __VA_ARGS__) } else { FM_DISPATCH_LPR(KERNEL, 1, true, false, __VA_ARGS__) } } \
-            else { if (nfm) { FM_DISPATCH_LPR(KERNEL, 1, false, true, __VA_ARGS__) } else { FM_DISPATCH_LPR(KERNEL, 1, false, false, __VA_ARGS__) } } \
-        }                                                                               \
-    } while (0)
+}
+template <int VEC>
+static auto backward_kernel(int lpr, bool hv, bool nfm) {
+    return hv ? (nfm ? backward_lpr<VEC, true, true>(lpr) : backward_lpr<VEC, true, false>(lpr))
+              : (nfm ? backward_lpr<VEC, false, true>(lpr) : backward_lpr<VEC, false, false>(lpr));
+}
 
 // Coalesced variant for K % 8 == 0: LPR = K/4 lanes cover one V row with float4 loads (a 64 B row is ONE request of two
 // fully used sectors instead of four scattered 16 B requests), so a warp gathers G = 32/LPR rows per load instruction.
@@ -400,6 +398,11 @@ fm_forward_coalesced_kernel(const int64_t* __restrict__ row_ptr, const uint32_t*
     if (!NFM && do_stats) publish_stats(loss, correct, partial, done, out_slot, false);
 }
 
+template <int K, bool HV, bool NF>
+static auto forward_kernel(bool co) {
+    return co ? fm_forward_coalesced_kernel<(K % 8 == 0) && K <= 32 ? K : 8, HV, NF> : fm_forward_kernel<K, HV, NF>;
+}
+
 template <int K>
 static int fwd_go(lctr_ctx* c, Slot& s, bool nfm, int64_t rb, int64_t re, double* out_slot, int stats, const int64_t* hdr) {
     constexpr bool kCoalesced = (K % 8 == 0) && K <= 32;
@@ -410,25 +413,11 @@ static int fwd_go(lctr_ctx* c, Slot& s, bool nfm, int64_t rb, int64_t re, double
     const int wpb = co ? 4 : 8;
     const unsigned grid = (unsigned)((re - rb + wpb - 1) / wpb);
     const size_t smem = co ? (size_t)wpb * (K + 2) * 68 * sizeof(float) : (size_t)wpb * 64 * (K + 4) * sizeof(float);
-    // past 48 KB of static + dynamic shared memory a launch needs the opt-in; the FM kernels' static part is publish_stats's
-    // scratch (K = 20: 48 KB of tile + that scratch).  `co` is fixed per process, so each site sees one kernel.
-#define FWD_GO(HV, NF)                                                                                         \
-    do {                                                                                                       \
-        auto kern = co ? fm_forward_coalesced_kernel<kCoalesced ? K : 8, HV, NF> : fm_forward_kernel<K, HV, NF>; \
-        static const size_t static_smem = [&] {                                                                \
-            cudaFuncAttributes a;                                                                              \
-            return cudaFuncGetAttributes(&a, kern) == cudaSuccess ? a.sharedSizeBytes : (size_t)48 * 1024;     \
-        }();                                                                                                   \
-        if (smem + static_smem > 48 * 1024)                                                                    \
-            LCTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));     \
-        kern<<<grid, wpb * 32, smem, c->stream>>>(s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val, s.label, c->cW, c->cV, s.pred, s.sumvx, c->z, \
-                                             s.wide, rb, re, c->stat_partial, c->stat_done, out_slot, stats, hdr,   \
-                                             c->fwd_quirk_sumvx, c->fwd_quirk_rows);                               \
-    } while (0)
-    if (s.has_val) { if (nfm) FWD_GO(true, true); else FWD_GO(true, false); }
-    else { if (nfm) FWD_GO(false, true); else FWD_GO(false, false); }
-#undef FWD_GO
-    return 0;
+    auto kern = s.has_val ? (nfm ? forward_kernel<K, true, true>(co) : forward_kernel<K, true, false>(co))
+                          : (nfm ? forward_kernel<K, false, true>(co) : forward_kernel<K, false, false>(co));
+    return launch(c, {grid, (unsigned)wpb * 32, smem, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val,
+                  s.label, c->cW, c->cV, s.pred, s.sumvx, c->z, s.wide, rb, re, c->stat_partial, c->stat_done, out_slot, stats, hdr,
+                  c->fwd_quirk_sumvx, c->fwd_quirk_rows);
 }
 
 int launch_fm_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm, bool stats) {
@@ -456,10 +445,7 @@ int launch_fm_forward_ex(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm,
             set_error("factor_cnt=%d is not instantiated (built: 1-8, 10, 12, 16, 20, 24, 32)", k);
             return 1;
     }
-    if (rc) return 1;
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return rc;
 }
 
 int launch_fm_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
@@ -470,11 +456,10 @@ int launch_fm_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
     if (rows <= 0) return 0;
     const unsigned grid = (unsigned)((rows + 7) / 8);
     ProfScope prof(c, PROF_FM_BWD_RED);
-    FM_DISPATCH(fm_backward_kernel, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val, s.label, c->cW, c->cV, k, s.pred, s.sumvx, c->dz, c->cgW,
-                c->cgV, c->cfg.world > 1 ? nullptr : c->touched, c->cfg.l2_reg, rb, re);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return launch(c, {grid, 256, 0, c->stream},
+                  sh.vec == 4 ? backward_kernel<4>(sh.lpr, s.has_val, nfm) : backward_kernel<1>(sh.lpr, s.has_val, nfm), s.row_ptr,
+                  c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val, s.label, c->cW, c->cV, k, s.pred, s.sumvx, c->dz, c->cgW, c->cgV,
+                  c->cfg.world > 1 ? nullptr : c->touched, c->cfg.l2_reg, rb, re);
 }
 
 
@@ -554,18 +539,9 @@ fm_backward_csc_kernel(const int64_t* __restrict__ seg_ptr, const uint32_t* __re
 }
 
 template <int LR>
-static void bwd_csc_go(lctr_ctx* c, Slot& s, bool nfm, unsigned grid, int k, int64_t sb, int64_t se, int64_t rb,
-                       const OptParams& P) {
-#define CSC_ARGS s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, sb, se, s.label, s.pred, s.sumvx, c->dz, rb, c->W, c->V, \
-                 c->s1W, c->s1V, c->s2W, c->s2V, k, c->cfg.l2_reg, P
-    if (s.has_val) {
-        if (nfm) fm_backward_csc_kernel<LR, true, true><<<grid, 256, 0, c->stream>>>(CSC_ARGS);
-        else fm_backward_csc_kernel<LR, true, false><<<grid, 256, 0, c->stream>>>(CSC_ARGS);
-    } else {
-        if (nfm) fm_backward_csc_kernel<LR, false, true><<<grid, 256, 0, c->stream>>>(CSC_ARGS);
-        else fm_backward_csc_kernel<LR, false, false><<<grid, 256, 0, c->stream>>>(CSC_ARGS);
-    }
-#undef CSC_ARGS
+static auto backward_csc_kernel(bool hv, bool nfm) {
+    return hv ? (nfm ? fm_backward_csc_kernel<LR, true, true> : fm_backward_csc_kernel<LR, true, false>)
+              : (nfm ? fm_backward_csc_kernel<LR, false, true> : fm_backward_csc_kernel<LR, false, false>);
 }
 
 int launch_fm_backward_csc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
@@ -584,15 +560,10 @@ int launch_fm_backward_csc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nf
     const int segs_per_cta = 8 * (32 / lr);
     const unsigned grid = (unsigned)((se - sb + segs_per_cta - 1) / segs_per_cta);
     ProfScope prof(c, PROF_FM_BWD_CSC);
-    switch (lr) {
-        case 4: bwd_csc_go<4>(c, s, nfm, grid, k, sb, se, rb, P); break;
-        case 8: bwd_csc_go<8>(c, s, nfm, grid, k, sb, se, rb, P); break;
-        case 16: bwd_csc_go<16>(c, s, nfm, grid, k, sb, se, rb, P); break;
-        default: bwd_csc_go<32>(c, s, nfm, grid, k, sb, se, rb, P); break;
-    }
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    auto kern = lr == 4 ? backward_csc_kernel<4>(s.has_val, nfm) : lr == 8 ? backward_csc_kernel<8>(s.has_val, nfm)
+              : lr == 16 ? backward_csc_kernel<16>(s.has_val, nfm) : backward_csc_kernel<32>(s.has_val, nfm);
+    return launch(c, {grid, 256, 0, c->stream}, kern, s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, sb, se, s.label, s.pred, s.sumvx,
+                  c->dz, rb, c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, k, c->cfg.l2_reg, P);
 }
 
 // FM_Predict quirk mode (predict/fm_predict.cpp:20-33): pred = sum w x - 0.5 sum|vx|^2 + 0.5|sumVX_train[rid]|^2, evaluated

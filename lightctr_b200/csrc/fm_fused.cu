@@ -97,42 +97,41 @@ int fused_build_slot(lctr_ctx* c, Slot& s, cudaStream_t st, const int64_t* hdr, 
         return 0;
     }
     const unsigned mkg = (unsigned)std::max<int64_t>(1, std::min<int64_t>((nnz_cap + 2047) / 2048, (int64_t)SM * 4));
-    slotmap_mark_kernel<<<mkg, 256, 0, st>>>(s.fid, hdr, nnz_cap, f->mark, f->T);
+    if (launch(c, {mkg, 256, 0, st}, slotmap_mark_kernel, s.fid, hdr, nnz_cap, f->mark, f->T)) return 1;
     const size_t ntiles = (128 * f->T + 511) / 512;
     const unsigned cg = (unsigned)std::max<size_t>(1, std::min<size_t>((ntiles + 7) / 8, (size_t)SM * 8));
-    slotmap_compact_kernel<<<cg, 256, 0, st>>>(f->mark, f->T, s.uniq, s.n_uniq, f->slot_of);
+    if (launch(c, {cg, 256, 0, st}, slotmap_compact_kernel, f->mark, f->T, s.uniq, s.n_uniq, f->slot_of)) return 1;
     const bool hot = c->grad_path == GRAD_COMPACT;  // replica rows only exist for the fused FM / NFM kernels
     if (hot) {
         const unsigned sg = (unsigned)std::min<int64_t>(((int64_t)kHotSampleRows * 128 + 255) / 256, (int64_t)SM * 8);
-        slotmap_sample_kernel<<<sg, 256, 0, st>>>(s.row_ptr, s.fid, hdr, rows_cap, f->slot_of, f->cnt);
-        slotmap_hot_kernel<<<SM * 2, 256, 0, st>>>(f->cnt, s.n_uniq, hdr, rows_cap, s.hot_of, s.hot_slot, s.n_hot);
-        c->launches += 2;
+        if (launch(c, {sg, 256, 0, st}, slotmap_sample_kernel, s.row_ptr, s.fid, hdr, rows_cap, f->slot_of, f->cnt) ||
+            launch(c, {(unsigned)SM * 2, 256, 0, st}, slotmap_hot_kernel, f->cnt, s.n_uniq, hdr, rows_cap, s.hot_of, s.hot_slot,
+                   s.n_hot))
+            return 1;
     }
     const unsigned ag = (unsigned)std::max<int64_t>(1, std::min<int64_t>((nnz_cap + 255) / 256, (int64_t)SM * 8));
-    slotmap_assign_kernel<<<ag, 256, 0, st>>>(s.fid, hdr, nnz_cap, f->slot_of, hot ? s.hot_of : nullptr, s.ent_slot,
-                                              c->cfg.world > 1 ? s.ent_pslot : nullptr);
-    c->launches += 3;
-    LCTR_CUDA(cudaGetLastError());
+    if (launch(c, {ag, 256, 0, st}, slotmap_assign_kernel, s.fid, hdr, nnz_cap, f->slot_of, hot ? s.hot_of : nullptr, s.ent_slot,
+               c->cfg.world > 1 ? s.ent_pslot : nullptr))
+        return 1;
     s.fused_valid = true;
     return 0;
 }
 
-// mode 1: FM forward + backward;  2: NFM forward (z, wide part);  3: NFM backward from dz
-void launch_slotmap_compact(lctr_ctx* c, uint8_t* mark, size_t T, uint32_t* uniq, unsigned int* n_uniq, cudaStream_t st) {
+int launch_slotmap_compact(lctr_ctx* c, uint8_t* mark, size_t T, uint32_t* uniq, unsigned int* n_uniq, cudaStream_t st) {
     const size_t ntiles = (128 * T + 511) / 512;
     const unsigned cg = (unsigned)std::max<size_t>(1, std::min<size_t>((ntiles + 7) / 8, (size_t)c->sm_count * 8));
-    slotmap_compact_kernel<<<cg, 256, 0, st>>>(mark, T, uniq, n_uniq, nullptr);
+    return launch(c, {cg, 256, 0, st}, slotmap_compact_kernel, mark, T, uniq, n_uniq, nullptr);
 }
 
-// programmatic dependent launches (updater behind the gradient kernel; dense kernels and the NFM backward behind their
-// predecessors): LCTR_PDL=0 turns them off; read per launch, the tests toggle it
-bool pdl_on() {
-    const char* e = getenv("LCTR_PDL");
-    return !(e && atoi(e) == 0);
+// mode 1: FM forward + backward;  2: NFM forward (z, wide part);  3: NFM backward from dz
+template <int K, bool HV>
+static auto fused_kernel(int mode) {
+    return mode == 1 ? fm_fused_kernel<K, HV, 1, false>
+         : mode == 2 ? fm_fused_kernel<K, HV, 2, false> : fm_fused_kernel<K, HV, 3, false>;
 }
 
 template <int K>
-static void fused_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, double* out_slot, const int64_t* hdr, int mode) {
+static int fused_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, double* out_slot, const int64_t* hdr, int mode) {
     FusedState* f = c->fused;
     const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((re - rb + 3) / 4, (int64_t)c->sm_count * 4));
     // one GPU: parameters straight from the tables (index = fid); several: from the batch-compact cache the owners filled
@@ -142,40 +141,23 @@ static void fused_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, do
     int nw = 0;
     unsigned long long ep = 0;
     if (multi && mode != 3) dist_wait_info(c, &wf, &nw, &ep);
-#define FUSED_ARGS s.row_ptr, multi ? s.ent_pslot : s.fid, s.ent_slot, s.val, s.label, c->cW, c->cV, s.pred, s.sumvx, nullptr, f->G, \
-                   f->Ghot, f->GS, c->cfg.l2_reg, rb, re, hdr, c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep
-#define FUSED_LAUNCH(HV)                                                                                                         \
-    do {                                                                                                                         \
-        if (mode == 1 && multi && pdl_on()) {  /* several GPUs: dependent on my own serve kernel; polls the owners' flags at its head */ \
-            cudaLaunchConfig_t cfg = {};                                                                                         \
-            cfg.gridDim = dim3(grid); cfg.blockDim = dim3(128); cfg.stream = c->stream;                                          \
-            cudaLaunchAttribute at[1];                                                                                           \
-            at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                       \
-            at[0].val.programmaticStreamSerializationAllowed = 1;                                                                \
-            cfg.attrs = at; cfg.numAttrs = 1;                                                                                    \
-            cudaLaunchKernelEx(&cfg, fm_fused_kernel<K, HV, 1, false>, (const int64_t*)s.row_ptr, (const uint32_t*)s.ent_pslot,  \
-                               (const uint32_t*)s.ent_slot, (const float*)s.val, (const float*)s.label, (const float*)c->cW,   \
-                               (const float*)c->cV, s.pred, s.sumvx, (float*)nullptr, f->G, f->Ghot, f->GS, c->cfg.l2_reg, rb, re, hdr, \
-                               c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep, (float*)nullptr, (float*)nullptr);    \
-        } else if (mode == 1) fm_fused_kernel<K, HV, 1, false><<<grid, 128, 0, c->stream>>>(FUSED_ARGS);                         \
-        else if (mode == 2) fm_fused_kernel<K, HV, 2, false><<<grid, 128, 0, c->stream>>>(FUSED_ARGS, c->z, s.wide);             \
-        else {  /* NFM backward: dependent on the dense kernels in front of it (it requests its batch data before their end) */ \
-            cudaLaunchConfig_t cfg = {};                                                                                         \
-            cfg.gridDim = dim3(grid); cfg.blockDim = dim3(128); cfg.stream = c->stream;                                          \
-            cudaLaunchAttribute at[1];                                                                                           \
-            at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                       \
-            at[0].val.programmaticStreamSerializationAllowed = 1;                                                                \
-            cfg.attrs = at; cfg.numAttrs = (!multi && pdl_on()) ? 1 : 0;                                                         \
-            cudaLaunchKernelEx(&cfg, fm_fused_kernel<K, HV, 3, false>, (const int64_t*)s.row_ptr, (const uint32_t*)(multi ? s.ent_pslot : s.fid), \
-                               (const uint32_t*)s.ent_slot, (const float*)s.val, (const float*)s.label, (const float*)c->cW,   \
-                               (const float*)c->cV, s.pred, s.sumvx, (float*)nullptr, f->G, f->Ghot, f->GS, c->cfg.l2_reg, rb, re, hdr, \
-                               c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep, c->dz, (float*)nullptr);              \
-        }                                                                                                                        \
-    } while (0)
-    if (s.has_val) FUSED_LAUNCH(true); else FUSED_LAUNCH(false);
-#undef FUSED_LAUNCH
-#undef FUSED_ARGS
+    // dependent launches: MODE 1 on several GPUs behind my own serve kernel (it polls the owners' flags at its head); the NFM
+    // backward on one GPU behind the dense kernels in front of it (it requests its batch data before their end)
+    const bool dependent = mode == 1 ? multi : mode == 3 && !multi;
+    return launch(c, {grid, 128, 0, c->stream, dependent}, s.has_val ? fused_kernel<K, true>(mode) : fused_kernel<K, false>(mode),
+                  s.row_ptr, multi ? s.ent_pslot : s.fid, s.ent_slot, s.val, s.label, c->cW, c->cV, s.pred, s.sumvx, nullptr, f->G,
+                  f->Ghot, f->GS, c->cfg.l2_reg, rb, re, hdr, c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep,
+                  mode == 2 ? c->z : mode == 3 ? c->dz : nullptr, mode == 2 ? s.wide : nullptr);
 }
+
+// FM k in {4, 8, 16, 32}: go<K>(args...) for the context's k (32 for any other)
+#define K_DISPATCH(go, ...)                                                                                                      \
+    switch ((int)c->cfg.factor_cnt) {                                                                                            \
+        case 4: return go<4>(__VA_ARGS__);                                                                                       \
+        case 8: return go<8>(__VA_ARGS__);                                                                                       \
+        case 16: return go<16>(__VA_ARGS__);                                                                                     \
+        default: return go<32>(__VA_ARGS__);                                                                                     \
+    }
 
 static int launch_fused_mode(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats, const int64_t* hdr, double* out_slot_override,
                              int mode, int prof_id) {
@@ -183,15 +165,7 @@ static int launch_fused_mode(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool 
     LCTR_CHECK(s.fused_valid, "fused FM step on a slot without its slot map (uploaded before the context supported it?)");
     double* out_slot = out_slot_override ? out_slot_override : c->stats + 2 * (c->step % kStatRing);
     ProfScope prof(c, prof_id);
-    switch ((int)c->cfg.factor_cnt) {
-        case 4: fused_go<4>(c, s, rb, re, stats ? 1 : 0, out_slot, hdr, mode); break;
-        case 8: fused_go<8>(c, s, rb, re, stats ? 1 : 0, out_slot, hdr, mode); break;
-        case 16: fused_go<16>(c, s, rb, re, stats ? 1 : 0, out_slot, hdr, mode); break;
-        default: fused_go<32>(c, s, rb, re, stats ? 1 : 0, out_slot, hdr, mode); break;
-    }
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    K_DISPATCH(fused_go, c, s, rb, re, stats ? 1 : 0, out_slot, hdr, mode)
 }
 
 // forward + RED backward of rows [rb, re) of the slot.  hdr != nullptr: `re` only sizes the grid, the row count comes
@@ -214,95 +188,44 @@ int launch_nfm_backward_fused(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
 // pCTR equals a single-GPU context's bit for bit), launched dependent on my serve kernel like the MODE 1 step, polling
 // the owners' "rows delivered" flags at its head.
 template <int K>
-static void fwd_tree_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, double* out_slot) {
-    const int GS = grad_stride(K);
+static int fwd_tree_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, double* out_slot) {
     const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((re - rb + 3) / 4, (int64_t)c->sm_count * 4));
-    if (c->cfg.world > 1) {
-        const unsigned long long* wf = nullptr;
-        int nw = 0;
-        unsigned long long ep = 0;
-        dist_wait_info(c, &wf, &nw, &ep);
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(128); cfg.stream = c->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;
-        auto kern = s.has_val ? fm_fused_kernel<K, true, 0, true> : fm_fused_kernel<K, false, 0, true>;
-        cudaLaunchKernelEx(&cfg, kern, (const int64_t*)s.row_ptr, (const uint32_t*)s.ent_pslot, (const uint32_t*)s.ent_pslot,
-                           (const float*)s.val, (const float*)s.label, (const float*)c->cW, (const float*)c->cV, s.pred, s.sumvx,
-                           (float*)nullptr, (float*)nullptr, (float*)nullptr, GS, c->cfg.l2_reg, rb, re, (const int64_t*)nullptr,
-                           c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep, (float*)nullptr, (float*)nullptr);
-        return;
-    }
-#define FWD_ARGS s.row_ptr, s.fid, s.fid, s.val, s.label, c->W, c->V, s.pred, s.sumvx, nullptr, nullptr, nullptr, GS, c->cfg.l2_reg, \
-                 rb, re, nullptr, c->stat_partial, c->stat_done, out_slot, stats
-    if (s.has_val) fm_fused_kernel<K, true, 0, true><<<grid, 128, 0, c->stream>>>(FWD_ARGS);
-    else fm_fused_kernel<K, false, 0, true><<<grid, 128, 0, c->stream>>>(FWD_ARGS);
-#undef FWD_ARGS
+    const bool multi = c->cfg.world > 1;
+    const unsigned long long* wf = nullptr;
+    int nw = 0;
+    unsigned long long ep = 0;
+    if (multi) dist_wait_info(c, &wf, &nw, &ep);
+    const uint32_t* fid = multi ? s.ent_pslot : s.fid;
+    return launch(c, {grid, 128, 0, c->stream, multi}, s.has_val ? fm_fused_kernel<K, true, 0, true> : fm_fused_kernel<K, false, 0, true>,
+                  s.row_ptr, fid, fid, s.val, s.label, multi ? c->cW : c->W, multi ? c->cV : c->V, s.pred, s.sumvx, nullptr, nullptr,
+                  nullptr, grad_stride(K), c->cfg.l2_reg, rb, re, nullptr, c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep,
+                  nullptr, nullptr);
 }
 int launch_fm_forward_tree(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
     if (re - rb <= 0) return 0;
     double* out_slot = c->stats + 2 * (c->step % kStatRing);
     ProfScope prof(c, PROF_FM_FWD);
-    switch ((int)c->cfg.factor_cnt) {
-        case 4: fwd_tree_go<4>(c, s, rb, re, stats ? 1 : 0, out_slot); break;
-        case 8: fwd_tree_go<8>(c, s, rb, re, stats ? 1 : 0, out_slot); break;
-        case 16: fwd_tree_go<16>(c, s, rb, re, stats ? 1 : 0, out_slot); break;
-        default: fwd_tree_go<32>(c, s, rb, re, stats ? 1 : 0, out_slot); break;
-    }
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    K_DISPATCH(fwd_tree_go, c, s, rb, re, stats ? 1 : 0, out_slot)
 }
 
 template <int K>
-static void apply_go(lctr_ctx* c, Slot& s, const OptParams& P, const OptParams* P_dev) {
+static int apply_go(lctr_ctx* c, Slot& s, const OptParams& P, const OptParams* P_dev) {
     FusedState* f = c->fused;
     const int main_blocks = c->sm_count * 3;
     const unsigned grid = (unsigned)(main_blocks + kHotMax / 8);  // + one warp per possible hot slot
-    // Programmatic dependent launch behind the gradient kernel (one GPU; LCTR_PDL=0 turns it off): the updater's CTAs start as
-    // the gradient kernel's retire, request their ids, parameter and state rows, and only then wait for its completion.
-    const bool pdl_off = !pdl_on();
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = 0; cfg.stream = c->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = (c->cfg.world == 1 && !pdl_off) ? 1 : 0;
-#define AC_GO(OPTC)                                                                                                          \
-    cudaLaunchKernelEx(&cfg, apply_compact_kernel<K, OPTC>, (const uint32_t*)s.uniq, (const unsigned int*)s.n_uniq, f->G,          \
-                       (const uint32_t*)s.hot_of, (const uint32_t*)s.hot_slot, (const unsigned int*)s.n_hot, f->Ghot, f->GS,     \
-                       main_blocks, c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, P, P_dev)
-    switch (P.opt) {
-        case LCTR_OPT_ADAGRAD: AC_GO(LCTR_OPT_ADAGRAD); break;
-        case LCTR_OPT_FTRL: AC_GO(LCTR_OPT_FTRL); break;
-        case LCTR_OPT_ADAM: AC_GO(LCTR_OPT_ADAM); break;
-        case LCTR_OPT_RMSPROP: AC_GO(LCTR_OPT_RMSPROP); break;
-        case LCTR_OPT_ADADELTA: AC_GO(LCTR_OPT_ADADELTA); break;
-        case LCTR_OPT_PS_SGD: AC_GO(LCTR_OPT_PS_SGD); break;
-        case LCTR_OPT_PS_ADAGRAD: AC_GO(LCTR_OPT_PS_ADAGRAD); break;
-        case LCTR_OPT_PS_DCASGD: AC_GO(LCTR_OPT_PS_DCASGD); break;
-        default: AC_GO(LCTR_OPT_PS_DCASGDA); break;
-    }
-#undef AC_GO
+    // Programmatic dependent launch behind the gradient kernel (one GPU): the updater's CTAs start as the gradient kernel's
+    // retire, request their ids, parameter and state rows, and only then wait for its completion.
+    return launch(c, {grid, 256, 0, c->stream, c->cfg.world == 1}, by_opt(P.opt, [](auto o) { return apply_compact_kernel<K, o.value>; }), s.uniq, s.n_uniq, f->G,
+                  s.hot_of, s.hot_slot, s.n_hot, f->Ghot, f->GS, main_blocks, c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, P, P_dev);
 }
 
 // updater over the slot's key set.  P_host (optional) / dP: parameters already staged in device memory (graph launches).
 int launch_apply_compact(lctr_ctx* c, Slot& s, int64_t rows_in_step, const OptParams* P_host, const OptParams* dP) {
     const OptParams P = P_host ? *P_host : make_opt_params(c, rows_in_step);
     ProfScope prof(c, PROF_APPLY_COMPACT);
-    switch ((int)c->cfg.factor_cnt) {
-        case 4: apply_go<4>(c, s, P, dP); break;
-        case 8: apply_go<8>(c, s, P, dP); break;
-        case 16: apply_go<16>(c, s, P, dP); break;
-        default: apply_go<32>(c, s, P, dP); break;
-    }
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    K_DISPATCH(apply_go, c, s, P, dP)
 }
+#undef K_DISPATCH
 
 void fused_opt_params(lctr_ctx* c, int64_t rows, void* out) { *reinterpret_cast<OptParams*>(out) = make_opt_params(c, rows); }
 void* fused_dev_opt(lctr_ctx* c) { return c->fused ? (void*)c->fused->d_opt : nullptr; }

@@ -97,12 +97,6 @@ namespace lctr {
 constexpr int kEvTile = 1024;  // rows per block of the eviction count / index kernels
 constexpr int kEvBins = 1 << 16;  // radix-select digit
 
-#define LCTR_LAUNCHED()                  \
-    do {                                 \
-        c->launches++;                   \
-        LCTR_CUDA(cudaGetLastError());   \
-    } while (0)
-
 // grid of a warp-per-item kernel over m items (8 warps a block), and of a grid-stride kernel of one thread per item
 static unsigned warp_grid(const lctr_ctx* c, size_t m) {
     return (unsigned)std::max<size_t>(1, std::min<size_t>((m + 7) / 8, (size_t)c->sm_count * 16));
@@ -757,8 +751,8 @@ static unsigned tile_grid(int64_t n) { return (unsigned)std::max<int64_t>(1, (n 
 int KeyIndex::rebuild(lctr_ctx* c, const KeyView& v, const unsigned long long* row_key, size_t n, const char* what) {
     if (clear(c->stream)) return 1;
     if (n) {
-        key_insert_fixed_kernel<<<tile_grid((int64_t)n), 256, 0, c->stream>>>(row_key, nullptr, (int64_t)n, v, 0);
-        LCTR_LAUNCHED();
+        if (launch(c, {tile_grid((int64_t)n), 256, 0, c->stream}, key_insert_fixed_kernel, row_key, nullptr, (int64_t)n, v, 0))
+            return 1;
     }
     LCTR_CUDA(cudaMemcpyAsync(h_flags, flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -794,7 +788,7 @@ static int admission_scratch(Admission* a, size_t cap) {
     if (!cap) return 0;
     if (dalloc(&a->scan, cap + 1) || dalloc(&a->tiles, cap / kEvTile + 1) || dalloc(&a->fid, cap) || dalloc(&a->field, cap) ||
         dalloc(&a->val, cap))
-        return 1;
+            return 1;
     a->cap = cap;
     return 0;
 }
@@ -807,7 +801,7 @@ static int evict_scratch(KeyTable* t, size_t cap) {
     if (!cap) return 0;
     if (dalloc(&t->ev_scan, cap + 1) || dalloc(&t->ev_rows, cap) || dalloc(&t->ev_tiles, cap / kEvTile + 1) ||
         dalloc(&t->ev_hist, (size_t)kEvBins) || dalloc(&t->ev_res, 4))
-        return 1;
+            return 1;
     LCTR_CUDA(cudaMallocHost((void**)&t->h_res, 4 * sizeof(unsigned long long)));
     return 0;
 }
@@ -825,9 +819,8 @@ int init_new_rows(lctr_ctx* c, int64_t max_new) {
     const bool tiered = tier_live(t);
     const auto kernel = tiered ? by_rowlen(c, key_init_kernel<true, true>, key_init_kernel<true, false>) : key_init_kernel<false, false>;
     HostTier* h = tiered ? t->tier : nullptr;
-    kernel<<<warp_grid(c, (size_t)max_new), 256, 0, c->stream>>>(view(t), h ? view(h) : KeyView{}, device_rows(c), h ? h->a : RowArrays{},
-                                                                 c->rowlen, h ? h->rel : nullptr, initial_s1(c->cfg), t->seed, t->scale);
-    LCTR_LAUNCHED();
+    if (launch(c, {warp_grid(c, (size_t)max_new), 256, 0, c->stream}, kernel, view(t), h ? view(h) : KeyView{}, device_rows(c),
+               h ? h->a : RowArrays{}, c->rowlen, h ? h->rel : nullptr, initial_s1(c->cfg), t->seed, t->scale)) return 1;
     return 0;
 }
 
@@ -961,9 +954,8 @@ static int tier_rebuild(lctr_ctx* c) {
 
 // survivors at or above n_live into the holes below it, for the rows of one table (wscan, holes: evict_move_kernel)
 static int launch_move(lctr_ctx* c, const RowArrays& a, size_t n_live, size_t n, const uint32_t* wscan, const uint32_t* holes) {
-    by_rowlen(c, evict_move_kernel<true>, evict_move_kernel<false>)<<<warp_grid(c, n - n_live), 256, 0, c->stream>>>(
-        a, c->rowlen, n_live, n, wscan, holes);
-    LCTR_LAUNCHED();
+    if (launch(c, {warp_grid(c, n - n_live), 256, 0, c->stream}, by_rowlen(c, evict_move_kernel<true>, evict_move_kernel<false>),
+               a, c->rowlen, n_live, n, wscan, holes)) return 1;
     return 0;
 }
 
@@ -1006,8 +998,8 @@ static int tier_compact(lctr_ctx* c) {
     if (!holes.empty())
         LCTR_CUDA(cudaMemcpyAsync(h->holes, holes.data(), holes.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     if (launch_move(c, h->a, n_live, n, h->wscan, h->holes)) return 1;
-    tier_reindex_kernel<<<tile_grid((int64_t)m), 256, 0, c->stream>>>(view(h), n_live, n, h->wscan, h->holes);
-    LCTR_LAUNCHED();
+    if (launch(c, {tile_grid((int64_t)m), 256, 0, c->stream}, tier_reindex_kernel, view(h), n_live, n, h->wscan, h->holes))
+        return 1;
     LCTR_CUDA(cudaMemsetAsync(h->ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
     h->ix.h_flags[0] = 0;
     h->n = n_live;
@@ -1036,26 +1028,24 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
         if (insert || restoring) {
             if (adm) {
                 const KeyView hv = restoring ? view(t->tier) : KeyView{};
-                key_count_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), hv, restoring, adm->sketch, adm->lw);
-                LCTR_LAUNCHED();
-                key_admit_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), hv, restoring, adm->sketch, adm->lw,
-                                                                      adm->min_count, adm->cnt + 1);
+                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_count_kernel, t->d_keys, n, view(t), hv, restoring,
+                           adm->sketch, adm->lw)) return 1;
+                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_admit_kernel, t->d_keys, n, view(t), hv, restoring,
+                           adm->sketch, adm->lw, adm->min_count, adm->cnt + 1)) return 1;
             } else if (insert) {
-                key_insert_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t));
+                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_insert_kernel, t->d_keys, n, view(t))) return 1;
             } else {
-                key_lookup_restore_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), view(t->tier));
+                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_lookup_restore_kernel, t->d_keys, n, view(t), view(t->tier)))
+                    return 1;
             }
-            LCTR_LAUNCHED();
             if (init_new_rows(c, std::min<int64_t>(n, (int64_t)t->cap))) return 1;
             if (!insert) {
-                key_tier_refused_kernel<<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), view(t->tier));
-                LCTR_LAUNCHED();
+                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_tier_refused_kernel, t->d_keys, n, view(t), view(t->tier)))
+                    return 1;
             }
         }
-        key_find_kernel<0><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0,
-                                                                insert ? t->last_seen : nullptr, t->clock,
-                                                                adm ? adm->cnt : nullptr);
-        LCTR_LAUNCHED();
+        if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_find_kernel<0>, t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0,
+                   insert ? t->last_seen : nullptr, t->clock, adm ? adm->cnt : nullptr)) return 1;
     }
     if (read_flags(c, adm != nullptr)) return 1;
     if (adm) {
@@ -1085,15 +1075,12 @@ int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, 
     {
         ProfScope prof(c, PROF_KEYS);
         const size_t ntiles = n / kEvTile + 1;  // tiles cover [0, n]: D(n) is read for row_ptr[rows] = n
-        evict_count_kernel<<<(unsigned)ntiles, kEvTile, 0, st>>>(DropFlag{s.fid}, n, a->tiles);
-        LCTR_LAUNCHED();
-        evict_scan_tiles_kernel<<<1, 1024, 0, st>>>(a->tiles, ntiles, a->cnt + 2);
-        LCTR_LAUNCHED();
-        evict_index_kernel<<<(unsigned)ntiles, kEvTile, 0, st>>>(DropFlag{s.fid}, n, a->tiles, a->scan, nullptr);
-        LCTR_LAUNCHED();
-        admit_compact_kernel<<<stride_grid(c, std::max(n, (size_t)rows + 1)), 256, 0, st>>>(s.fid, field, val, n, a->scan, s.row_ptr, (size_t)rows, a->fid,
-                                                   field ? a->field : nullptr, val ? a->val : nullptr);
-        LCTR_LAUNCHED();
+        if (launch(c, {(unsigned)ntiles, kEvTile, 0, st}, evict_count_kernel<DropFlag>, DropFlag{s.fid}, n, a->tiles)) return 1;
+        if (launch(c, {1, 1024, 0, st}, evict_scan_tiles_kernel, a->tiles, ntiles, a->cnt + 2)) return 1;
+        if (launch(c, {(unsigned)ntiles, kEvTile, 0, st}, evict_index_kernel<DropFlag>, DropFlag{s.fid}, n, a->tiles, a->scan, nullptr))
+            return 1;
+        if (launch(c, {stride_grid(c, std::max(n, (size_t)rows + 1)), 256, 0, st}, admit_compact_kernel, s.fid, field, val, n,
+                   a->scan, s.row_ptr, (size_t)rows, a->fid, field ? a->field : nullptr, val ? a->val : nullptr)) return 1;
     }
     if (kept) {
         LCTR_CUDA(cudaMemcpyAsync(s.fid, a->fid, kept * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
@@ -1108,8 +1095,8 @@ static int lookup_dev(lctr_ctx* c, const uint64_t* keys, int64_t n) {
     KeyTable* t = c->keys;
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
-    key_find_kernel<1><<<tile_grid(n), 256, 0, c->stream>>>(t->d_keys, n, view(t), nullptr, t->d_rows, 0, nullptr, 0, nullptr);
-    LCTR_LAUNCHED();
+    if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_find_kernel<1>, t->d_keys, n, view(t), nullptr, t->d_rows, 0, nullptr, 0,
+               nullptr)) return 1;
     return 0;
 }
 
@@ -1171,10 +1158,9 @@ static int radix_select_age(lctr_ctx* c, const unsigned long long* last_seen, si
         const int width = std::min(16, shift);
         shift -= width;
         LCTR_CUDA(cudaMemsetAsync(t->ev_hist, 0, ((size_t)1 << width) * sizeof(unsigned int), c->stream));
-        evict_hist_kernel<<<grid, 256, 0, c->stream>>>(last_seen, n, t->clock, max_idle, shift, width, pshift, prefix, t->ev_hist);
-        LCTR_LAUNCHED();
-        evict_pick_kernel<<<1, 1024, 0, c->stream>>>(t->ev_hist, 1 << width, rank, t->ev_res);
-        LCTR_LAUNCHED();
+        if (launch(c, {grid, 256, 0, c->stream}, evict_hist_kernel, last_seen, n, t->clock, max_idle, shift, width, pshift,
+                   prefix, t->ev_hist)) return 1;
+        if (launch(c, {1, 1024, 0, c->stream}, evict_pick_kernel, t->ev_hist, 1 << width, rank, t->ev_res)) return 1;
         if (read_res(c, 2)) return 1;
         prefix = (prefix << width) | t->h_res[0];
         rank -= t->h_res[1];
@@ -1197,8 +1183,8 @@ static int evict_plan(lctr_ctx* c, const EvTable& tb, uint64_t max_idle, uint64_
     const size_t n = tb.n;
     // 1 + 2: the rule
     LCTR_CUDA(cudaMemsetAsync(t->ev_res, 0, 2 * sizeof(unsigned long long), c->stream));
-    evict_survey_kernel<<<stride_grid(c, n), 256, 0, c->stream>>>(tb.a.last_seen, n, t->clock, max_idle, t->ev_res);
-    LCTR_LAUNCHED();
+    if (launch(c, {stride_grid(c, n), 256, 0, c->stream}, evict_survey_kernel, tb.a.last_seen, n, t->clock, max_idle, t->ev_res))
+        return 1;
     if (read_res(c, 2)) return 1;
     const unsigned long long survivors = t->h_res[0], max_age = t->h_res[1];
     *e = EvictRule{t->clock, max_idle, 0ull, 0};
@@ -1208,10 +1194,9 @@ static int evict_plan(lctr_ctx* c, const EvTable& tb, uint64_t max_idle, uint64_
     }
     // count and scan
     const size_t ntiles = n / kEvTile + 1;  // tiles cover [0, n]: E(n) is needed too
-    evict_count_kernel<<<(unsigned)ntiles, kEvTile, 0, c->stream>>>(EvictFlag{tb.a.last_seen, *e}, n, tb.tiles);
-    LCTR_LAUNCHED();
-    evict_scan_tiles_kernel<<<1, 1024, 0, c->stream>>>(tb.tiles, ntiles, t->ev_res);
-    LCTR_LAUNCHED();
+    if (launch(c, {(unsigned)ntiles, kEvTile, 0, c->stream}, evict_count_kernel<EvictFlag>, EvictFlag{tb.a.last_seen, *e}, n, tb.tiles))
+        return 1;
+    if (launch(c, {1, 1024, 0, c->stream}, evict_scan_tiles_kernel, tb.tiles, ntiles, t->ev_res)) return 1;
     if (read_res(c, 1)) return 1;
     *m = (size_t)t->h_res[0];
     return 0;
@@ -1220,9 +1205,8 @@ static int evict_plan(lctr_ctx* c, const EvTable& tb, uint64_t max_idle, uint64_
 // E(r) and the list of the m rows that leave, then their key, W and V into the caller's buffers (each may be null)
 static int evict_index_export(lctr_ctx* c, const EvTable& tb, const EvictRule& e, size_t m, uint64_t* keys_out, float* W_out,
                               float* V_out) {
-    evict_index_kernel<<<(unsigned)(tb.n / kEvTile + 1), kEvTile, 0, c->stream>>>(EvictFlag{tb.a.last_seen, e}, tb.n, tb.tiles,
-                                                                                  tb.scan, tb.rows);
-    LCTR_LAUNCHED();
+    if (launch(c, {(unsigned)(tb.n / kEvTile + 1), kEvTile, 0, c->stream}, evict_index_kernel<EvictFlag>, EvictFlag{tb.a.last_seen, e}, tb.n,
+               tb.tiles, tb.scan, tb.rows)) return 1;
     if (!(keys_out || W_out || V_out)) return 0;
     unsigned long long* dK = nullptr;
     float *dW = nullptr, *dV = nullptr;
@@ -1230,10 +1214,12 @@ static int evict_index_export(lctr_ctx* c, const EvTable& tb, const EvictRule& e
     if (keys_out && err == cudaSuccess) err = cudaMalloc((void**)&dK, m * sizeof(unsigned long long));
     if (W_out && err == cudaSuccess) err = cudaMalloc((void**)&dW, m * sizeof(float));
     if (V_out && err == cudaSuccess) err = cudaMalloc((void**)&dV, m * c->rowlen * sizeof(float));
-    if (err == cudaSuccess) {
-        evict_export_kernel<<<warp_grid(c, m), 256, 0, c->stream>>>(tb.rows, m, tb.a.row_key, tb.a.W, tb.a.V, c->rowlen, dK, dW, dV);
-        c->launches++;
-        err = cudaGetLastError();
+    // a failed launch frees the staging before it returns, like every other failure here
+    if (err == cudaSuccess && launch(c, {warp_grid(c, m), 256, 0, c->stream}, evict_export_kernel, tb.rows, m, tb.a.row_key,
+                              tb.a.W, tb.a.V, c->rowlen, dK, dW, dV)) {
+        cudaStreamSynchronize(c->stream);
+        cudaFree(dK); cudaFree(dW); cudaFree(dV);
+        return 1;
     }
     if (err == cudaSuccess && dK) err = cudaMemcpyAsync(keys_out, dK, m * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
     if (err == cudaSuccess && dW) err = cudaMemcpyAsync(W_out, dW, m * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
@@ -1273,9 +1259,8 @@ static int tier_spill(lctr_ctx* c, const EvTable& dev, size_t m) {
     HostTier* h = c->keys->tier;
     KeyIndex& ix = h->ix;
     LCTR_CUDA(cudaMemsetAsync(ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
-    by_rowlen(c, tier_spill_kernel<true>, tier_spill_kernel<false>)<<<warp_grid(c, m), 256, 0, c->stream>>>(
-        dev.rows, m, dev.a, h->a, h->n, c->rowlen, view(h));
-    LCTR_LAUNCHED();
+    if (launch(c, {warp_grid(c, m), 256, 0, c->stream}, by_rowlen(c, tier_spill_kernel<true>, tier_spill_kernel<false>), dev.rows,
+               m, dev.a, h->a, h->n, c->rowlen, view(h))) return 1;
     LCTR_CUDA(cudaMemcpyAsync(ix.h_flags, ix.flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     h->n += m;
@@ -1379,8 +1364,7 @@ static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* key
         LCTR_CUDA(cudaMemsetAsync(t->ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
         LCTR_CUDA(cudaMemcpyAsync(t->d_keys, new_keys.data(), (size_t)m * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
         LCTR_CUDA(cudaMemcpyAsync(t->d_rows, new_rows.data(), (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
-        key_insert_fixed_kernel<<<tile_grid(m), 256, 0, c->stream>>>(t->d_keys, t->d_rows, m, view(t), 1);
-        LCTR_LAUNCHED();
+        if (launch(c, {tile_grid(m), 256, 0, c->stream}, key_insert_fixed_kernel, t->d_keys, t->d_rows, m, view(t), 1)) return 1;
         const bool restoring = tier_live(t);  // tier keys bring their optimizer state back
         if (init_new_rows(c, m)) return 1;
         const unsigned long long cnt = used + (uint64_t)m;
@@ -1392,8 +1376,8 @@ static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* key
     if (t->last_seen || W || V)
         LCTR_CUDA(cudaMemcpyAsync(t->d_rows, rows.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
     if (t->last_seen) {  // every named row counts as met at the current clock
-        key_stamp_rows_kernel<<<stride_grid(c, (size_t)n), 256, 0, c->stream>>>(t->d_rows, n, t->last_seen, t->clock);
-        LCTR_LAUNCHED();
+        if (launch(c, {stride_grid(c, (size_t)n), 256, 0, c->stream}, key_stamp_rows_kernel, t->d_rows, n, t->last_seen, t->clock))
+            return 1;
     }
     if (W || V) {
         float *dW = nullptr, *dV = nullptr;
@@ -1405,12 +1389,12 @@ static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* key
             if (dalloc(&dV, (size_t)n * c->rowlen)) return 1;
             LCTR_CUDA(cudaMemcpyAsync(dV, V, (size_t)n * c->rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
         }
-        key_scatter_params_kernel<<<warp_grid(c, (size_t)n), 256, 0, c->stream>>>(t->d_rows, n, dW, dV, c->W, c->V, c->rowlen);
-        c->launches++;  // as LCTR_LAUNCHED, with the staging freed before an error returns
-        const cudaError_t e = cudaGetLastError();
+        // the staging is freed before an error returns
+        const int rc = launch(c, {warp_grid(c, (size_t)n), 256, 0, c->stream}, key_scatter_params_kernel, t->d_rows, n, dW, dV,
+                              c->W, c->V, c->rowlen);
         cudaStreamSynchronize(c->stream);
         dfree(dW); dfree(dV);
-        LCTR_CUDA(e);
+        if (rc) return 1;
     }
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
@@ -1466,8 +1450,8 @@ int lctr_decay_key_admission(lctr_ctx* c, uint32_t shift) {
     LCTR_CHECK(shift >= 1 && shift <= 32, "lctr_decay_key_admission: shift = %u outside [1, 32]", shift);
     const Admission* a = c->keys->adm;
     const size_t n4 = ((size_t)kSketchDepth << a->lw) / 4;
-    sketch_decay_kernel<<<stride_grid(c, n4), 256, 0, c->stream>>>(reinterpret_cast<uint4*>(a->sketch), n4, shift);
-    LCTR_LAUNCHED();
+    if (launch(c, {stride_grid(c, n4), 256, 0, c->stream}, sketch_decay_kernel, reinterpret_cast<uint4*>(a->sketch), n4, shift))
+        return 1;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }
@@ -1511,9 +1495,8 @@ int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t*
 
     // move, reset, rebuild
     if (launch_move(c, tb.a, n_live, n, t->ev_scan + n_live, t->ev_rows)) return 1;
-    by_rowlen(c, evict_reset_kernel<true>, evict_reset_kernel<false>)<<<warp_grid(c, m), 256, 0, c->stream>>>(
-        tb.a, c->rowlen, n_live, n, initial_s1(c->cfg));
-    LCTR_LAUNCHED();
+    if (launch(c, {warp_grid(c, m), 256, 0, c->stream}, by_rowlen(c, evict_reset_kernel<true>, evict_reset_kernel<false>), tb.a,
+               c->rowlen, n_live, n, initial_s1(c->cfg))) return 1;
     const unsigned long long cnt = n_live;
     LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
     if (t->ix.rebuild(c, view(t), t->row_key, n_live, "lctr_evict_keys: key table full while re-inserting")) return 1;

@@ -168,7 +168,7 @@ static int auc_scratch(lctr_ctx* c, AucScratch** out) {
 }
 
 // the three metrics of n device-resident (pCTR, label) pairs, in row order: histogram, compaction of the non-empty buckets,
-// and the two fp32 chains (five launches)
+// and the two fp32 chains
 static int eval_device(lctr_ctx* c, AucScratch* a, const float* pred, const float* label, int64_t n, float* loss_sum,
                        int64_t* correct, float* auc) {
     if ((size_t)n > a->list_cap) {
@@ -179,13 +179,12 @@ static int eval_device(lctr_ctx* c, AucScratch* a, const float* pred, const floa
         LCTR_CUDA(cudaMalloc((void**)&a->list, (size_t)(n + 32) * sizeof(uint2)));
         a->list_cap = (size_t)n;
     }
-    auc_hist_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(pred, label, n, a->pos, a->neg);
-    auc_tile_count_kernel<<<kAucTiles / 8, 256, 0, c->stream>>>(a->pos, a->neg, a->tile_cnt);
-    auc_tile_scan_kernel<<<1, 1024, 0, c->stream>>>(a->tile_cnt, a->tile_off, a->total);
-    auc_tile_write_kernel<<<kAucTiles / 8, 256, 0, c->stream>>>(a->pos, a->neg, a->tile_cnt, a->tile_off, a->list);
-    auc_chain_kernel<<<1, 32, 0, c->stream>>>(a->list, a->total, pred, label, n, a->out);
-    c->launches += 5;
-    LCTR_CUDA(cudaGetLastError());
+    if (launch(c, {(unsigned)((n + 255) / 256), 256, 0, c->stream}, auc_hist_kernel, pred, label, n, a->pos, a->neg) ||
+        launch(c, {kAucTiles / 8, 256, 0, c->stream}, auc_tile_count_kernel, a->pos, a->neg, a->tile_cnt) ||
+        launch(c, {1, 1024, 0, c->stream}, auc_tile_scan_kernel, a->tile_cnt, a->tile_off, a->total) ||
+        launch(c, {kAucTiles / 8, 256, 0, c->stream}, auc_tile_write_kernel, a->pos, a->neg, a->tile_cnt, a->tile_off, a->list) ||
+        launch(c, {1, 32, 0, c->stream}, auc_chain_kernel, a->list, a->total, pred, label, n, a->out))
+        return 1;
     float h[3];
     LCTR_CUDA(cudaMemcpyAsync(h, a->out, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));

@@ -209,53 +209,56 @@ int mlp_sync_dense_grad(lctr_ctx* c) {
 static inline unsigned mlp_blocks(int64_t n) { return (unsigned)((n + 255) / 256); }
 
 // Fully_Conn_Layer::forward down the chain (fullyconnLayer.h:80-118) on B rows of c->z; layer l's output in layers[l].act
-static void mlp_forward_dev(lctr_ctx* c, int B) {
+static int mlp_forward_dev(lctr_ctx* c, int B) {
     const int nl = c->n_layers;
     const float* x = c->z;
     for (int l = 0; l < nl; l++) {
         MlpLayer& L = c->layers[l];
-        fc_forward_kernel<<<mlp_blocks((int64_t)B * L.out), 256, 0, c->stream>>>(x, L.w, L.b, L.mask, L.act, B, L.in, L.out,
-                                                                                 l + 1 < nl ? 1 : 0, c->cfg.activation);
-        c->launches++;
+        if (launch(c, {mlp_blocks((int64_t)B * L.out), 256, 0, c->stream}, fc_forward_kernel, x, L.w, L.b, L.mask, L.act, B, L.in,
+                   L.out, l + 1 < nl ? 1 : 0, c->cfg.activation))
+            return 1;
         x = L.act;
     }
+    return 0;
 }
 // Fully_Conn_Layer::backward up the chain (fullyconnLayer.h:120-180) from layers[nl-1].delta: clip, inputDelta into
 // c->dz (first layer) / the previous layer's delta, weightDelta / biasDelta accumulated in the fused dense-gradient buffer
-static void mlp_backward_dev(lctr_ctx* c, int B) {
+static int mlp_backward_dev(lctr_ctx* c, int B) {
     const int nl = c->n_layers;
     for (int l = nl - 1; l >= 0; l--) {
         MlpLayer& L = c->layers[l];
         const bool has_next = l + 1 < nl;
         const float* xin = l == 0 ? c->z : c->layers[l - 1].act;
-        clip_kernel<<<mlp_blocks((int64_t)B * L.out), 256, 0, c->stream>>>(L.delta, (int64_t)B * L.out);
         float* dx = l == 0 ? c->dz : c->layers[l - 1].delta;
-        fc_input_delta_kernel<<<mlp_blocks((int64_t)B * L.in), 256, 0, c->stream>>>(
-            L.delta, L.w, L.mask, l > 0 ? c->layers[l - 1].act : nullptr, dx, B, L.in, L.out, has_next ? 1 : 0,
-            c->cfg.activation);
-        fc_weight_grad_kernel<<<mlp_blocks((int64_t)L.out * (L.in + 1)), 256, 0, c->stream>>>(xin, L.delta, L.dw, L.db, B,
-                                                                                              L.in, L.out);
-        c->launches += 3;
+        if (launch(c, {mlp_blocks((int64_t)B * L.out), 256, 0, c->stream}, clip_kernel, L.delta, (int64_t)B * L.out) ||
+            launch(c, {mlp_blocks((int64_t)B * L.in), 256, 0, c->stream}, fc_input_delta_kernel, L.delta, L.w, L.mask,
+                   l > 0 ? c->layers[l - 1].act : nullptr, dx, B, L.in, L.out, has_next ? 1 : 0, c->cfg.activation) ||
+            launch(c, {mlp_blocks((int64_t)L.out * (L.in + 1)), 256, 0, c->stream}, fc_weight_grad_kernel, xin, L.delta, L.dw, L.db,
+                   B, L.in, L.out))
+            return 1;
     }
+    return 0;
 }
 // Fully_Conn_Layer::applyBatchGradient (fullyconnLayer.h:194-197): Adagrad on bias then weights, per layer; deltas zeroed
-static void mlp_apply_dev(lctr_ctx* c, uint64_t mb) {
+static int mlp_apply_dev(lctr_ctx* c, uint64_t mb) {
     const float invB = (float)(1.0 / (double)mb);
     for (int l = 0; l < c->n_layers; l++) {
         MlpLayer& L = c->layers[l];
         const size_t nw = (size_t)L.out * L.in;
-        adagrad_dense_kernel<<<mlp_blocks(L.out), 256, 0, c->stream>>>(L.b, L.db, L.acc_b, L.out, invB, c->cfg.learning_rate);
-        adagrad_dense_kernel<<<mlp_blocks((int64_t)nw), 256, 0, c->stream>>>(L.w, L.dw, L.acc_w, nw, invB, c->cfg.learning_rate);
-        c->launches += 2;
+        if (launch(c, {mlp_blocks(L.out), 256, 0, c->stream}, adagrad_dense_kernel, L.b, L.db, L.acc_b, L.out, invB,
+                   c->cfg.learning_rate) ||
+            launch(c, {mlp_blocks((int64_t)nw), 256, 0, c->stream}, adagrad_dense_kernel, L.w, L.dw, L.acc_w, nw, invB,
+                   c->cfg.learning_rate))
+            return 1;
     }
+    return 0;
 }
 
 // forward only (fp32 reference-order layers) on the rows staged in c->z; *out = the last layer's output [rows]
 int mlp_forward_only(lctr_ctx* c, int64_t rows, const float** out) {
     LCTR_CHECK(c->cfg.mlp_precision == LCTR_MLP_FP32, "forward-only dense layers run in the fp32 mode");
-    mlp_forward_dev(c, (int)rows);
+    if (mlp_forward_dev(c, (int)rows)) return 1;
     *out = c->layers[c->n_layers - 1].act;
-    LCTR_CUDA(cudaGetLastError());
     return 0;
 }
 
@@ -269,19 +272,17 @@ int launch_nfm_mlp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_di
     // B == 0 (a rank's empty share on several GPUs): no rows, no gradient (the buffer is zero between steps); the rank
     // still joins the all-reduce and the replicated updater, so the collective stays matched and the layers stay equal
     if (B > 0) {
-        mlp_forward_dev(c, B);
-        // ---- loss, delta of the output layer
+        // forward, loss and delta of the output layer, backward
         double* out_slot = c->stats + 2 * (c->step % kStatRing);
         MlpLayer& last = c->layers[nl - 1];
-        nfm_loss_kernel<<<mlp_blocks(B), 256, 0, c->stream>>>(s.wide, last.act, s.label, s.pred, last.delta, rb, B,
-                                                              c->stat_partial, c->stat_done, out_slot);
-        c->launches++;
-        mlp_backward_dev(c, B);
+        if (mlp_forward_dev(c, B) ||
+            launch(c, {mlp_blocks(B), 256, 0, c->stream}, nfm_loss_kernel, s.wide, last.act, s.label, s.pred, last.delta, rb, B,
+                   c->stat_partial, c->stat_done, out_slot) ||
+            mlp_backward_dev(c, B))
+            return 1;
     }
     if (mlp_sync_dense_grad(c)) return 1;
-    if (!c->mlp_skip_update) mlp_apply_dev(c, c->cfg.minibatch_size ? c->cfg.minibatch_size : (uint64_t)rows_divisor);
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return c->mlp_skip_update ? 0 : mlp_apply_dev(c, c->cfg.minibatch_size ? c->cfg.minibatch_size : (uint64_t)rows_divisor);
 }
 
 }  // namespace lctr
@@ -296,8 +297,7 @@ int lctr_mlp_forward(lctr_ctx* c, int64_t rows, const float* x, float* out) {
     if (mlp_reserve(c, rows)) return 1;
     const size_t in0 = mlp_in0(c->cfg);
     LCTR_CUDA(cudaMemcpyAsync(c->z, x, (size_t)rows * in0 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    mlp_forward_dev(c, (int)rows);
-    LCTR_CUDA(cudaGetLastError());
+    if (mlp_forward_dev(c, (int)rows)) return 1;
     c->mlp_fwd_rows = rows;
     if (out) {
         MlpLayer& last = c->layers[c->n_layers - 1];
@@ -312,8 +312,7 @@ int lctr_mlp_backward(lctr_ctx* c, int64_t rows, const float* dout, float* dx) {
                "ran %lld", (long long)rows, (long long)c->mlp_fwd_rows);
     MlpLayer& last = c->layers[c->n_layers - 1];
     LCTR_CUDA(cudaMemcpyAsync(last.delta, dout, (size_t)rows * last.out * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    mlp_backward_dev(c, (int)rows);
-    LCTR_CUDA(cudaGetLastError());
+    if (mlp_backward_dev(c, (int)rows)) return 1;
     if (dx) {
         LCTR_CUDA(cudaMemcpyAsync(dx, c->dz, (size_t)rows * mlp_in0(c->cfg) * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -324,9 +323,7 @@ int lctr_mlp_apply(lctr_ctx* c, uint64_t minibatch) {
     LCTR_CHECK(c && c->n_layers > 0, "lctr_mlp_apply: the context has no dense layers");
     LCTR_CHECK(minibatch > 0, "lctr_mlp_apply: minibatch divisor must be > 0");
     if (mlp_sync_dense_grad(c)) return 1;
-    mlp_apply_dev(c, minibatch);
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return mlp_apply_dev(c, minibatch);
 }
 int lctr_mlp_upload(lctr_ctx* c, int layer, const float* weight, const float* bias) {
     LCTR_CHECK(c && layer >= 0 && layer < c->n_layers, "mlp layer %d out of range", layer);

@@ -421,10 +421,6 @@ int mlp_bf16_prepare(lctr_ctx* c) {
     if (need > 227 * 1024 - 1024) { need = bf16_layout(c, 64, P); c->mlp_tm = 64; }
     LCTR_CHECK(need <= 227 * 1024 - 1024, "bf16 MLP: layers need %zu B of shared memory per CTA (max %d)", need, 227 * 1024 - 1024);
     c->mlp_smem = need;
-    if (c->mlp_tm == 128)
-        LCTR_CUDA(cudaFuncSetAttribute(nfm_mlp_fused_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
-    else
-        LCTR_CUDA(cudaFuncSetAttribute(nfm_mlp_fused_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
     return 0;
 }
 
@@ -432,9 +428,8 @@ int mlp_bf16_refresh(lctr_ctx* c, int layer) {
     MlpLayer& L = c->layers[layer];
     if (!L.w16) return 0;
     const size_t n = (size_t)L.out * L.in;
-    to_bf16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(L.w, (__nv_bfloat16*)L.w16, (__nv_bfloat16*)L.w16t, L.in, L.out, n);
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return launch(c, {(unsigned)((n + 255) / 256), 256, 0, c->stream}, to_bf16_kernel, L.w, (__nv_bfloat16*)L.w16,
+                  (__nv_bfloat16*)L.w16t, L.in, L.out, n);
 }
 
 int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor) {
@@ -454,17 +449,13 @@ int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t ro
     // B == 0 (a rank's empty share on several GPUs): no rows, no gradient; the rank still joins the all-reduce and the
     // replicated updater below
     if (B > 0) {
-        if (c->mlp_umma && !c->mlp_has_mask) {  // wgmma kernel (mlp_umma.cu); dropout masks stay on the mma.sync kernel
-            if (launch_mlp_umma(c, s, rb, B, out_slot)) return 1;
-        } else if (c->mlp_tm == 128)
-            nfm_mlp_fused_kernel<128><<<grid, 256, c->mlp_smem, c->stream>>>(P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
-                                                                            c->stat_partial, c->stat_done, out_slot);
-        else
-            nfm_mlp_fused_kernel<64><<<grid, 128, c->mlp_smem, c->stream>>>(P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
-                                                                           c->stat_partial, c->stat_done, out_slot);
-        if (!(c->mlp_umma && !c->mlp_has_mask)) c->launches++;
+        const int rc = c->mlp_umma && !c->mlp_has_mask  // wgmma kernel (mlp_umma.cu); dropout masks stay on the mma.sync kernel
+            ? launch_mlp_umma(c, s, rb, B, out_slot)
+            : launch(c, {grid, c->mlp_tm == 128 ? 256u : 128u, c->mlp_smem, c->stream},
+                     c->mlp_tm == 128 ? nfm_mlp_fused_kernel<128> : nfm_mlp_fused_kernel<64>, P, c->z, c->dz, s.wide, s.label, s.pred,
+                     rb, B, c->stat_partial, c->stat_done, out_slot);
+        if (rc) return 1;
     }
-    LCTR_CUDA(cudaGetLastError());
     if (mlp_sync_dense_grad(c)) return 1;
     if (!c->mlp_skip_update) {
         DenseSegs S;
@@ -481,16 +472,9 @@ int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t ro
         }
         S.off[2 * nl] = off;
         const uint64_t mb = c->cfg.minibatch_size ? c->cfg.minibatch_size : (uint64_t)rows_divisor;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)((off + 255) / 256)); cfg.blockDim = dim3(256); cfg.stream = c->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = (c->cfg.world == 1 && pdl_on()) ? 1 : 0;
-        cudaLaunchKernelEx(&cfg, adagrad_dense_all_kernel, S, c->dense_grad, (float)(1.0 / (double)mb), c->cfg.learning_rate);
-        c->launches++;
+        return launch(c, {(unsigned)((off + 255) / 256), 256, 0, c->stream, c->cfg.world == 1}, adagrad_dense_all_kernel, S,
+                      c->dense_grad, (float)(1.0 / (double)mb), c->cfg.learning_rate);
     }
-    LCTR_CUDA(cudaGetLastError());
     return 0;
 }
 

@@ -486,8 +486,6 @@ int mlp_umma_prepare(lctr_ctx* c) {
     umma::Dev P;
     const size_t need = umma::layout(c, P);
     c->mlp_umma_smem = need;
-    LCTR_CUDA(cudaFuncSetAttribute(umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
-    LCTR_CUDA(cudaFuncSetAttribute(umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
     return 0;
 }
 
@@ -510,20 +508,11 @@ int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot) {
         P.trace = d_trace;
     }
     const unsigned grid = (unsigned)((B + umma::kTM - 1) / umma::kTM);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(umma::kThreads); cfg.dynamicSmemBytes = c->mlp_umma_smem; cfg.stream = c->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = (c->cfg.world == 1 && pdl_on()) ? 1 : 0;  // behind the embedding forward (fm_fused.cu, MODE 2)
-    if (P.act == LCTR_ACT_SIGMOID)
-        cudaLaunchKernelEx(&cfg, umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID>, P, (const float*)c->z, c->dz, (const float*)s.wide,
-                           (const float*)s.label, s.pred, rb, B, c->stat_partial, c->stat_done, out_slot);
-    else
-        cudaLaunchKernelEx(&cfg, umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH>, P, (const float*)c->z, c->dz, (const float*)s.wide,
-                           (const float*)s.label, s.pred, rb, B, c->stat_partial, c->stat_done, out_slot);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
+    // one GPU: dependent on the embedding forward in front of it (fm_fused.cu, MODE 2)
+    if (launch(c, {grid, (unsigned)umma::kThreads, c->mlp_umma_smem, c->stream, c->cfg.world == 1},
+               P.act == LCTR_ACT_SIGMOID ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH>, P,
+               c->z, c->dz, s.wide, s.label, s.pred, rb, B, c->stat_partial, c->stat_done, out_slot))
+        return 1;
     if (trace) {  // phase boundaries of CTA 0: setup | per layer (mma, epilogue) | output | per layer backward | stats
         unsigned long long h[64];
         LCTR_CUDA(cudaStreamSynchronize(c->stream));

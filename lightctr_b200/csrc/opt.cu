@@ -179,6 +179,34 @@ apply_kernel(const uint32_t* __restrict__ list, unsigned int* __restrict__ n_lis
     }
 }
 
+// the sparse apply's instance: Adagrad, FTRL, Adam, RMSprop and Adadelta are specialised on 4-wide rows, every other
+// updater and row shape takes OPT = -1
+template <int LPR, int VEC, int SPL, int U>
+static auto apply_instance(int opt) {
+    if (VEC != 4) return apply_kernel<LPR, VEC, SPL, U, -1>;
+    switch (opt) {
+        case LCTR_OPT_ADAGRAD: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_ADAGRAD>;
+        case LCTR_OPT_FTRL: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_FTRL>;
+        case LCTR_OPT_ADAM: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_ADAM>;
+        case LCTR_OPT_RMSPROP: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_RMSPROP>;
+        case LCTR_OPT_ADADELTA: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_ADADELTA>;
+        default: return apply_kernel<LPR, VEC, SPL, U, -1>;
+    }
+}
+template <int VEC>
+static auto apply_pick(int lpr, int spl, int opt) {
+    switch (lpr) {
+        case 1: return apply_instance<1, VEC, 1, 4>(opt);
+        case 2: return apply_instance<2, VEC, 1, 4>(opt);
+        case 4: return apply_instance<4, VEC, 1, 4>(opt);
+        case 8: return apply_instance<8, VEC, 1, 4>(opt);
+        case 16: return apply_instance<16, VEC, 1, 4>(opt);
+        default:
+            return spl == 1 ? apply_instance<32, VEC, 1, 4>(opt) : spl == 2 ? apply_instance<32, VEC, 2, 2>(opt)
+                 : spl == 3 ? apply_instance<32, VEC, 3, 1>(opt) : apply_instance<32, VEC, 4, 1>(opt);
+    }
+}
+
 int launch_apply(lctr_ctx* c, int64_t rows_in_step) {
     OptParams P = make_opt_params(c, rows_in_step);
     const int rowlen = (int)c->rowlen;
@@ -193,57 +221,9 @@ int launch_apply(lctr_ctx* c, int64_t rows_in_step) {
     if (grid_a == 0) grid_a = 1;
     const unsigned grid = (unsigned)c->sm_count * 2;
     ProfScope prof(c, PROF_APPLY);
-    compact_touched_kernel<<<grid_a, 256, 0, c->stream>>>(c->touched, c->Fl, c->touch_list, c->n_touch);
-    c->launches++;
-#define APPLY_ARGS c->touch_list, c->n_touch, c->apply_done, rowlen, c->W, c->V, c->gW, c->gV, c->s1W, c->s1V, c->s2W, c->s2V, P
-#define APPLY_GO(L, VV, S, UU, OO) apply_kernel<L, VV, S, UU, OO><<<grid, 256, 0, c->stream>>>(APPLY_ARGS)
-#define APPLY_CASE(L, VV, S, UU)                                             \
-    do {                                                                     \
-        if (VV != 4) { APPLY_GO(L, VV, S, UU, -1); break; }                  \
-        switch (P.opt) {                                                     \
-            case LCTR_OPT_ADAGRAD: APPLY_GO(L, VV, S, UU, LCTR_OPT_ADAGRAD); break;   \
-            case LCTR_OPT_FTRL: APPLY_GO(L, VV, S, UU, LCTR_OPT_FTRL); break;         \
-            case LCTR_OPT_ADAM: APPLY_GO(L, VV, S, UU, LCTR_OPT_ADAM); break;         \
-            case LCTR_OPT_RMSPROP: APPLY_GO(L, VV, S, UU, LCTR_OPT_RMSPROP); break;   \
-            case LCTR_OPT_ADADELTA: APPLY_GO(L, VV, S, UU, LCTR_OPT_ADADELTA); break; \
-            default: APPLY_GO(L, VV, S, UU, -1); break;                               \
-        }                                                                    \
-    } while (0)
-    if (vec == 4) {
-        switch (lpr) {
-            case 1: APPLY_CASE(1, 4, 1, 4); break;
-            case 2: APPLY_CASE(2, 4, 1, 4); break;
-            case 4: APPLY_CASE(4, 4, 1, 4); break;
-            case 8: APPLY_CASE(8, 4, 1, 4); break;
-            case 16: APPLY_CASE(16, 4, 1, 4); break;
-            default:
-                if (spl == 1) APPLY_CASE(32, 4, 1, 4);
-                else if (spl == 2) APPLY_CASE(32, 4, 2, 2);
-                else if (spl == 3) APPLY_CASE(32, 4, 3, 1);
-                else APPLY_CASE(32, 4, 4, 1);
-                break;
-        }
-    } else {
-        switch (lpr) {
-            case 1: APPLY_CASE(1, 1, 1, 4); break;
-            case 2: APPLY_CASE(2, 1, 1, 4); break;
-            case 4: APPLY_CASE(4, 1, 1, 4); break;
-            case 8: APPLY_CASE(8, 1, 1, 4); break;
-            case 16: APPLY_CASE(16, 1, 1, 4); break;
-            default:
-                if (spl == 1) APPLY_CASE(32, 1, 1, 4);
-                else if (spl == 2) APPLY_CASE(32, 1, 2, 2);
-                else if (spl == 3) APPLY_CASE(32, 1, 3, 1);
-                else APPLY_CASE(32, 1, 4, 1);
-                break;
-        }
-    }
-#undef APPLY_CASE
-#undef APPLY_GO
-#undef APPLY_ARGS
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    if (launch(c, {grid_a, 256, 0, c->stream}, compact_touched_kernel, c->touched, c->Fl, c->touch_list, c->n_touch)) return 1;
+    return launch(c, {grid, 256, 0, c->stream}, vec == 4 ? apply_pick<4>(lpr, spl, P.opt) : apply_pick<1>(lpr, spl, P.opt),
+                  c->touch_list, c->n_touch, c->apply_done, rowlen, c->W, c->V, c->gW, c->gV, c->s1W, c->s1V, c->s2W, c->s2V, P);
 }
 
 }  // namespace lctr

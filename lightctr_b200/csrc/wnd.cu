@@ -111,12 +111,9 @@ int launch_wnd_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     if (rows <= 0) return 0;
     LCTR_CHECK(s.has_field, "Wide&Deep batch uploaded without the field array");
     ProfScope prof(c, PROF_FM_FWD);
-    wnd_forward_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, c->stream>>>(s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.has_val ? s.val : nullptr,
-                                                                         c->cW, c->cV, (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt,
-                                                                         c->z, c->wnd_src, s.wide, rb, re);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return launch(c, {(unsigned)((rows + 7) / 8), 256, 0, c->stream}, wnd_forward_kernel, s.row_ptr,
+                  c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.has_val ? s.val : nullptr, c->cW, c->cV, (int)c->cfg.field_cnt,
+                  (int)c->cfg.factor_cnt, c->z, c->wnd_src, s.wide, rb, re);
 }
 
 // Distributed_Algo_Abst::Predict (distributed_algo_abst.h:163-174): pCTR = sigmoid(wide + chain output), no gradients
@@ -126,23 +123,17 @@ __global__ void wnd_pred_kernel(const float* __restrict__ wide, const float* __r
 }
 int launch_wnd_pred(lctr_ctx* c, Slot& s, const float* mlp_out, int64_t rb, int64_t re) {
     if (re - rb <= 0) return 0;
-    wnd_pred_kernel<<<(unsigned)((re - rb + 255) / 256), 256, 0, c->stream>>>(s.wide, mlp_out, s.pred, rb, re - rb);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return launch(c, {(unsigned)((re - rb + 255) / 256), 256, 0, c->stream}, wnd_pred_kernel, s.wide, mlp_out, s.pred, rb, re - rb);
 }
 
 int launch_wnd_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     const int64_t rows = re - rb;
     if (rows <= 0) return 0;
     ProfScope prof(c, PROF_FM_BWD_RED);
-    wnd_backward_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, c->stream>>>(s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.has_val ? s.val : nullptr, s.label, s.pred,
-                                                                          c->cW, c->wnd_src, c->dz, (int)c->cfg.field_cnt,
-                                                                          (int)c->cfg.factor_cnt, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched,
-                                                                          c->cfg.l2_reg, rb, re);
-    c->launches++;
-    LCTR_CUDA(cudaGetLastError());
-    return 0;
+    return launch(c, {(unsigned)((rows + 7) / 8), 256, 0, c->stream}, wnd_backward_kernel, s.row_ptr,
+                  c->cfg.world > 1 ? s.ent_pslot : s.fid, s.has_val ? s.val : nullptr, s.label, s.pred, c->cW, c->wnd_src, c->dz,
+                  (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched,
+                  c->cfg.l2_reg, rb, re);
 }
 
 }  // namespace lctr

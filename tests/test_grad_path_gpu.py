@@ -25,11 +25,16 @@ CASES = {
     "fm16_det2": (dict(model="FM", k=16, deterministic=2), "feature_major", True),
     "fm12_det0": (dict(model="FM", k=12, deterministic=0), "dense", True),
     "nfm16_fp32": (dict(model="NFM", k=16, deterministic=0, hidden=(32,)), "compact", False),
+    "nfm16_bf16": (dict(model="NFM", k=16, deterministic=0, hidden=(64,), mlp_precision="BF16"), "compact", False),
+    "nfm16_bf16_mask": (dict(model="NFM", k=16, deterministic=0, hidden=(64,), mlp_precision="BF16", mask=True), "compact",
+                        False),
     "ffm4_det0": (dict(model="FFM", k=4, deterministic=0, field_cnt=39), "dense", True),
+    "ffm4_det1": (dict(model="FFM", k=4, deterministic=1, field_cnt=39), "dense", True),
     "ffm4_det2": (dict(model="FFM", k=4, deterministic=2, field_cnt=39), "feature_major", True),
     "wnd": (dict(model="WND", k=8, deterministic=0, field_cnt=39, hidden=(32,)), "dense", True),
 }
 
+# NFM with mlp_precision = BF16 runs its dense chain on the wgmma kernel, or with a dropout mask on the mma.sync kernel.
 # lctr_launch_count deltas of (upload, first train step, predict) on one CriteoSynth batch of ROWS rows
 PINS = {
     "fm16_det0": (6, 2, 1),
@@ -37,7 +42,10 @@ PINS = {
     "fm16_det2": (5, 3, 1),
     "fm12_det0": (1, 4, 1),
     "nfm16_fp32": (6, 16, None),
+    "nfm16_bf16": (6, 5, None),
+    "nfm16_bf16_mask": (6, 5, None),
     "ffm4_det0": (1, 3, 1),
+    "ffm4_det1": (1, 3, 1),
     "ffm4_det2": (5, 2, 1),
     "wnd": (1, 17, 4),
 }
@@ -48,7 +56,19 @@ def _ctx(capi, name, **extra):
     a = dict(a)
     model = getattr(capi, "MODEL_" + a.pop("model"))
     k = a.pop("k")
-    return capi.Context(model, F, k, **a, **extra)
+    mask = a.pop("mask", False)
+    if "mlp_precision" in a:
+        a["mlp_precision"] = getattr(capi, "MLP_" + a["mlp_precision"])
+    ctx = capi.Context(model, F, k, **a, **extra)
+    if a.get("mlp_precision") == capi.MLP_BF16:  # mlp_upload writes the bf16 copies of the hidden layers
+        rng = np.random.default_rng(1)
+        dims = [k, *a["hidden"], 1]
+        for l in range(len(dims) - 1):
+            ctx.mlp_upload(l, (rng.standard_normal((dims[l + 1], dims[l])) / np.sqrt(dims[l])).astype(np.float32),
+                           np.zeros(dims[l + 1], np.float32))
+    if mask:  # one unit in four dropped
+        ctx.mlp_set_mask(0, (np.arange(a["hidden"][0]) % 4 != 0).astype(np.float32))
+    return ctx
 
 
 def _upload(ctx, slot, batch):

@@ -112,6 +112,7 @@ def test_predict_interleaved_with_training(tmp_path):
     for r in range(2):
         lp, ln = with_p[r]["launches"], without[r]["launches"]
         assert lp[0] == ln[0] and lp[1] == ln[1] + 1 and lp[2] == ln[2] + 1, (lp, ln)
+        assert list(lp) == [7, 8, 8] and list(ln) == [7, 7, 7], (r, list(lp), list(ln))
 
 
 def test_wnd_predict_twice_then_train(tmp_path):
