@@ -3,7 +3,8 @@
     RANK=r WORLD_SIZE=R MASTER_ADDR=127.0.0.1 MASTER_PORT=p python tests/dist_worker.py --out DIR [...]
 
 mode=gpu   : the real CUDA path (csrc/dist.cu); with --same-device every rank uses cuda:0 (IPC between processes on
-             one GPU -- slow barriers, but exercises every kernel), plumbing over gloo.
+             one GPU -- slow barriers, but exercises every kernel), plumbing over gloo.  --probe: the updater is a unit
+             SGD step (OPT_PS_SGD with lr = the global batch, so w1 = w0 - g) and each step's pCTR is saved as well.
 mode=emu   : CPU emulation of the same protocol with the oracle's arithmetic and gloo collectives (pull = all ranks
              read the owner's rows, push = all_to_all of (fid, grad row) records, owner merges + applies): checks that
              the protocol is the single-process step, on machines without a GPU."""
@@ -49,21 +50,24 @@ def run_gpu(args, rank, world):
     torch.cuda.set_device(dev)
     ctx = capi.Context(model, args.F, args.k, 39 if args.model == "ffm" else 0, device=dev, rank=rank, world=world,
                        minibatch_size=world * args.rows, max_nnz=args.rows * 200,
-                       hidden=NFM_HIDDEN if args.model == "nfm" else ())
+                       hidden=NFM_HIDDEN if args.model == "nfm" else (),
+                       **(dict(optimizer=capi.OPT_PS_SGD, lr=float(world * args.rows)) if args.probe else {}))
     ctx.upload_params(W0, V0)
     ldist.connect(ctx)
     if args.model == "nfm":
         for l, (w, b) in enumerate(make_mlp(args)):
             ctx.mlp_upload(l, w, b)
         ldist.attach_dense_allreduce(ctx)
-    stats = []
+    stats, preds = [], []
     for rp, fid, fld, lab in batches:
         ctx.upload_batch(0, rp, fid, fld if args.model == "ffm" else None, None, lab)
         l, c = ctx.train_step(0)
         stats.append(ldist.reduce_stats(l, c))
+        if args.probe:
+            preds.append(ctx.download_pred(0))
     dist.barrier()
     W, V = ctx.download_params()
-    extra = {}
+    extra = {"pred": np.concatenate(preds)} if args.probe else {}
     if args.model == "nfm":
         dims = [args.k] + list(NFM_HIDDEN) + [1]
         for l in range(len(dims) - 1):
@@ -139,6 +143,7 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--out", required=True)
     ap.add_argument("--same-device", action="store_true")
+    ap.add_argument("--probe", action="store_true")
     ap.add_argument("--backend", default="gloo")
     args = ap.parse_args()
     import torch.distributed as dist

@@ -4,8 +4,9 @@
     LCTR_FWD_COALESCED=0 python tests/kernel_shapes_worker.py IN.npz OUT.npz
 
 IN.npz: model, k, Fc, det, lr, the batch (rp, fid, fld, val -- empty = no values --, lab) and states W<i>, V<i>, S<i>
-(S = updater state s1).  For each state: upload it, then a train step (train = 1: loss<i>, cnt<i>, Wout<i>, Vout<i>) or a
-predict (train = 0: pctr<i>, and sumvx<i> for FM).  OUT.npz holds the results."""
+(S = updater state s1); optional opt (updater, default Adagrad), l2 (default 0.001) and mb (minibatch_size, default 0 =
+the rows of the step).  For each state: upload it, then a train step (train = 1: loss<i>, cnt<i>, Wout<i>, Vout<i> and the
+step's pCTR pred<i>) or a predict (train = 0: pctr<i>, and sumvx<i> for FM).  OUT.npz holds the results."""
 import os
 import sys
 
@@ -52,7 +53,10 @@ def run(inp):
     rp, fid, fld, lab = inp["rp"], inp["fid"], inp["fld"], inp["lab"]
     val = inp["val"] if len(inp["val"]) else None
     F = len(inp["W0"])
-    ctx = capi.Context(model, F, k, Fc, deterministic=det, lr=float(inp["lr"]))
+    opt = int(inp["opt"]) if "opt" in inp else capi.OPT_ADAGRAD
+    l2 = float(inp["l2"]) if "l2" in inp else 0.001
+    mb = int(inp["mb"]) if "mb" in inp else 0
+    ctx = capi.Context(model, F, k, Fc, deterministic=det, lr=float(inp["lr"]), optimizer=opt, l2=l2, minibatch_size=mb)
     ctx.upload_batch(0, rp, fid, fld if Fc else None, val, lab)
     out = {}
     i = 0
@@ -63,6 +67,7 @@ def run(inp):
         if int(inp["train"]):
             out[f"loss{i}"], out[f"cnt{i}"] = ctx.train_step(0)
             out[f"Wout{i}"], out[f"Vout{i}"] = ctx.download_params()
+            out[f"pred{i}"] = ctx.download_pred(0)
         else:
             out[f"pctr{i}"] = ctx.predict(0)
             if model == capi.MODEL_FM:

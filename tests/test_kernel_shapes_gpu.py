@@ -149,33 +149,6 @@ def test_dense_path_fm_step_vs_oracle(oracle_api, k, opt):
     ctx.close()
 
 
-@pytest.mark.parametrize("k", [pytest.param(k, id=f"fm_backward_kernel-LPR{l}-K{k}") for k, l in DENSE_FM])
-def test_dense_path_fm_gradient_vs_ref64(k):
-    """OPT_PS_SGD steps w -= g / (B / lr); with lr = B the divisor is exactly 1, so g = w0 - w1 up to the rounding of w1.
-    The recovered gradient must match ref64's float64 gradient (evaluated at the kernel's own pCTR, which
-    test_inorder_forward_vs_ref64 bounds) within 1e-5 * cond + one fp32 spacing of w1."""
-    from lightctr_b200 import capi
-    seed = 200 + k
-    rp, fid, fld, val, lab = make_batch(seed, F, with_val=True)
-    W0, V0 = make_params(seed, F, k)
-    B = len(lab)
-    ctx = capi.Context(capi.MODEL_FM, F, k, optimizer=capi.OPT_PS_SGD, deterministic=0, lr=float(B))
-    ctx.upload_params(W0, V0)
-    ctx.upload_batch(0, rp, fid, None, val, lab)
-    ctx.train_step(0)
-    W1, V1 = ctx.download_params()
-    pred = ctx.download_pred(0)
-    ctx.close()
-    s64, _z, p64, _sc, z_c = ref64.fm_forward(rp, fid, val, W0, V0, k)
-    _check_pctr(pred, p64, z_c)
-    gW, gV, gW_c, gV_c = ref64.fm_grad(rp, fid, val, lab, W0, V0, k, pred, s64, 0.001)
-    for w0, w1, g, c in ((W0, W1, gW, gW_c), (V0, V1, gV.ravel(), gV_c.ravel())):
-        got = w0.astype(np.float64) - w1.astype(np.float64)
-        ok, ex, at = _within(got, g, c, atol=np.spacing(np.abs(w1)).astype(np.float64))
-        assert ok, (ex, at, got[at], g[at])
-    assert np.count_nonzero(W1 != W0) == len(np.unique(fid))  # every batch feature moved, no other
-
-
 @pytest.mark.parametrize("k", [pytest.param(k, id=f"fm_backward_kernel-NFM-LPR{l}-K{k}") for k, l in DENSE_FM if k in (6, 12, 24)])
 def test_dense_path_nfm_step_vs_oracle(oracle_api, k):
     _nfm_step_vs_oracle(oracle_api, k, det=0, seed=300 + k)

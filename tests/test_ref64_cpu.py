@@ -137,3 +137,110 @@ def test_ffm_gradient_skips_rows_whose_prediction_equals_the_label():
     rp2 = np.concatenate([[0], np.cumsum(lens)])
     want = ref64.ffm_grad(rp2, fid[sel], fld[sel], val[sel], lab[keep], W, V, Fc, k, p[keep], 0.001)
     assert np.array_equal(got[0], want[0]) and np.array_equal(got[1], want[1])
+
+
+def _adagrad_recovered(w0, w1, accum, B):
+    """the gradient behind one oracle Adagrad step from a zero state: |g| = sqrt(accum) * B (accum = (g / B)^2), the sign
+    from the step; returns (g, sign_known)"""
+    mag = np.sqrt(accum.astype(np.float64)) * B
+    step = w0.astype(np.float64) - w1.astype(np.float64)
+    return np.sign(step) * mag, step != 0
+
+
+@pytest.mark.parametrize("act,hidden", [(0, [8]), (1, [8]), (0, [7, 5])], ids=["sigmoid-H8", "tanh-H8", "sigmoid-H7-5"])
+def test_nfm_head_and_gradient_match_the_oracle(oracle_api, act, hidden):
+    """One minibatch of NFMOracle from a zero Adagrad state (masks all 1, biases != 0): the loss from nfm_head's pCTR, and
+    the gradient recovered from the step (|g| from the accumulator, the sign from the step) against nfm_head + nfm_grad,
+    within 1e-5 of their condition figures (the oracle's own fp32 dz folded into gV's)."""
+    rng = np.random.default_rng(20 + act + len(hidden))
+    F, rows, k = 300, 40, 6
+    rp, fid, fld, val, lab = _batch(rng, F, rows)
+    W = (rng.standard_normal(F) * 0.05).astype(np.float32)
+    V = (rng.standard_normal(F * k) * 0.3).astype(np.float32)
+    ds = oracle_api.Dataset(rp, fid, fld, val, lab, F, 0)
+    o = oracle_api.NFMOracle(ds, k, hidden, W=W, V=V, batch_size=rows, minibatch=rows, lr=1.0, act=act)
+    layers = []
+    for l in range(len(hidden) + 1):
+        o.mlp.arrays("mask", l)[:] = 1.0
+        o.mlp.arrays("bias", l)[:] = (rng.standard_normal(len(o.mlp.arrays("bias", l))) * 0.1).astype(np.float32)
+        layers.append((o.mlp.arrays("weight", l).copy(), o.mlp.arrays("bias", l).copy()))
+    loss, _ = o.epoch()
+    z, wide, s64, z_c, w_c = ref64.nfm_forward(rp, fid, val, W, V, k)
+    p, dz, dz_c, _lc = ref64.nfm_head(z, wide, layers, act, None, lab, z_c, w_c)
+    loss64 = float(np.sum(np.where(lab == 1, -np.log(p), -np.log(1 - p))))
+    assert abs(loss - loss64) <= 1e-5 * loss64, (loss, loss64)
+    gW, gV, gW_c, gV_c = ref64.nfm_grad(rp, fid, val, lab, W, V, k, p, s64, dz, float(o.l2), dz_cond=dz_c)
+    for w0, w1, acc, g, c in ((W, o.W, o.accum[:F], gW, gW_c), (V, o.V, o.accum[F:], gV.ravel(), gV_c.ravel())):
+        got, known = _adagrad_recovered(w0, w1, acc, rows)
+        err = np.where(known, np.abs(got - g), np.minimum(np.abs(got - g), np.abs(-got - g)))
+        bound = 1e-5 * c + 1e-7
+        assert np.all(err <= bound), float(np.max(err - bound))
+    assert np.count_nonzero(gV) > F  # the batch touches most features
+
+
+def _hot_fm_problem(rows=2000, F=500, k=8, seed=31):
+    """every row holds id 0; returns the batch, parameters, the float64 forward and gradient"""
+    rng = np.random.default_rng(seed)
+    lens = rng.integers(2, 20, rows)
+    fid = np.concatenate([np.concatenate([[0], rng.choice(np.arange(1, F), n - 1, replace=False)]) for n in lens])
+    rp = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    val = (0.25 + 1.5 * rng.random(len(fid))).astype(np.float32)
+    lab = (rng.random(rows) < 0.4).astype(np.int32)
+    W = (rng.standard_normal(F) * 0.05).astype(np.float32)
+    V = (rng.standard_normal(F * k) * 0.1 / np.sqrt(k)).astype(np.float32)
+    return rp, fid.astype(np.uint32), val, lab, W, V
+
+
+def test_probe_bound_sees_a_dropped_or_doubled_share():
+    """The bound of the gradient probe (ref64.probe_excess) on the feature with the most rows: leaving out its largest
+    single-row term, or counting one of 32 replica shares twice, leaves the bound on every coordinate; so does an NFM dz
+    read from the neighbouring sample, and an FFM l2 count c_ib one too high at l2 = 5e-2 (on every touched row, and on
+    all but the factors whose V is near 0)."""
+    k, l2 = 8, 0.001
+    rp, fid, val, lab, W, V = _hot_fm_problem(k=k)
+    rows = len(lab)
+    s, _z, p, _sc, _zc = ref64.fm_forward(rp, fid, val, W, V, k)
+    gW, gV, gW_c, gV_c = ref64.fm_grad(rp, fid, val, lab, W, V, k, p, s, l2)
+    at = np.flatnonzero(fid == 0)
+    r = np.repeat(np.arange(rows), np.diff(rp))[at]
+    x = val[at].astype(np.float64)
+    gw_r = (p[r] - lab[r]) * x + l2 * W[0]
+    gv_r = (s[r] - x[:, None] * V[:k].astype(np.float64)) * gw_r[:, None] + l2 * V[:k]
+    terms = np.concatenate([gw_r[:, None], gv_r], 1)                      # [rows of id 0, 1 + k]
+    g = np.concatenate([[gW[0]], gV[0]])
+    cond = np.concatenate([[gW_c[0]], gV_c[0]])
+    w1 = (np.concatenate([[W[0]], V[:k]]).astype(np.float64) - g).astype(np.float32)
+    dropped = g - terms[np.argmax(np.abs(terms), 0), np.arange(k + 1)]
+    assert np.all(ref64.probe_excess(dropped, g, cond, w1) > 0)
+    doubled = g + terms[r % 32 == 5].sum(0)
+    assert np.all(ref64.probe_excess(doubled, g, cond, w1) > 0)
+    # NFM: dz of the neighbouring sample
+    rng = np.random.default_rng(3)
+    layers = [(rng.random((16, k)) - 0.5, np.zeros(16)), (rng.random((1, 16)) - 0.5, np.zeros(1))]
+    z, wide, s64, z_c, w_c = ref64.nfm_forward(rp, fid, val, W, V, k)
+    pn, dz, dz_c, _ = ref64.nfm_head(z, wide, layers, 0, None, lab, z_c, w_c)
+    _, gVn, _, gVn_c = ref64.nfm_grad(rp, fid, val, lab, W, V, k, pn, s64, dz, l2, dz_cond=dz_c)
+    _, gVs, _, _ = ref64.nfm_grad(rp, fid, val, lab, W, V, k, pn, s64, np.roll(dz, 1, 0), l2)
+    w1n = (V[:k].astype(np.float64) - gVn[0]).astype(np.float32)
+    assert np.all(ref64.probe_excess(gVs[0], gVn[0], gVn_c[0], w1n) > 0)
+    # FFM: c_ib = cnt[b] instead of cnt[b] - 1 for the entry's own field b = a_i
+    Fc, kf, l2f = 6, 4, 5e-2
+    rp2, fid2, fld2, val2, lab2 = _batch(np.random.default_rng(9), 200, 30, Fc)
+    Wf = (rng.standard_normal(200) * 0.05).astype(np.float32)
+    Vf = (rng.standard_normal(200 * Fc * kf) * 0.1).astype(np.float32)
+    _z, pf, _c = ref64.ffm_forward(rp2, fid2, fld2, val2, Wf, Vf, Fc, kf)
+    _, gVf, _, gVf_c = ref64.ffm_grad(rp2, fid2, fld2, val2, lab2, Wf, Vf, Fc, kf, pf, l2f)
+    V3 = Vf.reshape(-1, Fc, kf).astype(np.float64)
+    bad = gVf.copy()
+    hit = np.zeros(gVf.shape[:2], bool)
+    for row in range(len(lab2)):
+        f, a = fid2[rp2[row]:rp2[row + 1]].astype(np.int64), fld2[rp2[row]:rp2[row + 1]].astype(np.int64)
+        cnt = np.bincount(a, minlength=Fc)
+        for fi, ai in zip(f, a):
+            if cnt[ai] > 1:
+                bad[fi, ai] += l2f * V3[fi, ai]
+                hit[fi, ai] = True
+    w1f = (V3 - gVf).astype(np.float32)
+    assert hit.sum() > 10
+    out = ref64.probe_excess(bad, gVf, gVf_c, w1f)[hit]
+    assert np.mean(out > 0) > 0.95 and np.all(out.max(1) > 0)  # only factors with V ~ 0 may stay inside
