@@ -22,24 +22,19 @@ void set_error(const char* fmt, ...) {
 static int slot_reserve(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz) {
     const size_t k = c->cfg.factor_cnt;
     if (rows > s.cap_rows) {
-        int64_t cap = std::max<int64_t>(rows, s.cap_rows + s.cap_rows / 2);
-        dfree(s.row_ptr); dfree(s.label); dfree(s.pred); dfree(s.sumvx); dfree(s.wide);
-        if (dalloc(&s.row_ptr, (size_t)cap + 1)) return 1;
-        if (dalloc(&s.label, (size_t)cap)) return 1;
-        if (dalloc(&s.pred, (size_t)cap)) return 1;
-        if (dalloc(&s.wide, (size_t)cap)) return 1;
-        if (c->cfg.model != LCTR_MODEL_FFM) {
-            if (dalloc(&s.sumvx, (size_t)cap * k)) return 1;
-            LCTR_CUDA(cudaMemsetAsync(s.sumvx, 0, (size_t)cap * k * sizeof(float), c->stream));
-        }
+        const int64_t cap = std::max<int64_t>(rows, s.cap_rows + s.cap_rows / 2);
+        const size_t n = (size_t)cap, nk = c->cfg.model != LCTR_MODEL_FFM ? n * k : 0;
+        s.rows = 0; s.cap_rows = 0;
+        if (alloc_group(sized(s.row_ptr, n + 1), sized(s.label, n), sized(s.pred, n), sized(s.wide, n), sized(s.sumvx, nk)))
+            return 1;
+        if (nk) LCTR_CUDA(cudaMemsetAsync(s.sumvx, 0, nk * sizeof(float), c->stream));
         s.cap_rows = cap;
     }
     if (nnz > s.cap_nnz) {
-        int64_t cap = std::max<int64_t>(nnz, s.cap_nnz + s.cap_nnz / 2);
-        dfree(s.fid); dfree(s.field); dfree(s.val);
-        if (dalloc(&s.fid, (size_t)cap + 32)) return 1;
-        if (dalloc(&s.field, (size_t)cap + 32)) return 1;
-        if (dalloc(&s.val, (size_t)cap + 32)) return 1;
+        const int64_t cap = std::max<int64_t>(nnz, s.cap_nnz + s.cap_nnz / 2);
+        const size_t n = (size_t)cap + 32;
+        s.nnz = 0; s.cap_nnz = 0;
+        if (alloc_group(sized(s.fid, n), sized(s.field, n), sized(s.val, n))) return 1;
         s.cap_nnz = cap;
     }
     return 0;
@@ -137,18 +132,18 @@ static int build_csc(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz, const int6
     seg_ptr.push_back(out);
     const int64_t nseg = (int64_t)seg_fid.size();
     if (nseg > s.cap_segs) {
-        dfree(s.seg_ptr); dfree(s.seg_fid);
-        if (dalloc(&s.seg_ptr, (size_t)nseg + 1) || dalloc(&s.seg_fid, (size_t)nseg + 1)) return 1;
+        s.cap_segs = 0;
+        if (alloc_group(sized(s.seg_ptr, (size_t)nseg + 1), sized(s.seg_fid, (size_t)nseg + 1))) return 1;
         s.cap_segs = nseg;
     }
     if (nblocks > s.cap_blocks) {
-        dfree(s.blk_seg_ptr);
-        if (dalloc(&s.blk_seg_ptr, (size_t)nblocks + 1)) return 1;
+        s.cap_blocks = 0;
+        if (alloc_group(sized(s.blk_seg_ptr, (size_t)nblocks + 1))) return 1;
         s.cap_blocks = nblocks;
     }
     if (nnz > s.cap_ent) {
-        dfree(s.ent_row); dfree(s.ent_x);
-        if (dalloc(&s.ent_row, (size_t)nnz + 32) || dalloc(&s.ent_x, (size_t)nnz + 32)) return 1;
+        s.cap_ent = 0;
+        if (alloc_group(sized(s.ent_row, (size_t)nnz + 32), sized(s.ent_x, (size_t)nnz + 32))) return 1;
         s.cap_ent = nnz;
     }
     LCTR_CUDA(cudaMemcpyAsync(s.seg_ptr, seg_ptr.data(), (size_t)(nseg + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
@@ -159,8 +154,7 @@ static int build_csc(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz, const int6
         if (val) LCTR_CUDA(cudaMemcpyAsync(s.ent_x, ent_x.data(), (size_t)nnz * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     }
     LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the staging vectors die with this frame
-    if (!s.h_blk_seg_ptr) s.h_blk_seg_ptr = new std::vector<int64_t>();
-    *s.h_blk_seg_ptr = blk_seg_ptr;
+    s.h_blk_seg_ptr = blk_seg_ptr;
     s.csc_block = block; s.n_blocks = nblocks; s.n_segs = nseg;
     return 0;
 }
@@ -225,7 +219,8 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
     }
     LCTR_CHECK(cfg->device >= 0 && cfg->device < ndev, "lctr_create: device %d of %d", cfg->device, ndev);
     LCTR_CUDA(cudaSetDevice(cfg->device));
-    lctr_ctx* c = new lctr_ctx();
+    std::unique_ptr<lctr_ctx, decltype(&lctr_destroy)> own(new lctr_ctx(), lctr_destroy);  // released by every failure below
+    lctr_ctx* c = own.get();
     c->cfg = *cfg;
     if (c->cfg.ftrl_alpha == 0.f) {  // gradientUpdater.h:275
         c->cfg.ftrl_alpha = 0.15f; c->cfg.ftrl_lambda1 = 1.0f; c->cfg.ftrl_beta = 1.0f; c->cfg.ftrl_lambda2 = 1.0f;
@@ -247,23 +242,14 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
     const size_t nv = FL * c->rowlen;
     const bool two = cfg->optimizer == LCTR_OPT_FTRL || cfg->optimizer == LCTR_OPT_ADAM || cfg->optimizer == LCTR_OPT_ADADELTA ||
                      cfg->optimizer == LCTR_OPT_PS_DCASGD || cfg->optimizer == LCTR_OPT_PS_DCASGDA;
-    int rc = 0;
-    rc |= dalloc(&c->W, FL); rc |= dalloc(&c->V, nv);
-    if (update_g) { rc |= dalloc(&c->gW, FL); rc |= dalloc(&c->gV, nv); }
-    rc |= dalloc(&c->s1W, FL); rc |= dalloc(&c->s1V, nv);
-    if (two) { rc |= dalloc(&c->s2W, FL); rc |= dalloc(&c->s2V, nv); }
-    if (dense) {  // the sparse apply of opt.cu: touched map, its compacted list and counters
-        rc |= dalloc(&c->touched, FL + 512);
-        rc |= dalloc(&c->touch_list, FL + 32);
-        rc |= dalloc(&c->n_touch, 1);
-        rc |= dalloc(&c->apply_done, 1);
-    }
-    rc |= dalloc(&c->stats, (size_t)2 * kStatRing);
-    rc |= dalloc(&c->stat_partial, 2);
-    rc |= dalloc(&c->stat_done, 1);
-    if (rc) { lctr_destroy(c); return 1; }
-    LCTR_CUDA(cudaMallocHost((void**)&c->h_stats, 2 * sizeof(double)));
-    if (reset_table_rows(c)) { lctr_destroy(c); return 1; }
+    if (c->W.alloc(FL) || c->V.alloc(nv) || (update_g && (c->gW.alloc(FL) || c->gV.alloc(nv))) || c->s1W.alloc(FL) ||
+        c->s1V.alloc(nv) || (two && (c->s2W.alloc(FL) || c->s2V.alloc(nv))))
+        return 1;
+    // the sparse apply of opt.cu: touched map, its compacted list and counters
+    if (dense && (c->touched.alloc(FL + 512) || c->touch_list.alloc(FL + 32) || c->n_touch.alloc(1) || c->apply_done.alloc(1)))
+        return 1;
+    if (c->stats.alloc((size_t)2 * kStatRing) || c->stat_partial.alloc(2) || c->stat_done.alloc(1) || c->h_stats.alloc(2)) return 1;
+    if (reset_table_rows(c)) return 1;
     if (update_g) {
         LCTR_CUDA(cudaMemsetAsync(c->gW, 0, FL * sizeof(float), c->stream));
         LCTR_CUDA(cudaMemsetAsync(c->gV, 0, nv * sizeof(float), c->stream));
@@ -274,7 +260,7 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
         LCTR_CUDA(cudaMemsetAsync(c->apply_done, 0, sizeof(unsigned int), c->stream));
     }
     if (c->cfg.world > 1) {
-        if (dist_alloc(c)) { lctr_destroy(c); return 1; }
+        if (dist_alloc(c)) return 1;
     } else {
         c->cW = c->W; c->cV = c->V; c->cgW = c->gW; c->cgV = c->gV;
     }
@@ -282,12 +268,12 @@ int lctr_create(const lctr_cfg* cfg, lctr_ctx** out) {
     LCTR_CUDA(cudaMemsetAsync(c->stat_partial, 0, sizeof(double) * 2, c->stream));
     LCTR_CUDA(cudaMemsetAsync(c->stat_done, 0, sizeof(unsigned int), c->stream));
     if (cfg->model == LCTR_MODEL_NFM || cfg->model == LCTR_MODEL_WND) {
-        if (mlp_alloc(c)) { lctr_destroy(c); return 1; }
+        if (mlp_alloc(c)) return 1;
     }
-    if (cfg->key_mode == LCTR_KEYS_HASHED && keys_alloc(c)) { lctr_destroy(c); return 1; }
+    if (cfg->key_mode == LCTR_KEYS_HASHED && keys_alloc(c)) return 1;
     { const char* e = getenv("LCTR_CSC_IN_STEP"); c->csc_in_step = e && e[0] == '1'; }
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    *out = c;
+    *out = own.release();
     return 0;
 }
 
@@ -295,33 +281,12 @@ int lctr_destroy(lctr_ctx* c) {
     if (!c) return 0;
     cudaSetDevice(c->cfg.device);
     if (c->stream) cudaStreamSynchronize(c->stream);
-    dfree(c->W); dfree(c->V); dfree(c->gW); dfree(c->gV); dfree(c->s1W); dfree(c->s1V); dfree(c->s2W); dfree(c->s2V);
-    dfree(c->touched); dfree(c->touch_list); dfree(c->n_touch); dfree(c->apply_done); dfree(c->stats); dfree(c->stat_partial); dfree(c->stat_done);
-    for (auto& s : c->slots) {
-        dfree(s.row_ptr); dfree(s.fid); dfree(s.field); dfree(s.val); dfree(s.label); dfree(s.pred); dfree(s.sumvx);
-        dfree(s.wide);
-        dfree(s.blk_seg_ptr); dfree(s.seg_ptr); dfree(s.seg_fid); dfree(s.ent_row); dfree(s.ent_x); dfree(s.ent_field);
-        dfree(s.ent_slot); dfree(s.ent_pslot); dfree(s.hot_of); dfree(s.hot_slot); dfree(s.n_hot);
-        dfree(s.uniq); dfree(s.n_uniq); dfree(s.short_list); dfree(s.long_list); dfree(s.csc_totals); dfree(s.csc_acc); dfree(s.csc_arrived);
-        delete s.h_blk_seg_ptr; s.h_blk_seg_ptr = nullptr;
-    }
-    mlp_free(c);
-    ffm_grouped_free(c);
-    metrics_free(c);
-    wnd_free(c);
-    dist_free(c);
-    fused_free(c);
-    csc_scratch_free(c);
-    keys_free(c);
-    if (c->h_stats) cudaFreeHost(c->h_stats);
-    if (c->h_stat_ring) cudaFreeHost(c->h_stat_ring);
-    for (int p = 0; p < kPipe; p++) {
-        PipeGraph& g = c->pipe_graph[p];
+    if (c->copy_stream) cudaStreamSynchronize(c->copy_stream);
+    if (c->build_stream) cudaStreamSynchronize(c->build_stream);
+    if (c->dist) dist_close_peers(c);
+    for (PipeGraph& g : c->pipe_graph) {
         if (g.build) cudaGraphExecDestroy(g.build);
         if (g.step) cudaGraphExecDestroy(g.step);
-        if (g.d_hdr) cudaFree(g.d_hdr); if (g.h_hdr) cudaFreeHost(g.h_hdr);
-        if (g.d_opt) cudaFree(g.d_opt); if (g.h_opt) cudaFreeHost(g.h_opt);
-        if (g.d_stat) cudaFree(g.d_stat); if (g.h_stat) cudaFreeHost(g.h_stat);
     }
     if (c->copy_stream) {
         for (int i = 0; i < kPipe; i++) { cudaEventDestroy(c->ev_copied[i]); cudaEventDestroy(c->ev_computed[i]); cudaEventDestroy(c->ev_h2d[i]); }
@@ -330,7 +295,7 @@ int lctr_destroy(lctr_ctx* c) {
         cudaStreamDestroy(c->copy_stream);
     }
     if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
+    delete c;  // its buffers release themselves
     return 0;
 }
 
@@ -493,7 +458,7 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
         s.nnz = nnz;
     }
     const bool grouped = c->cfg.deterministic == 2 && rows > 0 && nnz > 0 && c->cfg.world == 1;
-    int32_t* tmp = reinterpret_cast<int32_t*>(s.pred);  // pred is overwritten by the next forward anyway
+    int32_t* tmp = reinterpret_cast<int32_t*>(s.pred.get());  // pred is overwritten by the next forward anyway
     if (rows) {
         // labels travel as int32 and are widened on device (the reference compares a `float target`)
         LCTR_CUDA(cudaMemcpyAsync(tmp, label, (size_t)rows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
@@ -732,8 +697,7 @@ static int pipe_init(lctr_ctx* c) {
         LCTR_CUDA(cudaEventCreateWithFlags(&c->ev_h2d[i], cudaEventDisableTiming));
     }
     for (int i = 0; i < kStatRing; i++) LCTR_CUDA(cudaEventCreateWithFlags(&c->ev_stat[i], cudaEventDisableTiming));
-    LCTR_CUDA(cudaMallocHost((void**)&c->h_stat_ring, sizeof(double) * 2 * kStatRing));
-    return 0;
+    return c->h_stat_ring.alloc(2 * kStatRing);
 }
 
 // Graph path of the streamed pipeline (FM, cfg.deterministic == 2, one GPU): per pipeline slot two captured graphs --
@@ -761,20 +725,13 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
     Slot& s = c->slots[kNumSlots - kPipe + p];
     if (g.build) { cudaGraphExecDestroy(g.build); g.build = nullptr; }
     if (g.step) { cudaGraphExecDestroy(g.step); g.step = nullptr; }
-    if (!g.d_hdr) {
-        LCTR_CUDA(cudaMalloc((void**)&g.d_hdr, 2 * sizeof(int64_t)));
-        LCTR_CUDA(cudaMallocHost((void**)&g.h_hdr, 2 * sizeof(int64_t)));
-        LCTR_CUDA(cudaMalloc((void**)&g.d_opt, csc_opt_params_size()));
-        LCTR_CUDA(cudaMallocHost((void**)&g.h_opt, csc_opt_params_size()));
-        LCTR_CUDA(cudaMalloc((void**)&g.d_stat, 2 * sizeof(double)));
-        LCTR_CUDA(cudaMallocHost((void**)&g.h_stat, 2 * sizeof(double)));
-    }
+    if (!g.h_stat && (g.d_hdr.alloc(2) || g.h_hdr.alloc(2) || g.d_opt.alloc(1) || g.h_opt.alloc(1) || g.d_stat.alloc(2) ||
+                      g.h_stat.alloc(2)))
+        return 1;
     s.has_val = has_val;
-    {   // the launchers pick their updater instance from the host copy at capture time: give it the context's updater
-        OptParams* hp = reinterpret_cast<OptParams*>(g.h_opt);
-        memset(hp, 0, csc_opt_params_size());
-        hp->opt = c->cfg.optimizer;
-    }
+    // the launchers pick their updater instance from the host copy at capture time: give it the context's updater
+    memset(g.h_opt, 0, sizeof(OptParams));
+    g.h_opt[0].opt = c->cfg.optimizer;
     cudaGraph_t graph;
     const bool fused = c->grad_path == GRAD_COMPACT;  // else device grouping (GRAD_FEATURE_MAJOR)
     // ---- build graph (copy stream)
@@ -783,10 +740,10 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
     if (!rc) {
         if (fused) {  // labels widened, then the slot map of the batch (fm_fused.cu)
             rc = launch(c, {(unsigned)((s.cap_rows + 255) / 256), 256, 0, c->copy_stream}, label_to_float_kernel,
-                        reinterpret_cast<int32_t*>(s.pred), s.label, s.cap_rows, g.d_hdr) ||
+                        reinterpret_cast<int32_t*>(s.pred.get()), s.label, s.cap_rows, g.d_hdr) ||
                  fused_build_slot(c, s, c->copy_stream, g.d_hdr, s.cap_rows, s.cap_nnz);
         } else {
-            rc = csc_build_device(c, s, c->copy_stream, reinterpret_cast<int32_t*>(s.pred), g.d_hdr, s.cap_rows, s.cap_nnz);
+            rc = csc_build_device(c, s, c->copy_stream, reinterpret_cast<int32_t*>(s.pred.get()), g.d_hdr, s.cap_rows, s.cap_nnz);
         }
     }
     cudaError_t ce = cudaStreamEndCapture(c->copy_stream, &graph);  // always closes the capture, also on error paths
@@ -796,15 +753,14 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
     cudaGraphDestroy(graph);
     // ---- step graph (compute stream)
     LCTR_CUDA(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-    rc = cudaMemcpyAsync(g.d_opt, g.h_opt, csc_opt_params_size(), cudaMemcpyHostToDevice, c->stream) != cudaSuccess;
+    rc = cudaMemcpyAsync(g.d_opt, g.h_opt, sizeof(OptParams), cudaMemcpyHostToDevice, c->stream) != cudaSuccess;
     if (!rc) {
         if (fused)
             rc = launch_fm_fused(c, s, 0, s.cap_rows, true, g.d_hdr, g.d_stat) ||
-                 launch_apply_compact(c, s, s.cap_rows, reinterpret_cast<const OptParams*>(g.h_opt),
-                                      reinterpret_cast<const OptParams*>(g.d_opt));
+                 launch_apply_compact(c, s, s.cap_rows, g.h_opt, g.d_opt);
         else
             rc = launch_fm_forward_ex(c, s, 0, s.cap_rows, false, true, g.d_hdr, g.d_stat) ||
-                 launch_fm_backward_devcsc_ex(c, s, 0, s.cap_rows, reinterpret_cast<const OptParams*>(g.h_opt), g.d_opt);
+                 launch_fm_backward_devcsc_ex(c, s, 0, s.cap_rows, g.h_opt, g.d_opt);
     }
     if (!rc) rc = cudaMemcpyAsync(g.h_stat, g.d_stat, 2 * sizeof(double), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess;
     ce = cudaStreamEndCapture(c->stream, &graph);
@@ -1016,23 +972,20 @@ int lctr_dense_grad_buffer(lctr_ctx* c, void** dev_ptr, size_t* n_floats) {
 
 int lctr_profile(lctr_ctx* c, int enable) {
     LCTR_CHECK(c, "null ctx");
-    if (enable && !c->prof_ev) { c->prof_ev = new std::vector<cudaEvent_t>(); c->prof_id = new std::vector<int>(); }
     c->profiling = enable ? 1 : 0;
     return 0;
 }
 int lctr_profile_read(lctr_ctx* c, double* ms, int64_t* counts, int n, int reset) {
     LCTR_CHECK(c && ms && counts, "null argument");
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    if (c->prof_ev) {
-        for (size_t i = 0; i < c->prof_id->size(); i++) {
-            float t = 0.f;
-            cudaEventElapsedTime(&t, (*c->prof_ev)[2 * i], (*c->prof_ev)[2 * i + 1]);
-            const int id = (*c->prof_id)[i];
-            if (id >= 0 && id < kNumProf) { c->prof_ms[id] += t; c->prof_cnt[id]++; }
-            cudaEventDestroy((*c->prof_ev)[2 * i]); cudaEventDestroy((*c->prof_ev)[2 * i + 1]);
-        }
-        c->prof_ev->clear(); c->prof_id->clear();
+    for (size_t i = 0; i < c->prof_id.size(); i++) {
+        float t = 0.f;
+        cudaEventElapsedTime(&t, c->prof_ev[2 * i], c->prof_ev[2 * i + 1]);
+        const int id = c->prof_id[i];
+        if (id >= 0 && id < kNumProf) { c->prof_ms[id] += t; c->prof_cnt[id]++; }
+        cudaEventDestroy(c->prof_ev[2 * i]); cudaEventDestroy(c->prof_ev[2 * i + 1]);
     }
+    c->prof_ev.clear(); c->prof_id.clear();
     for (int i = 0; i < n && i < kNumProf; i++) { ms[i] = c->prof_ms[i]; counts[i] = c->prof_cnt[i]; }
     if (reset) for (int i = 0; i < kNumProf; i++) { c->prof_ms[i] = 0; c->prof_cnt[i] = 0; }
     return 0;

@@ -292,9 +292,8 @@ __global__ void __launch_bounds__(256) reshard_scalars_kernel(const float* __res
 struct Stage {
     size_t rows = 0;
     std::vector<float> h;
-    float* d = nullptr;
-    uint32_t* dmap = nullptr;
-    ~Stage() { cudaFree(d); cudaFree(dmap); }
+    Buf<float> d;
+    Buf<uint32_t> dmap;
 };
 
 // one row section (n source rows of `rowlen` floats) of an open file into dst, chunk by chunk
@@ -304,17 +303,21 @@ static int scatter_section(lctr_ctx* c, Stage& st, FILE* f, float* dst, size_t n
     for (size_t l0 = 0; l0 < n; l0 += st.rows) {
         const size_t m = std::min(st.rows, n - l0);
         LCTR_CHECK(get(f, st.h.data(), m * rowlen * sizeof(float)), "checkpoint: short read");
-        LCTR_CUDA(cudaMemcpyAsync(st.d, st.h.data(), m * rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-        if (map) LCTR_CUDA(cudaMemcpyAsync(st.dmap, map + l0, m * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-        rule.map = map ? st.dmap : nullptr;
-        rule.l0 = l0;
-        const int rc = rowlen == 1
-            ? launch(c, {(unsigned)std::max<size_t>(1, std::min((m + 255) / 256, grid_cap)), 256, 0, c->stream},
-                     reshard_scalars_kernel, st.d, dst, m, rule)
-            : launch(c, {(unsigned)std::max<size_t>(1, std::min((m + 7) / 8, grid_cap)), 256, 0, c->stream},
-                     rowlen % 4 == 0 ? reshard_rows_kernel<true> : reshard_rows_kernel<false>, st.d, dst, m, rowlen, rule);
+        auto chunk = [&]() -> int {
+            LCTR_CUDA(cudaMemcpyAsync(st.d, st.h.data(), m * rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+            if (map) LCTR_CUDA(cudaMemcpyAsync(st.dmap, map + l0, m * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+            rule.map = map ? st.dmap.get() : nullptr;
+            rule.l0 = l0;
+            return rowlen == 1
+                ? launch(c, {(unsigned)std::max<size_t>(1, std::min((m + 255) / 256, grid_cap)), 256, 0, c->stream},
+                         reshard_scalars_kernel, st.d, dst, m, rule)
+                : launch(c, {(unsigned)std::max<size_t>(1, std::min((m + 7) / 8, grid_cap)), 256, 0, c->stream},
+                         rowlen % 4 == 0 ? reshard_rows_kernel<true> : reshard_rows_kernel<false>, st.d, dst, m, rowlen, rule);
+        };
+        const int rc = chunk();
+        // the host chunk is refilled next; after a failure the stage goes with the caller, while queued copies may read it
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
         if (rc) return 1;
-        LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the host chunk is refilled next
     }
     return 0;
 }
@@ -522,8 +525,7 @@ int lctr_load_checkpoint_shards(lctr_ctx* c, int n, const char* const* paths) {
         for (int r = 0; r < n; r++) src_rows = std::max<size_t>(src_rows, by_rank[r]->s.local_rows);
         st.rows = std::max<size_t>(1, std::min<size_t>(src_rows, ((size_t)16 << 20) / c->rowlen));
         st.h.resize(st.rows * c->rowlen);
-        LCTR_CUDA(cudaMalloc((void**)&st.d, st.rows * c->rowlen * sizeof(float)));
-        if (c->keys) LCTR_CUDA(cudaMalloc((void**)&st.dmap, st.rows * sizeof(uint32_t)));
+        if (st.d.alloc(st.rows * c->rowlen) || (c->keys && st.dmap.alloc(st.rows))) return 1;
     }
     const RowSections rs = row_sections(c);
     for (int r = 0; r < n; r++) {

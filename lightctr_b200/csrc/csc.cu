@@ -388,34 +388,26 @@ csc_backward_long_kernel(const uint2* __restrict__ work, const unsigned int* __r
 // host side
 // ------------------------------------------------------------------------------------------------
 struct CscScratch {
-    unsigned int* cnt = nullptr;   // F, all zero between builds
-    unsigned int* off = nullptr;   // F
-    uint2* tile_sum = nullptr;
-    uint2* tile_off = nullptr;
+    Buf<unsigned int> cnt;   // F, all zero between builds
+    Buf<unsigned int> off;   // F
+    Buf<uint2> tile_sum;
+    Buf<uint2> tile_off;
     size_t ntiles = 0;
 };
+void drop(CscScratch* p) { delete p; }
 
 static int scratch_get(lctr_ctx* c, CscScratch** out) {
     if (!c->csc_scratch) {
-        CscScratch* s = new CscScratch();
+        Owned<CscScratch> s(new CscScratch());  // the context's only once complete
         s->ntiles = (c->F + 511) / 512;
-        LCTR_CUDA(cudaMalloc((void**)&s->cnt, (c->F + 512) * sizeof(unsigned int)));
-        LCTR_CUDA(cudaMalloc((void**)&s->off, (c->F + 512) * sizeof(unsigned int)));
-        LCTR_CUDA(cudaMalloc((void**)&s->tile_sum, (s->ntiles + 1) * sizeof(uint2)));
-        LCTR_CUDA(cudaMalloc((void**)&s->tile_off, (s->ntiles + 1) * sizeof(uint2)));
+        if (s->cnt.alloc(c->F + 512) || s->off.alloc(c->F + 512) || s->tile_sum.alloc(s->ntiles + 1) ||
+            s->tile_off.alloc(s->ntiles + 1))
+            return 1;
         LCTR_CUDA(cudaMemset(s->cnt, 0, (c->F + 512) * sizeof(unsigned int)));
-        c->csc_scratch = s;
+        c->csc_scratch = std::move(s);
     }
-    *out = (CscScratch*)c->csc_scratch;
+    *out = c->csc_scratch.get();
     return 0;
-}
-
-void csc_scratch_free(lctr_ctx* c) {
-    CscScratch* s = (CscScratch*)c->csc_scratch;
-    if (!s) return;
-    cudaFree(s->cnt); cudaFree(s->off); cudaFree(s->tile_sum); cudaFree(s->tile_off);
-    delete s;
-    c->csc_scratch = nullptr;
 }
 
 // (re)allocate the per-slot arrays of the view for up to `max_nnz` entries
@@ -426,36 +418,30 @@ int csc_reserve(lctr_ctx* c, Slot& s, int64_t max_nnz) {
     if (max_segs > s.cap_segs || !s.short_list) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
         const int64_t cap = std::max<int64_t>(max_segs, s.cap_segs + s.cap_segs / 2);
-        if (s.seg_ptr) cudaFree(s.seg_ptr); if (s.seg_fid) cudaFree(s.seg_fid);
-        if (s.short_list) cudaFree(s.short_list); if (s.long_list) cudaFree(s.long_list);
-        LCTR_CUDA(cudaMalloc((void**)&s.seg_ptr, (size_t)(cap + 1) * sizeof(int64_t)));
-        LCTR_CUDA(cudaMalloc((void**)&s.seg_fid, (size_t)(cap + 1) * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&s.short_list, (size_t)(cap + 1) * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&s.long_list, (size_t)(max_nnz / 8 + cap + 1) * sizeof(uint2)));
-        if (s.csc_acc) cudaFree(s.csc_acc); if (s.csc_arrived) cudaFree(s.csc_arrived);
+        const size_t n = (size_t)(cap + 1);
         // FM: per-segment double accumulators; FFM meets in update_g instead (ffm_grouped.cu)
-        const size_t na = c->cfg.model == LCTR_MODEL_FFM ? 8 : (size_t)(cap + 1) * (c->cfg.factor_cnt + 1);
-        LCTR_CUDA(cudaMalloc((void**)&s.csc_acc, na * sizeof(double)));
-        LCTR_CUDA(cudaMalloc((void**)&s.csc_arrived, (size_t)(cap + 1) * sizeof(unsigned int)));
+        const size_t na = c->cfg.model == LCTR_MODEL_FFM ? 8 : n * (c->cfg.factor_cnt + 1);
+        s.cap_segs = 0; s.cap_long = 0;
+        if (alloc_group(sized(s.seg_ptr, n), sized(s.seg_fid, n), sized(s.short_list, n), sized(s.long_list, (size_t)max_nnz / 8 + n),
+                        sized(s.csc_acc, na), sized(s.csc_arrived, n)) ||
+            (!s.csc_totals && s.csc_totals.alloc(4)))
+            return 1;
         LCTR_CUDA(cudaMemset(s.csc_acc, 0, na * sizeof(double)));
-        LCTR_CUDA(cudaMemset(s.csc_arrived, 0, (size_t)(cap + 1) * sizeof(unsigned int)));
-        if (!s.csc_totals) LCTR_CUDA(cudaMalloc((void**)&s.csc_totals, 4 * sizeof(unsigned int)));
+        LCTR_CUDA(cudaMemset(s.csc_arrived, 0, n * sizeof(unsigned int)));
         s.cap_segs = cap;
         s.cap_long = max_nnz;
     } else if (max_nnz > s.cap_long) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        if (s.long_list) cudaFree(s.long_list);
-        LCTR_CUDA(cudaMalloc((void**)&s.long_list, (size_t)(max_nnz / 8 + s.cap_segs + 1) * sizeof(uint2)));
+        s.cap_long = 0;
+        if (alloc_group(sized(s.long_list, (size_t)(max_nnz / 8 + s.cap_segs + 1)))) return 1;
         s.cap_long = max_nnz;
     }
     if (max_nnz > s.cap_ent) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        if (s.ent_row) cudaFree(s.ent_row); if (s.ent_x) cudaFree(s.ent_x); if (s.ent_field) cudaFree(s.ent_field);
-        s.ent_field = nullptr;
         const int64_t cap = std::max<int64_t>(max_nnz, s.cap_ent + s.cap_ent / 2);
-        LCTR_CUDA(cudaMalloc((void**)&s.ent_row, (size_t)(cap + 32) * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&s.ent_x, (size_t)(cap + 32) * sizeof(float)));
-        if (c->cfg.model == LCTR_MODEL_FFM) LCTR_CUDA(cudaMalloc((void**)&s.ent_field, (size_t)(cap + 32) * sizeof(uint16_t)));
+        const size_t n = (size_t)(cap + 32);
+        s.cap_ent = 0;
+        if (alloc_group(sized(s.ent_row, n), sized(s.ent_x, n), sized(s.ent_field, c->cfg.model == LCTR_MODEL_FFM ? n : 0))) return 1;
         s.cap_ent = cap;
     }
     return 0;
@@ -479,9 +465,9 @@ int csc_build_device(lctr_ctx* c, Slot& s, cudaStream_t st, const int32_t* label
         launch(c, {std::max(gt, 1u), 256, 0, st}, csc_tile_reduce_kernel, sc->cnt, c->F, sc->tile_sum) ||
         launch(c, {1, 1024, 0, st}, csc_tile_scan_kernel, sc->tile_sum, sc->ntiles, sc->tile_off, s.csc_totals, s.seg_ptr) ||
         launch(c, {std::max(gt, 1u), 256, 0, st}, csc_tile_write_kernel, sc->cnt, c->F, sc->tile_off, sc->off, s.seg_fid, s.seg_ptr,
-               s.short_list, reinterpret_cast<uint2*>(s.long_list), s.csc_totals) ||
-        launch(c, {std::max(gf, 1u), 256, 0, st}, csc_fill_kernel, s.row_ptr, s.fid, s.has_val ? s.val : nullptr, s.rows, sc->off,
-               sc->cnt, s.ent_row, s.ent_x, hdr, s.has_field ? s.field : nullptr, s.ent_field))
+               s.short_list, s.long_list, s.csc_totals) ||
+        launch(c, {std::max(gf, 1u), 256, 0, st}, csc_fill_kernel, s.row_ptr, s.fid, s.has_val ? s.val.get() : nullptr, s.rows, sc->off,
+               sc->cnt, s.ent_row, s.ent_x, hdr, s.has_field ? s.field.get() : nullptr, s.ent_field))
         return 1;
     s.dev_csc = true;
     s.csc_block = 0;
@@ -493,7 +479,7 @@ static int bwd_go(lctr_ctx* c, Slot& s, const OptParams& P, const OptParams* dP)
     const unsigned grid = (unsigned)c->sm_count * 4;
     const CscView C{s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, s.label, s.pred, s.sumvx};
     const ParamView T{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V};
-    const uint2* longs = reinterpret_cast<const uint2*>(s.long_list);
+    const uint2* longs = s.long_list;
     return launch(c, {grid, 256, 0, c->stream}, s.has_val ? csc_backward_long_kernel<K, true> : csc_backward_long_kernel<K, false>,
                   longs, s.csc_totals, C, T, s.csc_acc, s.csc_arrived, c->cfg.l2_reg, P, dP) ||
            launch(c, {grid, 256, 0, c->stream}, s.has_val ? csc_backward_short_kernel<K, true> : csc_backward_short_kernel<K, false>,
@@ -530,7 +516,6 @@ void csc_opt_params(lctr_ctx* c, int64_t rows, void* out) {
     const OptParams P = make_opt_params(c, rows);
     memcpy(out, &P, sizeof(P));
 }
-size_t csc_opt_params_size() { return sizeof(OptParams); }
 
 bool csc_device_supported(const lctr_ctx* c) {
     const int k = (int)c->cfg.factor_cnt;

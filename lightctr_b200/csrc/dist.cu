@@ -87,27 +87,27 @@ constexpr long long kXlateWaitCycles = 1ll << 33;
 
 struct DistState {
     int rank = 0, world = 1, shift = 0;
-    unsigned char* arena = nullptr;
+    Buf<unsigned char> arena;
     ArenaLayout A;
     PeerTable peers;
     size_t cap_keys = 0, cap_pair = 0;
     int recw = 0;                     // floats per gradient-inbox record: rowlen + 4 ([gV | gW | pad])
     size_t rows_x = 0;                // world * cap_pair: rows of the exchange index space p
-    unsigned int* send_cnt = nullptr; // [kMaxWorld] records appended per owner by the running send_keys
-    unsigned int* seg_cnt = nullptr;  // [kNumSlots][kMaxWorld]: keys per owner of each slot's batch
-    uint32_t* opos = nullptr;         // [kNumSlots][cap_keys]: exchange row p of each of my slots
-    uint32_t* hot_p = nullptr;        // [kNumSlots][rows_x]: replica block of hot exchange rows (fused kernels), else ~0
-    unsigned int* done_ctr = nullptr; // [4] last-block counters
-    int* overflow = nullptr;          // device flag: a key list outgrew cap_pair
-    float *cgV = nullptr, *cgW = nullptr;  // [rows_x][rowlen], [rows_x]: compact gradient rows of the non-fused kernels
+    Buf<unsigned int> send_cnt;       // [kMaxWorld] records appended per owner by the running send_keys
+    Buf<unsigned int> seg_cnt;        // [kNumSlots][kMaxWorld]: keys per owner of each slot's batch
+    Buf<uint32_t> opos;               // [kNumSlots][cap_keys]: exchange row p of each of my slots
+    Buf<uint32_t> hot_p;              // [kNumSlots][rows_x]: replica block of hot exchange rows (fused kernels), else ~0
+    Buf<unsigned int> done_ctr;       // [4] last-block counters
+    Buf<int> overflow;                // device flag: a key list outgrew cap_pair
+    Buf<float> cgV, cgW;              // [rows_x][rowlen], [rows_x]: compact gradient rows of the non-fused kernels
     // owner side of the fused FM / NFM step: the UNION of the key lists the requesters sent for a slot's batch, built once per
     // upload, and for every union row its position in each requester's list (~0: not asked for) -- the updater walks it and
     // sums the gradient inboxes itself (no dense update_g, no touched map, no O(F / R) scan per step)
-    uint32_t* own_uniq = nullptr;     // [kNumSlots][cap_own] shard-local rows
-    unsigned int* n_own = nullptr;    // [kNumSlots]
-    uint32_t* own_pos = nullptr;      // [kNumSlots][world][cap_own]
-    uint32_t* posmap = nullptr;       // [world][Fl] scratch: list position of a row in requester q's current list (self-validating)
-    uint8_t* own_mark = nullptr;      // permuted byte map over the shard (128 * own_T)
+    Buf<uint32_t> own_uniq;           // [kNumSlots][cap_own] shard-local rows
+    Buf<unsigned int> n_own;          // [kNumSlots]
+    Buf<uint32_t> own_pos;            // [kNumSlots][world][cap_own]
+    Buf<uint32_t> posmap;             // [world][Fl] scratch: list position of a row in requester q's current list (self-validating)
+    Buf<uint8_t> own_mark;            // permuted byte map over the shard (128 * own_T)
     size_t cap_own = 0, own_T = 0;
     unsigned long long own_gen[kNumSlots] = {0};
     void* opened[kMaxWorld] = {nullptr};  // peers' arenas mapped by lctr_ipc_import
@@ -119,19 +119,20 @@ struct DistState {
     // keyed contexts (cfg.key_mode = LCTR_KEYS_HASHED): requester-side dedupe of a batch's keys into batch-local ids u,
     // an open-addressing table of bt_T >= 2 * cap_keys slots cleared by the list of the slots it claimed
     bool keyed = false;
-    unsigned long long* bt_key = nullptr;     // [bt_T] slot keys, kEmptyKey = free
-    uint32_t* bt_row = nullptr;               // [bt_T] batch-local id of the slot's key
-    uint32_t* bt_claimed = nullptr;           // [bt_T] slots claimed by the running dedupe
-    unsigned long long* bt_cnt = nullptr;     // keys claimed (the batch's U when <= cap_keys)
-    unsigned int* bt_flags = nullptr;         // [3] U > cap_keys, table full, (unused)
-    unsigned long long* batch_key = nullptr;  // [cap_keys] key of batch-local id u
-    unsigned long long* bt_stage = nullptr;   // the batch's keys, one per entry
+    Buf<unsigned long long> bt_key;           // [bt_T] slot keys, kEmptyKey = free
+    Buf<uint32_t> bt_row;                     // [bt_T] batch-local id of the slot's key
+    Buf<uint32_t> bt_claimed;                 // [bt_T] slots claimed by the running dedupe
+    Buf<unsigned long long> bt_cnt;           // keys claimed (the batch's U when <= cap_keys)
+    Buf<unsigned int> bt_flags;               // [3] U > cap_keys, table full, (unused)
+    Buf<unsigned long long> batch_key;        // [cap_keys] key of batch-local id u
+    Buf<unsigned long long> bt_stage;         // the batch's keys, one per entry
     size_t bt_T = 0, bt_stage_cap = 0;
-    unsigned int* xstat = nullptr;            // owner side: status of the running translation (wait kernel -> the others)
-    unsigned long long* xres = nullptr;       // [kMaxWorld] status every owner raised for this rank's upload
+    Buf<unsigned int> xstat;                  // owner side: status of the running translation (wait kernel -> the others)
+    Buf<unsigned long long> xres;             // [kMaxWorld] status every owner raised for this rank's upload
     unsigned long long xseq = 0;              // keyed uploads so far (the same on every rank: the upload is collective)
     bool posted = false;                      // this upload's lists (or its refusal) are out
 };
+void drop(DistState* p) { delete p; }
 
 __device__ __forceinline__ unsigned long long* flag_ptr(unsigned char* arena, const ArenaLayout& A, int row, int col) {
     return reinterpret_cast<unsigned long long*>(arena + A.flags) + (size_t)row * kMaxWorld + col;
@@ -711,8 +712,8 @@ static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 int dist_alloc(lctr_ctx* c) {
     const int R = c->cfg.world;
     LCTR_CHECK(R <= kMaxWorld && (R & (R - 1)) == 0, "world=%d: need a power of two <= %d", R, kMaxWorld);
-    DistState* d = new DistState();
-    c->dist = d;
+    c->dist.reset(new DistState());
+    DistState* d = c->dist.get();
     d->rank = c->cfg.rank; d->world = R;
     d->keyed = c->cfg.key_mode == LCTR_KEYS_HASHED;
     while ((1 << d->shift) < R) d->shift++;
@@ -743,37 +744,36 @@ int dist_alloc(lctr_ctx* c) {
     A.grad_region = align_up(d->cap_pair * (size_t)d->recw * sizeof(float), 256);
     A.grad_inbox = off; off += A.grad_region * R;
     A.total = off;
-    LCTR_CUDA(cudaMalloc((void**)&d->arena, A.total));
+    if (d->arena.alloc(A.total)) return 1;
     LCTR_CUDA(cudaMemsetAsync(d->arena, 0, A.total, c->stream));
     d->bytes += A.total;
-    LCTR_CUDA(cudaMalloc((void**)&d->send_cnt, kMaxWorld * sizeof(unsigned int)));
+    if (d->send_cnt.alloc(kMaxWorld)) return 1;
     LCTR_CUDA(cudaMemsetAsync(d->send_cnt, 0, kMaxWorld * sizeof(unsigned int), c->stream));
-    LCTR_CUDA(cudaMalloc((void**)&d->seg_cnt, (size_t)kNumSlots * kMaxWorld * sizeof(unsigned int)));
+    if (d->seg_cnt.alloc((size_t)kNumSlots * kMaxWorld)) return 1;
     LCTR_CUDA(cudaMemsetAsync(d->seg_cnt, 0, (size_t)kNumSlots * kMaxWorld * sizeof(unsigned int), c->stream));
-    LCTR_CUDA(cudaMalloc((void**)&d->opos, (size_t)kNumSlots * d->cap_keys * sizeof(uint32_t)));
+    if (d->opos.alloc((size_t)kNumSlots * d->cap_keys)) return 1;
     d->bytes += (size_t)kNumSlots * d->cap_keys * sizeof(uint32_t);
-    LCTR_CUDA(cudaMalloc((void**)&d->done_ctr, 4 * sizeof(unsigned int)));
+    if (d->done_ctr.alloc(4)) return 1;
     LCTR_CUDA(cudaMemsetAsync(d->done_ctr, 0, 4 * sizeof(unsigned int), c->stream));
-    LCTR_CUDA(cudaMalloc((void**)&d->overflow, sizeof(int)));
+    if (d->overflow.alloc(1)) return 1;
     LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), c->stream));
     if (c->grad_path == GRAD_COMPACT) {  // the fused FM / NFM kernels keep their gradients in fm_fused.cu's G / Ghot (rows p)
-        LCTR_CUDA(cudaMalloc((void**)&d->hot_p, (size_t)kNumSlots * d->rows_x * sizeof(uint32_t)));
+        if (d->hot_p.alloc((size_t)kNumSlots * d->rows_x)) return 1;
         LCTR_CUDA(cudaMemsetAsync(d->hot_p, 0xff, (size_t)kNumSlots * d->rows_x * sizeof(uint32_t), c->stream));
         d->bytes += (size_t)kNumSlots * d->rows_x * sizeof(uint32_t);
         d->cap_own = std::min<size_t>(c->Fl, d->rows_x);
         d->own_T = (c->Fl + 127) / 128;  // rows of the permuted byte map (fm_fused.cuh: mark_rows)
-        LCTR_CUDA(cudaMalloc((void**)&d->own_uniq, (size_t)kNumSlots * d->cap_own * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&d->own_pos, (size_t)kNumSlots * R * d->cap_own * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&d->n_own, kNumSlots * sizeof(unsigned int)));
+        if (d->own_uniq.alloc((size_t)kNumSlots * d->cap_own) || d->own_pos.alloc((size_t)kNumSlots * R * d->cap_own) ||
+            d->n_own.alloc(kNumSlots))
+            return 1;
         LCTR_CUDA(cudaMemsetAsync(d->n_own, 0, kNumSlots * sizeof(unsigned int), c->stream));
-        LCTR_CUDA(cudaMalloc((void**)&d->posmap, (size_t)R * c->Fl * sizeof(uint32_t)));
+        if (d->posmap.alloc((size_t)R * c->Fl)) return 1;
         LCTR_CUDA(cudaMemsetAsync(d->posmap, 0xff, (size_t)R * c->Fl * sizeof(uint32_t), c->stream));
-        LCTR_CUDA(cudaMalloc((void**)&d->own_mark, 128 * d->own_T));
+        if (d->own_mark.alloc(128 * d->own_T)) return 1;
         LCTR_CUDA(cudaMemsetAsync(d->own_mark, 0, 128 * d->own_T, c->stream));
         d->bytes += (size_t)kNumSlots * (R + 1) * d->cap_own * sizeof(uint32_t) + (size_t)R * c->Fl * sizeof(uint32_t) + 128 * d->own_T;
     } else {
-        LCTR_CUDA(cudaMalloc((void**)&d->cgW, d->rows_x * sizeof(float)));
-        LCTR_CUDA(cudaMalloc((void**)&d->cgV, d->rows_x * c->rowlen * sizeof(float)));
+        if (d->cgW.alloc(d->rows_x) || d->cgV.alloc(d->rows_x * c->rowlen)) return 1;
         LCTR_CUDA(cudaMemsetAsync(d->cgW, 0, d->rows_x * sizeof(float), c->stream));
         LCTR_CUDA(cudaMemsetAsync(d->cgV, 0, d->rows_x * c->rowlen * sizeof(float), c->stream));
         d->bytes += d->rows_x * (c->rowlen + 1) * sizeof(float);
@@ -782,14 +782,9 @@ int dist_alloc(lctr_ctx* c) {
         size_t T = kGroup;
         while (T < 2 * d->cap_keys) T <<= 1;
         d->bt_T = T;
-        LCTR_CUDA(cudaMalloc((void**)&d->bt_key, T * sizeof(unsigned long long)));
-        LCTR_CUDA(cudaMalloc((void**)&d->bt_row, T * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&d->bt_claimed, T * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&d->bt_cnt, sizeof(unsigned long long)));
-        LCTR_CUDA(cudaMalloc((void**)&d->bt_flags, 3 * sizeof(unsigned int)));
-        LCTR_CUDA(cudaMalloc((void**)&d->batch_key, d->cap_keys * sizeof(unsigned long long)));
-        LCTR_CUDA(cudaMalloc((void**)&d->xstat, sizeof(unsigned int)));
-        LCTR_CUDA(cudaMalloc((void**)&d->xres, kMaxWorld * sizeof(unsigned long long)));
+        if (d->bt_key.alloc(T) || d->bt_row.alloc(T) || d->bt_claimed.alloc(T) || d->bt_cnt.alloc(1) || d->bt_flags.alloc(3) ||
+            d->batch_key.alloc(d->cap_keys) || d->xstat.alloc(1) || d->xres.alloc(kMaxWorld))
+            return 1;
         LCTR_CUDA(cudaMemsetAsync(d->bt_key, 0xff, T * sizeof(unsigned long long), c->stream));
         LCTR_CUDA(cudaMemsetAsync(d->bt_row, 0xff, T * sizeof(uint32_t), c->stream));
         d->bytes += T * (sizeof(unsigned long long) + 2 * sizeof(uint32_t)) + d->cap_keys * sizeof(unsigned long long);
@@ -805,30 +800,16 @@ int dist_alloc(lctr_ctx* c) {
     return 0;
 }
 
-int dist_free(lctr_ctx* c) {
-    DistState* d = c->dist;
-    if (!d) return 0;
+void dist_close_peers(lctr_ctx* c) {
+    DistState* d = c->dist.get();
     for (int r = 0; r < d->world; r++)
         if (d->opened[r]) cudaIpcCloseMemHandle(d->opened[r]);
-    cudaFree(d->arena); cudaFree(d->send_cnt); cudaFree(d->seg_cnt); cudaFree(d->opos); cudaFree(d->done_ctr); cudaFree(d->overflow);
-    if (d->hot_p) cudaFree(d->hot_p);
-    if (d->own_uniq) { cudaFree(d->own_uniq); cudaFree(d->own_pos); cudaFree(d->n_own); cudaFree(d->posmap); cudaFree(d->own_mark); }
-    if (d->cgW) cudaFree(d->cgW);
-    if (d->cgV) cudaFree(d->cgV);
-    if (d->keyed) {
-        cudaFree(d->bt_key); cudaFree(d->bt_row); cudaFree(d->bt_claimed); cudaFree(d->bt_cnt); cudaFree(d->bt_flags);
-        cudaFree(d->batch_key); cudaFree(d->bt_stage); cudaFree(d->xstat); cudaFree(d->xres);
-    }
-    c->cW = c->cV = c->cgW = c->cgV = nullptr;
-    delete d;
-    c->dist = nullptr;
-    return 0;
 }
 
 size_t dist_bytes(const lctr_ctx* c) { return c->dist ? c->dist->bytes : 0; }
 
 void dist_wait_info(lctr_ctx* c, const unsigned long long** flags, int* n, unsigned long long* epoch) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     *flags = reinterpret_cast<const unsigned long long*>(d->arena + d->A.flags) + (size_t)FLAG_PULLED * kMaxWorld;
     *n = d->world;
     *epoch = d->epoch;
@@ -836,7 +817,7 @@ void dist_wait_info(lctr_ctx* c, const unsigned long long** flags, int* n, unsig
 
 // key lists of the slot's batch -> the owners' inboxes (after the slot map of fm_fused.cu has been built on `st`)
 int dist_send_keys(lctr_ctx* c, Slot& s, int slot, cudaStream_t st) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     LCTR_CHECK(d->imported, "multi-GPU upload before lctr_ipc_import");
     LCTR_CHECK((size_t)std::min<int64_t>(s.nnz, (int64_t)c->F) <= d->cap_keys,
                "batch of %lld entries exceeds the key capacity %zu of the multi-GPU context (cfg.max_nnz)", (long long)s.nnz, d->cap_keys);
@@ -850,26 +831,26 @@ int dist_send_keys(lctr_ctx* c, Slot& s, int slot, cudaStream_t st) {
     if (d->keyed) LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), st));
     if (launch(c, {grid, 256, 0, st}, d->keyed ? send_keys_kernel<true> : send_keys_kernel<false>, s.uniq, s.n_uniq, d->peers, d->A,
                d->rank, d->world, slot2, d->shift, (unsigned)d->cap_pair, d->send_cnt, opos, d->overflow,
-               d->keyed ? d->batch_key : nullptr) ||
+               d->keyed ? d->batch_key.get() : nullptr) ||
         launch(c, {1, 32, 0, st}, send_keys_finish_kernel, d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair,
-               d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow : nullptr, 0))
+               d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow.get() : nullptr, 0))
         return 1;
     d->posted = d->keyed;
     const unsigned rg = (unsigned)std::max<int64_t>(1, std::min<int64_t>((s.nnz + 255) / 256, (int64_t)c->sm_count * 8));
-    return launch(c, {rg, 256, 0, st}, remap_entries_kernel, nullptr, s.nnz, opos, s.ent_pslot, s.ent_slot, hot_p ? s.hot_of : nullptr,
+    return launch(c, {rg, 256, 0, st}, remap_entries_kernel, nullptr, s.nnz, opos, s.ent_pslot, s.ent_slot, hot_p ? s.hot_of.get() : nullptr,
                   s.n_uniq, hot_p);
 }
 
 // an empty share (0 rows or 0 entries): empty key lists and the generation flag on every owner, status OK -- the peers'
 // serve / translation of this upload then finds my lists like any other
 int dist_send_empty(lctr_ctx* c, int slot, cudaStream_t st) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     LCTR_CHECK(d->imported, "multi-GPU upload before lctr_ipc_import");
     d->gen[slot]++;
     const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
     if (d->keyed) LCTR_CUDA(cudaMemsetAsync(d->overflow, 0, sizeof(int), st));
     if (launch(c, {1, 32, 0, st}, send_keys_finish_kernel, d->peers, d->A, d->rank, d->world, slot2, slot, (unsigned)d->cap_pair,
-               d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow : nullptr, 0))
+               d->send_cnt, d->seg_cnt + (size_t)slot * kMaxWorld, d->gen[slot], d->keyed ? d->overflow.get() : nullptr, 0))
         return 1;
     d->posted = d->keyed;
     return 0;
@@ -877,7 +858,7 @@ int dist_send_empty(lctr_ctx* c, int slot, cudaStream_t st) {
 
 // ---- keyed upload, host side (capi.cu: lctr_upload_batch_keys on world > 1) -------------------------------------------
 int dist_keys_begin(lctr_ctx* c) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     LCTR_CHECK(d->imported, "multi-GPU upload before lctr_ipc_import");
     d->posted = false;
     return 0;
@@ -885,14 +866,12 @@ int dist_keys_begin(lctr_ctx* c) {
 
 // the batch's keys -> batch-local ids in s.fid (device), U of them; fails (nothing sent yet) when U > cap_keys
 int dist_keys_dedupe(lctr_ctx* c, Slot& s, const uint64_t* h_keys, int64_t nnz) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     if ((size_t)nnz > d->bt_stage_cap) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        cudaFree(d->bt_stage);
-        d->bt_stage = nullptr;
-        d->bt_stage_cap = 0;
         const size_t cap = (size_t)nnz + (size_t)nnz / 2;
-        LCTR_CUDA(cudaMalloc((void**)&d->bt_stage, cap * sizeof(unsigned long long)));
+        d->bt_stage_cap = 0;
+        if (alloc_group(sized(d->bt_stage, cap))) return 1;
         d->bt_stage_cap = cap;
     }
     LCTR_CUDA(cudaMemcpyAsync(d->bt_stage, h_keys, (size_t)nnz * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
@@ -921,7 +900,7 @@ int dist_keys_dedupe(lctr_ctx* c, Slot& s, const uint64_t* h_keys, int64_t nnz) 
 
 // a rank that cannot send its batch still posts empty lists, marked refused, so that every peer fails the upload at once
 int dist_keys_refuse(lctr_ctx* c, int slot) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     if (d->posted) return 0;
     d->gen[slot]++;
     const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
@@ -935,7 +914,7 @@ int dist_keys_refuse(lctr_ctx* c, int slot) {
 // owner side of the upload: translate what every requester sent me, raise my status on each, collect every owner's
 // status for my own lists.  Returns non-zero with the message every rank composes alike when an owner failed.
 int dist_keys_translate(lctr_ctx* c, int slot) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     const int slot2 = slot * 2 + (int)(d->gen[slot] & 1);
     d->posted = false;
     d->xseq++;
@@ -990,7 +969,7 @@ int dist_keys_translate(lctr_ctx* c, int slot) {
 // host-visible check (called where the host synchronises anyway): a key list that outgrew its inbox region is an error,
 // never a silent drop
 int dist_check_overflow(lctr_ctx* c) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     int h = 0;
     LCTR_CUDA(cudaMemcpyAsync(&h, d->overflow, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -1000,7 +979,7 @@ int dist_check_overflow(lctr_ctx* c) {
 
 // train = false: a pull-only round (no owner-side union: only the merge reads it); end it with dist_release
 int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait, bool train) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     LCTR_CHECK(d->imported, "multi-GPU step before lctr_ipc_import");
     LCTR_CHECK(s.fused_valid, "multi-GPU step on a slot without its key set");
     d->epoch++;
@@ -1038,21 +1017,21 @@ int dist_pre_step(lctr_ctx* c, Slot& s, int slot, bool in_kernel_wait, bool trai
 
 // end of a pull-only round (behind its forward): my cache is released to every owner for the next round
 int dist_release(lctr_ctx* c) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     if (launch(c, {1, 32, 0, c->stream}, release_cache_kernel, d->peers, d->A, d->rank, d->world, d->epoch)) return 1;
     d->released = d->epoch;
     return 0;
 }
 
 int dist_post_step(lctr_ctx* c, Slot& s, int slot, int64_t rows_divisor) {
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     const unsigned xgrid = (unsigned)std::max<int64_t>(8, std::min<int64_t>((int64_t)c->sm_count * 4,
         (std::min<int64_t>(s.nnz, (int64_t)c->F) * (int64_t)std::max<size_t>(1, c->rowlen / 16) + 255) / 256));
     const unsigned int* seg = d->seg_cnt + (size_t)slot * kMaxWorld;
     if (c->grad_path == GRAD_COMPACT) {  // push from G / Ghot, then merge + updater in one kernel over the owner-side union
         {
             ProfScope prof(c, PROF_DIST_PUSH);
-            FusedState* f = c->fused;
+            FusedState* f = c->fused.get();
             // dependent: behind the gradient kernel
             if (launch(c, {xgrid, 256, 0, c->stream, true}, push_rows_kernel, seg, f->G, f->GS, f->G + c->rowlen, f->GS,
                        d->hot_p + (size_t)slot * d->rows_x, f->Ghot, f->GS, (int)c->rowlen, d->recw, (unsigned)d->cap_pair, d->peers,
@@ -1108,7 +1087,7 @@ int lctr_ipc_import(lctr_ctx* c, const void* all_handles, size_t bytes_per_rank)
     LCTR_CHECK(bytes_per_rank == sizeof(cudaIpcMemHandle_t),
                "lctr_ipc_import: bytes_per_rank %zu, this build exports %zu (size the blob with lctr_ipc_export(ctx, NULL, 0, &n))",
                bytes_per_rank, sizeof(cudaIpcMemHandle_t));
-    DistState* d = c->dist;
+    DistState* d = c->dist.get();
     const unsigned char* base = reinterpret_cast<const unsigned char*>(all_handles);
     for (int r = 0; r < d->world; r++) {
         if (r == d->rank) continue;

@@ -552,7 +552,7 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
         const int tpb2 = std::max(64, (A + 31) / 32 * 32);
         return launch(c, {(unsigned)rows, (unsigned)tpb2, smem2, c->stream}, s.has_val ? ffm_tma_kernel<true> : ffm_tma_kernel<false>,
                       s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW,
-                      c->cgV, c->cfg.world > 1 ? nullptr : c->touched, c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot,
+                      c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot,
                       stats ? 1 : 0, CR);
     }
     // default for k % 4 == 0: the warp-per-sample kernel of ffm_warp.cu (LCTR_FFM_WARP=0 keeps the CTA-per-sample kernel below)
@@ -563,7 +563,7 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
     auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, train, bulk) : vec == 2 ? ffm_kernel<2>(s.has_val, train, bulk)
                                                                     : ffm_kernel<1>(s.has_val, train, bulk);
     return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid,
-                  s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched,
+                  s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(),
                   c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, stats ? 1 : 0, nullptr, nullptr);
 }
 

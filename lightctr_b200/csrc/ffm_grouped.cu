@@ -223,20 +223,11 @@ bool ffm_grouped_supported(const lctr_ctx* c) {
 int ffm_grouped_reserve(lctr_ctx* c, int64_t rows) {
     if ((size_t)rows <= c->ffm_T_rows) return 0;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    if (c->ffm_T) cudaFree(c->ffm_T);
-    if (c->ffm_cnt) cudaFree(c->ffm_cnt);
-    c->ffm_T = nullptr; c->ffm_cnt = nullptr; c->ffm_T_rows = 0;
+    c->ffm_T_rows = 0;
     const size_t Fc = c->cfg.field_cnt, k = c->cfg.factor_cnt;
-    LCTR_CUDA(cudaMalloc((void**)&c->ffm_T, (size_t)rows * Fc * Fc * k * sizeof(float)));
-    LCTR_CUDA(cudaMalloc((void**)&c->ffm_cnt, (size_t)rows * Fc * sizeof(uint16_t)));
+    if (alloc_group(sized(c->ffm_T, (size_t)rows * Fc * Fc * k), sized(c->ffm_cnt, (size_t)rows * Fc))) return 1;
     c->ffm_T_rows = (size_t)rows;
     return 0;
-}
-
-void ffm_grouped_free(lctr_ctx* c) {
-    if (c->ffm_T) cudaFree(c->ffm_T);
-    if (c->ffm_cnt) cudaFree(c->ffm_cnt);
-    c->ffm_T = nullptr; c->ffm_cnt = nullptr; c->ffm_T_rows = 0;
 }
 
 int launch_ffm_backward_grouped(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
@@ -247,7 +238,7 @@ int launch_ffm_backward_grouped(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     const int A = Fc * k / 4, NS = (A + 31) / 32;
     const OptParams P = make_opt_params(c, re - rb);
     const FfmView C{s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, s.ent_field, s.label, s.pred, c->ffm_T, c->ffm_cnt,
-                    s.short_list, reinterpret_cast<const uint2*>(s.long_list), s.csc_totals};
+                    s.short_list, s.long_list, s.csc_totals};
     const bool fuse = c->cfg.world == 1;
     const FfmParams T{fuse ? c->W : c->cW, fuse ? c->V : c->cV, c->s1W, c->s1V, c->s2W, c->s2V, c->cgW, c->cgV, s.csc_arrived};
     const unsigned grid = (unsigned)c->sm_count * 8;

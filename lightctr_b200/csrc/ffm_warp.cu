@@ -305,7 +305,7 @@ int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
     double* out_slot = c->stats + 2 * (c->step % kStatRing);
     ProfScope prof(c, PROF_FFM_FUSED);
     const uint32_t* ids = c->cfg.world > 1 ? s.ent_pslot : s.fid;
-    uint8_t* touched = c->cfg.world > 1 ? nullptr : c->touched;
+    uint8_t* touched = c->cfg.world > 1 ? nullptr : c->touched.get();
     auto kern = passes == 1 ? warp_kernel<1>(s.has_val) : passes == 2 ? warp_kernel<2>(s.has_val)
               : passes == 3 ? warp_kernel<3>(s.has_val) : warp_kernel<4>(s.has_val);
     return launch(c, {grid, (unsigned)warps * 32, smem, c->stream}, kern, s.row_ptr, ids, s.field, s.val, s.label, c->cW, c->cV, Fc,

@@ -459,7 +459,7 @@ int launch_fm_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
     return launch(c, {grid, 256, 0, c->stream},
                   sh.vec == 4 ? backward_kernel<4>(sh.lpr, s.has_val, nfm) : backward_kernel<1>(sh.lpr, s.has_val, nfm), s.row_ptr,
                   c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val, s.label, c->cW, c->cV, k, s.pred, s.sumvx, c->dz, c->cgW, c->cgV,
-                  c->cfg.world > 1 ? nullptr : c->touched, c->cfg.l2_reg, rb, re);
+                  c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb, re);
 }
 
 
@@ -547,12 +547,12 @@ static auto backward_csc_kernel(bool hv, bool nfm) {
 int launch_fm_backward_csc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
     const int k = (int)c->cfg.factor_cnt;
     LCTR_CHECK(k <= 32, "factor_cnt=%d unsupported by the feature-major backward (need k <= 32)", k);
-    LCTR_CHECK(s.csc_block > 0 && s.h_blk_seg_ptr, "deterministic step on a slot uploaded without the CSC view");
+    LCTR_CHECK(s.csc_block > 0 && !s.h_blk_seg_ptr.empty(), "deterministic step on a slot uploaded without the CSC view");
     LCTR_CHECK(rb % s.csc_block == 0 && (re == rb + s.csc_block || re == s.rows) && re - rb <= s.csc_block,
                "deterministic train_step rows [%lld,%lld) do not match the slot's row blocks of %lld",
                (long long)rb, (long long)re, (long long)s.csc_block);
     const int64_t bi = rb / s.csc_block;
-    const int64_t sb = (*s.h_blk_seg_ptr)[bi], se = (*s.h_blk_seg_ptr)[bi + 1];
+    const int64_t sb = s.h_blk_seg_ptr[bi], se = s.h_blk_seg_ptr[bi + 1];
     if (se <= sb) return 0;
     const OptParams P = make_opt_params(c, re - rb);
     int lr = 4;

@@ -10,64 +10,48 @@
 
 namespace lctr {
 
-void fused_free(lctr_ctx* c) {
-    FusedState* f = c->fused;
-    if (!f) return;
-    cudaFree(f->mark); cudaFree(f->slot_of); cudaFree(f->cnt); cudaFree(f->G); cudaFree(f->Ghot); cudaFree(f->d_opt);
-    delete f;
-    c->fused = nullptr;
-}
-
 static int fused_init(lctr_ctx* c) {
     if (c->fused) return 0;
-    FusedState* f = new FusedState();
-    c->fused = f;
+    auto f = std::make_unique<FusedState>();  // the context's only once complete
+    const bool compact = c->grad_path == GRAD_COMPACT;
     f->T = mark_rows(c->F);
-    LCTR_CUDA(cudaMalloc((void**)&f->mark, 128 * f->T + 512));
+    f->GS = compact ? grad_stride((int)c->cfg.factor_cnt) : 0;
+    const size_t n_hot = (size_t)kHotMax * kHotRep * f->GS;
+    if (f->mark.alloc(128 * f->T + 512) || f->slot_of.alloc(c->F) || f->Ghot.alloc(n_hot) || f->d_opt.alloc(1)) return 1;
     LCTR_CUDA(cudaMemsetAsync(f->mark, 0, 128 * f->T + 512, c->stream));
-    LCTR_CUDA(cudaMalloc((void**)&f->slot_of, c->F * sizeof(uint32_t)));
-    if (c->grad_path == GRAD_COMPACT) {
-        f->GS = grad_stride((int)c->cfg.factor_cnt);
-        LCTR_CUDA(cudaMalloc((void**)&f->Ghot, (size_t)kHotMax * kHotRep * f->GS * sizeof(float)));
-        LCTR_CUDA(cudaMemsetAsync(f->Ghot, 0, (size_t)kHotMax * kHotRep * f->GS * sizeof(float), c->stream));
-    }
-    LCTR_CUDA(cudaMalloc((void**)&f->d_opt, sizeof(OptParams)));
+    if (compact) LCTR_CUDA(cudaMemsetAsync(f->Ghot, 0, n_hot * sizeof(float), c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    c->fused = std::move(f);
     return 0;
 }
 
 // capacity for a batch of `nnz` entries in slot s (per-slot key set + per-context gradient buffer)
 int fused_reserve(lctr_ctx* c, Slot& s, int64_t nnz) {
     if (fused_init(c)) return 1;
-    FusedState* f = c->fused;
+    FusedState* f = c->fused.get();
     const int64_t need_u = std::min<int64_t>(std::max<int64_t>(nnz, 1), (int64_t)c->F);
     if (nnz > s.cap_ent_slot) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        if (s.ent_slot) cudaFree(s.ent_slot);
-        if (s.ent_pslot) cudaFree(s.ent_pslot);
-        s.ent_pslot = nullptr;
         const int64_t cap = std::max<int64_t>(nnz, s.cap_ent_slot + s.cap_ent_slot / 2);
-        LCTR_CUDA(cudaMalloc((void**)&s.ent_slot, (size_t)(cap + 64) * sizeof(uint32_t)));
-        if (c->cfg.world > 1) LCTR_CUDA(cudaMalloc((void**)&s.ent_pslot, (size_t)(cap + 64) * sizeof(uint32_t)));
+        s.cap_ent_slot = 0;
+        if (alloc_group(sized(s.ent_slot, (size_t)(cap + 64)), sized(s.ent_pslot, c->cfg.world > 1 ? (size_t)(cap + 64) : 0)))
+            return 1;
         s.cap_ent_slot = cap;
     }
     if (need_u > s.cap_uniq || !s.hot_of) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        if (s.uniq) cudaFree(s.uniq);
-        if (s.hot_of) cudaFree(s.hot_of);
         const int64_t cap = std::min<int64_t>(std::max<int64_t>(need_u, s.cap_uniq + s.cap_uniq / 2), (int64_t)c->F);
-        LCTR_CUDA(cudaMalloc((void**)&s.uniq, (size_t)(cap + 64) * sizeof(uint32_t)));
-        LCTR_CUDA(cudaMalloc((void**)&s.hot_of, (size_t)(cap + 64) * sizeof(uint32_t)));
-        if (!s.n_uniq) LCTR_CUDA(cudaMalloc((void**)&s.n_uniq, sizeof(unsigned int)));
-        if (!s.n_hot) LCTR_CUDA(cudaMalloc((void**)&s.n_hot, sizeof(unsigned int)));
-        if (!s.hot_slot) LCTR_CUDA(cudaMalloc((void**)&s.hot_slot, (size_t)kHotMax * sizeof(uint32_t)));
+        s.cap_uniq = 0;
+        if (alloc_group(sized(s.uniq, (size_t)(cap + 64)), sized(s.hot_of, (size_t)(cap + 64)))) return 1;
+        if ((!s.n_uniq && s.n_uniq.alloc(1)) || (!s.n_hot && s.n_hot.alloc(1)) || (!s.hot_slot && s.hot_slot.alloc(kHotMax)))
+            return 1;
         s.cap_uniq = cap;
     }
     if ((size_t)s.cap_uniq > f->cnt_cap) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
         if (c->copy_stream) LCTR_CUDA(cudaStreamSynchronize(c->copy_stream));
-        if (f->cnt) cudaFree(f->cnt);
-        LCTR_CUDA(cudaMalloc((void**)&f->cnt, (size_t)(s.cap_uniq + 64) * sizeof(unsigned int)));
+        f->cnt_cap = 0;
+        if (alloc_group(sized(f->cnt, (size_t)(s.cap_uniq + 64)))) return 1;
         LCTR_CUDA(cudaMemset(f->cnt, 0, (size_t)(s.cap_uniq + 64) * sizeof(unsigned int)));
         f->cnt_cap = (size_t)s.cap_uniq;
     }
@@ -75,8 +59,8 @@ int fused_reserve(lctr_ctx* c, Slot& s, int64_t nnz) {
     const size_t g_rows = c->cfg.world > 1 ? c->dist_rows : (size_t)s.cap_uniq;
     if (c->grad_path == GRAD_COMPACT && g_rows > f->G_rows) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        if (f->G) cudaFree(f->G);
-        LCTR_CUDA(cudaMalloc((void**)&f->G, (g_rows + 64) * f->GS * sizeof(float)));
+        f->G_rows = 0;
+        if (alloc_group(sized(f->G, (g_rows + 64) * f->GS))) return 1;
         LCTR_CUDA(cudaMemset(f->G, 0, (g_rows + 64) * f->GS * sizeof(float)));
         f->G_rows = g_rows;
     }
@@ -87,7 +71,7 @@ int fused_reserve(lctr_ctx* c, Slot& s, int64_t nnz) {
 // memory and the grids are sized for the slot's capacities.  An empty batch (0 rows or 0 entries) gets an empty map and no
 // kernel.
 int fused_build_slot(lctr_ctx* c, Slot& s, cudaStream_t st, const int64_t* hdr, int64_t rows_cap, int64_t nnz_cap) {
-    FusedState* f = c->fused;
+    FusedState* f = c->fused.get();
     s.fused_valid = false;
     const int SM = c->sm_count;
     LCTR_CUDA(cudaMemsetAsync(s.n_uniq, 0, sizeof(unsigned int), st));
@@ -110,8 +94,8 @@ int fused_build_slot(lctr_ctx* c, Slot& s, cudaStream_t st, const int64_t* hdr, 
             return 1;
     }
     const unsigned ag = (unsigned)std::max<int64_t>(1, std::min<int64_t>((nnz_cap + 255) / 256, (int64_t)SM * 8));
-    if (launch(c, {ag, 256, 0, st}, slotmap_assign_kernel, s.fid, hdr, nnz_cap, f->slot_of, hot ? s.hot_of : nullptr, s.ent_slot,
-               c->cfg.world > 1 ? s.ent_pslot : nullptr))
+    if (launch(c, {ag, 256, 0, st}, slotmap_assign_kernel, s.fid, hdr, nnz_cap, f->slot_of, hot ? s.hot_of.get() : nullptr, s.ent_slot,
+               c->cfg.world > 1 ? s.ent_pslot.get() : nullptr))
         return 1;
     s.fused_valid = true;
     return 0;
@@ -132,7 +116,7 @@ static auto fused_kernel(int mode) {
 
 template <int K>
 static int fused_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, double* out_slot, const int64_t* hdr, int mode) {
-    FusedState* f = c->fused;
+    FusedState* f = c->fused.get();
     const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((re - rb + 3) / 4, (int64_t)c->sm_count * 4));
     // one GPU: parameters straight from the tables (index = fid); several: from the batch-compact cache the owners filled
     // (index = plain slot), after the owners' "rows delivered" flags of this step (dist.cu)
@@ -147,7 +131,7 @@ static int fused_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, dou
     return launch(c, {grid, 128, 0, c->stream, dependent}, s.has_val ? fused_kernel<K, true>(mode) : fused_kernel<K, false>(mode),
                   s.row_ptr, multi ? s.ent_pslot : s.fid, s.ent_slot, s.val, s.label, c->cW, c->cV, s.pred, s.sumvx, nullptr, f->G,
                   f->Ghot, f->GS, c->cfg.l2_reg, rb, re, hdr, c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep,
-                  mode == 2 ? c->z : mode == 3 ? c->dz : nullptr, mode == 2 ? s.wide : nullptr);
+                  mode == 2 ? c->z : mode == 3 ? c->dz.get() : nullptr, mode == 2 ? s.wide.get() : nullptr);
 }
 
 // FM k in {4, 8, 16, 32}: go<K>(args...) for the context's k (32 for any other)
@@ -210,7 +194,7 @@ int launch_fm_forward_tree(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool st
 
 template <int K>
 static int apply_go(lctr_ctx* c, Slot& s, const OptParams& P, const OptParams* P_dev) {
-    FusedState* f = c->fused;
+    FusedState* f = c->fused.get();
     const int main_blocks = c->sm_count * 3;
     const unsigned grid = (unsigned)(main_blocks + kHotMax / 8);  // + one warp per possible hot slot
     // Programmatic dependent launch behind the gradient kernel (one GPU): the updater's CTAs start as the gradient kernel's
@@ -228,6 +212,6 @@ int launch_apply_compact(lctr_ctx* c, Slot& s, int64_t rows_in_step, const OptPa
 #undef K_DISPATCH
 
 void fused_opt_params(lctr_ctx* c, int64_t rows, void* out) { *reinterpret_cast<OptParams*>(out) = make_opt_params(c, rows); }
-void* fused_dev_opt(lctr_ctx* c) { return c->fused ? (void*)c->fused->d_opt : nullptr; }
+void* fused_dev_opt(lctr_ctx* c) { return c->fused ? c->fused->d_opt.get() : nullptr; }
 
 }  // namespace lctr

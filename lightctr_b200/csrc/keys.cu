@@ -121,10 +121,10 @@ struct RowArrays {
 // row, with three flag words whose meaning is the owner's ([1] is "full" for both) and their pinned mirror.  Both the
 // key table and the host tier index their rows with one.
 struct KeyIndex {
-    unsigned long long* key = nullptr;
-    uint32_t* row = nullptr;
-    unsigned int* flags = nullptr;
-    unsigned int* h_flags = nullptr;
+    Buf<unsigned long long> key;
+    Buf<uint32_t> row;
+    Buf<unsigned int> flags;
+    HostBuf<unsigned int> h_flags;
     size_t T = 0;
 
     int clear(cudaStream_t st) {
@@ -136,14 +136,8 @@ struct KeyIndex {
     int alloc(size_t cap, cudaStream_t st) {
         T = kGroup;
         while (T < 2 * cap) T <<= 1;
-        if (dalloc(&key, T) || dalloc(&row, T) || dalloc(&flags, 3)) return 1;
-        LCTR_CUDA(cudaMallocHost((void**)&h_flags, 3 * sizeof(unsigned int)));
+        if (key.alloc(T) || row.alloc(T) || flags.alloc(3) || h_flags.alloc(3)) return 1;
         return clear(st);
-    }
-    void free() {
-        dfree(key); dfree(row); dfree(flags);
-        if (h_flags) cudaFreeHost(h_flags);
-        h_flags = nullptr;
     }
     // emptied, then key row_key[i] re-inserted with row i for i < n (v: this index's view); fails naming `what` when full
     int rebuild(lctr_ctx* c, const KeyView& v, const unsigned long long* row_key, size_t n, const char* what);
@@ -154,56 +148,59 @@ struct KeyIndex {
 // from empty to a key only; a restored key keeps its slot with kNoRow, so `used` (slots holding a key) counts live and
 // dead slots, and the index is rebuilt from row_key[0, n) once it passes T / 2.
 struct HostTier {
-    RowArrays a{};                          // device-mapped host arrays of `cap` rows
+    RowArrays a{};                          // device-mapped host arrays of `cap` rows: views of the owners below
+    MappedBuf<unsigned long long> row_key, last_seen;
+    MappedBuf<float> p[6];                  // W, V, s1W, s1V, s2W, s2V
     KeyIndex ix;
     size_t cap = 0, n = 0, used = 0;
     // scratch of the compaction after a restore, sized with the key table's per-call scratch (at most one entry per new row)
-    uint32_t* rel = nullptr;                // tier rows released by the current call, in no order
-    uint32_t* wscan = nullptr;              // [m + 1] released rows in [n_live, n_live + i)
-    uint32_t* holes = nullptr;              // released rows below n_live, ascending
+    Buf<uint32_t> rel;                      // tier rows released by the current call, in no order
+    Buf<uint32_t> wscan;                    // [m + 1] released rows in [n_live, n_live + i)
+    Buf<uint32_t> holes;                    // released rows below n_live, ascending
 };
 
 // frequency admission (lctr_set_key_admission): the sketch, the counters of the last insert-upload, compaction scratch
 constexpr int kSketchDepth = 4;
 struct Admission {
-    uint32_t* sketch = nullptr;             // [kSketchDepth << lw] counters
+    Buf<uint32_t> sketch;                   // [kSketchDepth << lw] counters
     uint32_t min_count = 0, lw = 0;
-    unsigned long long* cnt = nullptr;      // [3] dropped entries, admitted keys of the current upload, scan total (device)
-    unsigned long long* h_cnt = nullptr;    // pinned mirror of [0, 2)
+    Buf<unsigned long long> cnt;            // [3] dropped entries, admitted keys of the current upload, scan total (device)
+    HostBuf<unsigned long long> h_cnt;      // pinned mirror of [0, 2)
     uint64_t dropped = 0, admitted = 0;     // of the last insert-upload
     uint64_t pending = 0;                   // entries of the upload in flight that keys_admission_compact removes
     // compaction scratch, grown on demand (per-call scratch: not counted by lctr_device_bytes)
     size_t cap = 0;
-    uint32_t *scan = nullptr, *tiles = nullptr, *fid = nullptr;
-    uint16_t* field = nullptr;
-    float* val = nullptr;
+    Buf<uint32_t> scan, tiles, fid;
+    Buf<uint16_t> field;
+    Buf<float> val;
 };
 
 struct KeyTable {
     KeyIndex ix;                            // row kNoRow when the capacity was exhausted; flags: [0] capacity exhausted,
                                             // [1] table full, [2] new rows of this upload
-    unsigned long long* row_key = nullptr;  // [capacity] key of each row
-    unsigned long long* count = nullptr;    // rows claimed (may pass capacity: claims that got no row)
-    uint32_t* new_rows = nullptr;           // rows created by this upload
-    unsigned long long* d_keys = nullptr;   // staging of the keys of one call
-    int64_t* d_rows = nullptr;              // lookup results / fixed rows of one call
+    Buf<unsigned long long> row_key;        // [capacity] key of each row
+    Buf<unsigned long long> count;          // rows claimed (may pass capacity: claims that got no row)
+    Buf<uint32_t> new_rows;                 // rows created by this upload
+    Buf<unsigned long long> d_keys;         // staging of the keys of one call
+    Buf<int64_t> d_rows;                    // lookup results / fixed rows of one call
     size_t cap_scratch = 0;
     size_t cap = 0;
     unsigned long long seed = 0;
     float scale = 1.f;
     // key_evict = 1
-    unsigned long long* last_seen = nullptr;  // [capacity] clock of the insert-upload that last met the row
+    Buf<unsigned long long> last_seen;        // [capacity] clock of the insert-upload that last met the row
     unsigned long long clock = 0;             // insert-uploads so far
     // scratch of lctr_evict_keys, allocated by its first call
-    uint32_t* ev_scan = nullptr;              // [capacity + 1] E(r)
-    uint32_t* ev_rows = nullptr;              // [capacity] evicted rows, ascending
-    uint32_t* ev_tiles = nullptr;             // [capacity / kEvTile + 1] per-tile counts -> offsets
-    unsigned int* ev_hist = nullptr;          // [65536] digit histogram of the radix select
-    unsigned long long* ev_res = nullptr;     // [4] counters read back by the host
-    unsigned long long* h_res = nullptr;      // pinned mirror
-    HostTier* tier = nullptr;                 // cfg.key_host_rows > 0
-    Admission* adm = nullptr;                 // lctr_set_key_admission with min_count > 1
+    Buf<uint32_t> ev_scan;                    // [capacity + 1] E(r)
+    Buf<uint32_t> ev_rows;                    // [capacity] evicted rows, ascending
+    Buf<uint32_t> ev_tiles;                   // [capacity / kEvTile + 1] per-tile counts -> offsets
+    Buf<unsigned int> ev_hist;                // [65536] digit histogram of the radix select
+    Buf<unsigned long long> ev_res;           // [4] counters read back by the host
+    HostBuf<unsigned long long> h_res;        // pinned mirror
+    std::unique_ptr<HostTier> tier;           // cfg.key_host_rows > 0
+    std::unique_ptr<Admission> adm;           // lctr_set_key_admission with min_count > 1
 };
+void drop(KeyTable* p) { delete p; }
 
 static KeyView view(const KeyTable* t) {
     return KeyView{t->ix.key, t->ix.row, t->row_key, t->count, t->ix.flags, t->new_rows, t->ix.T / kGroup, t->cap};
@@ -760,50 +757,38 @@ int KeyIndex::rebuild(lctr_ctx* c, const KeyView& v, const unsigned long long* r
     return 0;
 }
 
-// the per-call scratch of the key table and of the tier compaction for `cap` keys (0: freed)
-static int key_scratch(KeyTable* t, size_t cap) {
-    HostTier* h = t->tier;
-    dfree(t->d_keys); dfree(t->d_rows); dfree(t->new_rows);
-    if (h) { dfree(h->rel); dfree(h->wscan); dfree(h->holes); }
+// room for n keys in the per-call scratch of the key table and of the tier compaction, grown by half at least
+int scratch_reserve(lctr_ctx* c, size_t n) {
+    KeyTable* t = c->keys.get();
+    if (n <= t->cap_scratch) return 0;
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    const size_t cap = std::max(n, t->cap_scratch + t->cap_scratch / 2);
+    HostTier* h = t->tier.get();
     t->cap_scratch = 0;
-    if (!cap) return 0;
-    if (dalloc(&t->d_keys, cap) || dalloc(&t->d_rows, cap) || dalloc(&t->new_rows, cap)) return 1;
-    if (h && (dalloc(&h->rel, cap) || dalloc(&h->wscan, cap + 1) || dalloc(&h->holes, cap))) return 1;  // a call restores
-    t->cap_scratch = cap;                                                                              // <= 1 row per new row
+    if (h) { h->rel.reset(); h->wscan.reset(); h->holes.reset(); }
+    if (alloc_group(sized(t->d_keys, cap), sized(t->d_rows, cap), sized(t->new_rows, cap))) return 1;
+    if (h && alloc_group(sized(h->rel, cap), sized(h->wscan, cap + 1), sized(h->holes, cap))) {  // a call restores
+        t->d_keys.reset(); t->d_rows.reset(); t->new_rows.reset();                                // <= 1 row per new row
+        return 1;
+    }
+    t->cap_scratch = cap;
     return 0;
 }
 
-// room for n keys in the per-call scratch, grown by half at least
-int scratch_reserve(lctr_ctx* c, size_t n) {
-    KeyTable* t = c->keys;
-    if (n <= t->cap_scratch) return 0;
-    LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    return key_scratch(t, std::max(n, t->cap_scratch + t->cap_scratch / 2));
-}
-
-// the compaction scratch of admission for n entries (0: freed)
+// the compaction scratch of admission for n entries
 static int admission_scratch(Admission* a, size_t cap) {
-    dfree(a->scan); dfree(a->tiles); dfree(a->fid); dfree(a->field); dfree(a->val);
     a->cap = 0;
-    if (!cap) return 0;
-    if (dalloc(&a->scan, cap + 1) || dalloc(&a->tiles, cap / kEvTile + 1) || dalloc(&a->fid, cap) || dalloc(&a->field, cap) ||
-        dalloc(&a->val, cap))
-            return 1;
+    if (alloc_group(sized(a->scan, cap + 1), sized(a->tiles, cap / kEvTile + 1), sized(a->fid, cap), sized(a->field, cap),
+                    sized(a->val, cap)))
+        return 1;
     a->cap = cap;
     return 0;
 }
 
-// the scratch of lctr_evict_keys for a table of cap rows (0: freed); h_res, allocated last, marks it complete
+// the scratch of lctr_evict_keys for a table of cap rows; h_res, allocated last, marks it complete
 static int evict_scratch(KeyTable* t, size_t cap) {
-    dfree(t->ev_scan); dfree(t->ev_rows); dfree(t->ev_tiles); dfree(t->ev_hist); dfree(t->ev_res);
-    if (t->h_res) cudaFreeHost(t->h_res);
-    t->h_res = nullptr;
-    if (!cap) return 0;
-    if (dalloc(&t->ev_scan, cap + 1) || dalloc(&t->ev_rows, cap) || dalloc(&t->ev_tiles, cap / kEvTile + 1) ||
-        dalloc(&t->ev_hist, (size_t)kEvBins) || dalloc(&t->ev_res, 4))
-            return 1;
-    LCTR_CUDA(cudaMallocHost((void**)&t->h_res, 4 * sizeof(unsigned long long)));
-    return 0;
+    return alloc_group(sized(t->ev_scan, cap + 1), sized(t->ev_rows, cap), sized(t->ev_tiles, cap / kEvTile + 1),
+                       sized(t->ev_hist, (size_t)kEvBins), sized(t->ev_res, 4), sized(t->h_res, 4));
 }
 
 static RowArrays device_rows(lctr_ctx* c) {
@@ -815,19 +800,19 @@ static bool tier_live(const KeyTable* t) { return t->tier && t->tier->n > 0; }
 
 // the rows the last insert recorded (at most max_new), initialised or restored from the tier
 int init_new_rows(lctr_ctx* c, int64_t max_new) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     const bool tiered = tier_live(t);
     const auto kernel = tiered ? by_rowlen(c, key_init_kernel<true, true>, key_init_kernel<true, false>) : key_init_kernel<false, false>;
-    HostTier* h = tiered ? t->tier : nullptr;
+    HostTier* h = tiered ? t->tier.get() : nullptr;
     if (launch(c, {warp_grid(c, (size_t)max_new), 256, 0, c->stream}, kernel, view(t), h ? view(h) : KeyView{}, device_rows(c),
-               h ? h->a : RowArrays{}, c->rowlen, h ? h->rel : nullptr, initial_s1(c->cfg), t->seed, t->scale)) return 1;
+               h ? h->a : RowArrays{}, c->rowlen, h ? h->rel.get() : nullptr, initial_s1(c->cfg), t->seed, t->scale)) return 1;
     return 0;
 }
 
 // the key table's flags and, on a tiered context, the tier's, with one synchronisation; admission: also the counters of
 // an insert-upload
 static int read_flags(lctr_ctx* c, bool admission = false) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     LCTR_CUDA(cudaMemcpyAsync(t->ix.h_flags, t->ix.flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     if (t->tier)
         LCTR_CUDA(cudaMemcpyAsync(t->tier->ix.h_flags, t->tier->ix.flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
@@ -853,65 +838,36 @@ int check_keys_reserved(const uint64_t* keys, int64_t n, const char* who) {
 }
 
 int keys_alloc(lctr_ctx* c) {
-    KeyTable* t = new KeyTable();
-    c->keys = t;
+    c->keys.reset(new KeyTable());
+    KeyTable* t = c->keys.get();
     // several GPUs: this rank's shard holds the global rows l * world + rank below feature_cnt (dist.cu: placement)
     t->cap = owned_rows(c->F - 1, c->cfg.world, c->cfg.rank);
     t->scale = (float)(1.0 / sqrt((double)c->cfg.factor_cnt));
-    if (t->ix.alloc(t->cap, c->stream) || dalloc(&t->row_key, t->cap) || dalloc(&t->count, 1)) return 1;
+    if (t->ix.alloc(t->cap, c->stream) || t->row_key.alloc(t->cap) || t->count.alloc(1)) return 1;
     LCTR_CUDA(cudaMemsetAsync(t->count, 0, sizeof(unsigned long long), c->stream));
     if (c->cfg.key_evict) {
-        if (dalloc(&t->last_seen, t->cap)) return 1;
+        if (t->last_seen.alloc(t->cap)) return 1;
         LCTR_CUDA(cudaMemsetAsync(t->last_seen, 0, t->cap * sizeof(unsigned long long), c->stream));
     }
     if (c->cfg.key_host_rows) {
-        HostTier* h = new HostTier();
-        t->tier = h;
+        t->tier.reset(new HostTier());
+        HostTier* h = t->tier.get();
         h->cap = c->cfg.key_host_rows;
         if (h->ix.alloc(h->cap, c->stream)) return 1;
         // rows in pinned host memory mapped into the device address space: kernels read and write them over PCIe
-        auto host = [&](void** p, size_t bytes) {
-            return cudaHostAlloc(p, bytes, cudaHostAllocMapped) == cudaSuccess && (memset(*p, 0, bytes), true);
-        };
         const size_t R = h->cap, nv = R * c->rowlen;
-        bool ok = host((void**)&h->a.row_key, R * 8) && host((void**)&h->a.last_seen, R * 8) && host((void**)&h->a.W, R * 4) &&
-                  host((void**)&h->a.V, nv * 4) && host((void**)&h->a.s1W, R * 4) && host((void**)&h->a.s1V, nv * 4);
-        if (ok && c->s2W) ok = host((void**)&h->a.s2W, R * 4) && host((void**)&h->a.s2V, nv * 4);
+        const size_t np[6] = {R, nv, R, nv, c->s2W ? R : 0, c->s2W ? nv : 0};
+        bool ok = !h->row_key.alloc(R) && !h->last_seen.alloc(R);
+        for (int i = 0; i < 6 && ok; i++) ok = !h->p[i].alloc(np[i]);
         LCTR_CHECK(ok, "lctr_create: cannot allocate %llu rows of pinned host memory (cfg.key_host_rows)",
                    (unsigned long long)h->cap);
+        memset(h->row_key, 0, R * sizeof(unsigned long long));
+        memset(h->last_seen, 0, R * sizeof(unsigned long long));
+        for (int i = 0; i < 6; i++)
+            if (np[i]) memset(h->p[i], 0, np[i] * sizeof(float));
+        h->a = RowArrays{h->p[0], h->p[1], h->p[2], h->p[3], h->p[4], h->p[5], h->row_key, h->last_seen};
     }
     return 0;
-}
-
-static void admission_free(KeyTable* t) {
-    Admission* a = t->adm;
-    if (!a) return;
-    dfree(a->sketch); dfree(a->cnt);
-    admission_scratch(a, 0);
-    if (a->h_cnt) cudaFreeHost(a->h_cnt);
-    delete a;
-    t->adm = nullptr;
-}
-
-static void tier_free(HostTier* h) {
-    h->ix.free();
-    for (void* p : {(void*)h->a.row_key, (void*)h->a.last_seen, (void*)h->a.W, (void*)h->a.V, (void*)h->a.s1W, (void*)h->a.s1V,
-                    (void*)h->a.s2W, (void*)h->a.s2V})
-        if (p) cudaFreeHost(p);
-    delete h;
-}
-
-void keys_free(lctr_ctx* c) {
-    KeyTable* t = c->keys;
-    if (!t) return;
-    key_scratch(t, 0);  // the tier's compaction scratch too: before the tier goes
-    evict_scratch(t, 0);
-    if (t->tier) tier_free(t->tier);
-    admission_free(t);
-    t->ix.free();
-    dfree(t->row_key); dfree(t->count); dfree(t->last_seen);
-    delete t;
-    c->keys = nullptr;
 }
 
 bool keys_tracked(const lctr_ctx* c) { return c->keys && c->keys->last_seen; }
@@ -920,23 +876,23 @@ static int tier_rebuild(lctr_ctx* c);
 
 bool keys_tier(const lctr_ctx* c, TierRows* out) {
     if (!c->keys || !c->keys->tier) return false;
-    const HostTier* h = c->keys->tier;
+    const HostTier* h = c->keys->tier.get();
     *out = TierRows{h->a.row_key, h->a.last_seen, {h->a.W, h->a.V, h->a.s1W, h->a.s1V, h->a.s2W, h->a.s2V}, h->n, h->cap};
     return true;
 }
 
 int keys_tier_restore(lctr_ctx* c, uint64_t n) {
-    HostTier* h = c->keys->tier;
+    HostTier* h = c->keys->tier.get();
     LCTR_CHECK(n <= h->cap, "checkpoint: %llu host-tier rows exceed cfg.key_host_rows = %zu", (unsigned long long)n, h->cap);
     h->n = (size_t)n;
     return tier_rebuild(c);
 }
 
-KeyView keys_view(lctr_ctx* c) { return view(c->keys); }
+KeyView keys_view(lctr_ctx* c) { return view(c->keys.get()); }
 size_t keys_capacity(const lctr_ctx* c) { return c->keys->cap; }
 
 size_t keys_bytes(const lctr_ctx* c) {
-    const KeyTable* t = c->keys;
+    const KeyTable* t = c->keys.get();
     if (!t) return 0;
     return t->ix.T * (sizeof(unsigned long long) + sizeof(uint32_t)) + t->cap * sizeof(unsigned long long) +
            (t->last_seen ? t->cap * sizeof(unsigned long long) : 0) +
@@ -946,7 +902,7 @@ size_t keys_bytes(const lctr_ctx* c) {
 
 // the tier index emptied and rows [0, n) re-inserted with row = index
 static int tier_rebuild(lctr_ctx* c) {
-    HostTier* h = c->keys->tier;
+    HostTier* h = c->keys->tier.get();
     if (h->ix.rebuild(c, view(h), h->a.row_key, h->n, "host tier: index full while re-inserting")) return 1;
     h->used = h->n;
     return 0;
@@ -976,7 +932,7 @@ static void radix_sort_u32(std::vector<uint32_t>& v) {
 // ascending).  Planned on the host from the released list: O(m) copies and work (the sort is a radix sort), then one
 // move and one reindex launch over the window; nothing reads the rest of the tier.
 static int tier_compact(lctr_ctx* c) {
-    HostTier* h = c->keys->tier;
+    HostTier* h = c->keys->tier.get();
     if (!h || !h->ix.h_flags[0]) return 0;
     const size_t m = h->ix.h_flags[0], n = h->n, n_live = n - m;
     std::vector<uint32_t> rel(m), holes;
@@ -1012,8 +968,8 @@ static int tier_compact(lctr_ctx* c) {
 // Admission on, insert = 1: count + admit replace the insert, entries of keys not admitted get the drop marker, and the
 // dropped count is left for keys_admission_compact.
 int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid) {
-    KeyTable* t = c->keys;
-    Admission* adm = insert ? t->adm : nullptr;
+    KeyTable* t = c->keys.get();
+    Admission* adm = insert ? t->adm.get() : nullptr;
     if (insert) t->clock++;  // the clock counts insert-uploads, empty ones included
     if (t->adm) t->adm->pending = 0;
     if (adm) adm->dropped = adm->admitted = 0;
@@ -1027,7 +983,7 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
         ProfScope prof(c, PROF_KEYS);
         if (insert || restoring) {
             if (adm) {
-                const KeyView hv = restoring ? view(t->tier) : KeyView{};
+                const KeyView hv = restoring ? view(t->tier.get()) : KeyView{};
                 if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_count_kernel, t->d_keys, n, view(t), hv, restoring,
                            adm->sketch, adm->lw)) return 1;
                 if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_admit_kernel, t->d_keys, n, view(t), hv, restoring,
@@ -1035,17 +991,17 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
             } else if (insert) {
                 if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_insert_kernel, t->d_keys, n, view(t))) return 1;
             } else {
-                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_lookup_restore_kernel, t->d_keys, n, view(t), view(t->tier)))
+                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_lookup_restore_kernel, t->d_keys, n, view(t), view(t->tier.get())))
                     return 1;
             }
             if (init_new_rows(c, std::min<int64_t>(n, (int64_t)t->cap))) return 1;
             if (!insert) {
-                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_tier_refused_kernel, t->d_keys, n, view(t), view(t->tier)))
+                if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_tier_refused_kernel, t->d_keys, n, view(t), view(t->tier.get())))
                     return 1;
             }
         }
         if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_find_kernel<0>, t->d_keys, n, view(t), fid, nullptr, insert ? 1 : 0,
-                   insert ? t->last_seen : nullptr, t->clock, adm ? adm->cnt : nullptr)) return 1;
+                   insert ? t->last_seen.get() : nullptr, t->clock, adm ? adm->cnt.get() : nullptr)) return 1;
     }
     if (read_flags(c, adm != nullptr)) return 1;
     if (adm) {
@@ -1062,7 +1018,7 @@ int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, 
 // after keys_translate dropped entries of the slot's batch (row_ptr, fid, field, val on the device): the kept entries in
 // order, the new row_ptr, *nnz = the kept count.  Nothing runs when no entry was dropped.
 int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, int64_t* nnz) {
-    Admission* a = c->keys ? c->keys->adm : nullptr;
+    Admission* a = c->keys ? c->keys->adm.get() : nullptr;
     if (!a || !a->pending) return 0;
     const size_t n = (size_t)*nnz, kept = n - a->pending;
     a->pending = 0;
@@ -1070,8 +1026,8 @@ int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, 
         LCTR_CUDA(cudaStreamSynchronize(st));
         if (admission_scratch(a, std::max(n, a->cap + a->cap / 2))) return 1;
     }
-    const uint16_t* field = s.has_field ? s.field : nullptr;
-    const float* val = s.has_val ? s.val : nullptr;
+    const uint16_t* field = s.has_field ? s.field.get() : nullptr;
+    const float* val = s.has_val ? s.val.get() : nullptr;
     {
         ProfScope prof(c, PROF_KEYS);
         const size_t ntiles = n / kEvTile + 1;  // tiles cover [0, n]: D(n) is read for row_ptr[rows] = n
@@ -1080,7 +1036,7 @@ int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, 
         if (launch(c, {(unsigned)ntiles, kEvTile, 0, st}, evict_index_kernel<DropFlag>, DropFlag{s.fid}, n, a->tiles, a->scan, nullptr))
             return 1;
         if (launch(c, {stride_grid(c, std::max(n, (size_t)rows + 1)), 256, 0, st}, admit_compact_kernel, s.fid, field, val, n,
-                   a->scan, s.row_ptr, (size_t)rows, a->fid, field ? a->field : nullptr, val ? a->val : nullptr)) return 1;
+                   a->scan, s.row_ptr, (size_t)rows, a->fid, field ? a->field.get() : nullptr, val ? a->val.get() : nullptr)) return 1;
     }
     if (kept) {
         LCTR_CUDA(cudaMemcpyAsync(s.fid, a->fid, kept * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
@@ -1092,7 +1048,7 @@ int keys_admission_compact(lctr_ctx* c, Slot& s, cudaStream_t st, int64_t rows, 
 }
 
 static int lookup_dev(lctr_ctx* c, const uint64_t* keys, int64_t n) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     if (scratch_reserve(c, (size_t)n)) return 1;
     LCTR_CUDA(cudaMemcpyAsync(t->d_keys, keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
     if (launch(c, {tile_grid(n), 256, 0, c->stream}, key_find_kernel<1>, t->d_keys, n, view(t), nullptr, t->d_rows, 0, nullptr, 0,
@@ -1102,7 +1058,7 @@ static int lookup_dev(lctr_ctx* c, const uint64_t* keys, int64_t n) {
 
 // rebuild from a row -> key array (checkpoint restore): key i gets row i, parameters are left as they are
 int keys_restore(lctr_ctx* c, const uint64_t* row_key, uint64_t n) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     LCTR_CHECK(n <= t->cap, "checkpoint: %llu keyed rows exceed the capacity %zu", (unsigned long long)n, t->cap);
     const unsigned long long cnt = n;
     LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));
@@ -1121,7 +1077,7 @@ int keys_download(lctr_ctx* c, std::vector<uint64_t>& out) {
 }
 
 int keys_download_stamps(lctr_ctx* c, uint64_t n, std::vector<uint64_t>& stamps, uint64_t* clock) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     stamps.resize(n);
     *clock = t->clock;
     if (n) LCTR_CUDA(cudaMemcpyAsync(stamps.data(), t->last_seen, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
@@ -1130,7 +1086,7 @@ int keys_download_stamps(lctr_ctx* c, uint64_t n, std::vector<uint64_t>& stamps,
 }
 
 int keys_restore_stamps(lctr_ctx* c, const uint64_t* stamps, uint64_t n, uint64_t clock) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     LCTR_CHECK(n <= t->cap, "checkpoint: %llu stamps exceed the capacity %zu", (unsigned long long)n, t->cap);
     LCTR_CUDA(cudaMemsetAsync(t->last_seen, 0, t->cap * sizeof(uint64_t), c->stream));
     if (n) LCTR_CUDA(cudaMemcpyAsync(t->last_seen, stamps, n * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
@@ -1140,7 +1096,7 @@ int keys_restore_stamps(lctr_ctx* c, const uint64_t* stamps, uint64_t n, uint64_
 }
 
 static int read_res(lctr_ctx* c, int n) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     LCTR_CUDA(cudaMemcpyAsync(t->h_res, t->ev_res, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
@@ -1149,7 +1105,7 @@ static int read_res(lctr_ctx* c, int n) {
 // the age of rank `rank` (0-based, ascending) among the rows of age <= max_idle, of which the largest is max_age
 static int radix_select_age(lctr_ctx* c, const unsigned long long* last_seen, size_t n, unsigned long long max_idle,
                             unsigned long long max_age, unsigned long long rank, unsigned long long* out) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     const int bits = std::max(1, 64 - __builtin_clzll(max_age | 1ull));
     const unsigned grid = stride_grid(c, n);
     unsigned long long prefix = 0;
@@ -1179,7 +1135,7 @@ struct EvTable {
 
 // survey, select, count and scan of the stamp rule against the upload clock: *m rows of the table leave by rule *l
 static int evict_plan(lctr_ctx* c, const EvTable& tb, uint64_t max_idle, uint64_t max_rows, EvictRule* e, size_t* m) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     const size_t n = tb.n;
     // 1 + 2: the rule
     LCTR_CUDA(cudaMemsetAsync(t->ev_res, 0, 2 * sizeof(unsigned long long), c->stream));
@@ -1208,38 +1164,32 @@ static int evict_index_export(lctr_ctx* c, const EvTable& tb, const EvictRule& e
     if (launch(c, {(unsigned)(tb.n / kEvTile + 1), kEvTile, 0, c->stream}, evict_index_kernel<EvictFlag>, EvictFlag{tb.a.last_seen, e}, tb.n,
                tb.tiles, tb.scan, tb.rows)) return 1;
     if (!(keys_out || W_out || V_out)) return 0;
-    unsigned long long* dK = nullptr;
-    float *dW = nullptr, *dV = nullptr;
-    cudaError_t err = cudaSuccess;
-    if (keys_out && err == cudaSuccess) err = cudaMalloc((void**)&dK, m * sizeof(unsigned long long));
-    if (W_out && err == cudaSuccess) err = cudaMalloc((void**)&dW, m * sizeof(float));
-    if (V_out && err == cudaSuccess) err = cudaMalloc((void**)&dV, m * c->rowlen * sizeof(float));
-    // a failed launch frees the staging before it returns, like every other failure here
-    if (err == cudaSuccess && launch(c, {warp_grid(c, m), 256, 0, c->stream}, evict_export_kernel, tb.rows, m, tb.a.row_key,
-                              tb.a.W, tb.a.V, c->rowlen, dK, dW, dV)) {
-        cudaStreamSynchronize(c->stream);
-        cudaFree(dK); cudaFree(dW); cudaFree(dV);
-        return 1;
-    }
-    if (err == cudaSuccess && dK) err = cudaMemcpyAsync(keys_out, dK, m * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream);
-    if (err == cudaSuccess && dW) err = cudaMemcpyAsync(W_out, dW, m * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
-    if (err == cudaSuccess && dV) err = cudaMemcpyAsync(V_out, dV, m * c->rowlen * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
-    const cudaError_t es = cudaStreamSynchronize(c->stream);
-    cudaFree(dK); cudaFree(dW); cudaFree(dV);
-    LCTR_CUDA(err);
-    LCTR_CUDA(es);
-    return 0;
+    Buf<unsigned long long> dK;
+    Buf<float> dW, dV;
+    if (dK.alloc(keys_out ? m : 0) || dW.alloc(W_out ? m : 0) || dV.alloc(V_out ? m * c->rowlen : 0)) return 1;
+    auto copy_out = [&]() -> int {
+        if (launch(c, {warp_grid(c, m), 256, 0, c->stream}, evict_export_kernel, tb.rows, m, tb.a.row_key, tb.a.W, tb.a.V,
+                   c->rowlen, dK, dW, dV))
+            return 1;
+        if (dK) LCTR_CUDA(cudaMemcpyAsync(keys_out, dK, m * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+        if (dW) LCTR_CUDA(cudaMemcpyAsync(W_out, dW, m * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        if (dV) LCTR_CUDA(cudaMemcpyAsync(V_out, dV, m * c->rowlen * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        return 0;
+    };
+    const int rc = copy_out();
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the queued work reads the staging, which goes on return
+    return rc;
 }
 
 bool keys_admission(const lctr_ctx* c, uint32_t* min_count, uint32_t* log2_width) {
-    const Admission* a = c->keys ? c->keys->adm : nullptr;
+    const Admission* a = c->keys ? c->keys->adm.get() : nullptr;
     *min_count = a ? a->min_count : 0;
     *log2_width = a ? a->lw : 0;
     return a != nullptr;
 }
 
 int keys_admission_download(lctr_ctx* c, std::vector<uint32_t>& sketch) {
-    const Admission* a = c->keys->adm;
+    const Admission* a = c->keys->adm.get();
     sketch.resize((size_t)kSketchDepth << a->lw);
     LCTR_CUDA(cudaMemcpyAsync(sketch.data(), a->sketch, sketch.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -1247,7 +1197,7 @@ int keys_admission_download(lctr_ctx* c, std::vector<uint32_t>& sketch) {
 }
 
 int keys_admission_restore(lctr_ctx* c, const uint32_t* sketch) {
-    Admission* a = c->keys->adm;
+    Admission* a = c->keys->adm.get();
     LCTR_CUDA(cudaMemcpyAsync(a->sketch, sketch, ((size_t)kSketchDepth << a->lw) * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     a->dropped = a->admitted = a->pending = 0;
@@ -1256,7 +1206,7 @@ int keys_admission_restore(lctr_ctx* c, const uint32_t* sketch) {
 
 // the m rows of the device table's eviction list appended to the tier at rows [n, n + m), keys claimed in its index
 static int tier_spill(lctr_ctx* c, const EvTable& dev, size_t m) {
-    HostTier* h = c->keys->tier;
+    HostTier* h = c->keys->tier.get();
     KeyIndex& ix = h->ix;
     LCTR_CUDA(cudaMemsetAsync(ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
     if (launch(c, {warp_grid(c, m), 256, 0, c->stream}, by_rowlen(c, tier_spill_kernel<true>, tier_spill_kernel<false>), dev.rows,
@@ -1339,7 +1289,7 @@ int lctr_upload_keyed_params(lctr_ctx* c, int64_t n, const uint64_t* keys, const
 
 // the keys of one rank's table (all of them on one GPU), validated by the caller
 static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* keys, const float* W, const float* V) {
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     if (lookup_dev(c, keys, n)) return 1;
     std::vector<int64_t> rows((size_t)n);
@@ -1380,20 +1330,16 @@ static int upload_keyed_params_local(lctr_ctx* c, int64_t n, const uint64_t* key
             return 1;
     }
     if (W || V) {
-        float *dW = nullptr, *dV = nullptr;
-        if (W) {
-            if (dalloc(&dW, (size_t)n)) return 1;
-            LCTR_CUDA(cudaMemcpyAsync(dW, W, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-        }
-        if (V) {
-            if (dalloc(&dV, (size_t)n * c->rowlen)) return 1;
-            LCTR_CUDA(cudaMemcpyAsync(dV, V, (size_t)n * c->rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-        }
-        // the staging is freed before an error returns
-        const int rc = launch(c, {warp_grid(c, (size_t)n), 256, 0, c->stream}, key_scatter_params_kernel, t->d_rows, n, dW, dV,
-                              c->W, c->V, c->rowlen);
-        cudaStreamSynchronize(c->stream);
-        dfree(dW); dfree(dV);
+        Buf<float> dW, dV;
+        if (dW.alloc(W ? (size_t)n : 0) || dV.alloc(V ? (size_t)n * c->rowlen : 0)) return 1;
+        auto scatter = [&]() -> int {
+            if (W) LCTR_CUDA(cudaMemcpyAsync(dW, W, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+            if (V) LCTR_CUDA(cudaMemcpyAsync(dV, V, (size_t)n * c->rowlen * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+            return launch(c, {warp_grid(c, (size_t)n), 256, 0, c->stream}, key_scatter_params_kernel, t->d_rows, n, dW, dV, c->W,
+                          c->V, c->rowlen);
+        };
+        const int rc = scatter();
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the queued work reads the staging, which goes with this block
         if (rc) return 1;
     }
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -1416,26 +1362,25 @@ int lctr_set_key_admission(lctr_ctx* c, uint32_t min_count, uint32_t log2_width)
                                   "built before the owners translate, so it cannot drop entries)", c->cfg.world);
     LCTR_CHECK(c->cfg.model != LCTR_MODEL_WND, "lctr_set_key_admission: Wide&Deep reads the first id of each field, and dropping "
                                                "entries would change which id that is");
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     if (min_count <= 1) {  // off: the context behaves and launches as one that never set it
-        admission_free(t);
+        t->adm.reset();
         return 0;
     }
     LCTR_CHECK(log2_width >= 10 && log2_width <= 28, "lctr_set_key_admission: log2_width = %u outside [10, 28]", log2_width);
     if (!t->adm || t->adm->lw != log2_width) {
-        admission_free(t);
-        Admission* a = new Admission();
-        t->adm = a;
+        t->adm.reset();
+        auto a = std::make_unique<Admission>();
         a->lw = log2_width;
-        if (dalloc(&a->sketch, (size_t)kSketchDepth << log2_width) || dalloc(&a->cnt, 3) ||
-            cudaMallocHost((void**)&a->h_cnt, 2 * sizeof(unsigned long long)) != cudaSuccess) {
-            admission_free(t);
-            LCTR_CHECK(false, "lctr_set_key_admission: cannot allocate a sketch of %llu bytes (admission is off)",
-                       (unsigned long long)(((size_t)kSketchDepth << log2_width) * sizeof(uint32_t)));
+        if (a->sketch.alloc((size_t)kSketchDepth << log2_width) || a->cnt.alloc(3) || a->h_cnt.alloc(2)) {
+            set_error("lctr_set_key_admission: cannot allocate a sketch of %llu bytes (admission is off)",
+                      (unsigned long long)(((size_t)kSketchDepth << log2_width) * sizeof(uint32_t)));
+            return 1;
         }
+        t->adm = std::move(a);
     }
-    Admission* a = t->adm;
+    Admission* a = t->adm.get();
     a->min_count = min_count;
     a->dropped = a->admitted = a->pending = 0;
     LCTR_CUDA(cudaMemsetAsync(a->sketch, 0, ((size_t)kSketchDepth << a->lw) * sizeof(uint32_t), c->stream));
@@ -1448,9 +1393,9 @@ int lctr_decay_key_admission(lctr_ctx* c, uint32_t shift) {
     LCTR_CHECK(c->keys && c->keys->adm, "lctr_decay_key_admission: admission is off (lctr_set_key_admission with min_count > 1 "
                                         "turns it on)");
     LCTR_CHECK(shift >= 1 && shift <= 32, "lctr_decay_key_admission: shift = %u outside [1, 32]", shift);
-    const Admission* a = c->keys->adm;
+    const Admission* a = c->keys->adm.get();
     const size_t n4 = ((size_t)kSketchDepth << a->lw) / 4;
-    if (launch(c, {stride_grid(c, n4), 256, 0, c->stream}, sketch_decay_kernel, reinterpret_cast<uint4*>(a->sketch), n4, shift))
+    if (launch(c, {stride_grid(c, n4), 256, 0, c->stream}, sketch_decay_kernel, reinterpret_cast<uint4*>(a->sketch.get()), n4, shift))
         return 1;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
@@ -1459,7 +1404,7 @@ int lctr_decay_key_admission(lctr_ctx* c, uint32_t shift) {
 int lctr_key_admission_stats(lctr_ctx* c, uint64_t* dropped_entries, uint64_t* admitted_keys) {
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(c->keys, "lctr_key_admission_stats: the context was not created with key_mode = LCTR_KEYS_HASHED");
-    const Admission* a = c->keys->adm;
+    const Admission* a = c->keys->adm.get();
     if (dropped_entries) *dropped_entries = a ? a->dropped : 0;
     if (admitted_keys) *admitted_keys = a ? a->admitted : 0;
     return 0;
@@ -1470,7 +1415,7 @@ int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t*
     LCTR_CHECK(c && n_evicted, "null argument");
     LCTR_CHECK(c->keys, "lctr_evict_keys: the context was not created with key_mode = LCTR_KEYS_HASHED");
     LCTR_CHECK(c->keys->last_seen, "lctr_evict_keys: the context was not created with key_evict = 1 (rows record no last use)");
-    KeyTable* t = c->keys;
+    KeyTable* t = c->keys.get();
     *n_evicted = 0;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     int rc = 0;
@@ -1486,7 +1431,7 @@ int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t*
     const bool exporting = keys_out || W_out || V_out;
     LCTR_CHECK(!exporting || cap_out >= m, "lctr_evict_keys: room for %llu evicted rows, %zu would leave (nothing was changed)",
                (unsigned long long)cap_out, m);
-    HostTier* h = t->tier;
+    HostTier* h = t->tier.get();
     LCTR_CHECK(!h || h->n + m <= h->cap, "lctr_evict_keys: %zu rows would leave for the host tier, which holds %zu rows "
                "(cfg.key_host_rows) with %zu free (nothing was changed)", m, h ? h->cap : 0, h ? h->cap - h->n : 0);
     const size_t n_live = n - m;
@@ -1510,38 +1455,40 @@ int lctr_evict_host_tier(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint
                          uint64_t cap_out, uint64_t* n_evicted) {
     LCTR_CHECK(c && n_evicted, "null argument");
     LCTR_CHECK(c->keys && c->keys->tier, "lctr_evict_host_tier: the context was not created with a host tier (cfg.key_host_rows)");
-    HostTier* h = c->keys->tier;
+    HostTier* h = c->keys->tier.get();
     *n_evicted = 0;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     const size_t n = h->n;
     if (n == 0) return 0;
-    if (!c->keys->h_res && evict_scratch(c->keys, c->keys->cap)) return 1;
+    if (!c->keys->h_res && evict_scratch(c->keys.get(), c->keys->cap)) return 1;
     // scratch of the tier's size for this call only: a tier eviction reads every tier row anyway
-    struct Scratch {
-        uint32_t *scan = nullptr, *rows = nullptr, *tiles = nullptr;
-        ~Scratch() { cudaFree(scan); cudaFree(rows); cudaFree(tiles); }
-    } sc;
-    if (dalloc(&sc.scan, n + 1) || dalloc(&sc.rows, n) || dalloc(&sc.tiles, n / kEvTile + 1)) return 1;
-    const EvTable tb{h->a, n, sc.scan, sc.rows, sc.tiles};
-    EvictRule e;
-    size_t m = 0;
-    if (evict_plan(c, tb, max_idle, max_rows, &e, &m)) return 1;
-    if (m == 0) return 0;
-    LCTR_CHECK(!(keys_out || W_out || V_out) || cap_out >= m,
-               "lctr_evict_host_tier: room for %llu evicted rows, %zu would leave (nothing was changed)", (unsigned long long)cap_out, m);
-    if (evict_index_export(c, tb, e, m, keys_out, W_out, V_out)) return 1;
-    if (launch_move(c, h->a, n - m, n, sc.scan + (n - m), sc.rows)) return 1;
-    h->n = n - m;
-    if (tier_rebuild(c)) return 1;
-    *n_evicted = m;
-    return 0;
+    Buf<uint32_t> scan, rows, tiles;
+    if (scan.alloc(n + 1) || rows.alloc(n) || tiles.alloc(n / kEvTile + 1)) return 1;
+    auto evict = [&]() -> int {
+        const EvTable tb{h->a, n, scan, rows, tiles};
+        EvictRule e;
+        size_t m = 0;
+        if (evict_plan(c, tb, max_idle, max_rows, &e, &m)) return 1;
+        if (m == 0) return 0;
+        LCTR_CHECK(!(keys_out || W_out || V_out) || cap_out >= m,
+                   "lctr_evict_host_tier: room for %llu evicted rows, %zu would leave (nothing was changed)", (unsigned long long)cap_out, m);
+        if (evict_index_export(c, tb, e, m, keys_out, W_out, V_out)) return 1;
+        if (launch_move(c, h->a, n - m, n, scan + (n - m), rows)) return 1;
+        h->n = n - m;
+        if (tier_rebuild(c)) return 1;
+        *n_evicted = m;
+        return 0;
+    };
+    const int rc = evict();
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the queued work reads the scratch, which goes on return
+    return rc;
 }
 
 int lctr_download_host_tier(lctr_ctx* c, uint64_t* keys, float* W, float* V, uint64_t cap, uint64_t* n_rows) {
     LCTR_CHECK(c && n_rows, "null argument");
     LCTR_CHECK(c->keys && c->keys->tier, "lctr_download_host_tier: the context was not created with a host tier (cfg.key_host_rows)");
     LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the tier's rows change only on the ctx stream
-    const HostTier* h = c->keys->tier;
+    const HostTier* h = c->keys->tier.get();
     *n_rows = h->n;
     if (!keys && !W && !V) return 0;
     LCTR_CHECK(cap >= h->n, "lctr_download_host_tier: room for %llu rows, the tier holds %zu", (unsigned long long)cap, h->n);

@@ -131,39 +131,27 @@ __global__ void auc_chain_kernel(const uint2* __restrict__ list, const unsigned 
 }
 
 struct AucScratch {
-    unsigned int *pos = nullptr, *neg = nullptr, *tile_cnt = nullptr, *tile_off = nullptr, *total = nullptr;
-    uint2* list = nullptr;
+    Buf<unsigned int> pos, neg, tile_cnt, tile_off, total;
+    Buf<uint2> list;
     size_t list_cap = 0;
-    float* out = nullptr;
-    float *in_pred = nullptr, *in_label = nullptr;  // lctr_eval_pred: the caller's arrays on the device
+    Buf<float> out;
+    Buf<float> in_pred, in_label;  // lctr_eval_pred: the caller's arrays on the device
     size_t in_cap = 0;
 };
-
-void metrics_free(lctr_ctx* c) {
-    AucScratch* a = (AucScratch*)c->auc_scratch;
-    if (!a) return;
-    cudaFree(a->pos); cudaFree(a->neg); cudaFree(a->tile_cnt); cudaFree(a->tile_off); cudaFree(a->total);
-    cudaFree(a->list); cudaFree(a->out); cudaFree(a->in_pred); cudaFree(a->in_label);
-    delete a;
-    c->auc_scratch = nullptr;
-}
+void drop(AucScratch* p) { delete p; }
 
 static int auc_scratch(lctr_ctx* c, AucScratch** out) {
-    AucScratch* a = (AucScratch*)c->auc_scratch;
-    if (!a) {
-        a = new AucScratch();
-        c->auc_scratch = a;
-        const size_t hb = (size_t)(kHashLen + 1) * sizeof(unsigned int);
-        LCTR_CUDA(cudaMalloc((void**)&a->pos, hb));
-        LCTR_CUDA(cudaMalloc((void**)&a->neg, hb));
-        LCTR_CUDA(cudaMemsetAsync(a->pos, 0, hb, c->stream));
-        LCTR_CUDA(cudaMemsetAsync(a->neg, 0, hb, c->stream));
-        LCTR_CUDA(cudaMalloc((void**)&a->tile_cnt, kAucTiles * sizeof(unsigned int)));
-        LCTR_CUDA(cudaMalloc((void**)&a->tile_off, kAucTiles * sizeof(unsigned int)));
-        LCTR_CUDA(cudaMalloc((void**)&a->total, sizeof(unsigned int)));
-        LCTR_CUDA(cudaMalloc((void**)&a->out, 4 * sizeof(float)));
+    if (!c->auc_scratch) {
+        Owned<AucScratch> a(new AucScratch());  // the context's only once complete
+        const size_t hn = (size_t)(kHashLen + 1);
+        if (a->pos.alloc(hn) || a->neg.alloc(hn) || a->tile_cnt.alloc(kAucTiles) || a->tile_off.alloc(kAucTiles) ||
+            a->total.alloc(1) || a->out.alloc(4))
+            return 1;
+        LCTR_CUDA(cudaMemsetAsync(a->pos, 0, hn * sizeof(unsigned int), c->stream));
+        LCTR_CUDA(cudaMemsetAsync(a->neg, 0, hn * sizeof(unsigned int), c->stream));
+        c->auc_scratch = std::move(a);
     }
-    *out = a;
+    *out = c->auc_scratch.get();
     return 0;
 }
 
@@ -173,10 +161,8 @@ static int eval_device(lctr_ctx* c, AucScratch* a, const float* pred, const floa
                        int64_t* correct, float* auc) {
     if ((size_t)n > a->list_cap) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        if (a->list) cudaFree(a->list);
-        a->list = nullptr;
         a->list_cap = 0;
-        LCTR_CUDA(cudaMalloc((void**)&a->list, (size_t)(n + 32) * sizeof(uint2)));
+        if (alloc_group(sized(a->list, (size_t)(n + 32)))) return 1;
         a->list_cap = (size_t)n;
     }
     if (launch(c, {(unsigned)((n + 255) / 256), 256, 0, c->stream}, auc_hist_kernel, pred, label, n, a->pos, a->neg) ||
@@ -219,11 +205,8 @@ int lctr_eval_pred(lctr_ctx* c, int64_t n, const float* pctr, const int32_t* lab
     if (auc_scratch(c, &a)) return 1;
     if ((size_t)n > a->in_cap) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        cudaFree(a->in_pred); cudaFree(a->in_label);
-        a->in_pred = a->in_label = nullptr;
         a->in_cap = 0;
-        LCTR_CUDA(cudaMalloc((void**)&a->in_pred, (size_t)n * sizeof(float)));
-        LCTR_CUDA(cudaMalloc((void**)&a->in_label, (size_t)n * sizeof(float)));
+        if (alloc_group(sized(a->in_pred, (size_t)n), sized(a->in_label, (size_t)n))) return 1;
         a->in_cap = (size_t)n;
     }
     std::vector<float> y((size_t)n);  // as upload_batch widens them: (float) of the int32 label

@@ -132,17 +132,13 @@ int mlp_alloc(lctr_ctx* c) {
         in = L.out;
     }
     c->dense_grad_n = total;
-    LCTR_CUDA(cudaMalloc((void**)&c->dense_grad, total * sizeof(float)));
+    if (c->dense_grad.alloc(total)) return 1;
     LCTR_CUDA(cudaMemsetAsync(c->dense_grad, 0, total * sizeof(float), c->stream));
     size_t off = 0;
     for (int l = 0; l < c->n_layers; l++) {
         MlpLayer& L = c->layers[l];
         const size_t nw = (size_t)L.out * L.in;
-        LCTR_CUDA(cudaMalloc((void**)&L.w, nw * sizeof(float)));
-        LCTR_CUDA(cudaMalloc((void**)&L.b, L.out * sizeof(float)));
-        LCTR_CUDA(cudaMalloc((void**)&L.mask, L.out * sizeof(float)));
-        LCTR_CUDA(cudaMalloc((void**)&L.acc_w, nw * sizeof(float)));
-        LCTR_CUDA(cudaMalloc((void**)&L.acc_b, L.out * sizeof(float)));
+        if (L.w.alloc(nw) || L.b.alloc(L.out) || L.mask.alloc(L.out) || L.acc_w.alloc(nw) || L.acc_b.alloc(L.out)) return 1;
         LCTR_CUDA(cudaMemsetAsync(L.w, 0, nw * sizeof(float), c->stream));
         LCTR_CUDA(cudaMemsetAsync(L.b, 0, L.out * sizeof(float), c->stream));
         LCTR_CUDA(cudaMemsetAsync(L.acc_w, 0, nw * sizeof(float), c->stream));
@@ -159,35 +155,20 @@ int mlp_alloc(lctr_ctx* c) {
     return 0;
 }
 
-int mlp_free(lctr_ctx* c) {
-    for (int l = 0; l < c->n_layers; l++) {
-        MlpLayer& L = c->layers[l];
-        if (L.w) cudaFree(L.w); if (L.b) cudaFree(L.b); if (L.mask) cudaFree(L.mask);
-        if (L.acc_w) cudaFree(L.acc_w); if (L.acc_b) cudaFree(L.acc_b);
-        if (L.act) cudaFree(L.act); if (L.delta) cudaFree(L.delta); if (L.w16) cudaFree(L.w16); if (L.w16t) cudaFree(L.w16t);
-        L = MlpLayer();
-    }
-    if (c->dense_grad) cudaFree(c->dense_grad);
-    if (c->z) cudaFree(c->z); if (c->dz) cudaFree(c->dz); if (c->mlp_out) cudaFree(c->mlp_out);
-    c->dense_grad = c->z = c->dz = c->mlp_out = nullptr;
-    c->n_layers = 0;
-    return 0;
-}
-
 int mlp_reserve(lctr_ctx* c, int64_t rows) {
     if ((size_t)rows <= c->mlp_cap_rows) return 0;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     const size_t cap = (size_t)rows;
     const size_t k = mlp_in0(c->cfg);
-    if (c->z) cudaFree(c->z); if (c->dz) cudaFree(c->dz); if (c->mlp_out) cudaFree(c->mlp_out);
-    LCTR_CUDA(cudaMalloc((void**)&c->z, cap * k * sizeof(float)));
-    LCTR_CUDA(cudaMalloc((void**)&c->dz, cap * k * sizeof(float)));
-    LCTR_CUDA(cudaMalloc((void**)&c->mlp_out, cap * sizeof(float)));
+    c->mlp_cap_rows = 0;
+    if (alloc_group(sized(c->z, cap * k), sized(c->dz, cap * k), sized(c->mlp_out, cap))) return 1;
     for (int l = 0; l < c->n_layers && c->cfg.mlp_precision == LCTR_MLP_FP32; l++) {  // bf16 mode keeps activations on chip
         MlpLayer& L = c->layers[l];
-        if (L.act) cudaFree(L.act); if (L.delta) cudaFree(L.delta);
-        LCTR_CUDA(cudaMalloc((void**)&L.act, cap * L.out * sizeof(float)));
-        LCTR_CUDA(cudaMalloc((void**)&L.delta, cap * (size_t)std::max(L.out, L.in) * sizeof(float)));
+        if (alloc_group(sized(L.act, cap * L.out), sized(L.delta, cap * (size_t)std::max(L.out, L.in)))) {
+            for (MlpLayer& M : c->layers) { M.act.reset(); M.delta.reset(); }  // the whole group goes
+            c->z.reset(); c->dz.reset(); c->mlp_out.reset();
+            return 1;
+        }
     }
     c->mlp_cap_rows = cap;
     return 0;
@@ -232,7 +213,7 @@ static int mlp_backward_dev(lctr_ctx* c, int B) {
         float* dx = l == 0 ? c->dz : c->layers[l - 1].delta;
         if (launch(c, {mlp_blocks((int64_t)B * L.out), 256, 0, c->stream}, clip_kernel, L.delta, (int64_t)B * L.out) ||
             launch(c, {mlp_blocks((int64_t)B * L.in), 256, 0, c->stream}, fc_input_delta_kernel, L.delta, L.w, L.mask,
-                   l > 0 ? c->layers[l - 1].act : nullptr, dx, B, L.in, L.out, has_next ? 1 : 0, c->cfg.activation) ||
+                   l > 0 ? c->layers[l - 1].act.get() : nullptr, dx, B, L.in, L.out, has_next ? 1 : 0, c->cfg.activation) ||
             launch(c, {mlp_blocks((int64_t)L.out * (L.in + 1)), 256, 0, c->stream}, fc_weight_grad_kernel, xin, L.delta, L.dw, L.db,
                    B, L.in, L.out))
             return 1;

@@ -408,8 +408,9 @@ int mlp_bf16_prepare(lctr_ctx* c) {
         LCTR_CHECK(c->layers[l].in % 16 == 0 && c->layers[l].in <= 512,
                    "bf16 MLP: layer %d input width %d must be a multiple of 16 (<= 512)", l, c->layers[l].in);
         if (l < nh && !c->layers[l].w16) {
-            LCTR_CUDA(cudaMalloc((void**)&c->layers[l].w16, (size_t)c->layers[l].out * c->layers[l].in * 2));
-            LCTR_CUDA(cudaMalloc((void**)&c->layers[l].w16t, (size_t)c->layers[l].out * c->layers[l].in * 2));
+            if (c->layers[l].w16.alloc((size_t)c->layers[l].out * c->layers[l].in) ||
+                c->layers[l].w16t.alloc((size_t)c->layers[l].out * c->layers[l].in))
+                return 1;
         }
     }
     c->mlp_umma = mlp_umma_supported(c) ? 1 : 0;
@@ -428,8 +429,7 @@ int mlp_bf16_refresh(lctr_ctx* c, int layer) {
     MlpLayer& L = c->layers[layer];
     if (!L.w16) return 0;
     const size_t n = (size_t)L.out * L.in;
-    return launch(c, {(unsigned)((n + 255) / 256), 256, 0, c->stream}, to_bf16_kernel, L.w, (__nv_bfloat16*)L.w16,
-                  (__nv_bfloat16*)L.w16t, L.in, L.out, n);
+    return launch(c, {(unsigned)((n + 255) / 256), 256, 0, c->stream}, to_bf16_kernel, L.w, L.w16, L.w16t, L.in, L.out, n);
 }
 
 int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor) {
@@ -441,7 +441,7 @@ int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t ro
     P.nl = nl; P.act = c->cfg.activation; P.has_mask = c->mlp_has_mask;
     for (int l = 0; l < nl; l++) {
         MlpLayer& L = c->layers[l];
-        P.w16[l] = (const __nv_bfloat16*)L.w16; P.bias[l] = L.b; P.mask[l] = L.mask; P.dw[l] = L.dw; P.db[l] = L.db;
+        P.w16[l] = L.w16; P.bias[l] = L.b; P.mask[l] = L.mask; P.dw[l] = L.dw; P.db[l] = L.db;
     }
     P.w32_last = c->layers[nh].w;
     double* out_slot = c->stats + 2 * (c->step % kStatRing);
@@ -463,8 +463,8 @@ int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t ro
         size_t off = 0;
         for (int l = 0; l < nl; l++) {
             MlpLayer& L = c->layers[l];
-            S.off[2 * l] = off; S.w[2 * l] = L.w; S.acc[2 * l] = L.acc_w; S.w16[2 * l] = (__nv_bfloat16*)L.w16;
-            S.w16t[2 * l] = (__nv_bfloat16*)L.w16t; S.in[2 * l] = L.in; S.out[2 * l] = L.out;
+            S.off[2 * l] = off; S.w[2 * l] = L.w; S.acc[2 * l] = L.acc_w; S.w16[2 * l] = L.w16;
+            S.w16t[2 * l] = L.w16t; S.in[2 * l] = L.in; S.out[2 * l] = L.out;
             S.w16t[2 * l + 1] = nullptr; S.in[2 * l + 1] = 1; S.out[2 * l + 1] = L.out;
             off += (size_t)L.out * L.in;
             S.off[2 * l + 1] = off; S.w[2 * l + 1] = L.b; S.acc[2 * l + 1] = L.acc_b; S.w16[2 * l + 1] = nullptr;

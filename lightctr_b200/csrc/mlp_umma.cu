@@ -496,7 +496,7 @@ int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot) {
     P.act = c->cfg.activation;
     for (int l = 0; l < nl; l++) {
         MlpLayer& L = c->layers[l];
-        P.w16t[l] = (const __nv_bfloat16*)L.w16t; P.bias[l] = L.b; P.dw[l] = L.dw; P.db[l] = L.db;
+        P.w16t[l] = L.w16t; P.bias[l] = L.b; P.dw[l] = L.dw; P.db[l] = L.db;
     }
     P.w32_last = c->layers[nh].w;
     P.trace = nullptr;

@@ -94,16 +94,10 @@ wnd_backward_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restr
 int wnd_reserve(lctr_ctx* c, int64_t rows) {
     if ((size_t)rows <= c->wnd_cap_rows) return 0;
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    if (c->wnd_src) cudaFree(c->wnd_src);
-    c->wnd_src = nullptr; c->wnd_cap_rows = 0;
-    LCTR_CUDA(cudaMalloc((void**)&c->wnd_src, (size_t)rows * c->cfg.field_cnt * sizeof(uint32_t)));
+    c->wnd_cap_rows = 0;
+    if (alloc_group(sized(c->wnd_src, (size_t)rows * c->cfg.field_cnt))) return 1;
     c->wnd_cap_rows = (size_t)rows;
     return 0;
-}
-
-void wnd_free(lctr_ctx* c) {
-    if (c->wnd_src) cudaFree(c->wnd_src);
-    c->wnd_src = nullptr; c->wnd_cap_rows = 0;
 }
 
 int launch_wnd_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
@@ -112,7 +106,7 @@ int launch_wnd_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     LCTR_CHECK(s.has_field, "Wide&Deep batch uploaded without the field array");
     ProfScope prof(c, PROF_FM_FWD);
     return launch(c, {(unsigned)((rows + 7) / 8), 256, 0, c->stream}, wnd_forward_kernel, s.row_ptr,
-                  c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.has_val ? s.val : nullptr, c->cW, c->cV, (int)c->cfg.field_cnt,
+                  c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.has_val ? s.val.get() : nullptr, c->cW, c->cV, (int)c->cfg.field_cnt,
                   (int)c->cfg.factor_cnt, c->z, c->wnd_src, s.wide, rb, re);
 }
 
@@ -131,8 +125,8 @@ int launch_wnd_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     if (rows <= 0) return 0;
     ProfScope prof(c, PROF_FM_BWD_RED);
     return launch(c, {(unsigned)((rows + 7) / 8), 256, 0, c->stream}, wnd_backward_kernel, s.row_ptr,
-                  c->cfg.world > 1 ? s.ent_pslot : s.fid, s.has_val ? s.val : nullptr, s.label, s.pred, c->cW, c->wnd_src, c->dz,
-                  (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched,
+                  c->cfg.world > 1 ? s.ent_pslot : s.fid, s.has_val ? s.val.get() : nullptr, s.label, s.pred, c->cW, c->wnd_src, c->dz,
+                  (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(),
                   c->cfg.l2_reg, rb, re);
 }
 
