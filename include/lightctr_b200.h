@@ -378,6 +378,41 @@ typedef struct lctr_keyed_dataset {
 } lctr_keyed_dataset;
 int lctr_load_libffm_keys(const char* path, uint64_t field_cnt_in, lctr_keyed_dataset** out);
 int lctr_free_keyed_dataset(lctr_keyed_dataset* d);
+/* ---- libffm text parsed on the device ------------------------------------------------------------ */
+/* Parses libffm text into `slot` on the GPU.  Split a text T at line boundaries into calls, LCTR_TEXT_BEGIN on the first
+ * and LCTR_TEXT_END on the last: the slots of the calls, concatenated in call order, hold bit for bit what
+ * lctr_load_libffm(T) + lctr_upload_batch give (row_ptr rebased per slot, ids, fields, value bits, the first `rows`
+ * labels); keyed contexts: lctr_load_libffm_keys(T) + lctr_upload_batch_keys.  The reference parser's quirks carry across
+ * calls: a line with a label but no features is dropped while its label is kept, shifting every later row's label; a
+ * two-field token keeps the value of the token before it, also from an earlier line or call.  Lines that a token outside
+ * the fast grammar (`digits:digits:plain-decimal`, <= 18 digits per id, label <= 9 digits) makes the device decline
+ * are parsed by the host parser, in order (info->host_lines counts them).  A slot whose values are all exactly 1.0f
+ * stores no val array, as lctr_upload_batch(val = NULL).
+ * Errors name the line (counted from 1 at LCTR_TEXT_BEGIN): those lctr_load_libffm raises (an id >= 2^32 on a dense
+ * context, a field >= 2^16), then those of the upload (field >= field_cnt for FFM / Wide&Deep, fid >= feature_cnt, the
+ * reserved key).  After a failed call the parser state is unchanged and the slot holds no usable batch; keys inserted
+ * before the failure keep their rows.  Text after the last '\n' is not consumed unless LCTR_TEXT_END is set.  The call
+ * ends in a stream synchronise, so `text` (pinned memory copies fastest) may be reused when it returns.
+ * Refused: world > 1, deterministic = 1 (its feature-major view is built on the host from host arrays), a slot out of
+ * range, LCTR_TEXT_LOOKUP on a dense context.  Not covered: multi-GPU text uploads, the exact-order mode
+ * (deterministic = 1), overlapping text uploads with steps (lctr_train_batch_async takes host CSR), FM_Predict's own
+ * test-set loader quirks (its first feature dropped); the host shims keep lctr_load_libffm. */
+#define LCTR_TEXT_BEGIN 1  /* this text starts a file: reset the state the reference's loop carries across lines */
+#define LCTR_TEXT_END 2    /* this text ends the file: a last line without '\n' is parsed too */
+#define LCTR_TEXT_LOOKUP 4 /* keyed contexts: insert = 0 (unseen keys -> the null row), as lctr_upload_batch_keys */
+typedef struct lctr_text_info {
+    int64_t rows, nnz;               /* what the slot now holds */
+    int64_t lines, labels;           /* lines consumed; labels parsed from them */
+    uint64_t feature_cnt, field_cnt; /* max id + 1, max field + 1 over the consumed lines (0 without entries) */
+    int64_t host_lines;              /* lines the device grammar declined, parsed by the host parser */
+    size_t consumed;                 /* bytes consumed: whole lines only */
+} lctr_text_info;
+int lctr_upload_libffm(lctr_ctx* ctx, int slot, const char* text, size_t bytes, int flags, lctr_text_info* info);
+/* a slot read back: *rows / *nnz, row_ptr [rows + 1], fid [nnz] (rows of the key table on keyed contexts), field [nnz]
+ * (zeros when the slot has none), val [nnz] (1.0f when it has no val array), label [rows] as the floats the slot holds.
+ * Any pointer may be NULL; query the sizes first. */
+int lctr_download_batch(lctr_ctx* ctx, int slot, int64_t* rows, int64_t* nnz, int64_t* row_ptr, uint32_t* fid,
+                        uint16_t* field, float* val, float* label);
 /* binary CSR cache of a parsed file: the sscanf-per-token parse is paid once (SURVEY.md 8f-2) */
 int lctr_save_dataset_bin(const lctr_dataset* d, const char* path);
 int lctr_load_dataset_bin(const char* path, lctr_dataset** out);

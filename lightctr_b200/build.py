@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "liblightctr_b200.so")
-SOURCES = ["capi.cu", "fm.cu", "fm_fused.cu", "ffm.cu", "ffm_warp.cu", "ffm_grouped.cu", "opt.cu", "mlp.cu", "mlp_bf16.cu", "mlp_umma.cu", "dist.cu", "csc.cu", "checkpoint.cu", "metrics.cu", "wnd.cu", "keys.cu", "loader.cpp"]
+SOURCES = ["capi.cu", "fm.cu", "fm_fused.cu", "ffm.cu", "ffm_warp.cu", "ffm_grouped.cu", "opt.cu", "mlp.cu", "mlp_bf16.cu", "mlp_umma.cu", "dist.cu", "csc.cu", "checkpoint.cu", "metrics.cu", "wnd.cu", "keys.cu", "text.cu", "loader.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false: the reference is built without FMA (-mavx only, Makefile:3); keeping mul and add
 # separately rounded keeps per-coordinate updates comparable bit-for-bit.  All kernels here are

@@ -34,9 +34,10 @@ SYMBOLS = [
     "lctr_upload_batch_keys", "lctr_lookup_keys", "lctr_download_keys", "lctr_upload_keyed_params", "lctr_set_key_init",
     "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys", "lctr_load_checkpoint_shards", "lctr_eval_pred",
     "lctr_download_host_tier", "lctr_evict_host_tier", "lctr_set_key_admission", "lctr_decay_key_admission",
-    "lctr_key_admission_stats",
+    "lctr_key_admission_stats", "lctr_upload_libffm", "lctr_download_batch",
 ]
 NO_LIMIT = (1 << 64) - 1  # lctr_evict_keys: UINT64_MAX = no limit
+TEXT_BEGIN, TEXT_END, TEXT_LOOKUP = 1, 2, 4  # lctr_upload_libffm flags
 
 
 class Cfg(C.Structure):
@@ -65,6 +66,12 @@ class KeyedDatasetC(C.Structure):
     _fields_ = [("rows", C.c_int64), ("nnz", C.c_int64), ("label_cnt", C.c_int64), ("field_cnt", C.c_uint64),
                 ("row_ptr", C.POINTER(C.c_int64)), ("key", C.POINTER(C.c_uint64)), ("field", C.POINTER(C.c_uint16)),
                 ("val", C.POINTER(C.c_float)), ("label", C.POINTER(C.c_int32))]
+
+
+class TextInfo(C.Structure):
+    """lctr_text_info: what one lctr_upload_libffm call parsed"""
+    _fields_ = [("rows", C.c_int64), ("nnz", C.c_int64), ("lines", C.c_int64), ("labels", C.c_int64),
+                ("feature_cnt", C.c_uint64), ("field_cnt", C.c_uint64), ("host_lines", C.c_int64), ("consumed", C.c_size_t)]
 
 
 _lib = None
@@ -137,6 +144,8 @@ def load_library():
     L.lctr_set_key_admission.argtypes = [vp, C.c_uint32, C.c_uint32]
     L.lctr_decay_key_admission.argtypes = [vp, C.c_uint32]
     L.lctr_key_admission_stats.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    L.lctr_upload_libffm.argtypes = [vp, C.c_int, vp, C.c_size_t, C.c_int, C.POINTER(TextInfo)]
+    L.lctr_download_batch.argtypes = [vp, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64), vp, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -429,6 +438,28 @@ class Context:
         _chk(self.L.lctr_key_admission_stats(self.h, C.byref(d), C.byref(a)))
         return d.value, a.value
 
+    def upload_libffm(self, slot, data, begin=True, end=True, lookup=False):
+        """libffm text (bytes or any buffer; pinned memory copies fastest) parsed into `slot` on the device -> TextInfo.
+        Consecutive calls continue one file: begin=True on its first part, end=True on its last."""
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        flags = (TEXT_BEGIN if begin else 0) | (TEXT_END if end else 0) | (TEXT_LOOKUP if lookup else 0)
+        info = TextInfo()
+        self.slot_rows[slot] = 0
+        _chk(self.L.lctr_upload_libffm(self.h, slot, buf.ctypes.data, len(data), flags, C.byref(info)))
+        self.slot_rows[slot] = info.rows
+        return info
+
+    def download_batch(self, slot):
+        """the slot read back -> (row_ptr, fid, field, val, label): fid holds table rows on keyed contexts, val is 1.0f
+        where the slot stores none, label the floats the slot trains on"""
+        rows, nnz = C.c_int64(), C.c_int64()
+        _chk(self.L.lctr_download_batch(self.h, slot, C.byref(rows), C.byref(nnz), None, None, None, None, None))
+        r, n = rows.value, nnz.value
+        row_ptr, fid, field = np.empty(r + 1, np.int64), np.empty(n, np.uint32), np.empty(n, np.uint16)
+        val, label = np.empty(n, np.float32), np.empty(r, np.float32)
+        _chk(self.L.lctr_download_batch(self.h, slot, None, None, *[a.ctypes.data for a in (row_ptr, fid, field, val, label)]))
+        return row_ptr, fid, field, val, label
+
     def upload_dataset(self, slot, ds, all_ones_as_null=True):
         val = ds.val
         if val is not None and all_ones_as_null and np.all(val == 1.0):
@@ -563,7 +594,7 @@ class Context:
 
     PROF_NAMES = ["fm_forward", "fm_backward_red", "apply", "ffm_fused", "fm_backward_csc", "mlp", "dist_mark", "dist_compact",
                   "dist_pull", "dist_push", "dist_barrier0", "dist_merge", "dist_barrier1", "csc_build", "fm_fused", "apply_compact",
-                  "keys_translate"]
+                  "keys_translate", "text_parse"]
 
     def profile(self, enable=True):
         _chk(self.L.lctr_profile(self.h, 1 if enable else 0))

@@ -167,6 +167,56 @@ static GradPath grad_path_of(const lctr_cfg& cf) {
         return GRAD_FEATURE_MAJOR;
     return GRAD_DENSE;
 }
+
+// room in the slot for a batch of rows x nnz; buffers are only reallocated once the stream has let go of them
+int slot_fit(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz) {
+    if (rows > s.cap_rows || nnz > s.cap_nnz || !s.row_ptr) {  // (!row_ptr: an empty first upload still has row_ptr[0])
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));  // buffers about to be reallocated may still be in use
+        if (slot_reserve(c, s, std::max<int64_t>(rows, 1), nnz)) return 1;
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    }
+    return 0;
+}
+
+// The end of every single-slot upload, once the batch sits in the slot (row_ptr, field, val; fid, or for `keyed` the rows
+// the translate wrote there; s.has_val / s.has_field set) and its int32 labels in s.pred: key admission's compaction, the
+// labels widened, the slot map, the grouping.  h_row_ptr / h_fid / h_val: the batch on the host, which only the host-built
+// view of deterministic = 1 reads.
+int upload_tail(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows, int64_t nnz, bool keyed, const int64_t* h_row_ptr,
+                const uint32_t* h_fid, const float* h_val) {
+    Slot& s = c->slots[slot];
+    if (keyed && c->keys) {  // key admission dropped entries: the slot holds the kept ones, before the slot map
+        if (keys_admission_compact(c, s, st, rows, &nnz)) return 1;
+        s.nnz = nnz;
+    }
+    const bool grouped = c->cfg.deterministic == 2 && rows > 0 && nnz > 0 && c->cfg.world == 1;
+    int32_t* tmp = reinterpret_cast<int32_t*>(s.pred.get());  // pred is overwritten by the next forward anyway
+    // labels travel as int32 and are widened on device (the reference compares a `float target`)
+    if (rows && !grouped && launch(c, {(unsigned)((rows + 255) / 256), 256, 0, st}, label_to_float_kernel, tmp, s.label, rows, nullptr))
+        return 1;
+    s.fused_valid = false;
+    s.key_state = SLOT_KEYS_OK;
+    if (c->grad_path == GRAD_COMPACT || c->cfg.world > 1) {
+        // slot map of the batch: the gradient rows of the compact path; on several GPUs also the key set of the pull / push
+        // exchange, whose per-owner lists go out right away (posted stores, overlapping the previous step).  An empty batch
+        // (0 rows or 0 entries) gets an empty map, and the compact gradient buffers are reserved all the same (a train step
+        // reads them).  On several GPUs it still posts its (empty) key lists: the peers' serve waits for every rank's lists
+        const bool empty = rows == 0 || nnz == 0;
+        if (fused_reserve(c, s, nnz) || fused_build_slot(c, s, st, nullptr, rows, nnz)) return 1;
+        if (c->cfg.world > 1 && (empty ? dist_send_empty(c, slot, st) : dist_send_keys(c, s, slot, st))) return 1;
+    }
+    s.csc_block = 0;
+    s.dev_csc = false;
+    if (grouped) {
+        LCTR_CHECK(csc_device_supported(c), "cfg.deterministic=2 (device-grouped backward) needs FM with k in {4,8,16,32} "
+                                            "or FFM with k %% 4 == 0 and field_cnt * k <= 512");
+        if (csc_build_device(c, s, st, tmp, nullptr, rows, nnz)) return 1;  // widens the labels in its first kernel
+    } else if (c->cfg.deterministic == 1 && c->cfg.model != LCTR_MODEL_FFM && rows > 0) {
+        LCTR_CUDA(cudaStreamSynchronize(st));
+        if (build_csc(c, s, rows, nnz, h_row_ptr, h_fid, h_val)) return 1;
+    }
+    return 0;
+}
 }  // namespace lctr
 
 using namespace lctr;
@@ -439,11 +489,7 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
     LCTR_CHECK((c->cfg.model != LCTR_MODEL_FFM && c->cfg.model != LCTR_MODEL_WND) || field || nnz == 0,
                "upload_batch: FFM / Wide&Deep need the field array");
     Slot& s = c->slots[slot];
-    if (rows > s.cap_rows || nnz > s.cap_nnz || !s.row_ptr) {  // (!row_ptr: an empty first upload still has row_ptr[0])
-        LCTR_CUDA(cudaStreamSynchronize(c->stream));  // buffers about to be reallocated may still be in use
-        if (slot_reserve(c, s, std::max<int64_t>(rows, 1), nnz)) return 1;
-        LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    }
+    if (slot_fit(c, s, rows, nnz)) return 1;
     s.rows = rows; s.nnz = nnz;
     s.has_val = val != nullptr;
     s.has_field = field != nullptr;
@@ -453,40 +499,8 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
         if (field) LCTR_CUDA(cudaMemcpyAsync(s.field, field, (size_t)nnz * sizeof(uint16_t), cudaMemcpyHostToDevice, st));
         if (val) LCTR_CUDA(cudaMemcpyAsync(s.val, val, (size_t)nnz * sizeof(float), cudaMemcpyHostToDevice, st));
     }
-    if (fid_resident && c->keys) {  // key admission dropped entries: the slot holds the kept ones, before the slot map
-        if (keys_admission_compact(c, s, st, rows, &nnz)) return 1;
-        s.nnz = nnz;
-    }
-    const bool grouped = c->cfg.deterministic == 2 && rows > 0 && nnz > 0 && c->cfg.world == 1;
-    int32_t* tmp = reinterpret_cast<int32_t*>(s.pred.get());  // pred is overwritten by the next forward anyway
-    if (rows) {
-        // labels travel as int32 and are widened on device (the reference compares a `float target`)
-        LCTR_CUDA(cudaMemcpyAsync(tmp, label, (size_t)rows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-        if (!grouped && launch(c, {(unsigned)((rows + 255) / 256), 256, 0, st}, label_to_float_kernel, tmp, s.label, rows, nullptr))
-            return 1;
-    }
-    s.fused_valid = false;
-    s.key_state = SLOT_KEYS_OK;
-    if (c->grad_path == GRAD_COMPACT || c->cfg.world > 1) {
-        // slot map of the batch: the gradient rows of the compact path; on several GPUs also the key set of the pull / push
-        // exchange, whose per-owner lists go out right away (posted stores, overlapping the previous step).  An empty batch
-        // (0 rows or 0 entries) gets an empty map, and the compact gradient buffers are reserved all the same (a train step
-        // reads them).  On several GPUs it still posts its (empty) key lists: the peers' serve waits for every rank's lists
-        const bool empty = rows == 0 || nnz == 0;
-        if (fused_reserve(c, s, nnz) || fused_build_slot(c, s, st, nullptr, rows, nnz)) return 1;
-        if (c->cfg.world > 1 && (empty ? dist_send_empty(c, slot, st) : dist_send_keys(c, s, slot, st))) return 1;
-    }
-    s.csc_block = 0;
-    s.dev_csc = false;
-    if (grouped) {
-        LCTR_CHECK(csc_device_supported(c), "cfg.deterministic=2 (device-grouped backward) needs FM with k in {4,8,16,32} "
-                                            "or FFM with k %% 4 == 0 and field_cnt * k <= 512");
-        if (csc_build_device(c, s, st, tmp, nullptr, rows, nnz)) return 1;  // widens the labels in its first kernel
-    } else if (c->cfg.deterministic == 1 && c->cfg.model != LCTR_MODEL_FFM && rows > 0) {
-        LCTR_CUDA(cudaStreamSynchronize(st));
-        if (build_csc(c, s, rows, nnz, row_ptr, fid, val)) return 1;
-    }
-    return 0;
+    if (rows) LCTR_CUDA(cudaMemcpyAsync(s.pred, label, (size_t)rows * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return upload_tail(c, st, slot, rows, nnz, fid_resident, row_ptr, fid, val);
 }
 
 // the CSR structure of an upload (`who` prefixes the messages): row_ptr from 0 to nnz, never decreasing, and the fields
@@ -959,6 +973,29 @@ int lctr_download_pred(lctr_ctx* c, int slot, float* out) {
     LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
     Slot& s = c->slots[slot];
     LCTR_CUDA(cudaMemcpyAsync(out, s.pred, (size_t)s.rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+int lctr_download_batch(lctr_ctx* c, int slot, int64_t* rows, int64_t* nnz, int64_t* row_ptr, uint32_t* fid, uint16_t* field,
+                        float* val, float* label) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
+    Slot& s = c->slots[slot];
+    const size_t r = (size_t)s.rows, n = (size_t)s.nnz;
+    if (rows) *rows = s.rows;
+    if (nnz) *nnz = s.nnz;
+    if (row_ptr && s.row_ptr) LCTR_CUDA(cudaMemcpyAsync(row_ptr, s.row_ptr, (r + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+    if (n && fid) LCTR_CUDA(cudaMemcpyAsync(fid, s.fid, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    if (n && field) {
+        if (s.has_field) LCTR_CUDA(cudaMemcpyAsync(field, s.field, n * sizeof(uint16_t), cudaMemcpyDeviceToHost, c->stream));
+        else memset(field, 0, n * sizeof(uint16_t));
+    }
+    if (n && val) {
+        if (s.has_val) LCTR_CUDA(cudaMemcpyAsync(val, s.val, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        else std::fill(val, val + n, 1.0f);
+    }
+    if (r && label) LCTR_CUDA(cudaMemcpyAsync(label, s.label, r * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }

@@ -114,10 +114,12 @@ struct DistState;
 struct KeyTable;
 struct CscScratch;
 struct AucScratch;
+struct TextState;
 void drop(DistState* p);
 void drop(KeyTable* p);
 void drop(CscScratch* p);
 void drop(AucScratch* p);
+void drop(TextState* p);
 struct Drop {
     template <typename T>
     void operator()(T* p) const { drop(p); }
@@ -127,8 +129,8 @@ using Owned = std::unique_ptr<T, Drop>;
 
 constexpr int kNumSlots = 8;
 constexpr int kPipe = LCTR_PIPE_DEPTH;  // streamed pipeline: batches in flight (the last kPipe slots are its buffers)
-constexpr int kNumProf = 17;  // per-kernel timing buckets
-enum { PROF_FM_FWD = 0, PROF_FM_BWD_RED = 1, PROF_APPLY = 2, PROF_FFM_FUSED = 3, PROF_FM_BWD_CSC = 4, PROF_MLP = 5, PROF_DIST_MARK = 6, PROF_DIST_COMPACT = 7, PROF_DIST_PULL = 8, PROF_DIST_PUSH = 9, PROF_DIST_BAR0 = 10, PROF_DIST_MERGE = 11, PROF_DIST_BAR1 = 12, PROF_CSC_BUILD = 13, PROF_FM_FUSED = 14, PROF_APPLY_COMPACT = 15, PROF_KEYS = 16 };
+constexpr int kNumProf = 18;  // per-kernel timing buckets
+enum { PROF_FM_FWD = 0, PROF_FM_BWD_RED = 1, PROF_APPLY = 2, PROF_FFM_FUSED = 3, PROF_FM_BWD_CSC = 4, PROF_MLP = 5, PROF_DIST_MARK = 6, PROF_DIST_COMPACT = 7, PROF_DIST_PULL = 8, PROF_DIST_PUSH = 9, PROF_DIST_BAR0 = 10, PROF_DIST_MERGE = 11, PROF_DIST_BAR1 = 12, PROF_CSC_BUILD = 13, PROF_FM_FUSED = 14, PROF_APPLY_COMPACT = 15, PROF_KEYS = 16, PROF_TEXT = 17 };
 constexpr int kStatRing = 64;
 constexpr int kHotRep = 32;      // fm_fused: replica rows per hot slot of the batch-compact gradient buffer
 constexpr int kHotMax = 2048;    // hot slots per batch (ids beyond the cap stay ordinary slots)
@@ -304,6 +306,7 @@ struct lctr_ctx {
     const float* fwd_quirk_sumvx = nullptr;  // FM_Predict quirk: training sumVX rows used by the next forward launch
     int64_t fwd_quirk_rows = 0;
     lctr::Owned<lctr::CscScratch> csc_scratch;  // csc.cu: dense count / offset arrays of the device-side grouping
+    lctr::Owned<lctr::TextState> text;          // text.cu: staging and parser state of lctr_upload_libffm
     // optional per-kernel timing (lctr_profile): events bracket every launch on the ctx stream
     int profiling = 0;
     std::vector<cudaEvent_t> prof_ev;   // flat list of (start, stop) pairs
@@ -514,6 +517,9 @@ int launch_nfm_mlp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_di
 int keys_alloc(lctr_ctx* c);
 size_t keys_bytes(const lctr_ctx* c);
 int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid);
+// the translate's key scratch, room for n keys (valid until the next keyed call), and the translation of its first n keys
+int keys_scratch(lctr_ctx* c, size_t n, uint64_t** d_keys);
+int keys_translate_scratch(lctr_ctx* c, int64_t n, bool insert, uint32_t* fid);
 // fails naming `who` when one of the n keys is ~0, the empty marker of the key table
 int check_keys_reserved(const uint64_t* keys, int64_t n, const char* who);
 int keys_restore(lctr_ctx* c, const uint64_t* row_key, uint64_t n);
@@ -547,6 +553,10 @@ inline float initial_s1(const lctr_cfg& cf) {
 }
 // W, V, s1 and s2 of this rank's shard back to the state lctr_create gives (capi.cu)
 int reset_table_rows(lctr_ctx* c);
+// single-slot uploads (capi.cu): room in the slot for rows x nnz, and the common end once the batch sits in the slot
+int slot_fit(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz);
+int upload_tail(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows, int64_t nnz, bool keyed, const int64_t* h_row_ptr,
+                const uint32_t* h_fid, const float* h_val);
 
 }  // namespace lctr
 

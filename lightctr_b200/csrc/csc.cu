@@ -467,7 +467,7 @@ int csc_build_device(lctr_ctx* c, Slot& s, cudaStream_t st, const int32_t* label
         launch(c, {std::max(gt, 1u), 256, 0, st}, csc_tile_write_kernel, sc->cnt, c->F, sc->tile_off, sc->off, s.seg_fid, s.seg_ptr,
                s.short_list, s.long_list, s.csc_totals) ||
         launch(c, {std::max(gf, 1u), 256, 0, st}, csc_fill_kernel, s.row_ptr, s.fid, s.has_val ? s.val.get() : nullptr, s.rows, sc->off,
-               sc->cnt, s.ent_row, s.ent_x, hdr, s.has_field ? s.field.get() : nullptr, s.ent_field))
+               sc->cnt, s.ent_row, s.ent_x, hdr, s.has_field && s.ent_field ? s.field.get() : nullptr, s.ent_field))  // FFM only
         return 1;
     s.dev_csc = true;
     s.csc_block = 0;

@@ -963,19 +963,33 @@ static int tier_compact(lctr_ctx* c) {
     return 0;
 }
 
-// keys of one upload -> rows in fid (device, n entries); insert: create and initialise rows for new keys first.  Tiered:
+// keys of one upload (host) -> rows in fid (device, n entries): the keys copied into the scratch, then translated there.
+// keys_translate_scratch: the translation of the n keys a caller has put into the scratch (keys_scratch); insert: create and initialise rows for new keys first.  Tiered:
 // new keys the tier holds are restored from it; insert = 0 gives rows to the keys the tier holds, and to no other.
 // Admission on, insert = 1: count + admit replace the insert, entries of keys not admitted get the drop marker, and the
 // dropped count is left for keys_admission_compact.
 int keys_translate(lctr_ctx* c, const uint64_t* h_keys, int64_t n, bool insert, uint32_t* fid) {
+    uint64_t* d_keys = nullptr;
+    if (n > 0) {
+        if (keys_scratch(c, (size_t)n, &d_keys)) return 1;
+        LCTR_CUDA(cudaMemcpyAsync(d_keys, h_keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
+    }
+    return keys_translate_scratch(c, n, insert, fid);
+}
+
+int keys_scratch(lctr_ctx* c, size_t n, uint64_t** d_keys) {
+    if (scratch_reserve(c, n)) return 1;
+    *d_keys = reinterpret_cast<uint64_t*>(c->keys->d_keys.get());
+    return 0;
+}
+
+int keys_translate_scratch(lctr_ctx* c, int64_t n, bool insert, uint32_t* fid) {
     KeyTable* t = c->keys.get();
     Admission* adm = insert ? t->adm.get() : nullptr;
     if (insert) t->clock++;  // the clock counts insert-uploads, empty ones included
     if (t->adm) t->adm->pending = 0;
     if (adm) adm->dropped = adm->admitted = 0;
     if (n == 0) return 0;
-    if (scratch_reserve(c, (size_t)n)) return 1;
-    LCTR_CUDA(cudaMemcpyAsync(t->d_keys, h_keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
     LCTR_CUDA(cudaMemsetAsync(t->ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
     if (adm) LCTR_CUDA(cudaMemsetAsync(adm->cnt, 0, 2 * sizeof(unsigned long long), c->stream));
     const bool restoring = tier_live(t);
