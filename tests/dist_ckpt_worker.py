@@ -2,8 +2,8 @@
 
     RANK=r WORLD_SIZE=R MASTER_ADDR=127.0.0.1 MASTER_PORT=p python tests/dist_ckpt_worker.py --out DIR --mode M [...]
 
-Every rank uses cuda:0 (CUDA IPC between processes on one GPU), plumbing over gloo; batches are the CriteoSynth ones of
-tests/dist_worker.py (seed 100 + rank), keyed runs use key = fmix64(fid).
+Every rank uses cuda:0 (CUDA IPC between processes on one GPU), plumbing over gloo; batches are the CriteoSynth train
+batches of tests/multirank.py, keyed runs use key = fmix64(fid).
 
 mode=resume : 6 uninterrupted steps, then 3 steps + save_sharded + fresh contexts (create, connect, load_sharded, upload
               again) + 3 steps; writes rank<r>.npz with both runs' per-step stats and final global downloads (params, optimizer
@@ -13,79 +13,26 @@ mode=from1  : load_checkpoint_shards([--single]) of a single-GPU file; writes th
               that a collective upload + step runs on the loaded state.
 mode=refuse : the refused loads, each followed by downloads equal to the ones before it; writes rank<r>.json."""
 import argparse
-import json
 import os
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import multirank as mr
 
-NFM_HIDDEN = (32, 16)
-WND_HIDDEN = (16,)
-CAP_MULT = 2  # keyed capacity = CAP_MULT * F
-HALF = 3      # resume: steps before the save
+HALF = 3  # resume: steps before the save
 
 
-def model_id(name):
-    from lightctr_b200 import capi
-    return {"ffm": capi.MODEL_FFM, "fm": capi.MODEL_FM, "nfm": capi.MODEL_NFM, "wnd": capi.MODEL_WND}[name]
-
-
-def make_context(args, rank, world, k=None, cap=None):
-    from lightctr_b200 import capi
-    k = k or args.k
-    fc = 39 if args.model in ("ffm", "wnd") else 0
-    hidden = NFM_HIDDEN if args.model == "nfm" else WND_HIDDEN if args.model == "wnd" else ()
-    kw = dict(device=0, rank=rank, world=world, minibatch_size=2 * args.rows, max_nnz=args.rows * 200, optimizer=args.opt,
-              hidden=hidden)
-    if args.keyed:
-        return capi.Context(model_id(args.model), cap or CAP_MULT * args.F, k, fc, key_mode=capi.KEYS_HASHED, **kw)
-    return capi.Context(model_id(args.model), args.F, k, fc, **kw)
-
-
-def make_problem(args, rank):
-    from lightctr_b200.data import CriteoSynth
-    gen = CriteoSynth(args.F, seed=100 + rank)
-    batches = [gen.batch(args.rows) for _ in range(2 * HALF)]
-    rng = np.random.default_rng(5)
-    W0 = (rng.standard_normal(args.F) * 0.01).astype(np.float32)
-    rowlen = args.k * (39 if args.model == "ffm" else 1)
-    V0 = (rng.standard_normal(args.F * rowlen) / np.sqrt(args.k)).astype(np.float32)
-    return batches, W0, V0
-
-
-def layer_dims(args):
-    if args.model == "nfm":
-        return [args.k] + list(NFM_HIDDEN) + [1]
-    if args.model == "wnd":
-        return [39 * args.k] + list(WND_HIDDEN) + [1]
-    return []
-
-
-def make_mlp(args):
-    rng = np.random.default_rng(77)
-    dims = layer_dims(args)
-    return [((rng.random((dims[i + 1], dims[i]), dtype=np.float32) - 0.5).astype(np.float32),
-             np.zeros(dims[i + 1], np.float32)) for i in range(len(dims) - 1)]
-
-
-def upload(ctx, args, slot, batch):
-    from lightctr_b200 import dist as ldist
-    rp, fid, fld, lab = batch
-    fld = fld if args.model in ("ffm", "wnd") else None
-    if args.keyed:
-        ctx.upload_batch_keys(slot, rp, ldist.fmix64(fid), fld, None, lab)
-    else:
-        ctx.upload_batch(slot, rp, fid, fld, None, lab)
+def context(args, rank, world, **kw):
+    """the context of every run here; world = 1 gives its single-GPU twin"""
+    return mr.make_context(args.model, args.F, args.k, rank, world, minibatch_size=2 * args.rows,
+                           max_nnz=args.rows * 200, optimizer=args.opt, keyed=args.keyed, **kw)
 
 
 def train(ctx, args, batches):
     from lightctr_b200 import dist as ldist
     stats = []
     for b in batches:
-        upload(ctx, args, 0, b)
+        mr.upload(ctx, args.model, 0, b, args.keyed)
         stats.append(ldist.reduce_stats(*ctx.train_step(0)))
     return stats
 
@@ -105,7 +52,7 @@ def snapshot(ctx, args):
     out = {"W": W, "V": V, "s1": s1, "s2": s2}
     if args.keyed:
         out["keys"] = ctx.download_keys()
-    dims = layer_dims(args)
+    dims = mr.layer_dims(args.model, args.k)
     for l in range(len(dims) - 1):
         out["mlp_w%d" % l], out["mlp_b%d" % l] = ctx.mlp_download(l, dims[l], dims[l + 1])
     return out
@@ -117,14 +64,14 @@ def same(a, b):
 
 def fresh(args, rank, world, W0=None, V0=None):
     from lightctr_b200 import dist as ldist
-    ctx = make_context(args, rank, world)
+    ctx = context(args, rank, world)
     ldist.connect(ctx)
     if args.model == "nfm":
         ldist.attach_dense_allreduce(ctx)
     if W0 is not None and not args.keyed:
         ctx.upload_params(W0, V0)
     if W0 is not None:
-        for l, (w, b) in enumerate(make_mlp(args)):
+        for l, (w, b) in enumerate(mr.dense_layers(args.model, args.k)):
             ctx.mlp_upload(l, w, b)
     return ctx
 
@@ -132,7 +79,7 @@ def fresh(args, rank, world, W0=None, V0=None):
 def run_resume(args, rank, world):
     import torch.distributed as dist
     from lightctr_b200 import dist as ldist
-    batches, W0, V0 = make_problem(args, rank)
+    batches, (W0, V0) = mr.train_batches(args.F, args.rows, 2 * HALF, rank), mr.make_params(args.F, args.k, args.model)
     ctx = fresh(args, rank, world, W0, V0)
     stats_a = train(ctx, args, batches)
     snap_a = snapshot(ctx, args)
@@ -150,8 +97,8 @@ def run_resume(args, rank, world):
     stats_b += train(ctx, args, batches[HALF:])
     snap_b = snapshot(ctx, args)
     ldist.save_sharded(ctx, os.path.join(args.out, "final"))
-    np.savez(os.path.join(args.out, "rank%d.npz" % rank), stats_a=np.array(stats_a), stats_b=np.array(stats_b),
-             round_trip=round_trip, **{"a_" + x: v for x, v in snap_a.items()}, **{"b_" + x: v for x, v in snap_b.items()})
+    mr.save(args.out, rank, dict(stats_a=np.array(stats_a), stats_b=np.array(stats_b), round_trip=round_trip,
+                                 **{"a_" + x: v for x, v in snap_a.items()}, **{"b_" + x: v for x, v in snap_b.items()}))
     dist.barrier()
     ctx.close()
 
@@ -159,11 +106,11 @@ def run_resume(args, rank, world):
 def run_from1(args, rank, world):
     import torch.distributed as dist
     from lightctr_b200 import capi, dist as ldist
-    batches, _, _ = make_problem(args, rank)
+    batches = mr.train_batches(args.F, args.rows, 2, rank)
     ctx = fresh(args, rank, world)
     out = {}
     if args.keyed:  # slot 1 holds a translated batch before the load
-        upload(ctx, args, 1, batches[0])
+        mr.upload(ctx, args.model, 1, batches[0], args.keyed)
     ctx.load_checkpoint_shards([args.single])
     snap = snapshot(ctx, args)
     if args.keyed:
@@ -173,13 +120,11 @@ def run_from1(args, rank, world):
             out["stale"] = None
         except capi.LctrError as e:
             out["stale"] = str(e)
-        upload(ctx, args, 1, batches[1])
+        mr.upload(ctx, args.model, 1, batches[1], args.keyed)
         out["after_upload"] = ldist.reduce_stats(*ctx.train_step(1))[0]
     else:
         out["after_upload"] = train(ctx, args, batches[:1])[0][0]
-    np.savez(os.path.join(args.out, "rank%d.npz" % rank), **snap)
-    with open(os.path.join(args.out, "rank%d.json" % rank), "w") as f:
-        json.dump(out, f)
+    mr.save(args.out, rank, snap, out)
     dist.barrier()
     ctx.close()
 
@@ -202,7 +147,7 @@ def run_refuse(args, rank, world):
     out = {"rank": rank}
     other = 1 - rank
     # dense FM: sets A (1 step) and B (2 steps)
-    batches, W0, V0 = make_problem(args, rank)
+    batches, (W0, V0) = mr.train_batches(args.F, args.rows, 2 * HALF, rank), mr.make_params(args.F, args.k, args.model)
     ctx = fresh(args, rank, world, W0, V0)
     train(ctx, args, batches[:1])
     a = os.path.join(args.out, "A")
@@ -223,30 +168,29 @@ def run_refuse(args, rank, world):
     ctx.close()
     # Wide&Deep without a dense all-reduce: per-rank layers, which a world-1 context refuses
     wargs = argparse.Namespace(**dict(vars(args), model="wnd", k=4, keyed=False))
-    wb, _, _ = make_problem(wargs, rank)
-    ctx = make_context(wargs, rank, world)
+    wb = mr.train_batches(args.F, args.rows, 1, rank)
+    ctx = context(wargs, rank, world)
     ldist.connect(ctx)
-    for l, (w, bb) in enumerate(make_mlp(wargs)):
+    for l, (w, bb) in enumerate(mr.dense_layers("wnd", wargs.k)):
         ctx.mlp_upload(l, w, bb)
     train(ctx, wargs, wb[:1])
     wp = os.path.join(args.out, "W")
     ldist.save_sharded(ctx, wp)
-    ctx1 = make_context(wargs, 0, 1)
+    ctx1 = context(wargs, 0, 1)
     out["wnd_layers"] = refused(ctx1, wargs, lambda: ctx1.load_checkpoint_shards([sp(wp, 0, 2), sp(wp, 1, 2)]))
     ctx1.close()
     dist.barrier()
     ctx.close()
     # keyed: a single-GPU file whose keys all belong to rank 1 under world 2 overflows rank 1's shard
     kargs = argparse.Namespace(**dict(vars(args), keyed=True, k=8))
-    ctx = make_context(kargs, rank, world, cap=64)
+    ctx = context(kargs, rank, world, cap=64)
     ldist.connect(ctx)
     pool = ldist.fmix64(np.arange(1, 2000))
     ctx.upload_keyed_params(pool[:6], np.ones(6, np.float32), None)  # each rank seeds the keys of the 6 it owns
     out["keyed_overflow"] = refused(ctx, kargs, lambda: ctx.load_checkpoint_shards([args.skewed]))
     dist.barrier()
     ctx.close()
-    with open(os.path.join(args.out, "rank%d.json" % rank), "w") as f:
-        json.dump(out, f)
+    mr.save(args.out, rank, messages=out)
     dist.barrier()
 
 
@@ -264,13 +208,8 @@ def main():
     ap.add_argument("--skewed", default="")
     ap.add_argument("--out", required=True)
     args = ap.parse_args()
-    import torch
-    import torch.distributed as dist
-    torch.cuda.set_device(0)
-    rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    {"resume": run_resume, "from1": run_from1, "refuse": run_refuse}[args.mode](args, rank, world)
-    dist.destroy_process_group()
+    run = {"resume": run_resume, "from1": run_from1, "refuse": run_refuse}[args.mode]
+    mr.main(lambda rank, world: run(args, rank, world), device=0)
 
 
 if __name__ == "__main__":

@@ -3,7 +3,7 @@
     RANK=r WORLD_SIZE=R MASTER_ADDR=127.0.0.1 MASTER_PORT=p python tests/dist_keyed_worker.py --out DIR [...]
 
 Every rank uses cuda:0 (CUDA IPC between processes on one GPU), plumbing over gloo.  Keys are fmix64(fid) of the
-CriteoSynth batches (seed 100 + rank, as tests/dist_worker.py), rows created by lazy init or seeded with
+CriteoSynth train batches of tests/multirank.py, rows created by lazy init or seeded with
 upload_keyed_params (--seeded: the same arrays on every rank).
 
 mode=train : --steps collective uploads + steps; writes rank<r>.npz with the rank's row -> key map, its download_params
@@ -11,67 +11,34 @@ mode=train : --steps collective uploads + steps; writes rank<r>.npz with the ran
 mode=edge  : FM on a tiny capacity: a batch overflowing one owner's shard, refused uploads (insert = 0, and on one rank
              only), recovery after each, and key_evict or a missing max_nnz refused with world > 1; writes rank<r>.json with what happened."""
 import argparse
-import json
-import os
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-NFM_HIDDEN = (32, 16)
-CAP_MULT = 2  # keyed capacity = CAP_MULT * F: every key a run can meet fits each owner's shard
-
-
-def make_problem(F, k, rows, steps, model, rank):
-    from lightctr_b200.data import CriteoSynth
-    gen = CriteoSynth(F, seed=100 + rank)
-    batches = [gen.batch(rows) for _ in range(steps)]
-    rng = np.random.default_rng(5)
-    W0 = (rng.standard_normal(F) * 0.01).astype(np.float32)
-    rowlen = k * (39 if model == "ffm" else 1)
-    V0 = (rng.standard_normal(F * rowlen) / np.sqrt(k)).astype(np.float32)
-    return batches, W0, V0
-
-
-def make_mlp(k):
-    rng = np.random.default_rng(77)
-    dims = [k] + list(NFM_HIDDEN) + [1]
-    return [((rng.random((dims[i + 1], dims[i]), dtype=np.float32) - 0.5).astype(np.float32),
-             np.zeros(dims[i + 1], np.float32)) for i in range(len(dims) - 1)]
-
-
-def make_context(model, cap, k, rank, world, rows, **kw):
-    from lightctr_b200 import capi
-    mid = {"ffm": capi.MODEL_FFM, "fm": capi.MODEL_FM, "nfm": capi.MODEL_NFM}[model]
-    return capi.Context(mid, cap, k, 39 if model == "ffm" else 0, device=0, rank=rank, world=world,
-                        minibatch_size=world * rows, max_nnz=rows * 200, key_mode=capi.KEYS_HASHED,
-                        hidden=NFM_HIDDEN if model == "nfm" else (), **kw)
+import multirank as mr
 
 
 def run_train(args, rank, world):
     import torch.distributed as dist
     from lightctr_b200 import dist as ldist
-    batches, W0, V0 = make_problem(args.F, args.k, args.rows, args.steps, args.model, rank)
-    ctx = make_context(args.model, CAP_MULT * args.F, args.k, rank, world, args.rows)
+    ctx = mr.make_context(args.model, args.F, args.k, rank, world, minibatch_size=world * args.rows,
+                          max_nnz=args.rows * 200, keyed=True)
     ldist.connect(ctx)
     if args.seeded:
-        ctx.upload_keyed_params(ldist.fmix64(np.arange(args.F)), W0, V0)
+        ctx.upload_keyed_params(ldist.fmix64(np.arange(args.F)), *mr.make_params(args.F, args.k, args.model))
     if args.model == "nfm":
-        for l, (w, b) in enumerate(make_mlp(args.k)):
+        for l, (w, b) in enumerate(mr.dense_layers(args.model, args.k)):
             ctx.mlp_upload(l, w, b)
         ldist.attach_dense_allreduce(ctx)
     stats = []
-    for rp, fid, fld, lab in batches:
-        ctx.upload_batch_keys(0, rp, ldist.fmix64(fid), fld if args.model == "ffm" else None, None, lab)
+    for b in mr.train_batches(args.F, args.rows, args.steps, rank):
+        mr.upload(ctx, args.model, 0, b, keyed=True)
         l, c = ctx.train_step(0)
         stats.append(ldist.reduce_stats(l, c))
     dist.barrier()
     keys = ctx.download_keys()
     W, V = ctx.download_params()
-    np.savez(os.path.join(args.out, "rank%d.npz" % rank), keys=keys, W=W, V=V, rows=ctx.lookup_keys(keys),
-             stats=np.array(stats), launches=ctx.launch_count())
+    mr.save(args.out, rank, dict(keys=keys, W=W, V=V, rows=ctx.lookup_keys(keys), stats=np.array(stats),
+                                 launches=ctx.launch_count()))
     dist.barrier()
     ctx.close()
 
@@ -100,7 +67,7 @@ def run_edge(args, rank, world):
         out["no_max_nnz_create"] = None
     except capi.LctrError as e:
         out["no_max_nnz_create"] = str(e)
-    ctx = make_context("fm", cap, k, rank, world, rows)
+    ctx = mr.make_context("fm", 0, k, rank, world, minibatch_size=world * rows, max_nnz=rows * 200, keyed=True, cap=cap)
     ldist.connect(ctx)
     pool = ldist.fmix64(np.arange(1, 20000))
     own = [pool[ldist.owner_of_key(pool, world) == o] for o in range(world)]
@@ -144,8 +111,7 @@ def run_edge(args, rank, world):
     out["d_upload"] = upload(batch_a)
     out["d_loss"] = step()
     dist.barrier()
-    with open(os.path.join(args.out, "rank%d.json" % rank), "w") as f:
-        json.dump(out, f)
+    mr.save(args.out, rank, messages=out)
     dist.barrier()
     ctx.close()
 
@@ -161,13 +127,8 @@ def main():
     ap.add_argument("--seeded", action="store_true")
     ap.add_argument("--out", required=True)
     args = ap.parse_args()
-    import torch
-    import torch.distributed as dist
-    torch.cuda.set_device(0)
-    rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    (run_train if args.mode == "train" else run_edge)(args, rank, world)
-    dist.destroy_process_group()
+    run = run_train if args.mode == "train" else run_edge
+    mr.main(lambda rank, world: run(args, rank, world), device=0)
 
 
 if __name__ == "__main__":

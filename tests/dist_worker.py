@@ -1,4 +1,4 @@
-"""One rank of a multi-process run of the multi-GPU path (launched by tests/test_dist_*.py and usable by hand):
+"""One rank of a multi-process run of the multi-GPU path (launched by tests/test_dist.py and usable by hand):
 
     RANK=r WORLD_SIZE=R MASTER_ADDR=127.0.0.1 MASTER_PORT=p python tests/dist_worker.py --out DIR [...]
 
@@ -9,71 +9,44 @@ mode=emu   : CPU emulation of the same protocol with the oracle's arithmetic and
              read the owner's rows, push = all_to_all of (fid, grad row) records, owner merges + applies): checks that
              the protocol is the single-process step, on machines without a GPU."""
 import argparse
-import os
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def make_problem(args, rank):
-    from lightctr_b200.data import CriteoSynth
-    gen = CriteoSynth(args.F, seed=100 + rank)
-    batches = [gen.batch(args.rows) for _ in range(args.steps)]
-    rng = np.random.default_rng(5)
-    W0 = (rng.standard_normal(args.F) * 0.01).astype(np.float32)
-    rowlen = args.k * (39 if args.model == "ffm" else 1)
-    V0 = (rng.standard_normal(args.F * rowlen) / np.sqrt(args.k)).astype(np.float32)
-    return batches, W0, V0
-
-
-NFM_HIDDEN = (32, 16)
-
-
-def make_mlp(args):
-    """Initial dense layers of the NFM runs (identical on every rank: the layers are replicated)."""
-    rng = np.random.default_rng(77)
-    dims = [args.k] + list(NFM_HIDDEN) + [1]
-    return [((rng.random((dims[i + 1], dims[i]), dtype=np.float32) - 0.5).astype(np.float32),
-             np.zeros(dims[i + 1], np.float32)) for i in range(len(dims) - 1)]
+import multirank as mr
 
 
 def run_gpu(args, rank, world):
+    import torch
     import torch.distributed as dist
     from lightctr_b200 import capi, dist as ldist
-    batches, W0, V0 = make_problem(args, rank)
-    model = {"ffm": capi.MODEL_FFM, "fm": capi.MODEL_FM, "nfm": capi.MODEL_NFM}[args.model]
+    batches, (W0, V0) = mr.train_batches(args.F, args.rows, args.steps, rank), mr.make_params(args.F, args.k, args.model)
     dev = 0 if args.same_device else rank
-    import torch
     torch.cuda.set_device(dev)
-    ctx = capi.Context(model, args.F, args.k, 39 if args.model == "ffm" else 0, device=dev, rank=rank, world=world,
-                       minibatch_size=world * args.rows, max_nnz=args.rows * 200,
-                       hidden=NFM_HIDDEN if args.model == "nfm" else (),
-                       **(dict(optimizer=capi.OPT_PS_SGD, lr=float(world * args.rows)) if args.probe else {}))
+    ctx = mr.make_context(args.model, args.F, args.k, rank, world, minibatch_size=world * args.rows,
+                          max_nnz=args.rows * 200, device=dev,
+                          **(dict(optimizer=capi.OPT_PS_SGD, lr=float(world * args.rows)) if args.probe else {}))
     ctx.upload_params(W0, V0)
     ldist.connect(ctx)
     if args.model == "nfm":
-        for l, (w, b) in enumerate(make_mlp(args)):
+        for l, (w, b) in enumerate(mr.dense_layers(args.model, args.k)):
             ctx.mlp_upload(l, w, b)
         ldist.attach_dense_allreduce(ctx)
     stats, preds = [], []
-    for rp, fid, fld, lab in batches:
-        ctx.upload_batch(0, rp, fid, fld if args.model == "ffm" else None, None, lab)
+    for b in batches:
+        mr.upload(ctx, args.model, 0, b)
         l, c = ctx.train_step(0)
         stats.append(ldist.reduce_stats(l, c))
         if args.probe:
             preds.append(ctx.download_pred(0))
     dist.barrier()
     W, V = ctx.download_params()
-    extra = {"pred": np.concatenate(preds)} if args.probe else {}
-    if args.model == "nfm":
-        dims = [args.k] + list(NFM_HIDDEN) + [1]
-        for l in range(len(dims) - 1):
-            w, b = ctx.mlp_download(l, dims[l], dims[l + 1])
-            extra["mlp_w%d" % l], extra["mlp_b%d" % l] = w, b
-    np.savez(os.path.join(args.out, "rank%d.npz" % rank), W=W, V=V, stats=np.array(stats), **extra)
+    arrs = {"W": W, "V": V, "stats": np.array(stats)}
+    if args.probe:
+        arrs["pred"] = np.concatenate(preds)
+    dims = mr.layer_dims(args.model, args.k)
+    for l in range(len(dims) - 1):
+        arrs["mlp_w%d" % l], arrs["mlp_b%d" % l] = ctx.mlp_download(l, dims[l], dims[l + 1])
+    mr.save(args.out, rank, arrs)
     dist.barrier()
     ctx.close()
 
@@ -82,7 +55,7 @@ def run_emu(args, rank, world):
     import torch
     import torch.distributed as dist
     from oracle import api
-    batches, W0, V0 = make_problem(args, rank)
+    batches, (W0, V0) = mr.train_batches(args.F, args.rows, args.steps, rank), mr.make_params(args.F, args.k, args.model)
     F, k = args.F, args.k
     mine = np.arange(rank, F, world)
     W, V = W0[mine].copy(), V0.reshape(F, k)[mine].copy()          # my shard
@@ -129,7 +102,7 @@ def run_emu(args, rank, world):
         stats.append((float(t[0]), float(t[1])))
     Wf, Vf = np.zeros(F, np.float32), np.zeros((F, k), np.float32)
     Wf[mine], Vf[mine] = W, V
-    np.savez(os.path.join(args.out, "rank%d.npz" % rank), W=Wf, V=Vf.reshape(-1), stats=np.array(stats))
+    mr.save(args.out, rank, {"W": Wf, "V": Vf.reshape(-1), "stats": np.array(stats)})
     dist.barrier()
 
 
@@ -146,11 +119,8 @@ def main():
     ap.add_argument("--probe", action="store_true")
     ap.add_argument("--backend", default="gloo")
     args = ap.parse_args()
-    import torch.distributed as dist
-    rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-    dist.init_process_group(args.backend, rank=rank, world_size=world)
-    (run_gpu if args.mode == "gpu" else run_emu)(args, rank, world)
-    dist.destroy_process_group()
+    run = run_gpu if args.mode == "gpu" else run_emu
+    mr.main(lambda rank, world: run(args, rank, world), backend=args.backend)
 
 
 if __name__ == "__main__":

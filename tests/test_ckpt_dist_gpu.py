@@ -1,50 +1,19 @@
 """Checkpoints of sharded trainers (csrc/checkpoint.cu): 2 ranks sharing cuda:0 over CUDA IPC save per-rank shard files,
 resume from them, and reshard them onto one GPU; a single-GPU file is resharded onto 2 ranks; the refused loads leave the
 context as it was."""
-import json
 import os
-import socket
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
-
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-import dist_ckpt_worker as wk  # noqa: E402
+import dist_ckpt_worker as wk
+import multirank as mr
 
 pytestmark = pytest.mark.gpu
-WORKER = os.path.join(ROOT, "tests", "dist_ckpt_worker.py")
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _run(tmp_path, extra, world=2, timeout=900):
-    port = _free_port()
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port),
-                   LOCAL_RANK=str(r))
-        procs.append(subprocess.Popen([sys.executable, WORKER, "--out", str(tmp_path)] + extra, env=env,
-                                      stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    logs = []
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            for q in procs:
-                q.kill()
-            raise
-        logs.append(o)
-    assert all(p.returncode == 0 for p in procs), "\n".join(logs)
+def _run(tmp_path, extra):
+    mr.launch("dist_ckpt_worker.py", tmp_path, extra)
 
 
 def _args(**kw):
@@ -79,11 +48,6 @@ def _bits(a):
     return np.ascontiguousarray(a).view(np.uint32)
 
 
-def _single_context(a):
-    """the world-1 twin of the workers' contexts"""
-    return wk.make_context(a, 0, 1)
-
-
 def _keyed_rows(keys, W, V, S1, S2, F, rowlen):
     """key -> (W, V row, s1 row, s2 row) of a 2-rank keyed save, from the ranks' global downloads"""
     out = {}
@@ -110,9 +74,9 @@ def test_resume_and_reshard_to_one_gpu(tmp_path, case):
     from lightctr_b200 import dist as ldist
     a = CASES[case]
     _run(tmp_path, ["--mode", "resume"] + _cli(a))
-    parts = [np.load(os.path.join(str(tmp_path), "rank%d.npz" % r)) for r in range(2)]
+    parts = mr.load(tmp_path)
     rowlen = a.k * (39 if a.model == "ffm" else 1)
-    F = wk.CAP_MULT * a.F if a.keyed else a.F
+    F = mr.CAP_MULT * a.F if a.keyed else a.F
     # the save -> load round trip itself is exact: every download equal bit for bit
     assert all(bool(p["round_trip"]) for p in parts)
     # the continuation: deterministic = 0 (the only mode on several GPUs) sums gradients with REDs in arbitrary order, so
@@ -134,7 +98,8 @@ def test_resume_and_reshard_to_one_gpu(tmp_path, case):
         for key, va in ka.items():
             for x, y, t in zip(va, kb[key], (1e-5, 1e-5, 1e-4, 1e-4, 1e-4, 1e-4)):
                 assert np.allclose(x, y, rtol=t, atol=t), key
-    for l in range(len(wk.layer_dims(a)) - 1):
+    dims = mr.layer_dims(a.model, a.k)
+    for l in range(len(dims) - 1):
         for r in range(2):
             assert np.allclose(parts[r]["a_mlp_w%d" % l], parts[r]["b_mlp_w%d" % l], rtol=1e-5, atol=1e-6)
 
@@ -142,7 +107,7 @@ def test_resume_and_reshard_to_one_gpu(tmp_path, case):
     final = os.path.join(str(tmp_path), "final")
     paths, world = ldist.find_shards(final)
     assert world == 2
-    c = _single_context(a)
+    c = wk.context(a, 0, 1)
     c.load_checkpoint_shards(paths)
     W, V = c.download_params()
     s1, s2 = c.download_opt_state()
@@ -151,8 +116,7 @@ def test_resume_and_reshard_to_one_gpu(tmp_path, case):
     step1 = ldist.checkpoint_info(path1)[:2]
     assert step1 == ldist.checkpoint_info(paths[0])[:2] == ldist.checkpoint_info(paths[1])[:2]
     assert step1[0] == 2 * wk.HALF and (step1[1] > 0) == (a.opt == 2)
-    for l in range(len(wk.layer_dims(a)) - 1):
-        dims = wk.layer_dims(a)
+    for l in range(len(dims) - 1):
         w, b = c.mlp_download(l, dims[l], dims[l + 1])
         assert np.array_equal(_bits(w), _bits(parts[0]["b_mlp_w%d" % l])) and np.array_equal(_bits(b), _bits(parts[0]["b_mlp_b%d" % l]))
     if not a.keyed:
@@ -178,23 +142,12 @@ def test_resume_and_reshard_to_one_gpu(tmp_path, case):
 
 def _single_file(tmp_path, a, name, steps=3):
     """a single-GPU checkpoint of `a`'s world-1 context after `steps` steps on the global batches of 2 ranks"""
-    from lightctr_b200 import dist as ldist
-    per_rank = [wk.make_problem(a, r) for r in range(2)]
-    c = _single_context(a)
+    per_rank = [mr.train_batches(a.F, a.rows, steps, r) for r in range(2)]
+    c = wk.context(a, 0, 1)
     if not a.keyed:
-        c.upload_params(per_rank[0][1], per_rank[0][2])
+        c.upload_params(*mr.make_params(a.F, a.k, a.model))
     for s in range(steps):
-        rps, fids, labs, off = [np.zeros(1, np.int64)], [], [], 0
-        for r in range(2):
-            rp, fid, _, lab = per_rank[r][0][s]
-            rps.append(rp[1:] + off)
-            off += rp[-1]
-            fids.append(fid); labs.append(lab)
-        fid = np.concatenate(fids)
-        if a.keyed:
-            c.upload_batch_keys(0, np.concatenate(rps), ldist.fmix64(fid), None, None, np.concatenate(labs))
-        else:
-            c.upload_batch(0, np.concatenate(rps), fid, None, None, np.concatenate(labs))
+        mr.upload(c, a.model, 0, mr.global_batch([b[s] for b in per_rank]), a.keyed)
         c.train_step(0)
     path = os.path.join(str(tmp_path), name)
     c.save_checkpoint(path)
@@ -213,9 +166,8 @@ def test_reshard_one_gpu_file_onto_two_ranks(tmp_path, keyed):
     if keyed:
         np.save(path + ".keys.npy", single["keys"])
     _run(tmp_path, ["--mode", "from1", "--single", path] + _cli(a))
-    parts = [np.load(os.path.join(str(tmp_path), "rank%d.npz" % r)) for r in range(2)]
-    res = [json.load(open(os.path.join(str(tmp_path), "rank%d.json" % r))) for r in range(2)]
-    F = wk.CAP_MULT * a.F if keyed else a.F
+    parts, res = mr.load(tmp_path), mr.load_json(tmp_path)
+    F = mr.CAP_MULT * a.F if keyed else a.F
     rowlen = a.k
     for o in res:
         assert np.isfinite(o["after_upload"])
@@ -246,7 +198,7 @@ def test_refused_loads_leave_the_context_unchanged(tmp_path):
     single, _ = _single_file(tmp_path, a, "single", steps=1)
     other, _ = _single_file(tmp_path, _args(k=8), "other_cfg", steps=1)
     # keyed FM, capacity 64: 40 keys all owned by rank 1 under world 2, whose shard holds 32 rows
-    c = wk.make_context(_args(keyed=True, k=8), 0, 1, cap=64)
+    c = wk.context(_args(keyed=True, k=8), 0, 1, cap=64)
     pool = ldist.fmix64(np.arange(1, 2000))
     skew = pool[ldist.owner_of_key(pool, 2) == 1][:40]
     c.upload_keyed_params(skew, np.ones(40, np.float32), None)
@@ -254,7 +206,7 @@ def test_refused_loads_leave_the_context_unchanged(tmp_path):
     c.save_checkpoint(skewed)
     c.close()
     _run(tmp_path, ["--mode", "refuse", "--single", single, "--other-cfg", other, "--skewed", skewed] + _cli(a))
-    res = [json.load(open(os.path.join(str(tmp_path), "rank%d.json" % r))) for r in range(2)]
+    res = mr.load_json(tmp_path)
     for r, o in enumerate(res):
         for x in ("other_rank", "single_file", "incomplete", "duplicate", "steps", "cfg", "wnd_layers"):
             assert o[x] != "NOT REFUSED" and not o[x].startswith("CHANGED"), (x, o[x])
@@ -270,7 +222,7 @@ def test_refused_loads_leave_the_context_unchanged(tmp_path):
     msg = res[1]["keyed_overflow"]
     assert "rank 1 would hold 40 keys" in msg and "capacity is 32" in msg and not msg.startswith("CHANGED"), msg
     # a shard file through a single-GPU context's lctr_load_checkpoint
-    c = _single_context(a)
+    c = wk.context(a, 0, 1)
     with pytest.raises(capi.LctrError, match="load_checkpoint_shards"):
         c.load_checkpoint(ldist.shard_path(os.path.join(str(tmp_path), "A"), 0, 2))
     c.close()

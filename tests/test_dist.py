@@ -3,69 +3,21 @@
 CPU (gloo, world_size 2): the process-group plumbing and an emulation of the exchange protocol with the oracle's
 arithmetic must equal the single-process oracle step on the concatenated global batch.
 GPU (-m gpu): the CUDA implementation, 2 ranks (both on cuda:0 over CUDA IPC), against the same oracle."""
-import os
-import socket
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
-
-WORKER = os.path.join(ROOT, "tests", "dist_worker.py")
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _launch(world, out, extra, timeout=600):
-    port = _free_port()
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port),
-                   LOCAL_RANK=str(r))
-        procs.append(subprocess.Popen([sys.executable, WORKER, "--out", out] + extra, env=env, stdout=subprocess.PIPE,
-                                      stderr=subprocess.STDOUT, text=True))
-    logs = []
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            for q in procs:
-                q.kill()
-            raise
-        logs.append(o)
-    assert all(p.returncode == 0 for p in procs), "\n".join(logs)
+import multirank as mr
 
 
 def _oracle_global(oracle_api, world, F, k, rows, steps, model="fm"):
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import dist_worker
-
-    class A:
-        pass
-    a = A()
-    a.F, a.k, a.rows, a.steps, a.model = F, k, rows, steps, model
-    per_rank = [dist_worker.make_problem(a, r) for r in range(world)]
-    W, V = per_rank[0][1].copy(), per_rank[0][2].copy()
+    per_rank = [mr.train_batches(F, rows, steps, r) for r in range(world)]
+    W, V = mr.make_params(F, k, model)
     Fc = 39 if model == "ffm" else 0
     accum = np.zeros(F * (k * max(Fc, 1) + 1), np.float32)
     stats = []
     for s in range(steps):
-        rps, fids, flds, labs, off = [np.zeros(1, np.int64)], [], [], [], 0
-        for r in range(world):
-            rp, fid, fld, lab = per_rank[r][0][s]
-            rps.append(rp[1:] + off)
-            off += rp[-1]
-            fids.append(fid); flds.append(fld); labs.append(lab)
-        ds = oracle_api.Dataset(np.concatenate(rps), np.concatenate(fids), np.concatenate(flds).astype(np.uint32),
-                                np.ones(off, np.float32), np.concatenate(labs), F, Fc)
+        rp, fid, fld, lab = mr.global_batch([b[s] for b in per_rank])
+        ds = oracle_api.Dataset(rp, fid, fld.astype(np.uint32), np.ones(len(fid), np.float32), lab, F, Fc)
         if model == "ffm":
             o = oracle_api.FFMOracle(ds, k, W, V)
             o.s1[:] = accum
@@ -82,32 +34,19 @@ def _oracle_global(oracle_api, world, F, k, rows, steps, model="fm"):
 
 def _oracle_global_nfm(oracle_api, world, F, k, rows, steps):
     """Single-process NFM oracle on the concatenated global batch: one minibatch of world*rows samples per step, masks
-    all ones, the same initial dense layers as tests/dist_worker.py."""
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import dist_worker
-
-    class A:
-        pass
-    a = A()
-    a.F, a.k, a.rows, a.steps, a.model = F, k, rows, steps, "nfm"
-    per_rank = [dist_worker.make_problem(a, r) for r in range(world)]
-    W, V = per_rank[0][1].copy(), per_rank[0][2].copy()
+    all ones, the same initial dense layers as the ranks."""
+    per_rank = [mr.train_batches(F, rows, steps, r) for r in range(world)]
+    W, V = mr.make_params(F, k, "nfm")
     accum = np.zeros(F * (k + 1), np.float32)
-    mlp0 = dist_worker.make_mlp(a)
+    mlp0 = mr.dense_layers("nfm", k)
     nl = len(mlp0)
     state = {"weight": [w.reshape(-1).copy() for w, _ in mlp0], "bias": [b.copy() for _, b in mlp0], "accum": None}
     stats = []
     for s in range(steps):
-        rps, fids, flds, labs, off = [np.zeros(1, np.int64)], [], [], [], 0
-        for r in range(world):
-            rp, fid, fld, lab = per_rank[r][0][s]
-            rps.append(rp[1:] + off)
-            off += rp[-1]
-            fids.append(fid); flds.append(fld); labs.append(lab)
-        ds = oracle_api.Dataset(np.concatenate(rps), np.concatenate(fids), np.concatenate(flds).astype(np.uint32),
-                                np.ones(off, np.float32), np.concatenate(labs), F, 0)
+        rp, fid, fld, lab = mr.global_batch([b[s] for b in per_rank])
+        ds = oracle_api.Dataset(rp, fid, fld.astype(np.uint32), np.ones(len(fid), np.float32), lab, F, 0)
         B = world * rows
-        o = oracle_api.NFMOracle(ds, k, list(dist_worker.NFM_HIDDEN), W=W, V=V, batch_size=B, minibatch=B)
+        o = oracle_api.NFMOracle(ds, k, list(mr.NFM_HIDDEN), W=W, V=V, batch_size=B, minibatch=B)
         o.accum[:] = accum
         for l in range(nl):
             o.mlp.arrays("weight", l)[:] = state["weight"][l]
@@ -124,7 +63,7 @@ def _oracle_global_nfm(oracle_api, world, F, k, rows, steps):
 
 def _check(out, world, F, k, oracle, tol):
     from lightctr_b200 import dist as ldist
-    parts = [np.load(os.path.join(out, "rank%d.npz" % r)) for r in range(world)]
+    parts = mr.load(out, world)
     W = ldist.merge_shards([p["W"] for p in parts], world, F)
     V = ldist.merge_shards([p["V"] for p in parts], world, F)
     Wo, Vo, so = oracle
@@ -150,26 +89,27 @@ def test_shard_arithmetic():
 def test_protocol_emulation_gloo_world2(oracle_api, tmp_path):
     """world_size-2 gloo run of the pull / push / owner-update protocol == single-process oracle on the global batch."""
     F, k, rows, steps = 5000, 8, 64, 3
-    _launch(2, str(tmp_path), ["--mode", "emu", "--F", str(F), "--k", str(k), "--rows", str(rows), "--steps", str(steps)])
-    _check(str(tmp_path), 2, F, k, _oracle_global(oracle_api, 2, F, k, rows, steps), 2e-6)
+    mr.launch("dist_worker.py", tmp_path, ["--mode", "emu", "--F", str(F), "--k", str(k), "--rows", str(rows), "--steps",
+                                           str(steps)], timeout=600)
+    _check(tmp_path, 2, F, k, _oracle_global(oracle_api, 2, F, k, rows, steps), 2e-6)
 
 
 @pytest.mark.gpu
 def test_cuda_two_ranks_one_device(oracle_api, tmp_path):
     """The CUDA multi-GPU path with 2 ranks sharing cuda:0 (CUDA IPC between processes), vs the oracle."""
     F, k, rows, steps = 20000, 16, 256, 3
-    _launch(2, str(tmp_path), ["--mode", "gpu", "--same-device", "--F", str(F), "--k", str(k), "--rows", str(rows),
-                               "--steps", str(steps)], timeout=900)
-    _check(str(tmp_path), 2, F, k, _oracle_global(oracle_api, 2, F, k, rows, steps), 2e-5)
+    mr.launch("dist_worker.py", tmp_path, ["--mode", "gpu", "--same-device", "--F", str(F), "--k", str(k), "--rows",
+                                           str(rows), "--steps", str(steps)])
+    _check(tmp_path, 2, F, k, _oracle_global(oracle_api, 2, F, k, rows, steps), 2e-5)
 
 
 @pytest.mark.gpu
 def test_cuda_two_ranks_ffm(oracle_api, tmp_path):
     """FFM (39 fields, k=4) over 2 ranks: rows of Fc*k floats travel through the same pull / push kernels."""
     F, k, rows, steps = 6000, 4, 128, 2
-    _launch(2, str(tmp_path), ["--mode", "gpu", "--same-device", "--model", "ffm", "--F", str(F), "--k", str(k),
-                               "--rows", str(rows), "--steps", str(steps)], timeout=900)
-    _check(str(tmp_path), 2, F, k, _oracle_global(oracle_api, 2, F, k, rows, steps, model="ffm"), 5e-5)
+    mr.launch("dist_worker.py", tmp_path, ["--mode", "gpu", "--same-device", "--model", "ffm", "--F", str(F), "--k",
+                                           str(k), "--rows", str(rows), "--steps", str(steps)])
+    _check(tmp_path, 2, F, k, _oracle_global(oracle_api, 2, F, k, rows, steps, model="ffm"), 5e-5)
 
 
 @pytest.mark.gpu
@@ -177,11 +117,11 @@ def test_cuda_two_ranks_nfm(oracle_api, tmp_path):
     """NFM over 2 ranks: embeddings owner-sharded (pull / push), dense layers replicated with the per-rank dW / db summed
     through lctr_set_dense_allreduce before the dense Adagrad (gloo through the host here: both ranks share cuda:0)."""
     F, k, rows, steps = 8000, 16, 128, 3
-    _launch(2, str(tmp_path), ["--mode", "gpu", "--same-device", "--model", "nfm", "--F", str(F), "--k", str(k),
-                               "--rows", str(rows), "--steps", str(steps)], timeout=900)
+    mr.launch("dist_worker.py", tmp_path, ["--mode", "gpu", "--same-device", "--model", "nfm", "--F", str(F), "--k",
+                                           str(k), "--rows", str(rows), "--steps", str(steps)])
     Wo, Vo, so, mlp = _oracle_global_nfm(oracle_api, 2, F, k, rows, steps)
-    _check(str(tmp_path), 2, F, k, (Wo, Vo, so), 5e-5)
-    parts = [np.load(os.path.join(str(tmp_path), "rank%d.npz" % r)) for r in range(2)]
+    _check(tmp_path, 2, F, k, (Wo, Vo, so), 5e-5)
+    parts = mr.load(tmp_path)
     for l in range(len(mlp["weight"])):
         for r in range(2):  # replicas stay identical and equal to the oracle's layers
             assert np.max(np.abs(parts[r]["mlp_w%d" % l] - mlp["weight"][l])) < 5e-5

@@ -12,6 +12,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import multirank as mr
 from conftest import ROOT
 
 pytestmark = pytest.mark.gpu
@@ -89,14 +90,10 @@ def test_two_workers_share_the_tables(exe, oracle_api, tmp_path):
         _make_file("%s_%d.csv" % (prefix, r), rng, rows, F, Fc)
     rdv = str(tmp_path / "rdv")
     os.makedirs(rdv)
-    procs, outs = [], []
-    for r in range(2):
-        env = dict(os.environ, LIGHTCTR_B200_RANK=str(r), LIGHTCTR_B200_WORLD="2", LIGHTCTR_B200_DEVICE="0", LIGHTCTR_B200_RDV=rdv)
-        out = str(tmp_path / ("params_%d.bin" % r))
-        outs.append(out)
-        procs.append(subprocess.Popen([exe, prefix, str(epochs), str(seed), out], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    logs = [p.communicate(timeout=600)[0] for p in procs]
-    assert all(p.returncode == 0 for p in procs), "\n".join(logs)
+    outs = [str(tmp_path / ("params_%d.bin" % r)) for r in range(2)]
+    logs = mr.run(2, lambda r: [exe, prefix, str(epochs), str(seed), outs[r]], timeout=600,
+                  env=lambda r: dict(LIGHTCTR_B200_RANK=str(r), LIGHTCTR_B200_WORLD="2", LIGHTCTR_B200_DEVICE="0",
+                                     LIGHTCTR_B200_RDV=rdv))
     for lg in logs:
         losses = [float(v) for v in re.findall(r"\[Worker Train\] epoch = \d+ loss = ([0-9.eE+-]+)", lg)]
         assert len(losses) == epochs and all(np.isfinite(losses)) and losses[-1] < losses[0], lg

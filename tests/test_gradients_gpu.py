@@ -17,6 +17,7 @@ import sys
 import numpy as np
 import pytest
 
+import multirank as mr
 import ref64
 from conftest import ROOT
 from kernel_shapes_worker import make_batch, make_params, run
@@ -24,7 +25,6 @@ from kernel_shapes_worker import make_batch, make_params, run
 pytestmark = pytest.mark.gpu
 
 WORKER = os.path.join(ROOT, "tests", "kernel_shapes_worker.py")
-DIST_WORKER = os.path.join(ROOT, "tests", "dist_worker.py")
 L2 = 0.001
 
 
@@ -365,30 +365,6 @@ def test_ffm_other_kernels_gradient_vs_ref64(tmp_path, Fc, k, det, env, l2):
 # two ranks on one device (CUDA IPC): push_rows_kernel's hot fold + merge_apply_kernel (FM / NFM), merge_kernel + the
 # sparse apply (FFM)
 # ------------------------------------------------------------------------------------------------------------------------
-def _launch_two(out, extra):
-    import socket
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = []
-    for r in range(2):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE="2", MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), LOCAL_RANK=str(r))
-        procs.append(subprocess.Popen([sys.executable, DIST_WORKER, "--out", out, "--mode", "gpu", "--same-device", "--probe",
-                                       "--steps", "1"] + extra, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
-                                      text=True))
-    logs = []
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=900)
-        except subprocess.TimeoutExpired:
-            for q in procs:
-                q.kill()
-            raise
-        logs.append(o)
-    assert all(p.returncode == 0 for p in procs), "\n".join(logs)
-
-
 @pytest.mark.parametrize("model,F,k,rows", [
     pytest.param("fm", 20000, 16, 2048, id="push_rows_kernel-hot+merge_apply_kernel-FM-K16"),
     pytest.param("nfm", 20000, 16, 1024, id="push_rows_kernel+merge_apply_kernel-NFM-K16"),
@@ -398,30 +374,18 @@ def test_two_ranks_gradient_vs_ref64(tmp_path, model, F, k, rows):
     """lr = minibatch_size = the global batch; 2048 Criteo-shaped rows per rank put the frequent ids of the FM case over
     the hot threshold (32 hits in the first 512 rows)."""
     from lightctr_b200 import dist as ldist
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import dist_worker
-
-    class A:
-        pass
-    a = A()
-    a.F, a.k, a.rows, a.steps, a.model = F, k, rows, 1, model
-    _launch_two(str(tmp_path), ["--model", model, "--F", str(F), "--k", str(k), "--rows", str(rows)])
-    parts = [np.load(os.path.join(str(tmp_path), "rank%d.npz" % r)) for r in range(2)]
+    mr.launch("dist_worker.py", tmp_path, ["--mode", "gpu", "--same-device", "--probe", "--steps", "1", "--model", model,
+                                           "--F", str(F), "--k", str(k), "--rows", str(rows)])
+    parts = mr.load(tmp_path)
     W1 = ldist.merge_shards([p["W"] for p in parts], 2, F)
     V1 = ldist.merge_shards([p["V"] for p in parts], 2, F)
     pred = np.concatenate([p["pred"] for p in parts])
-    probs = [dist_worker.make_problem(a, r) for r in range(2)]
-    W0, V0 = probs[0][1], probs[0][2]
-    rps, fids, flds, labs, off = [np.zeros(1, np.int64)], [], [], [], 0
-    for r in range(2):
-        rp, fid, fld, lab = probs[r][0][0]
-        rps.append(rp[1:] + off)
-        off += rp[-1]
-        fids.append(fid); flds.append(fld); labs.append(lab)
-    batch = (np.concatenate(rps), np.concatenate(fids), np.concatenate(flds), None, np.concatenate(labs))
+    W0, V0 = mr.make_params(F, k, model)
+    rp, fid, fld, lab = mr.global_batch([mr.train_batches(F, rows, 1, r)[0] for r in range(2)])
+    batch = (rp, fid, fld, None, lab)
     if model == "fm":
         _check_fm(batch, W0, V0, W1, V1, pred, k)
     elif model == "nfm":
-        _check_nfm(batch, W0, V0, W1, V1, pred, k, [(w, b) for w, b in dist_worker.make_mlp(a)])
+        _check_nfm(batch, W0, V0, W1, V1, pred, k, mr.dense_layers(model, k))
     else:
         _check_ffm(batch, W0, V0, W1, V1, pred, 39, k, L2)

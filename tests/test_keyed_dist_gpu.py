@@ -1,74 +1,28 @@
 """Keyed mode on several GPUs (csrc/dist.cu, keyed upload): 2 ranks sharing cuda:0 over CUDA IPC against a single-GPU
 keyed context trained on the concatenated global batch.  Lazy init depends on (seed, key, element) only, so both start
 from the same values and every key's W and V must agree after training; each key must live on its owner only."""
-import json
-import os
-import socket
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
-
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-import dist_keyed_worker as wk  # noqa: E402
+import multirank as mr
 
 pytestmark = pytest.mark.gpu
-WORKER = os.path.join(ROOT, "tests", "dist_keyed_worker.py")
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _run(tmp_path, extra, world=2, timeout=900):
-    port = _free_port()
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port),
-                   LOCAL_RANK=str(r))
-        procs.append(subprocess.Popen([sys.executable, WORKER, "--out", str(tmp_path)] + extra, env=env,
-                                      stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    logs = []
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            for q in procs:
-                q.kill()
-            raise
-        logs.append(o)
-    assert all(p.returncode == 0 for p in procs), "\n".join(logs)
 
 
 def _single_gpu(model, F, k, rows, steps, seeded, world=2):
     """one keyed context on the global batch (every rank's rows, rank order), same capacity and lazy init"""
     from lightctr_b200 import dist as ldist
-    per_rank = [wk.make_problem(F, k, rows, steps, model, r) for r in range(world)]
-    ctx = wk.make_context(model, wk.CAP_MULT * F, k, 0, 1, world * rows)
+    per_rank = [mr.train_batches(F, rows, steps, r) for r in range(world)]
+    ctx = mr.make_context(model, F, k, 0, 1, minibatch_size=world * rows, max_nnz=world * rows * 200, keyed=True)
     if seeded:
-        ctx.upload_keyed_params(ldist.fmix64(np.arange(F)), per_rank[0][1], per_rank[0][2])
-    if model == "nfm":
-        for l, (w, b) in enumerate(wk.make_mlp(k)):
-            ctx.mlp_upload(l, w, b)
+        ctx.upload_keyed_params(ldist.fmix64(np.arange(F)), *mr.make_params(F, k, model))
+    for l, (w, b) in enumerate(mr.dense_layers(model, k)):
+        ctx.mlp_upload(l, w, b)
     stats, seen = [], set()
     for s in range(steps):
-        rps, keys, flds, labs, off = [np.zeros(1, np.int64)], [], [], [], 0
-        for r in range(world):
-            rp, fid, fld, lab = per_rank[r][0][s]
-            rps.append(rp[1:] + off)
-            off += rp[-1]
-            keys.append(ldist.fmix64(fid)); flds.append(fld); labs.append(lab)
-        keys = np.concatenate(keys)
-        seen.update(keys.tolist())
-        ctx.upload_batch_keys(0, np.concatenate(rps), keys, np.concatenate(flds) if model == "ffm" else None, None,
-                              np.concatenate(labs))
+        batch = mr.global_batch([b[s] for b in per_rank])
+        seen.update(ldist.fmix64(batch[1]).tolist())
+        mr.upload(ctx, model, 0, batch, keyed=True)
         stats.append(ctx.train_step(0))
     kk = ctx.download_keys()
     W, V = ctx.download_params()
@@ -81,8 +35,8 @@ def _single_gpu(model, F, k, rows, steps, seeded, world=2):
 def _check_train(tmp_path, model, F, k, rows, steps, tol, seeded=False):
     from lightctr_b200 import dist as ldist
     extra = ["--model", model, "--F", str(F), "--k", str(k), "--rows", str(rows), "--steps", str(steps)]
-    _run(tmp_path, extra + (["--seeded"] if seeded else []))
-    parts = [np.load(os.path.join(str(tmp_path), "rank%d.npz" % r)) for r in range(2)]
+    mr.launch("dist_keyed_worker.py", tmp_path, extra + (["--seeded"] if seeded else []))
+    parts = mr.load(tmp_path)
     got = ldist.merge_keyed_shards([p["keys"] for p in parts], [p["W"] for p in parts], [p["V"] for p in parts], 2)
     ref, stats, seen = _single_gpu(model, F, k, rows, steps, seeded)
     for (lg, cg), (lo, co) in zip(parts[0]["stats"], stats):
@@ -125,8 +79,8 @@ def test_keyed_fm_two_ranks_seeded(tmp_path):
 
 
 def test_keyed_two_ranks_overflow_and_refusals(tmp_path):
-    _run(tmp_path, ["--mode", "edge"])
-    res = [json.load(open(os.path.join(str(tmp_path), "rank%d.json" % r))) for r in range(2)]
+    mr.launch("dist_keyed_worker.py", tmp_path, ["--mode", "edge"])
+    res = mr.load_json(tmp_path)
     for r, o in enumerate(res):
         assert o["evict_create"] is not None and "key_evict" in o["evict_create"]
         assert o["no_max_nnz_create"] is not None and "max_nnz" in o["no_max_nnz_create"]

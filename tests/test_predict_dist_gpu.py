@@ -1,54 +1,19 @@
 """Collective predict and global test metrics on multi-GPU trainers (csrc/capi.cu: predict_dist, csrc/dist.cu: pull-only
 rounds and the cache release, lightctr_b200/dist.py: eval_global): 2 ranks sharing cuda:0 over CUDA IPC against a
 single-GPU context of the same cfg holding the merged parameters."""
-import json
-import os
-import socket
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
-
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-import dist_predict_worker as wk  # noqa: E402
+import dist_predict_worker as wk
+import multirank as mr
 
 pytestmark = pytest.mark.gpu
-WORKER = os.path.join(ROOT, "tests", "dist_predict_worker.py")
 TOL = 1e-5  # parameters of two sharded runs: the sparse scatter sums in arbitrary order
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _run(out, extra, world=2, timeout=900):
-    os.makedirs(out, exist_ok=True)
-    port = _free_port()
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port),
-                   LOCAL_RANK=str(r))
-        procs.append(subprocess.Popen([sys.executable, WORKER, "--out", out] + extra, env=env,
-                                      stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    logs = []
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            for q in procs:
-                q.kill()
-            raise
-        logs.append(o)
-    assert all(p.returncode == 0 for p in procs), "\n".join(logs)
-    return ([dict(np.load(os.path.join(out, "rank%d.npz" % r))) for r in range(world)],
-            [json.load(open(os.path.join(out, "rank%d.json" % r))) for r in range(world)])
+def _run(out, extra):
+    mr.launch("dist_predict_worker.py", out, extra)
+    return mr.load(out), mr.load_json(out)
 
 
 def _merged(parts, F, wkey="W", vkey="V"):
@@ -58,11 +23,11 @@ def _merged(parts, F, wkey="W", vkey="V"):
 
 def _reference_pctr(model, F, k, rows, W, V, batches):
     """world-1 context of the same cfg holding W / V: the pCTR of each batch"""
-    ctx = wk.make_context(model, F, k, 0, 1, rows)
+    ctx = wk.context(model, F, k, 0, 1, rows)
     ctx.upload_params(W, V)
     out = []
     for b in batches:
-        wk.upload(ctx, model, 1, b)
+        mr.upload(ctx, model, 1, b)
         out.append(ctx.predict(1))
     ctx.close()
     return out
@@ -80,7 +45,7 @@ def test_predict_parity_with_merged_single_gpu(tmp_path, model, k):
     parts, _ = _run(str(tmp_path), ["--mode", "parity", "--model", model, "--k", str(k), "--F", str(F), "--rows", str(rows),
                                     "--test-rows", str(test_rows)])
     W, V = _merged(parts, F)
-    tests = [wk.test_batches(F, test_rows, 1, r)[0] for r in range(2)]
+    tests = [mr.test_batches(F, test_rows, 1, r)[0] for r in range(2)]
     ref = _reference_pctr(model, F, k, rows, W, V, tests)
     for r in range(2):
         assert len(parts[r]["pctr"]) == test_rows
@@ -96,7 +61,7 @@ def test_predict_interleaved_with_training(tmp_path):
                                            "--test-rows", str(test_rows)])
     without, _ = _run(str(tmp_path / "n"), ["--mode", "interleave", "--model", "fm", "--k", str(k), "--rows", str(rows),
                                             "--test-rows", str(test_rows), "--no-predict"])
-    tests = [wk.test_batches(F, test_rows, 2, r) for r in range(2)]
+    tests = [mr.test_batches(F, test_rows, 2, r) for r in range(2)]
     W0, V0 = _merged(with_p, F, "W0", "V0")
     W1, V1 = _merged(with_p, F, "W1", "V1")
     ref0 = _reference_pctr("fm", F, k, rows, W0, V0, [tests[r][0] for r in range(2)])
@@ -133,30 +98,30 @@ def test_empty_share_predicts_and_trains(tmp_path, model, k):
     parts, res = _run(str(tmp_path), ["--mode", "empty", "--model", model, "--k", str(k), "--rows", str(rows),
                                       "--test-rows", str(test_rows)])
     assert res[1]["stats"] == [0.0, 0.0]
-    W0, V0 = wk.make_params(F, k, model)
-    dense = wk.dense_layers(model, k) if model in ("nfm", "wnd") else []
+    W0, V0 = mr.make_params(F, k, model)
+    dense = mr.dense_layers(model, k)
     if model != "nfm":
         assert len(parts[1]["pctr"]) == 0 and len(parts[1]["pctr_after"]) == 0
-        test0 = wk.test_batches(F, test_rows, 1, 0)[0]
-        ctx = wk.make_context(model, F, k, 0, 1, rows)
+        test0 = mr.test_batches(F, test_rows, 1, 0)[0]
+        ctx = wk.context(model, F, k, 0, 1, rows)
         ctx.upload_params(W0, V0)
         for l, (w, b) in enumerate(dense):
             ctx.mlp_upload(l, w, b)
-        wk.upload(ctx, model, 1, test0)
+        mr.upload(ctx, model, 1, test0)
         ref = ctx.predict(1)
         ctx.close()
         if model == "wnd":
             assert np.allclose(parts[0]["pctr"], ref, rtol=1e-6, atol=0)
         else:
             assert _same_bits(parts[0]["pctr"], ref)
-    ctx = wk.make_context(model, F, k, 0, 1, rows)
+    ctx = wk.context(model, F, k, 0, 1, rows)
     ctx.upload_params(W0, V0)
     for l, (w, b) in enumerate(dense):
         ctx.mlp_upload(l, w, b)
-    wk.upload(ctx, model, 0, wk.train_batches(F, rows, 1, 0)[0])
+    mr.upload(ctx, model, 0, mr.train_batches(F, rows, 1, 0)[0])
     loss, correct = ctx.train_step(0)
     W, V = ctx.download_params()
-    dims = wk.layer_dims(model, k) if dense else []
+    dims = mr.layer_dims(model, k)
     layers = [ctx.mlp_download(l, dims[l], dims[l + 1]) for l in range(len(dims) - 1)]
     ctx.close()
     got_loss, got_correct = res[0]["reduced"]
@@ -182,11 +147,11 @@ def test_keyed_predict_parity_with_merged_single_gpu(tmp_path):
                                     "--test-rows", str(test_rows), "--keyed"])
     got = ldist.merge_keyed_shards([p["keys"] for p in parts], [p["W"] for p in parts], [p["V"] for p in parts], 2)
     keys = np.array(sorted(got), np.uint64)
-    ctx = wk.make_context("fm", F, k, 0, 1, rows, keyed=True)
+    ctx = wk.context("fm", F, k, 0, 1, rows, keyed=True)
     ctx.upload_keyed_params(keys, np.array([got[int(x)][0] for x in keys], np.float32),
                             np.concatenate([got[int(x)][1] for x in keys]).astype(np.float32))
     for r in range(2):
-        rp, fid, _, lab = wk.test_batches(F, test_rows, 1, r)[0]
+        rp, fid, _, lab = mr.test_batches(F, test_rows, 1, r)[0]
         ctx.upload_batch_keys(1, rp, ldist.fmix64(fid), None, None, lab, insert=False)  # every key is in the merged map
         ref = ctx.predict(1)
         assert len(parts[r]["pctr"]) == test_rows
@@ -217,15 +182,8 @@ def test_eval_global_equals_single_gpu_eval(tmp_path, shares):
     assert res[0]["predicted"] == res[1]["predicted"] and res[0]["crafted"] == res[1]["crafted"]
     for o in res:  # rank 1's label count did not match: both ranks raised
         assert o["mismatch"] is not None and "rank(s) [1]" in o["mismatch"], o["mismatch"]
-    batches = [wk.test_batches(F, n[r], 1, r)[0] for r in range(2) if n[r]]
-    rp = [np.zeros(1, np.int64)]
-    off = 0
-    for b in batches:
-        rp.append(b[0][1:] + off)
-        off += b[0][-1]
-    cat = (np.concatenate(rp), np.concatenate([b[1] for b in batches]), None, np.concatenate([b[3] for b in batches]))
-    ctx = wk.make_context("fm", F, k, 0, 1, rows)
-    wk.upload(ctx, "fm", 1, cat)
+    ctx = wk.context("fm", F, k, 0, 1, rows)
+    mr.upload(ctx, "fm", 1, mr.global_batch([mr.test_batches(F, n[r], 1, r)[0] for r in range(2) if n[r]]))
     for key in ("pctr", "crafted"):
         ctx.upload_pred(1, np.concatenate([parts[r][key] for r in range(2)]))
         want = ctx.eval_metrics(1)
@@ -239,10 +197,10 @@ def test_eval_global_equals_single_gpu_eval(tmp_path, shares):
 def test_eval_pred_equals_eval_single_gpu():
     """lctr_eval_pred over host arrays equals lctr_eval on the slot holding the same pCTR and labels, bit for bit"""
     F, k, rows = 20000, 16, 3000
-    b = wk.test_batches(F, rows, 1, 0)[0]
-    ctx = wk.make_context("fm", F, k, 0, 1, rows)
-    ctx.upload_params(*wk.make_params(F, k, "fm"))
-    wk.upload(ctx, "fm", 1, b)
+    b = mr.test_batches(F, rows, 1, 0)[0]
+    ctx = wk.context("fm", F, k, 0, 1, rows)
+    ctx.upload_params(*mr.make_params(F, k, "fm"))
+    mr.upload(ctx, "fm", 1, b)
     pred = ctx.predict(1)
     for p in (pred, wk.crafted_pctr(rows, 0)):
         ctx.upload_pred(1, p)
