@@ -296,6 +296,23 @@ int lctr_wait(lctr_ctx* ctx, uint64_t ticket, float* loss_sum, float* acc_cnt);
  * list that outgrew its inbox (cfg.max_nnz) fails the call with the overflow message.  Refused with world > 1:
  * quirk_sumvx_slot >= 0, and NFM (no NFM predictor exists on any world). */
 int lctr_predict(lctr_ctx* ctx, int slot, int quirk_sumvx_slot, float* pctr);
+/* The forward half of lctr_train_step(ctx, slot, row_begin, row_end, ...) alone: pctr[i] (row_end - row_begin floats,
+ * host; may be NULL: then no copy and no synchronisation) is, bit for bit, the pCTR that train step would compute for row
+ * row_begin + i from the current state -- for every model (FM, FFM, NFM, Wide&Deep), every gradient path the context
+ * chose and both dense-layer precisions.  The same values are left in the slot's pred array, so lctr_eval,
+ * lctr_download_pred and the global metrics of several GPUs work after a score as after a predict.
+ * No side effects: no parameter, optimizer state, dense layer, bf16 weight copy, step counter or statistics entry changes
+ * and no gradient is written; a train step after a score runs exactly as it would have without it.
+ * Dropout masks apply as they stand, because that is the step's forward; a caller who wants a mask-free forward sets
+ * all-ones masks with lctr_mlp_set_mask first.
+ * NFM and Wide&Deep score the rows in blocks of at most max(65536, the largest dense batch the context has run) rows, so
+ * the dense scratch stays bounded whatever the slot's size.
+ * Slots as for lctr_predict: an invalid or stale keyed slot is refused; a lookup-only keyed slot (insert = 0, one GPU) is
+ * scored with its unseen keys on the null row.  world > 1: a COLLECTIVE call like a train step (one pull-only round; every
+ * rank calls it for the same slot in the same order and receives the pCTR of its own rows; an empty share takes part and
+ * receives 0 rows).  NFM's replicated dense layers make each rank's pCTR that of one GPU holding the merged parameters;
+ * Wide&Deep without a dense all-reduce uses the rank's own layers. */
+int lctr_score(lctr_ctx* ctx, int slot, int64_t row_begin, int64_t row_end, float* pctr);
 /* sumVX[rows*k] of a slot as left by the last forward over it (FM_Algo_Abst::sumVX, fm_algo_abst.h:145). */
 int lctr_download_sumvx(lctr_ctx* ctx, int slot, float* sumVX);
 /* per-row sigmoid(pred) of the last forward over the slot */

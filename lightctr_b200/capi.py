@@ -27,7 +27,7 @@ ABI_VERSION = 1
 SYMBOLS = [
     "lctr_last_error", "lctr_abi_version", "lctr_create", "lctr_destroy", "lctr_sync", "lctr_upload_params",
     "lctr_download_params", "lctr_fill_params", "lctr_download_opt_state", "lctr_upload_opt_state", "lctr_upload_batch",
-    "lctr_train_step", "lctr_train_batch", "lctr_train_batch_async", "lctr_wait", "lctr_predict", "lctr_download_sumvx", "lctr_download_pred",
+    "lctr_train_step", "lctr_train_batch", "lctr_train_batch_async", "lctr_wait", "lctr_predict", "lctr_score", "lctr_download_sumvx", "lctr_download_pred",
     "lctr_mlp_forward", "lctr_mlp_backward", "lctr_mlp_apply", "lctr_mlp_upload", "lctr_mlp_download", "lctr_mlp_set_mask", "lctr_mlp_download_grad", "lctr_set_dense_allreduce", "lctr_save_checkpoint", "lctr_load_checkpoint",
     "lctr_save_dataset_bin", "lctr_load_dataset_bin", "lctr_eval", "lctr_upload_pred", "lctr_ipc_export", "lctr_ipc_import",
     "lctr_dense_grad_buffer", "lctr_device_bytes", "lctr_load_libffm", "lctr_free_dataset", "lctr_launch_count", "lctr_stream", "lctr_profile", "lctr_profile_read",
@@ -102,6 +102,7 @@ def load_library():
     L.lctr_train_batch_async.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp, C.POINTER(C.c_uint64)]
     L.lctr_wait.argtypes = [vp, C.c_uint64, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     L.lctr_predict.argtypes = [vp, C.c_int, C.c_int, f32p]
+    L.lctr_score.argtypes = [vp, C.c_int, i64, i64, f32p]
     L.lctr_download_sumvx.argtypes = [vp, C.c_int, f32p]
     L.lctr_download_pred.argtypes = [vp, C.c_int, f32p]
     L.lctr_mlp_upload.argtypes = [vp, C.c_int, f32p, f32p]
@@ -502,6 +503,18 @@ class Context:
     def predict_resident(self, slot, quirk_sumvx_slot=-1):
         """forward only, predictions stay on the device (no host copy, no synchronisation)"""
         _chk(self.L.lctr_predict(self.h, slot, quirk_sumvx_slot, None))
+
+    def score(self, slot, row_begin=0, row_end=None, download=True):
+        """the pCTR a train step on rows [row_begin, row_end) would compute, bit for bit, with no side effects (they are
+        also left in the slot's pred array); download=False keeps them on the device (no copy, no synchronisation)"""
+        if row_end is None:
+            row_end = self.slot_rows[slot]
+        if not download:
+            _chk(self.L.lctr_score(self.h, slot, row_begin, row_end, None))
+            return None
+        out = np.empty(max(row_end - row_begin, 0), np.float32)
+        _chk(self.L.lctr_score(self.h, slot, row_begin, row_end, out.ctypes.data))
+        return out
 
     def download_sumvx(self, slot):
         out = np.empty(self.slot_rows[slot] * self.k, np.float32)

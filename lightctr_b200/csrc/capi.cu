@@ -692,6 +692,58 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
     return read_stats(c, step, loss_sum, acc_cnt);
 }
 
+// lctr_score: the forward of lctr_train_step on rows [rb, re) of the slot -- the launchers of the context's path, with
+// statistics off and the forward-only instances of the kernels that fuse a backward.  NFM and Wide&Deep run their rows in
+// blocks of at most max(kScoreBlock, the rows the dense scratch already holds), which bounds c->z, the fp32 activations
+// and the Wide&Deep source map whatever the slot's size.  On several GPUs the rows are already pulled into the cache.
+constexpr int64_t kScoreBlock = 65536;
+static int score_rows(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
+    const bool compact = c->grad_path == GRAD_COMPACT;
+    switch (c->cfg.model) {
+        case LCTR_MODEL_FM:  // the order-free step's forward is MODE 0 of its kernel family
+            return compact ? launch_fm_forward_tree(c, s, rb, re, false) : launch_fm_forward(c, s, rb, re, false, false);
+        case LCTR_MODEL_FFM: return launch_ffm_score(c, s, rb, re);
+        default: break;
+    }
+    const bool wnd = c->cfg.model == LCTR_MODEL_WND;
+    const int64_t block = std::max<int64_t>(kScoreBlock, (int64_t)c->mlp_cap_rows);
+    for (int64_t b = rb; b < re; b += block) {
+        const int64_t e = std::min(re, b + block);
+        if (mlp_reserve(c, e - b) || (wnd && wnd_reserve(c, e - b))) return 1;
+        const int rc = wnd ? launch_wnd_forward(c, s, b, e)
+                     : compact ? launch_nfm_forward_fused(c, s, b, e) : launch_fm_forward(c, s, b, e, true, false);
+        if (rc || launch_dense_score(c, s, b, e)) return 1;
+    }
+    return 0;
+}
+
+int lctr_score(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* pctr) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
+    Slot& s = c->slots[slot];
+    LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "lctr_score: slot %d holds no usable batch (its last keyed upload failed)", slot);
+    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "lctr_score: slot %d is stale: lctr_evict_keys or a keyed checkpoint load "
+                                               "renumbered rows after it was uploaded; upload it again", slot);
+    LCTR_CHECK(rb >= 0 && re <= s.rows && rb <= re, "lctr_score: rows [%lld,%lld) outside slot (%lld rows)", (long long)rb,
+               (long long)re, (long long)s.rows);
+    if (c->cfg.world > 1) {
+        // one pull-only round for the whole call (no push, merge or updater); the forward waits for the owners' rows as
+        // the step's does: in-kernel on the order-free path, behind a wait kernel otherwise
+        if (dist_pre_step(c, s, slot, c->grad_path == GRAD_COMPACT, false)) return 1;
+        const int rc = score_rows(c, s, rb, re);
+        if (dist_release(c)) return 1;  // also after a failed forward: the owners' next serve waits for it
+        if (rc) return 1;
+        if (dist_check_overflow(c)) return 1;  // a truncated key list gives no score
+    } else if (score_rows(c, s, rb, re)) {
+        return 1;
+    }
+    if (pctr && re > rb) {
+        LCTR_CUDA(cudaMemcpyAsync(pctr, s.pred + rb, (size_t)(re - rb) * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
+    }
+    return 0;
+}
+
 int lctr_train_batch(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
                      const uint16_t* field, const float* val, const int32_t* label, float* loss_sum, float* acc_cnt) {
     LCTR_CHECK(c, "null ctx");

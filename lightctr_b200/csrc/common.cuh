@@ -495,6 +495,7 @@ int mlp_reserve(lctr_ctx* c, int64_t rows);
 bool ffm_grouped_supported(const lctr_ctx* c);
 int ffm_grouped_reserve(lctr_ctx* c, int64_t rows);
 int launch_ffm_forward_tiles(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
+int launch_ffm_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
 int launch_ffm_backward_grouped(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
 int wnd_reserve(lctr_ctx* c, int64_t rows);
 int launch_wnd_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
@@ -508,11 +509,15 @@ inline size_t mlp_in0(const lctr_cfg& cf) {
 int mlp_sync_dense_grad(lctr_ctx* c);
 // scan + clear of a permuted byte map (fm_fused.cuh): appends the ids of the set positions to uniq, counts in *n_uniq
 int launch_slotmap_compact(lctr_ctx* c, uint8_t* mark, size_t T, uint32_t* uniq, unsigned int* n_uniq, cudaStream_t st);
-int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats);  // 0 launched, -1 shape not covered, 1 error
+int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats, bool train);  // 0 launched, -1 shape not covered, 1 error
 int mlp_bf16_prepare(lctr_ctx* c);
 int mlp_bf16_refresh(lctr_ctx* c, int layer);
 int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor);
 int launch_nfm_mlp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor);
+// lctr_score's dense chain on the rows staged in c->z (rows [rb, re) of the slot): pred = sigmoid(wide + out) by the step's
+// kernels without loss, backward or update (fp32: the reference-order layers; bf16: the forward-only tensor-core instances)
+int launch_mlp_bf16_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
+int launch_dense_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
 // keyed mode (keys.cu)
 int keys_alloc(lctr_ctx* c);
 size_t keys_bytes(const lctr_ctx* c);

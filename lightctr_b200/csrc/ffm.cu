@@ -300,7 +300,8 @@ __device__ __forceinline__ void bulk_load(void* sdst, const void* gsrc, uint32_t
                  ::"r"(smem_u32(sdst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-template <bool HAS_VAL>
+// TRAIN = false: the forward-only instance of lctr_score (phases 1 and 2, the pCTR; no statistics, no gradient)
+template <bool HAS_VAL, bool TRAIN>
 __global__ void ffm_tma_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ fid,
                                const uint16_t* __restrict__ field, const float* __restrict__ val,
                                const float* __restrict__ label, const float* __restrict__ W, const float* __restrict__ V,
@@ -407,6 +408,7 @@ __global__ void ffm_tma_kernel(const int64_t* __restrict__ row_ptr, const uint32
         }
         __syncthreads();
     }
+    if (!TRAIN) return;
     const float p = red[64];
     double loss = 0.0, correct = 0.0;
     const float y = label[r];
@@ -507,7 +509,11 @@ static auto ffm_kernel(bool hv, bool train, bool bulk) {
               : (train ? ffm_kernel<VEC, false, true>(bulk) : ffm_kernel<VEC, false, false>(bulk));
 }
 
-static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, bool stats, bool grouped = false) {
+// train: the kernel of a train step (stats: with its statistics); otherwise the forward-only CTA-per-sample kernel.  score:
+// the kernel a train step would choose, in its forward-only instance (lctr_score: the pCTR of the step, no statistics, no
+// gradient)
+static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, bool stats, bool grouped = false,
+                      bool score = false) {
     const int k = (int)c->cfg.factor_cnt, Fc = (int)c->cfg.field_cnt;
     const int64_t rows = re - rb;
     if (rows <= 0) return 0;
@@ -537,6 +543,7 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
     // instruction count but leaves 2 CTAs = 4 warps per SM next to the field-pair tile, against 16 warps of the
     // register-staged kernel, which was the faster of the two on B200s.  The choice has not been re-measured on H100s.
     static const bool use_tma = getenv("LCTR_FFM_TMA") && atoi(getenv("LCTR_FFM_TMA")) == 1;
+    const bool tr = train && !score;  // the instance: forward + backward, or forward only
     if (use_tma && train && vec == 4 && !bulk) {
         // rows per chunk: as many as leave 3 (narrow rows) or 2 CTAs per SM, at least 40, at most 96
         const size_t stage_bytes = ((size_t)A * 16 + 127) / 128 * 128;
@@ -550,21 +557,23 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
         LCTR_CHECK(CR >= 8, "FFM field-pair tile + row buffer do not fit 227 KB shared memory: Fc=%d k=%d", Fc, k);
         const size_t smem2 = (size_t)CR * (stage_bytes + 14) + fixed;
         const int tpb2 = std::max(64, (A + 31) / 32 * 32);
-        return launch(c, {(unsigned)rows, (unsigned)tpb2, smem2, c->stream}, s.has_val ? ffm_tma_kernel<true> : ffm_tma_kernel<false>,
-                      s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW,
+        auto tma = s.has_val ? (tr ? ffm_tma_kernel<true, true> : ffm_tma_kernel<true, false>)
+                             : (tr ? ffm_tma_kernel<false, true> : ffm_tma_kernel<false, false>);
+        return launch(c, {(unsigned)rows, (unsigned)tpb2, smem2, c->stream}, tma, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW,
                       c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot,
-                      stats ? 1 : 0, CR);
+                      stats && tr ? 1 : 0, CR);
     }
     // default for k % 4 == 0: the warp-per-sample kernel of ffm_warp.cu (LCTR_FFM_WARP=0 keeps the CTA-per-sample kernel below)
     if (train && !bulk && vec == 4) {
-        const int rc = launch_ffm_warp(c, s, rb, re, stats);
+        const int rc = launch_ffm_warp(c, s, rb, re, stats && tr, tr);
         if (rc >= 0) return rc;
     }
-    auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, train, bulk) : vec == 2 ? ffm_kernel<2>(s.has_val, train, bulk)
-                                                                    : ffm_kernel<1>(s.has_val, train, bulk);
+    // (a forward-only instance of the bulk kernel is the plain one: ffm_kernel takes the bulk path with training only)
+    auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, tr, bulk) : vec == 2 ? ffm_kernel<2>(s.has_val, tr, bulk)
+                                                                 : ffm_kernel<1>(s.has_val, tr, bulk);
     return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid,
                   s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(),
-                  c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, stats ? 1 : 0, nullptr, nullptr);
+                  c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, stats && tr ? 1 : 0, nullptr, nullptr);
 }
 
 // forward + backward are one fused kernel (stats: a train step; otherwise forward only)
@@ -574,6 +583,12 @@ int launch_ffm_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats)
 // forward half of the feature-grouped step: predictions, loss, and the T tiles for ffm_grouped.cu
 int launch_ffm_forward_tiles(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     return ffm_launch(c, s, rb, re, true, true, true);
+}
+// lctr_score: the pCTR a train step computes, by the forward code of the kernel it runs.  The feature-grouped step's
+// kernel (deterministic = 2) is the CTA-per-sample kernel with its T tiles stored, whose forward-only instance is the
+// plain one
+int launch_ffm_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
+    return ffm_launch(c, s, rb, re, c->grad_path != GRAD_FEATURE_MAJOR, false, false, true);
 }
 
 }  // namespace lctr

@@ -39,7 +39,8 @@ __device__ __forceinline__ void acc4(float4& acc, const float4& v, float x) {
 
 constexpr int max_warps(int passes) { return passes <= 2 ? 10 : 5; }  // 3-4 passes keep kU rows of 3-4 x 16 B per lane: 255 registers
 
-template <int PASSES, bool HAS_VAL>
+// TRAIN = false: the forward-only instance of lctr_score (phases 1 and 2, the pCTR; no statistics, no gradient)
+template <int PASSES, bool HAS_VAL, bool TRAIN>
 __global__ void __launch_bounds__(max_warps(PASSES) * 32, 1)
 ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ fid, const uint16_t* __restrict__ field,
                 const float* __restrict__ val, const float* __restrict__ label, const float* __restrict__ W,
@@ -206,6 +207,7 @@ ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
         const float pr = ref_sigmoid(fm_pred);
         const float y = label[r];
         if (lane == 0) pred[r] = pr;
+        if (!TRAIN) continue;
         const float d = pr - y;
         if (d == 0.f) continue;  // train_ffm_algo.cpp:81-83: rows with pred == label contribute nothing at all
         if (lane == 0 && do_stats) {
@@ -278,16 +280,20 @@ ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
         }
         __syncwarp();  // T is rewritten by the next sample
     }
-    if (do_stats) publish_stats(loss, correct, partial, done, out_slot, false);
+    if (TRAIN && do_stats) publish_stats(loss, correct, partial, done, out_slot, false);
 }
 
 }  // namespace
 
-// returns 0 when launched, -1 when the shape is not covered (caller falls back to ffm.cu), 1 on error
+// returns 0 when launched, -1 when the shape is not covered (caller falls back to ffm.cu), 1 on error.  train = false: the
+// forward-only instance (stats unused)
 template <int PASSES>
-static auto warp_kernel(bool hv) { return hv ? ffm_warp_kernel<PASSES, true> : ffm_warp_kernel<PASSES, false>; }
+static auto warp_kernel(bool hv, bool train) {
+    return hv ? (train ? ffm_warp_kernel<PASSES, true, true> : ffm_warp_kernel<PASSES, true, false>)
+              : (train ? ffm_warp_kernel<PASSES, false, true> : ffm_warp_kernel<PASSES, false, false>);
+}
 
-int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
+int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats, bool train) {
     static const bool off = getenv("LCTR_FFM_WARP") && atoi(getenv("LCTR_FFM_WARP")) == 0;
     const int k = (int)c->cfg.factor_cnt, Fc = (int)c->cfg.field_cnt;
     if (off || k % 4 != 0 || Fc > 64) return -1;
@@ -306,8 +312,8 @@ int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
     ProfScope prof(c, PROF_FFM_FUSED);
     const uint32_t* ids = c->cfg.world > 1 ? s.ent_pslot : s.fid;
     uint8_t* touched = c->cfg.world > 1 ? nullptr : c->touched.get();
-    auto kern = passes == 1 ? warp_kernel<1>(s.has_val) : passes == 2 ? warp_kernel<2>(s.has_val)
-              : passes == 3 ? warp_kernel<3>(s.has_val) : warp_kernel<4>(s.has_val);
+    auto kern = passes == 1 ? warp_kernel<1>(s.has_val, train) : passes == 2 ? warp_kernel<2>(s.has_val, train)
+              : passes == 3 ? warp_kernel<3>(s.has_val, train) : warp_kernel<4>(s.has_val, train);
     return launch(c, {grid, (unsigned)warps * 32, smem, c->stream}, kern, s.row_ptr, ids, s.field, s.val, s.label, c->cW, c->cV, Fc,
                   k, s.pred, c->cgW, c->cgV, touched, c->cfg.l2_reg, rb, rows, (int)tile, c->stat_partial, c->stat_done, out_slot,
                   stats ? 1 : 0);

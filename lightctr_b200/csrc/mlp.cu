@@ -243,6 +243,15 @@ int mlp_forward_only(lctr_ctx* c, int64_t rows, const float** out) {
     return 0;
 }
 
+int launch_dense_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
+    if (re - rb <= 0) return 0;
+    if (c->cfg.mlp_precision == LCTR_MLP_BF16) return launch_mlp_bf16_forward(c, s, rb, re);
+    ProfScope prof(c, PROF_MLP);
+    const float* out = nullptr;
+    // wnd_pred_kernel's sigmoid(wide + out) is the expression nfm_loss_kernel writes
+    return mlp_forward_only(c, re - rb, &out) || launch_wnd_pred(c, s, out, rb, re);
+}
+
 // forward MLP on c->z, loss, backward to c->dz, accumulate dW/db, Adagrad on the MLP (fp32, reference order).
 int launch_nfm_mlp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor) {
     const int B = (int)(re - rb);

@@ -139,7 +139,9 @@ __device__ __forceinline__ void warp_gemm_tn(uint32_t d_base, int d_stride, int 
     }
 }
 
-template <int TM>
+// TRAIN = false: the forward-only instance of lctr_score -- the same staging, forward and output layer, then the pCTR
+// alone: no labels, loss, statistics, deltas or dW / db (dz, label and the statistics arguments are unused).
+template <int TM, bool TRAIN>
 __global__ void __launch_bounds__(TM * 2, 1)
 nfm_mlp_fused_kernel(MlpDev P, const float* __restrict__ z, float* __restrict__ dz, const float* __restrict__ wide,
                      const float* __restrict__ label, float* __restrict__ pred, int64_t rb, int B, double* partial,
@@ -240,6 +242,10 @@ nfm_mlp_fused_kernel(MlpDev P, const float* __restrict__ z, float* __restrict__ 
             if (row < valid) {
                 const int64_t gi = rb + row0 + row;
                 const float p = ref_sigmoid(wide[gi] + o);  // train_nfm_algo.cpp:101-116
+                if (!TRAIN) {
+                    if (lane == 0) pred[gi] = p;
+                    continue;
+                }
                 const float yv = label[gi];
                 if (lane == 0) {
                     pred[gi] = p;
@@ -249,6 +255,7 @@ nfm_mlp_fused_kernel(MlpDev P, const float* __restrict__ z, float* __restrict__ 
                 }
                 d3 = clip15(p - yv);
             }
+            if (!TRAIN) continue;
             dbl += d3;
 #pragma unroll
             for (int q = 0; q < 4; q++) {
@@ -265,16 +272,18 @@ nfm_mlp_fused_kernel(MlpDev P, const float* __restrict__ z, float* __restrict__ 
                 }
             }
         }
+        if (TRAIN) {
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
-            const int c = 2 * lane + 64 * q;
-            if (c < K) red_add_v2(P.dw[nh] + c, dwl[q][0], dwl[q][1]);
+            for (int q = 0; q < 4; q++) {
+                const int c = 2 * lane + 64 * q;
+                if (c < K) red_add_v2(P.dw[nh] + c, dwl[q][0], dwl[q][1]);
+            }
+            if (lane == 0) atomicAdd(P.db[nh], dbl);
         }
-        if (lane == 0) atomicAdd(P.db[nh], dbl);
     }
 
     // ---- backward through the hidden layers (fullyconnLayer.h:120-180)
-    for (int l = nh - 1; l >= 0; l--) {
+    for (int l = nh - 1; TRAIN && l >= 0; l--) {
         const int K = P.in[l], N = P.out[l];
         const int xs = (K + kPad) * 2, ds = (N + kPad) * 2;
         const uint32_t d_base = sbase + P.x_off[l + 1], x_base = sbase + P.x_off[l];
@@ -338,7 +347,7 @@ nfm_mlp_fused_kernel(MlpDev P, const float* __restrict__ z, float* __restrict__ 
             }
         }
     }
-    publish_stats(loss, correct, partial, done, out_slot, false);
+    if (TRAIN) publish_stats(loss, correct, partial, done, out_slot, false);
 }
 
 // fp32 -> bf16 copy of one weight matrix
@@ -432,10 +441,13 @@ int mlp_bf16_refresh(lctr_ctx* c, int layer) {
     return launch(c, {(unsigned)((n + 255) / 256), 256, 0, c->stream}, to_bf16_kernel, L.w, L.w16, L.w16t, L.in, L.out, n);
 }
 
-int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor) {
-    const int B = (int)(re - rb);
+// the dense chain on the B rows staged in c->z (rows [rb, rb + B) of the slot): the wgmma kernel (mlp_umma.cu) or, with a
+// dropout mask or a shape it does not take, the mma.sync kernel.  train: forward, loss and backward of a step; otherwise
+// the forward-only instances, which write the rows' pred alone.
+static int launch_mlp_bf16_kernel(lctr_ctx* c, Slot& s, int64_t rb, int B, bool train) {
     const int nl = c->n_layers, nh = nl - 1;
-    ProfScope prof(c, PROF_MLP);
+    double* out_slot = c->stats + 2 * (c->step % kStatRing);
+    if (c->mlp_umma && !c->mlp_has_mask) return launch_mlp_umma(c, s, rb, B, out_slot, train);
     MlpDev P;
     bf16_layout(c, c->mlp_tm, P);
     P.nl = nl; P.act = c->cfg.activation; P.has_mask = c->mlp_has_mask;
@@ -444,18 +456,27 @@ int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t ro
         P.w16[l] = L.w16; P.bias[l] = L.b; P.mask[l] = L.mask; P.dw[l] = L.dw; P.db[l] = L.db;
     }
     P.w32_last = c->layers[nh].w;
-    double* out_slot = c->stats + 2 * (c->step % kStatRing);
     const unsigned grid = (unsigned)((B + c->mlp_tm - 1) / c->mlp_tm);
+    const bool t128 = c->mlp_tm == 128;
+    auto kern = train ? (t128 ? nfm_mlp_fused_kernel<128, true> : nfm_mlp_fused_kernel<64, true>)
+                      : (t128 ? nfm_mlp_fused_kernel<128, false> : nfm_mlp_fused_kernel<64, false>);
+    return launch(c, {grid, t128 ? 256u : 128u, c->mlp_smem, c->stream}, kern, P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
+                  c->stat_partial, c->stat_done, out_slot);
+}
+
+int launch_mlp_bf16_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
+    if (re - rb <= 0) return 0;
+    ProfScope prof(c, PROF_MLP);
+    return launch_mlp_bf16_kernel(c, s, rb, (int)(re - rb), false);
+}
+
+int launch_nfm_mlp_bf16(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_divisor) {
+    const int B = (int)(re - rb);
+    const int nl = c->n_layers;
+    ProfScope prof(c, PROF_MLP);
     // B == 0 (a rank's empty share on several GPUs): no rows, no gradient; the rank still joins the all-reduce and the
     // replicated updater below
-    if (B > 0) {
-        const int rc = c->mlp_umma && !c->mlp_has_mask  // wgmma kernel (mlp_umma.cu); dropout masks stay on the mma.sync kernel
-            ? launch_mlp_umma(c, s, rb, B, out_slot)
-            : launch(c, {grid, c->mlp_tm == 128 ? 256u : 128u, c->mlp_smem, c->stream},
-                     c->mlp_tm == 128 ? nfm_mlp_fused_kernel<128> : nfm_mlp_fused_kernel<64>, P, c->z, c->dz, s.wide, s.label, s.pred,
-                     rb, B, c->stat_partial, c->stat_done, out_slot);
-        if (rc) return 1;
-    }
+    if (B > 0 && launch_mlp_bf16_kernel(c, s, rb, B, true)) return 1;
     if (mlp_sync_dense_grad(c)) return 1;
     if (!c->mlp_skip_update) {
         DenseSegs S;

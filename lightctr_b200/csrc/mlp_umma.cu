@@ -265,7 +265,9 @@ __device__ __forceinline__ void backward_layer(const Dev& P, unsigned char* smem
     }
 }
 
-template <int ACT>
+// TRAIN = false: the forward-only instance of lctr_score -- the same staging, forward passes and output layer, then the
+// pCTR alone: no labels, loss, statistics, deltas or dW / db (dz, label and the statistics arguments are unused).
+template <int ACT, bool TRAIN>
 __global__ void __launch_bounds__(kThreads, 1)
 nfm_mlp_umma_kernel(Dev P, const float* __restrict__ z, float* __restrict__ dz, const float* __restrict__ wide,
                     const float* __restrict__ label, float* __restrict__ pred, int64_t rb, int B, double* partial,
@@ -310,7 +312,7 @@ nfm_mlp_umma_kernel(Dev P, const float* __restrict__ z, float* __restrict__ dz, 
     for (int h = 0; h < 2; h++) {
         const bool ok = r0 + 8 * h < valid;
         wide_r[h] = ok ? wide[rb + row0 + r0 + 8 * h] : 0.f;
-        label_r[h] = ok ? label[rb + row0 + r0 + 8 * h] : 0.f;
+        label_r[h] = TRAIN && ok ? label[rb + row0 + r0 + 8 * h] : 0.f;
     }
     {   // z tile -> bf16, chunk-major
         const int k = P.in[0], chunks = k / 8;
@@ -395,6 +397,7 @@ nfm_mlp_umma_kernel(Dev P, const float* __restrict__ z, float* __restrict__ dz, 
                 d3[h] = clip15(p - label_r[h]);
             }
         }
+        if constexpr (!TRAIN) return;
         unsigned char* x = smem + P.x_off[nh];
         for (int t = 0; t < K / 64; t++) {
             float sw[16], sd[16];
@@ -489,7 +492,7 @@ int mlp_umma_prepare(lctr_ctx* c) {
     return 0;
 }
 
-int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot) {
+int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot, bool train) {
     umma::Dev P;
     umma::layout(c, P);
     const int nl = c->n_layers, nh = nl - 1;
@@ -508,10 +511,12 @@ int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot) {
         P.trace = d_trace;
     }
     const unsigned grid = (unsigned)((B + umma::kTM - 1) / umma::kTM);
-    // one GPU: dependent on the embedding forward in front of it (fm_fused.cu, MODE 2)
-    if (launch(c, {grid, (unsigned)umma::kThreads, c->mlp_umma_smem, c->stream, c->cfg.world == 1},
-               P.act == LCTR_ACT_SIGMOID ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH>, P,
-               c->z, c->dz, s.wide, s.label, s.pred, rb, B, c->stat_partial, c->stat_done, out_slot))
+    // one GPU: dependent on the embedding forward in front of it (fm_fused.cu, MODE 2), in a train step and in a score alike
+    const bool sig = P.act == LCTR_ACT_SIGMOID;
+    auto kern = train ? (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, true> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, true>)
+                      : (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, false> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, false>);
+    if (launch(c, {grid, (unsigned)umma::kThreads, c->mlp_umma_smem, c->stream, c->cfg.world == 1}, kern, P, c->z, c->dz, s.wide,
+               s.label, s.pred, rb, B, c->stat_partial, c->stat_done, out_slot))
         return 1;
     if (trace) {  // phase boundaries of CTA 0: setup | per layer (mma, epilogue) | output | per layer backward | stats
         unsigned long long h[64];

@@ -34,6 +34,7 @@ __host__ __device__ __forceinline__ size_t tiled_index(size_t j, int in, int out
 
 bool mlp_umma_supported(const lctr_ctx* c);
 int mlp_umma_prepare(lctr_ctx* c);
-int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot);
+// train = false: the forward-only instance (pred of rows [rb, rb + B) only; out_slot unused)
+int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot, bool train);
 
 }  // namespace lctr
