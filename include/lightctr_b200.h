@@ -287,6 +287,10 @@ int lctr_wait(lctr_ctx* ctx, uint64_t ticket, float* loss_sum, float* acc_cnt);
 /* Forward only on a resident slot; pctr (rows floats, host; may be NULL) receives sigmoid(pred).
  * quirk_sumvx_slot >= 0 reproduces FM_Predict's use of the TRAINING sumVX of the same row index
  * (predict/fm_predict.cpp:27-32); -1 computes the proper FM prediction.
+ * Without the quirk, FM and Wide&Deep run the forward of lctr_score, so their pCTR equals lctr_score(ctx, slot, 0, rows)
+ * bit for bit; Wide&Deep runs the rows in blocks as lctr_score does (a bounded dense scratch), and is refused with bf16
+ * dense layers (cfg.mlp_precision = LCTR_MLP_BF16).  FFM predicts with the plain CTA-per-sample forward, or in the
+ * reference's own pair loop order under cfg.deterministic = 1.
  * world > 1 (FM, FFM, Wide&Deep): a COLLECTIVE call, like a train step: every rank calls it for the same slot, in the same
  * order relative to the other collective calls, and receives the pCTR of its own rows.  The owners serve the rows from
  * their shards as they stand after every step issued before the call; no gradient moves and the step counter does not

@@ -623,17 +623,25 @@ static int read_stats(lctr_ctx* c, uint64_t step, float* loss_sum, float* acc_cn
     return 0;
 }
 
-int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_sum, float* acc_cnt) {
+// the slot of a forward entry point (`who` prefixes the messages): in range, holding a usable batch that has rows [rb, re).
+// A keyed slot uploaded with insert = 0 is refused for training only
+static int check_slot(lctr_ctx* c, const char* who, int slot, int64_t rb, int64_t re, bool train) {
     LCTR_CHECK(c, "null ctx");
     LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
+    const Slot& s = c->slots[slot];
+    LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "%s: slot %d holds no usable batch (its last keyed upload failed)", who, slot);
+    LCTR_CHECK(!train || s.key_state != SLOT_KEYS_LOOKUP, "%s: slot %d was uploaded with insert = 0 (lookup only: unseen "
+                                                          "keys sit on the null row, which is never trained)", who, slot);
+    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "%s: slot %d is stale: lctr_evict_keys or a keyed checkpoint load renumbered "
+                                               "rows after it was uploaded; upload it again", who, slot);
+    LCTR_CHECK(rb >= 0 && re <= s.rows && rb <= re, "%s: rows [%lld,%lld) outside slot (%lld rows)", who, (long long)rb,
+               (long long)re, (long long)s.rows);
+    return 0;
+}
+
+int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_sum, float* acc_cnt) {
+    if (check_slot(c, "train_step", slot, rb, re, true)) return 1;
     Slot& s = c->slots[slot];
-    LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "train_step: slot %d holds no usable batch (its last keyed upload failed)", slot);
-    LCTR_CHECK(s.key_state != SLOT_KEYS_LOOKUP, "train_step: slot %d was uploaded with insert = 0 (lookup only: unseen keys "
-                                                "sit on the null row, which is never trained)", slot);
-    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "train_step: slot %d is stale: lctr_evict_keys or a keyed checkpoint load "
-                                               "renumbered rows after it was uploaded; upload it again", slot);
-    LCTR_CHECK(rb >= 0 && re <= s.rows && rb <= re, "train_step: rows [%lld,%lld) outside slot (%lld rows)",
-               (long long)rb, (long long)re, (long long)s.rows);
     LCTR_CHECK(c->cfg.world == 1 || c->cfg.minibatch_size > 0,
                "train_step: multi-GPU contexts need cfg.minibatch_size = the GLOBAL batch (the updater's divisor)");
     const uint64_t step = c->step;
@@ -674,7 +682,7 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
             if (multi && dist_pre_step(c, s, slot, false)) return 1;
             switch (c->cfg.model) {
                 case LCTR_MODEL_FM: rc = launch_fm_forward(c, s, rb, re, false, true) || launch_fm_backward(c, s, rb, re, false); break;
-                case LCTR_MODEL_FFM: rc = launch_ffm_forward(c, s, rb, re, true); break;
+                case LCTR_MODEL_FFM: rc = launch_ffm_forward(c, s, rb, re); break;
                 case LCTR_MODEL_WND:
                     rc = mlp_reserve(c, rows) || wnd_reserve(c, rows) || launch_wnd_forward(c, s, rb, re) ||
                          launch_nfm_mlp(c, s, rb, re, rows) || launch_wnd_backward(c, s, rb, re);
@@ -692,17 +700,19 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
     return read_stats(c, step, loss_sum, acc_cnt);
 }
 
-// lctr_score: the forward of lctr_train_step on rows [rb, re) of the slot -- the launchers of the context's path, with
-// statistics off and the forward-only instances of the kernels that fuse a backward.  NFM and Wide&Deep run their rows in
-// blocks of at most max(kScoreBlock, the rows the dense scratch already holds), which bounds c->z, the fp32 activations
-// and the Wide&Deep source map whatever the slot's size.  On several GPUs the rows are already pulled into the cache.
+// The forward of lctr_score / lctr_predict on rows [rb, re) of the slot, with statistics off and the forward-only instances
+// of the kernels that fuse a backward.  as_step (lctr_score): FFM runs the kernel the train step chooses, so the pCTR is
+// the step's; otherwise (lctr_predict) the plain CTA-per-sample kernel.  The other models run the step's launchers for both.
+// NFM and Wide&Deep run their rows in blocks of at most max(kScoreBlock, the rows the dense scratch already holds), which
+// bounds c->z, the fp32 activations and the Wide&Deep source map whatever the slot's size.  On several GPUs the rows are
+// already pulled into the cache.
 constexpr int64_t kScoreBlock = 65536;
-static int score_rows(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
+static int score_rows(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool as_step) {
     const bool compact = c->grad_path == GRAD_COMPACT;
     switch (c->cfg.model) {
         case LCTR_MODEL_FM:  // the order-free step's forward is MODE 0 of its kernel family
             return compact ? launch_fm_forward_tree(c, s, rb, re, false) : launch_fm_forward(c, s, rb, re, false, false);
-        case LCTR_MODEL_FFM: return launch_ffm_score(c, s, rb, re);
+        case LCTR_MODEL_FFM: return launch_ffm_score(c, s, rb, re, as_step);
         default: break;
     }
     const bool wnd = c->cfg.model == LCTR_MODEL_WND;
@@ -717,24 +727,19 @@ static int score_rows(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     return 0;
 }
 
-int lctr_score(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* pctr) {
-    LCTR_CHECK(c, "null ctx");
-    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
-    Slot& s = c->slots[slot];
-    LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "lctr_score: slot %d holds no usable batch (its last keyed upload failed)", slot);
-    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "lctr_score: slot %d is stale: lctr_evict_keys or a keyed checkpoint load "
-                                               "renumbered rows after it was uploaded; upload it again", slot);
-    LCTR_CHECK(rb >= 0 && re <= s.rows && rb <= re, "lctr_score: rows [%lld,%lld) outside slot (%lld rows)", (long long)rb,
-               (long long)re, (long long)s.rows);
+// score_rows, and the pCTR to pctr.  On several GPUs a collective pull-only round (dist.cu): the owners serve the slot's
+// rows from their shards into the batch-compact cache, the forward runs on that cache and the cache is released to the
+// owners.  No push, merge or updater; the step counter does not advance.
+static int forward_round(lctr_ctx* c, Slot& s, int slot, int64_t rb, int64_t re, bool as_step, float* pctr) {
     if (c->cfg.world > 1) {
-        // one pull-only round for the whole call (no push, merge or updater); the forward waits for the owners' rows as
-        // the step's does: in-kernel on the order-free path, behind a wait kernel otherwise
+        // the forward waits for the owners' rows as the step's does: in-kernel on the order-free path, behind a wait kernel
+        // otherwise
         if (dist_pre_step(c, s, slot, c->grad_path == GRAD_COMPACT, false)) return 1;
-        const int rc = score_rows(c, s, rb, re);
+        const int rc = score_rows(c, s, rb, re, as_step);
         if (dist_release(c)) return 1;  // also after a failed forward: the owners' next serve waits for it
         if (rc) return 1;
-        if (dist_check_overflow(c)) return 1;  // a truncated key list gives no score
-    } else if (score_rows(c, s, rb, re)) {
+        if (dist_check_overflow(c)) return 1;  // a truncated key list gives no pCTR
+    } else if (score_rows(c, s, rb, re, as_step)) {
         return 1;
     }
     if (pctr && re > rb) {
@@ -742,6 +747,11 @@ int lctr_score(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* pctr) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
     }
     return 0;
+}
+
+int lctr_score(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* pctr) {
+    if (check_slot(c, "lctr_score", slot, rb, re, false)) return 1;
+    return forward_round(c, c->slots[slot], slot, rb, re, true, pctr);
 }
 
 int lctr_train_batch(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
@@ -932,82 +942,30 @@ int lctr_wait(lctr_ctx* c, uint64_t ticket, float* loss_sum, float* acc_cnt) {
     return 0;
 }
 
-// world > 1, FM / FFM: a collective pull-only round on the slot (dist.cu): the owners serve its rows from their shards into
-// the batch-compact cache, the single-GPU forward runs on that cache, and the cache is released to the owners.  No push,
-// merge or updater; the step counter does not advance.  Refused before anything is launched, alike on every rank that
-// passes the same arguments.
-static int predict_dist(lctr_ctx* c, Slot& s, int slot, int quirk_sumvx_slot, float* pctr) {
-    if (c->cfg.model == LCTR_MODEL_NFM) {
-        set_error("lctr_predict: the reference ships no NFM predictor (main.cpp:230-233)");
-        return 1;
-    }
-    LCTR_CHECK(quirk_sumvx_slot < 0, "lctr_predict: quirk_sumvx_slot is single-GPU: the quirk predictor reads another slot's "
-                                     "sumVX, which a sharded context does not keep for the rows of this slot (world %d)",
-               c->cfg.world);
-    const bool fm_tree = c->cfg.model == LCTR_MODEL_FM && c->grad_path == GRAD_COMPACT;
-    // the order-free FM forward waits for the owners' rows in-kernel; FFM and the other FM kernels behind a wait kernel
-    if (dist_pre_step(c, s, slot, fm_tree, false)) return 1;
-    int rc;
-    if (c->cfg.model == LCTR_MODEL_FFM) rc = launch_ffm_forward(c, s, 0, s.rows, false);
-    else if (fm_tree) rc = launch_fm_forward_tree(c, s, 0, s.rows, false);
-    else rc = launch_fm_forward(c, s, 0, s.rows, false, false);
-    if (dist_release(c)) return 1;  // also after a failed forward: the owners' next serve waits for it
-    if (rc) return 1;
-    if (dist_check_overflow(c)) return 1;  // a truncated key list gives no prediction
-    if (pctr && s.rows > 0) {
-        LCTR_CUDA(cudaMemcpyAsync(pctr, s.pred, (size_t)s.rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-        LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    }
-    return 0;
-}
-
+// forward_round over the whole slot, or one of the single-GPU predictors only lctr_predict has (the FM quirk predictor, the
+// FFM parity predictor).  Every refusal comes before anything is launched and follows from the arguments and the
+// configuration, so every rank that passes the same arguments refuses alike.
 int lctr_predict(lctr_ctx* c, int slot, int quirk_sumvx_slot, float* pctr) {
-    LCTR_CHECK(c, "null ctx");
-    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "slot %d out of range", slot);
+    if (check_slot(c, "lctr_predict", slot, 0, 0, false)) return 1;  // (rows [0, 0) lie in every slot)
     Slot& s = c->slots[slot];
-    LCTR_CHECK(s.key_state != SLOT_KEYS_INVALID, "lctr_predict: slot %d holds no usable batch (its last keyed upload failed)", slot);
-    LCTR_CHECK(s.key_state != SLOT_KEYS_STALE, "lctr_predict: slot %d is stale: lctr_evict_keys or a keyed checkpoint load "
-                                               "renumbered rows after it was uploaded; upload it again", slot);
-    int rc = 0;
-    if (c->cfg.world > 1 && c->cfg.model != LCTR_MODEL_WND) return predict_dist(c, s, slot, quirk_sumvx_slot, pctr);
-    if (c->cfg.model == LCTR_MODEL_WND) {
-        // Distributed_Algo_Abst::Predict (distributed_algo_abst.h:163-174): a forward pass over the slot; with several
-        // ranks a collective pull-only round (every rank serves the rows its peers need, then releases its cache)
-        const bool multi = c->cfg.world > 1;
-        if (multi && dist_pre_step(c, s, slot, false, false)) return 1;
-        const float* out = nullptr;
-        rc = mlp_reserve(c, s.rows) || wnd_reserve(c, s.rows) || launch_wnd_forward(c, s, 0, s.rows) ||
-             (s.rows > 0 && (mlp_forward_only(c, s.rows, &out) || launch_wnd_pred(c, s, out, 0, s.rows)));
-        if (multi && dist_release(c)) return 1;
-        if (rc) return 1;
-        if (multi && dist_check_overflow(c)) return 1;  // a truncated key list gives no prediction
-        if (pctr) {
-            LCTR_CUDA(cudaMemcpyAsync(pctr, s.pred, (size_t)s.rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-            LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        }
-        return 0;
-    }
-    if (c->cfg.model == LCTR_MODEL_FFM) {
-        // parity mode: the reference's own pair loop order; otherwise the field-pair factorised forward
-        rc = c->cfg.deterministic == 1 ? launch_ffm_predict_inorder(c, s) : launch_ffm_forward(c, s, 0, s.rows, false);
-    } else if (c->cfg.model == LCTR_MODEL_FM) {
-        if (quirk_sumvx_slot >= 0) {
-            LCTR_CHECK(quirk_sumvx_slot < kNumSlots, "quirk slot out of range");
-            rc = launch_predict_quirk(c, s, c->slots[quirk_sumvx_slot]);
-        } else {
-            // order-free contexts predict with the shuffle-tree forward; parity contexts with the in-order one
-            rc = c->grad_path == GRAD_COMPACT ? launch_fm_forward_tree(c, s, 0, s.rows, false) : launch_fm_forward(c, s, 0, s.rows, false, false);
-        }
+    const int model = c->cfg.model;
+    LCTR_CHECK(model != LCTR_MODEL_NFM, "lctr_predict: the reference ships no NFM predictor (main.cpp:230-233)");
+    LCTR_CHECK(quirk_sumvx_slot < 0 || model == LCTR_MODEL_WND || c->cfg.world == 1,
+               "lctr_predict: quirk_sumvx_slot is single-GPU: the quirk predictor reads another slot's sumVX, which a sharded "
+               "context does not keep for the rows of this slot (world %d)", c->cfg.world);
+    LCTR_CHECK(model != LCTR_MODEL_WND || c->cfg.mlp_precision == LCTR_MLP_FP32, "forward-only dense layers run in the fp32 mode");
+    int rc;
+    if (model == LCTR_MODEL_FM && quirk_sumvx_slot >= 0) {
+        LCTR_CHECK(quirk_sumvx_slot < kNumSlots, "quirk slot out of range");
+        rc = launch_predict_quirk(c, s, c->slots[quirk_sumvx_slot]);
+    } else if (model == LCTR_MODEL_FFM && c->cfg.deterministic == 1) {
+        rc = launch_ffm_predict_inorder(c, s);  // parity mode: the reference's own pair loop order
     } else {
-        set_error("lctr_predict: the reference ships no NFM predictor (main.cpp:230-233)");
-        return 1;
+        // FM_Predict::Predict / Distributed_Algo_Abst::Predict (distributed_algo_abst.h:163-174): a forward over the slot
+        return forward_round(c, s, slot, 0, s.rows, false, pctr);
     }
     if (rc) return 1;
-    if (pctr) {
-        LCTR_CUDA(cudaMemcpyAsync(pctr, s.pred, (size_t)s.rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-        LCTR_CUDA(cudaStreamSynchronize(c->stream));
-    }
-    return 0;
+    return pctr ? lctr_download_pred(c, slot, pctr) : 0;
 }
 
 int lctr_download_sumvx(lctr_ctx* c, int slot, float* out) {

@@ -447,7 +447,7 @@ struct ProfScope {
 };
 int launch_fm_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm, bool stats);
 int launch_fm_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm);
-int launch_ffm_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats);
+int launch_ffm_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
 int launch_apply(lctr_ctx* c, int64_t rows_in_step);
 int launch_fm_backward_csc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm);
 // csc.cu: feature-major view built on the device at upload + atomic-free backward with fused updater
@@ -495,13 +495,12 @@ int mlp_reserve(lctr_ctx* c, int64_t rows);
 bool ffm_grouped_supported(const lctr_ctx* c);
 int ffm_grouped_reserve(lctr_ctx* c, int64_t rows);
 int launch_ffm_forward_tiles(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
-int launch_ffm_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
+int launch_ffm_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool as_step);
 int launch_ffm_backward_grouped(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
 int wnd_reserve(lctr_ctx* c, int64_t rows);
 int launch_wnd_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
 int launch_wnd_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
 int launch_wnd_pred(lctr_ctx* c, Slot& s, const float* mlp_out, int64_t rb, int64_t re);
-int mlp_forward_only(lctr_ctx* c, int64_t rows, const float** out);
 // width of the dense chain's input: k (NFM bi-interaction) or Fc * d (Wide&Deep concat)
 inline size_t mlp_in0(const lctr_cfg& cf) {
     return cf.model == LCTR_MODEL_WND ? (size_t)cf.field_cnt * cf.factor_cnt : (size_t)cf.factor_cnt;

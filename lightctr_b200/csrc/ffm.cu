@@ -509,11 +509,9 @@ static auto ffm_kernel(bool hv, bool train, bool bulk) {
               : (train ? ffm_kernel<VEC, false, true>(bulk) : ffm_kernel<VEC, false, false>(bulk));
 }
 
-// train: the kernel of a train step (stats: with its statistics); otherwise the forward-only CTA-per-sample kernel.  score:
-// the kernel a train step would choose, in its forward-only instance (lctr_score: the pCTR of the step, no statistics, no
-// gradient)
-static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, bool stats, bool grouped = false,
-                      bool score = false) {
+// step_kernel: the kernel a train step chooses, otherwise the plain CTA-per-sample kernel; train (implies step_kernel): that
+// kernel's forward + backward instance with the step's statistics, otherwise its forward-only instance
+static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool step_kernel, bool train, bool grouped = false) {
     const int k = (int)c->cfg.factor_cnt, Fc = (int)c->cfg.field_cnt;
     const int64_t rows = re - rb;
     if (rows <= 0) return 0;
@@ -525,7 +523,7 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
     // TMA bulk reduce-add of whole gradient rows is built but off by default: on B200s it was no faster than the vector
     // REDs (both end in the same L2 reductions); not re-measured on H100s.
     static const bool use_bulk = getenv("LCTR_FFM_BULK") && atoi(getenv("LCTR_FFM_BULK")) == 1;
-    const bool bulk = use_bulk && train && vec == 4 && (Fc * k * 4) % 16 == 0;
+    const bool bulk = use_bulk && step_kernel && vec == 4 && (Fc * k * 4) % 16 == 0;
     const size_t smem = ((size_t)Fc * A * vec * 4 + (size_t)Fc * 4 + 80 * 4 + (size_t)kFfmStage * 10 + 15) / 16 * 16 +
                         (bulk ? (size_t)FFM_UNROLL * A * vec * 4 : 0);
     LCTR_CHECK(smem <= 227 * 1024, "FFM field-pair tile needs %zu B shared memory (> 227 KB): Fc=%d k=%d", smem, Fc, k);
@@ -536,15 +534,14 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
         return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream},
                       s.has_val ? ffm_fused_kernel<4, true, true, false, true> : ffm_fused_kernel<4, false, true, false, true>,
                       s.row_ptr, s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, nullptr, c->cfg.l2_reg, rb,
-                      c->stat_partial, c->stat_done, out_slot, stats ? 1 : 0, c->ffm_T, c->ffm_cnt);
+                      c->stat_partial, c->stat_done, out_slot, train ? 1 : 0, c->ffm_T, c->ffm_cnt);
     }
     // LCTR_FFM_TMA=1 selects the TMA-staged kernel (cp.async.bulk rows + mbarrier).  It is parity-green but NOT the
     // default: both kernels are issue-bound rather than memory-bound, and staging whole rows in shared memory cuts the
     // instruction count but leaves 2 CTAs = 4 warps per SM next to the field-pair tile, against 16 warps of the
     // register-staged kernel, which was the faster of the two on B200s.  The choice has not been re-measured on H100s.
     static const bool use_tma = getenv("LCTR_FFM_TMA") && atoi(getenv("LCTR_FFM_TMA")) == 1;
-    const bool tr = train && !score;  // the instance: forward + backward, or forward only
-    if (use_tma && train && vec == 4 && !bulk) {
+    if (use_tma && step_kernel && vec == 4 && !bulk) {
         // rows per chunk: as many as leave 3 (narrow rows) or 2 CTAs per SM, at least 40, at most 96
         const size_t stage_bytes = ((size_t)A * 16 + 127) / 128 * 128;
         const size_t fixed = (size_t)Fc * A * 16 + (size_t)Fc * 4 + 80 * 4 + 64 + 1024;
@@ -557,38 +554,38 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool train, 
         LCTR_CHECK(CR >= 8, "FFM field-pair tile + row buffer do not fit 227 KB shared memory: Fc=%d k=%d", Fc, k);
         const size_t smem2 = (size_t)CR * (stage_bytes + 14) + fixed;
         const int tpb2 = std::max(64, (A + 31) / 32 * 32);
-        auto tma = s.has_val ? (tr ? ffm_tma_kernel<true, true> : ffm_tma_kernel<true, false>)
-                             : (tr ? ffm_tma_kernel<false, true> : ffm_tma_kernel<false, false>);
+        auto tma = s.has_val ? (train ? ffm_tma_kernel<true, true> : ffm_tma_kernel<true, false>)
+                             : (train ? ffm_tma_kernel<false, true> : ffm_tma_kernel<false, false>);
         return launch(c, {(unsigned)rows, (unsigned)tpb2, smem2, c->stream}, tma, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW,
                       c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot,
-                      stats && tr ? 1 : 0, CR);
+                      train ? 1 : 0, CR);
     }
     // default for k % 4 == 0: the warp-per-sample kernel of ffm_warp.cu (LCTR_FFM_WARP=0 keeps the CTA-per-sample kernel below)
-    if (train && !bulk && vec == 4) {
-        const int rc = launch_ffm_warp(c, s, rb, re, stats && tr, tr);
+    if (step_kernel && !bulk && vec == 4) {
+        const int rc = launch_ffm_warp(c, s, rb, re, train, train);
         if (rc >= 0) return rc;
     }
     // (a forward-only instance of the bulk kernel is the plain one: ffm_kernel takes the bulk path with training only)
-    auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, tr, bulk) : vec == 2 ? ffm_kernel<2>(s.has_val, tr, bulk)
-                                                                 : ffm_kernel<1>(s.has_val, tr, bulk);
+    auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, train, bulk) : vec == 2 ? ffm_kernel<2>(s.has_val, train, bulk)
+                                                                    : ffm_kernel<1>(s.has_val, train, bulk);
     return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid,
                   s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(),
-                  c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, stats && tr ? 1 : 0, nullptr, nullptr);
+                  c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, train ? 1 : 0, nullptr, nullptr);
 }
 
-// forward + backward are one fused kernel (stats: a train step; otherwise forward only)
-int launch_ffm_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
-    return ffm_launch(c, s, rb, re, /*train=*/stats, stats);
+// the train step: forward + backward are one fused kernel
+int launch_ffm_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
+    return ffm_launch(c, s, rb, re, true, true);
 }
 // forward half of the feature-grouped step: predictions, loss, and the T tiles for ffm_grouped.cu
 int launch_ffm_forward_tiles(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     return ffm_launch(c, s, rb, re, true, true, true);
 }
-// lctr_score: the pCTR a train step computes, by the forward code of the kernel it runs.  The feature-grouped step's
-// kernel (deterministic = 2) is the CTA-per-sample kernel with its T tiles stored, whose forward-only instance is the
-// plain one
-int launch_ffm_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
-    return ffm_launch(c, s, rb, re, c->grad_path != GRAD_FEATURE_MAJOR, false, false, true);
+// forward only.  as_step (lctr_score): the pCTR a train step computes, by the forward code of the kernel it runs -- the
+// feature-grouped step's kernel (deterministic = 2) is the CTA-per-sample kernel with its T tiles stored, whose
+// forward-only instance is the plain one.  Otherwise (lctr_predict) the plain CTA-per-sample kernel
+int launch_ffm_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool as_step) {
+    return ffm_launch(c, s, rb, re, as_step && c->grad_path != GRAD_FEATURE_MAJOR, false);
 }
 
 }  // namespace lctr

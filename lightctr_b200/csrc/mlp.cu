@@ -235,21 +235,12 @@ static int mlp_apply_dev(lctr_ctx* c, uint64_t mb) {
     return 0;
 }
 
-// forward only (fp32 reference-order layers) on the rows staged in c->z; *out = the last layer's output [rows]
-int mlp_forward_only(lctr_ctx* c, int64_t rows, const float** out) {
-    LCTR_CHECK(c->cfg.mlp_precision == LCTR_MLP_FP32, "forward-only dense layers run in the fp32 mode");
-    if (mlp_forward_dev(c, (int)rows)) return 1;
-    *out = c->layers[c->n_layers - 1].act;
-    return 0;
-}
-
 int launch_dense_score(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     if (re - rb <= 0) return 0;
     if (c->cfg.mlp_precision == LCTR_MLP_BF16) return launch_mlp_bf16_forward(c, s, rb, re);
     ProfScope prof(c, PROF_MLP);
-    const float* out = nullptr;
     // wnd_pred_kernel's sigmoid(wide + out) is the expression nfm_loss_kernel writes
-    return mlp_forward_only(c, re - rb, &out) || launch_wnd_pred(c, s, out, rb, re);
+    return mlp_forward_dev(c, (int)(re - rb)) || launch_wnd_pred(c, s, c->layers[c->n_layers - 1].act, rb, re);
 }
 
 // forward MLP on c->z, loss, backward to c->dz, accumulate dW/db, Adagrad on the MLP (fp32, reference order).

@@ -1,4 +1,4 @@
-"""Collective predict and global test metrics on multi-GPU trainers (csrc/capi.cu: predict_dist, csrc/dist.cu: pull-only
+"""Collective predict and global test metrics on multi-GPU trainers (csrc/capi.cu: forward_round, csrc/dist.cu: pull-only
 rounds and the cache release, lightctr_b200/dist.py: eval_global): 2 ranks sharing cuda:0 over CUDA IPC against a
 single-GPU context of the same cfg holding the merged parameters."""
 import numpy as np

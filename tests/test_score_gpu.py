@@ -7,7 +7,9 @@
   * no side effects: parameters, optimizer state, dense layers and the following loss trajectory equal a twin context's
     that never scored;
   * blocks: NFM / Wide&Deep score a slot past 2 x 65536 rows in blocks, with the same bits as sub-range scores;
-  * keyed slots, refusals and launch counts."""
+  * keyed slots, refusals and launch counts;
+  * lctr_predict shares the forward: it equals the score bit for bit wherever both run the same kernel (FM, fp32
+    Wide&Deep in blocks, FFM on the plain CTA-per-sample kernel), and its refusals launch nothing."""
 import numpy as np
 import pytest
 
@@ -195,7 +197,10 @@ def test_blocks_of_a_large_slot(name, monkeypatch):
     for l, (w, b) in enumerate(layers):
         c.mlp_upload(l, w, b)
     c.upload_batch(0, *_batch(6, rows, Fc, nnz_per=6, distinct=False))
+    pred = c.predict(0) if model == capi.MODEL_WND else None  # first, so the predict itself runs in blocks
     whole = c.score(0)
+    if pred is not None:
+        assert np.array_equal(_bits(pred), _bits(whole))
     cuts = [0, 1000, 70001, 131072, rows]
     parts = np.concatenate([c.score(0, a, b) for a, b in zip(cuts[:-1], cuts[1:])])
     assert np.array_equal(_bits(whole), _bits(parts))
@@ -225,6 +230,47 @@ def test_nfm_bf16_score_vs_emulation(name, monkeypatch):
     p_ref, _, _ = _emulate(torch, capi, rp, fid, label, info["W"], info["V"], info["k"], info["layers"], capi.ACT_SIGMOID,
                            info["masks"])
     assert np.max(np.abs(s - p_ref)) < 3e-3, np.max(np.abs(s - p_ref))  # bf16-ulp flips of single activations
+    c.close()
+
+
+@pytest.mark.parametrize("name", ["fm_k16_compact", "fm_k16_compact_val", "fm_k10_dense", "fm_det1", "fm_det2", "ffm_det2",
+                                  "wnd_fp32"])
+def test_predict_equals_score(name, monkeypatch):
+    """where lctr_predict runs the forward of lctr_score, before and after updates"""
+    from lightctr_b200 import capi
+    c, _ = _make(capi, monkeypatch, name, 300)
+    for rnd in range(2):
+        assert np.array_equal(_bits(c.predict(0)), _bits(c.score(0))), (name, rnd)
+        for _ in range(3):
+            c.train_step(0)
+    c.close()
+
+
+def test_ffm_predict_is_the_plain_cta_forward(monkeypatch):
+    """FFM with deterministic = 0 predicts on the plain CTA-per-sample kernel, not on its step's warp kernel: the score of
+    a deterministic = 2 twin (whose step runs the CTA kernel) holding the same parameters and batch"""
+    from lightctr_b200 import capi
+    rows = 300
+    a, info = _make(capi, monkeypatch, "ffm_det0_warp", rows)
+    b = capi.Context(capi.MODEL_FFM, F, info["k"], field_cnt=info["Fc"], deterministic=2, minibatch_size=rows)
+    b.upload_batch(0, *info["batch"])
+    for rnd in range(2):
+        b.upload_params(*a.download_params())
+        assert np.array_equal(_bits(a.predict(0)), _bits(b.score(0))), rnd
+        for _ in range(3):
+            a.train_step(0)
+    a.close(); b.close()
+
+
+@pytest.mark.parametrize("name, msg", [("nfm_fp32_det0", "ships no NFM predictor"),
+                                       ("wnd_bf16", "forward-only dense layers run in the fp32 mode")])
+def test_predict_refusals_launch_nothing(name, msg, monkeypatch):
+    from lightctr_b200 import capi
+    c, _ = _make(capi, monkeypatch, name, 300)
+    n0 = c.launch_count()
+    with pytest.raises(capi.LctrError, match=msg):
+        c.predict(0)
+    assert c.launch_count() == n0
     c.close()
 
 
