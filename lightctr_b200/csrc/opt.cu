@@ -3,7 +3,7 @@
 // Reference: AdagradUpdater_Num::update (util/gradientUpdater.h:139-150), FTRLUpdater::update
 // (:252-273), AdamUpdater_Num::update (util/momentumUpdater.h:187-210), applied by
 // Train_*_Algo::ApplyGrad as a DENSE sweep over all F*(rowlen+1) coordinates.  Every updater
-// skips coordinates whose batch gradient is exactly 0, and a gradient is only ever produced
+// skips coordinates whose batch gradient is exactly 0 (opt.cuh), and a gradient is only ever produced
 // for the fids present in the batch (L2 terms are added inside the nnz loops), so visiting only
 // the touched fids is exactly equivalent (SURVEY.md 8a-7).  The backward kernels mark
 // touched[fid] = 1 (plain byte store, idempotent); this kernel scans the byte map 16 B per lane,

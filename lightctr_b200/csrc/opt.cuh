@@ -1,5 +1,11 @@
-// lightctr_b200/csrc/opt.cuh -- per-coordinate updater arithmetic shared by the sparse apply kernel (opt.cu)
-// and the fused feature-major backward (fm.cu).
+// lightctr_b200/csrc/opt.cuh -- per-coordinate updater arithmetic shared by every applier: the sparse apply kernel
+// (opt.cu), the compact updater (fm_fused.cuh), the feature-major backwards (fm.cu, csc.cu, ffm_grouped.cu) and the
+// owner-side merge of several GPUs (dist.cu).
+//
+// Contract: a coordinate whose batch gradient is exactly zero keeps its parameter and its state, under all nine rules.
+// An applier may therefore visit any set of coordinates that holds the nonzero ones -- whole rows of the batch's
+// features, only their nonzero 4-wide slices, or only the rows a merge saw a nonzero record for -- and every applier
+// gives the same result.  tests/test_updaters_gpu.py holds each applier to the oracle bit for bit under every rule.
 #pragma once
 #include <math.h>
 
@@ -70,6 +76,9 @@ __device__ __forceinline__ void update_one(const OptParams& P, float corr, float
         // operand (distributed_algo_abst.h:39-72: `a * b` is `a.w *= b.w; return a`), which the sequences below follow.
         // corr == 0: scalar parameters (the W call); corr != 0: tensors (the V call) -- Wide&Deep tensors take the tensor
         // SGD form under LCTR_OPT_PS_SGD when P.tensor_v is set.
+        // A zero gradient is never pushed (Value::checkPreferredValue, push.h:62-65), so it changes nothing here either:
+        // without this, DCASGD would still copy w into its shadow and DCASGDA would still decay its accumulator.
+        if (g == 0.f) return;
         if (P.opt == LCTR_OPT_PS_SGD) {
             if (corr != 0.f && P.tensor_v) {  // :232-237  scaler = -lr / minibatch (double expression narrowed to float)
                 const float scaler = (float)(-1.0 * (double)P.lr / (double)P.mb);

@@ -225,10 +225,13 @@ class FMOracle:
                 L.orc_adam(hi - lo, w, g, a, self.s2[lo:hi], C.byref(self.iter), B, self.lr,
                            np.float32(getattr(self, "beta1", 0.8)), np.float32(getattr(self, "beta2", 0.999)))
             elif opt.startswith("ps_"):
-                # the PS only touches the keys a worker pushed (paramserver.h:214-216): the batch's features
+                # the PS only touches the keys a worker pushed (paramserver.h:214-216): the batch's features, and of
+                # those only the coordinates whose gradient is nonzero -- the worker never pushes a zero
+                # (Value::checkPreferredValue, push.h:62-65), so a zero leaves DCASGD's shadow and DCASGDA's decay alone
                 kind = {"ps_sgd": 0, "ps_adagrad": 1, "ps_dcasgd": 2, "ps_dcasgda": 3}[opt]
                 keys = np.unique(self.ds.fid).astype(np.int64)
                 idx = keys if lo == 0 else (keys[:, None] * k + np.arange(k)[None, :]).ravel()
+                idx = idx[g[idx] != 0]
                 ww, gg, aa = w[idx].copy(), g[idx].copy(), a[idx].copy()
                 sh = self.s2[lo:hi][idx].copy() if kind >= 2 else np.zeros(1, np.float32)
                 L.orc_ps_update(kind, len(idx), ww, gg, aa, sh, B, self.lr, 0)
