@@ -270,6 +270,28 @@ int lctr_key_admission_stats(lctr_ctx* ctx, uint64_t* dropped_entries, uint64_t*
  * loss_sum / acc_cnt (may be NULL: then no host sync happens) receive the summed logloss and the
  * number of correct rows of this step, the quantities the reference prints per epoch. */
 int lctr_train_step(lctr_ctx* ctx, int slot, int64_t row_begin, int64_t row_end, float* loss_sum, float* acc_cnt);
+/* Per-row weights of the batch resident in `slot`: rows must equal the slot's row count; weight = NULL drops them.
+ * Each weight must be finite and >= 0; a refused call writes nothing to the device.  Returns once `weight` may be reused.
+ * THE RULE: a train step over rows [rb, re) of a weighted slot trains row r as if its whole per-row objective were
+ * multiplied by w_r.
+ *   - head: wherever a kernel forms d_r = p_r - y_r it uses fl(w_r (p_r - y_r)) (FM, FFM, the dense layers' output delta,
+ *     the NFM and Wide&Deep wide terms);
+ *   - L2: every term the reference adds per occurrence inside the row loop uses fl(w_r l2) for l2 (FM's l2 W, also inside
+ *     the V multiplier, and l2 V; FFM's per-pair l2 c_ib; NFM's l2 W and l2 V; Wide&Deep's l2 W);
+ *   - the dense layers' +-15 clip (fullyconnLayer.h:129-131) applies to the weighted deltas;
+ *   - FFM's early return on d == 0 tests the weighted d, so a zero-weight row contributes nothing;
+ *   - the updater's divisor stays cfg.minibatch_size, or the rows of the step;
+ *   - loss_sum = sum w_r loss_r and acc_cnt = sum w_r [correct_r].
+ * So w = 1 everywhere is bit for bit an unweighted step; a row of w = 0 is an absent row, except that its entries still
+ * mark rows for change tracking; an integer w equals w copies of the row (fixed minibatch_size) up to re-association and
+ * the clip.  Weights change gradients and statistics, not pCTR: lctr_score, lctr_predict and lctr_eval / lctr_eval_pred
+ * ignore them (a weighted AUC needs non-integer buckets and is not offered).  They are batch data: any later upload into
+ * the slot (lctr_upload_batch, lctr_upload_batch_keys with insert 0 or 1, lctr_upload_libffm, lctr_train_batch) drops
+ * them, and checkpoints do not carry them.  Key admission removes entries, never rows, so weights stay aligned with the
+ * rows of a keyed slot.  On several GPUs each rank weights its own rows (no collective).
+ * Every model, deterministic mode and world trains weighted slots.  The statistics cost one more launch, and only when
+ * loss_sum or acc_cnt is requested.  Not covered: the streamed pipeline (lctr_train_batch_async takes no weights). */
+int lctr_set_row_weights(lctr_ctx* ctx, int slot, int64_t rows, const float* weight);
 /* End-to-end convenience: upload_batch(slot 0) + train_step + result readback, host buffers in. */
 int lctr_train_batch(lctr_ctx* ctx, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
                      const uint16_t* field, const float* val, const int32_t* label, float* loss_sum,

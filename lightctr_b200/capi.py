@@ -35,7 +35,7 @@ SYMBOLS = [
     "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys", "lctr_load_checkpoint_shards", "lctr_eval_pred",
     "lctr_download_host_tier", "lctr_evict_host_tier", "lctr_set_key_admission", "lctr_decay_key_admission",
     "lctr_key_admission_stats", "lctr_upload_libffm", "lctr_download_batch", "lctr_track_changes", "lctr_save_checkpoint_delta",
-    "lctr_load_checkpoint_chain", "lctr_checkpoint_hash",
+    "lctr_load_checkpoint_chain", "lctr_checkpoint_hash", "lctr_set_row_weights",
 ]
 NO_LIMIT = (1 << 64) - 1  # lctr_evict_keys: UINT64_MAX = no limit
 TEXT_BEGIN, TEXT_END, TEXT_LOOKUP = 1, 2, 4  # lctr_upload_libffm flags
@@ -99,6 +99,7 @@ def load_library():
     L.lctr_upload_opt_state.argtypes = [vp, f32p, f32p]
     L.lctr_upload_batch.argtypes = [vp, C.c_int, i64, i64, vp, vp, vp, vp, vp]
     L.lctr_train_step.argtypes = [vp, C.c_int, i64, i64, C.POINTER(C.c_float), C.POINTER(C.c_float)]
+    L.lctr_set_row_weights.argtypes = [vp, C.c_int, i64, f32p]
     L.lctr_train_batch.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     L.lctr_train_batch_async.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp, C.POINTER(C.c_uint64)]
     L.lctr_wait.argtypes = [vp, C.c_uint64, C.POINTER(C.c_float), C.POINTER(C.c_float)]
@@ -478,6 +479,15 @@ class Context:
         if val is not None and all_ones_as_null and np.all(val == 1.0):
             val = None
         self.upload_batch(slot, ds.row_ptr, ds.fid, ds.field, val, ds.label[:len(ds.row_ptr) - 1])
+
+    def set_row_weights(self, slot, weights):
+        """Per-row weights (float32, one per row of the batch in `slot`) for the train steps on that batch; None drops
+        them.  Any later upload into the slot drops them too (include/lightctr_b200.h states the rule)."""
+        if weights is None:
+            _chk(self.L.lctr_set_row_weights(self.h, slot, 0, None))
+            return
+        w = np.ascontiguousarray(weights, np.float32)
+        _chk(self.L.lctr_set_row_weights(self.h, slot, len(w), _p(w)))
 
     def train_step(self, slot=0, row_begin=0, row_end=None, want_stats=True):
         if row_end is None:

@@ -4,6 +4,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <vector>
 
 #include "opt.cuh"
@@ -67,6 +68,32 @@ __global__ void label_to_float_kernel(const int32_t* in, float* out, int64_t n_a
     const int64_t n = hdr ? hdr[0] : n_arg;
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = (float)in[i];
+}
+
+// Statistics of a weighted step: sum w loss and sum w [correct] over rows [rb, re), from the predictions the step left in
+// the slot and the same loss_terms as the unweighted kernels, written over the ring slot those kernels published to.
+// A zero-weight row is absent; FFM (skip_zero_head) also leaves out every row whose weighted head fl(w (p - y)) is zero,
+// as its kernels do
+__global__ void weighted_stats_kernel(const float* __restrict__ pred, const float* __restrict__ label, const float* __restrict__ rw,
+                                      int64_t rb, int64_t re, int skip_zero_head, double* partial, unsigned int* done,
+                                      double* out_slot) {
+    double loss = 0.0, correct = 0.0;
+    for (int64_t r = rb + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < re; r += (int64_t)gridDim.x * blockDim.x) {
+        const float w = rw[r];
+        if (w == 0.f || (skip_zero_head && w * (pred[r] - label[r]) == 0.f)) continue;
+        double l1, c1;
+        loss_terms(pred[r], label[r], l1, c1);
+        loss += (double)w * l1;
+        correct += (double)w * c1;
+    }
+    publish_stats(loss, correct, partial, done, out_slot, false);
+}
+
+int launch_weighted_stats(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
+    if (re <= rb) return 0;
+    const unsigned grid = (unsigned)std::min<int64_t>((re - rb + 255) / 256, (int64_t)c->sm_count * 4);
+    return launch(c, {grid, 256, 0, c->stream}, weighted_stats_kernel, s.pred, s.label, s.rw, rb, re,
+                  c->cfg.model == LCTR_MODEL_FFM ? 1 : 0, c->stat_partial, c->stat_done, c->stats + 2 * (c->step % kStatRing));
 }
 
 // synthetic initialisation on the device (bench only): W = 0, V[f][j] = scale * N(0,1) from a counter-based hash of
@@ -185,6 +212,7 @@ int slot_fit(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz) {
 int upload_tail(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows, int64_t nnz, bool keyed, const int64_t* h_row_ptr,
                 const uint32_t* h_fid, const float* h_val) {
     Slot& s = c->slots[slot];
+    s.has_rw = false;  // weights belong to the batch they were set for (key admission drops entries, never rows)
     if (keyed && c->keys) {  // key admission dropped entries: the slot holds the kept ones, before the slot map
         if (keys_admission_compact(c, s, st, rows, &nnz)) return 1;
         s.nnz = nnz;
@@ -493,6 +521,7 @@ static int upload_batch_on(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows,
     LCTR_CHECK((c->cfg.model != LCTR_MODEL_FFM && c->cfg.model != LCTR_MODEL_WND) || field || nnz == 0,
                "upload_batch: FFM / Wide&Deep need the field array");
     Slot& s = c->slots[slot];
+    s.has_rw = false;
     if (slot_fit(c, s, rows, nnz)) return 1;
     s.rows = rows; s.nnz = nnz;
     s.has_val = val != nullptr;
@@ -616,6 +645,33 @@ int lctr_upload_batch_keys(lctr_ctx* c, int slot, int64_t rows, int64_t nnz, con
     return 0;
 }
 
+int lctr_set_row_weights(lctr_ctx* c, int slot, int64_t rows, const float* weight) {
+    LCTR_CHECK(c, "null ctx");
+    LCTR_CHECK(slot >= 0 && slot < kNumSlots, "lctr_set_row_weights: slot %d out of range", slot);
+    Slot& s = c->slots[slot];
+    if (!weight) {
+        s.has_rw = false;
+        return 0;
+    }
+    LCTR_CHECK(s.rows > 0, "lctr_set_row_weights: slot %d holds no rows", slot);
+    LCTR_CHECK(rows == s.rows, "lctr_set_row_weights: %lld weights for the %lld rows of slot %d", (long long)rows, (long long)s.rows,
+               slot);
+    for (int64_t r = 0; r < rows; r++)
+        LCTR_CHECK(std::isfinite(weight[r]) && weight[r] >= 0.f, "lctr_set_row_weights: weight %g of row %lld is not a finite "
+                   "value >= 0", (double)weight[r], (long long)r);
+    s.has_rw = false;  // until the new weights are in place
+    if (rows > s.cap_rw) {
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));  // a step may still read the old array
+        s.cap_rw = 0;
+        if (alloc_group(sized(s.rw, (size_t)s.cap_rows))) return 1;
+        s.cap_rw = s.cap_rows;
+    }
+    LCTR_CUDA(cudaMemcpyAsync(s.rw, weight, (size_t)rows * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    LCTR_CUDA(cudaStreamSynchronize(c->stream));  // the caller's buffer may be reused on return
+    s.has_rw = true;
+    return 0;
+}
+
 static int read_stats(lctr_ctx* c, uint64_t step, float* loss_sum, float* acc_cnt) {
     if (!loss_sum && !acc_cnt) return 0;
     if (c->cfg.world > 1 && dist_check_overflow(c)) return 1;
@@ -699,6 +755,9 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
             rc = rc || (multi ? dist_post_step(c, s, slot, rows) : launch_apply(c, rows));
             break;
     }
+    // a weighted slot's statistics are the weighted sums, computed from the step's predictions once its kernels are done,
+    // when the caller reads them
+    if (!rc && s.has_rw && (loss_sum || acc_cnt)) rc = launch_weighted_stats(c, s, rb, re);
     // change tracking: the rows the stepped entries name, behind the updater (several GPUs: the owner marks the rows it
     // served, dist_post_step)
     if (rc || (!multi && track_mark_entries(c, s, rb, re, nullptr, c->stream))) return 1;
@@ -873,7 +932,7 @@ static int train_batch_async_graph(lctr_ctx* c, int64_t rows, int64_t nnz, const
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
         if (pipe_graph_capture(c, p, val != nullptr)) return 1;
     }
-    s.rows = rows; s.nnz = nnz; s.has_val = val != nullptr; s.has_field = false;
+    s.rows = rows; s.nnz = nnz; s.has_val = val != nullptr; s.has_field = false; s.has_rw = false;
     if (c->pipe_issued >= (uint64_t)kPipe) LCTR_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_computed[p], 0));
     LCTR_CUDA(cudaMemcpyAsync(s.row_ptr, row_ptr, (size_t)(rows + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, c->copy_stream));
     LCTR_CUDA(cudaMemcpyAsync(s.fid, fid, (size_t)nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, c->copy_stream));

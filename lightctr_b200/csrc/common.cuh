@@ -186,7 +186,14 @@ struct Slot {
     // keyed upload failed, nothing may run on the slot until it is uploaded again; SLOT_KEYS_STALE = lctr_evict_keys
     // renumbered rows after the upload, so the slot's row ids are out of date until it is uploaded again
     int key_state = 0;
+    // per-row weights of the resident batch (lctr_set_row_weights): rw[r] scales row r's loss head, its per-occurrence L2
+    // terms and its statistics.  Every upload into the slot clears has_rw; rw keeps its storage (cap_rw rows)
+    Buf<float> rw;
+    int64_t cap_rw = 0;
+    bool has_rw = false;
 };
+// the weights a train step over the slot applies, or null when the slot has none (kernels take their unweighted instance)
+inline const float* row_weights(const Slot& s) { return s.has_rw ? s.rw.get() : nullptr; }
 enum { SLOT_KEYS_OK = 0, SLOT_KEYS_LOOKUP = 1, SLOT_KEYS_INVALID = 2, SLOT_KEYS_STALE = 3 };
 
 struct OptParams;
@@ -401,6 +408,16 @@ __device__ __forceinline__ void loss_terms(float p, float y, double& loss, doubl
     loss = (y == 1.f) ? (double)(-logf(p)) : -log(1.0 - (double)p);
     correct = ((p > 0.5f && y == 1.f) || (p < 0.5f && y == 0.f)) ? 1.0 : 0.0;
 }
+// the head of a weighted row: fl(w (p - y)); the unweighted instances (RW = false) form p - y alone
+template <bool RW>
+__device__ __forceinline__ float row_head(float p, float y, const float* __restrict__ rw, int64_t r) {
+    return RW ? __ldg(rw + r) * (p - y) : p - y;
+}
+// the per-occurrence L2 coefficient of a weighted row: fl(w l2)
+template <bool RW>
+__device__ __forceinline__ float row_l2(float l2, const float* __restrict__ rw, int64_t r) {
+    return RW ? __ldg(rw + r) * l2 : l2;
+}
 
 // Block-level accumulation of (loss, correct) into ctx statistics; the last block to finish publishes
 // the step totals into the ring slot and re-arms the accumulators (no memset launches between steps).
@@ -581,6 +598,9 @@ int flags_to_list(lctr_ctx* c, const uint8_t* flags, size_t n, uint32_t* list, s
 int keys_reset_rows(lctr_ctx* c, size_t lo, size_t hi);
 // single-slot uploads (capi.cu): room in the slot for rows x nnz, and the common end once the batch sits in the slot
 int slot_fit(lctr_ctx* c, Slot& s, int64_t rows, int64_t nnz);
+// weighted slots (capi.cu): the statistics of rows [rb, re) as sum w loss and sum w [correct], from the step's predictions,
+// written over what the step's kernels published
+int launch_weighted_stats(lctr_ctx* c, Slot& s, int64_t rb, int64_t re);
 int upload_tail(lctr_ctx* c, cudaStream_t st, int slot, int64_t rows, int64_t nnz, bool keyed, const int64_t* h_row_ptr,
                 const uint32_t* h_fid, const float* h_val);
 

@@ -245,10 +245,11 @@ __device__ __forceinline__ void apply_update(const ParamView& T, const OptParams
 
 // SHORT segments (<= 8 entries): one LPR-lane group per segment.  The <= 8 row indices are fetched with one load
 // per lane, then all <= 8 sumVX / pred / label gathers are in flight together: two memory round trips per segment.
-template <int K, bool HAS_VAL>
+// RW (both kernels): the slot's row weights rw scale each entry's head and L2 terms by its row's weight
+template <int K, bool HAS_VAL, bool RW = false>
 __global__ void __launch_bounds__(256)
 csc_backward_short_kernel(const uint32_t* __restrict__ work, const unsigned int* __restrict__ totals, CscView C,
-                          ParamView T, float l2, OptParams P_arg, const OptParams* __restrict__ dP) {
+                          ParamView T, float l2, OptParams P_arg, const OptParams* __restrict__ dP, const float* __restrict__ rw) {
     const OptParams P = dP ? *dP : P_arg;
     constexpr int LPR = K / 4;
     constexpr int G = 32 / LPR;
@@ -277,18 +278,19 @@ csc_backward_short_kernel(const uint32_t* __restrict__ work, const unsigned int*
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (sv) v = *reinterpret_cast<const float4*>(T.V + (size_t)f * K + 4 * q);
         float4 s[kShortMax];
-        float d[kShortMax], x[kShortMax];
+        float d[kShortMax], x[kShortMax], l2e[kShortMax];
 #pragma unroll
         for (int e = 0; e < kShortMax; e++) {
             const uint32_t r = __shfl_sync(kFull, rows[e / LPR], (e % LPR), LPR);
             x[e] = HAS_VAL ? __shfl_sync(kFull, xs[e / LPR], (e % LPR), LPR) : 1.f;
             s[e] = ldg_f4(C.sumvx + (size_t)r * K + 4 * q);       // row 0 for e >= n: valid address, masked below
-            d[e] = __ldg(C.pred + r) - __ldg(C.label + r);
+            d[e] = row_head<RW>(__ldg(C.pred + r), __ldg(C.label + r), rw, r);
+            l2e[e] = row_l2<RW>(l2, rw, r);
         }
         double u[4] = {0.0, 0.0, 0.0, 0.0}, gws = 0.0;
 #pragma unroll
         for (int e = 0; e < kShortMax; e++)
-            if (e < n) accumulate<K>(u, gws, s[e], d[e], x[e], w, v, l2);
+            if (e < n) accumulate<K>(u, gws, s[e], d[e], x[e], w, v, RW ? l2e[e] : l2);
         if (sv) apply_update<K>(T, P, f, q, w, v, u, gws);
     }
 }
@@ -297,11 +299,11 @@ csc_backward_short_kernel(const uint32_t* __restrict__ work, const unsigned int*
 // fetched with one coalesced load, the next chunk's indices are prefetched while the current one is reduced.
 // Segments of more than kTaskLen entries are covered by several tasks whose partial sums meet in acc[seg] (double
 // atomics); the task that arrives last applies the update and re-arms the accumulator.
-template <int K, bool HAS_VAL>
+template <int K, bool HAS_VAL, bool RW = false>
 __global__ void __launch_bounds__(256)
 csc_backward_long_kernel(const uint2* __restrict__ work, const unsigned int* __restrict__ totals, CscView C, ParamView T,
                          double* __restrict__ acc, unsigned int* __restrict__ arrived, float l2, OptParams P_arg,
-                         const OptParams* __restrict__ dP) {
+                         const OptParams* __restrict__ dP, const float* __restrict__ rw) {
     const OptParams P = dP ? *dP : P_arg;
     constexpr int LPR = K / 4;
     constexpr int G = 32 / LPR;
@@ -330,18 +332,19 @@ csc_backward_long_kernel(const uint2* __restrict__ work, const unsigned int* __r
             rows_n = nb < n ? __ldg(C.ent_row + eb + nb) : 0u;
             if (HAS_VAL) xs_n = nb < n ? __ldg(C.ent_x + eb + nb) : 0.f;
             float4 s[LPR];
-            float d[LPR], x[LPR];
+            float d[LPR], x[LPR], l2e[LPR];
 #pragma unroll
             for (int j = 0; j < LPR; j++) {
                 const int e = j * G + g;
                 const uint32_t r = __shfl_sync(kFull, rows, e);
                 x[j] = HAS_VAL ? __shfl_sync(kFull, xs, e) : 1.f;
                 s[j] = ldg_f4(C.sumvx + (size_t)r * K + 4 * q);
-                d[j] = __ldg(C.pred + r) - __ldg(C.label + r);
+                d[j] = row_head<RW>(__ldg(C.pred + r), __ldg(C.label + r), rw, r);
+                l2e[j] = row_l2<RW>(l2, rw, r);
             }
 #pragma unroll
             for (int j = 0; j < LPR; j++)
-                if (base + j * G + g < n) accumulate<K>(u, gws, s[j], d[j], x[j], w, v, l2);
+                if (base + j * G + g < n) accumulate<K>(u, gws, s[j], d[j], x[j], w, v, RW ? l2e[j] : l2);
         }
         // fold the G entry slots (lanes with the same q) in a fixed tree
 #pragma unroll
@@ -480,10 +483,14 @@ static int bwd_go(lctr_ctx* c, Slot& s, const OptParams& P, const OptParams* dP)
     const CscView C{s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, s.label, s.pred, s.sumvx};
     const ParamView T{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V};
     const uint2* longs = s.long_list;
-    return launch(c, {grid, 256, 0, c->stream}, s.has_val ? csc_backward_long_kernel<K, true> : csc_backward_long_kernel<K, false>,
-                  longs, s.csc_totals, C, T, s.csc_acc, s.csc_arrived, c->cfg.l2_reg, P, dP) ||
-           launch(c, {grid, 256, 0, c->stream}, s.has_val ? csc_backward_short_kernel<K, true> : csc_backward_short_kernel<K, false>,
-                  s.short_list, s.csc_totals, C, T, c->cfg.l2_reg, P, dP);
+    const bool rw = s.has_rw;
+    auto lk = s.has_val ? (rw ? csc_backward_long_kernel<K, true, true> : csc_backward_long_kernel<K, true>)
+                        : (rw ? csc_backward_long_kernel<K, false, true> : csc_backward_long_kernel<K, false>);
+    auto sk = s.has_val ? (rw ? csc_backward_short_kernel<K, true, true> : csc_backward_short_kernel<K, true>)
+                        : (rw ? csc_backward_short_kernel<K, false, true> : csc_backward_short_kernel<K, false>);
+    return launch(c, {grid, 256, 0, c->stream}, lk, longs, s.csc_totals, C, T, s.csc_acc, s.csc_arrived, c->cfg.l2_reg, P, dP,
+                  row_weights(s)) ||
+           launch(c, {grid, 256, 0, c->stream}, sk, s.short_list, s.csc_totals, C, T, c->cfg.l2_reg, P, dP, row_weights(s));
 }
 
 // dP != nullptr (graph capture): the updater parameters are read from device memory at run time

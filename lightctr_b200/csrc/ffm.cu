@@ -64,14 +64,16 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 // GROUPED (with TRAIN): the gradient phase is replaced by storing the sample's field-pair tile T (as [a][b][k], so that
 // {T[a][b]}_b -- what an entry of field a needs -- is one contiguous row) and its per-field counts; the feature-grouped
 // backward of ffm_grouped.cu consumes them.
-template <int VEC, bool HAS_VAL, bool TRAIN, bool BULK, bool GROUPED = false>
+// RW (training instances): the slot's row weights rw scale the head d and the per-pair L2 coefficient of each row
+template <int VEC, bool HAS_VAL, bool TRAIN, bool BULK, bool GROUPED = false, bool RW = false>
 __global__ void ffm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ fid,
                                  const uint16_t* __restrict__ field, const float* __restrict__ val,
                                  const float* __restrict__ label, const float* __restrict__ W,
                                  const float* __restrict__ V, int Fc, int k, float* __restrict__ pred,
                                  float* __restrict__ gW, float* __restrict__ gV, uint8_t* __restrict__ touched,
-                                 float l2, int64_t rb, double* partial, unsigned int* done, double* out_slot,
-                                 int do_stats, float* __restrict__ Tbuf, uint16_t* __restrict__ cntbuf) {
+                                 float l2_arg, int64_t rb, double* partial, unsigned int* done, double* out_slot,
+                                 int do_stats, float* __restrict__ Tbuf, uint16_t* __restrict__ cntbuf,
+                                 const float* __restrict__ rw) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int A = Fc * k / VEC;   // slots per row
     const int PPF = k / VEC;      // slots (parts) per field
@@ -181,7 +183,8 @@ __global__ void ffm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint
     double loss = 0.0, correct = 0.0;
     if (TRAIN) {
         const float y = label[r];
-        const float d = p - y;
+        const float d = row_head<RW>(p, y, rw, r);
+        const float l2 = row_l2<RW>(l2_arg, rw, r);
         if (d != 0.f) {  // train_ffm_algo.cpp:81-83: rows with pred == label contribute nothing at all
             if (t == 0 && do_stats) loss_terms(p, y, loss, correct);
             if (GROUPED) {
@@ -301,13 +304,14 @@ __device__ __forceinline__ void bulk_load(void* sdst, const void* gsrc, uint32_t
 }
 
 // TRAIN = false: the forward-only instance of lctr_score (phases 1 and 2, the pCTR; no statistics, no gradient)
-template <bool HAS_VAL, bool TRAIN>
+// RW: as ffm_fused_kernel
+template <bool HAS_VAL, bool TRAIN, bool RW = false>
 __global__ void ffm_tma_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ fid,
                                const uint16_t* __restrict__ field, const float* __restrict__ val,
                                const float* __restrict__ label, const float* __restrict__ W, const float* __restrict__ V,
                                int Fc, int k, float* __restrict__ pred, float* __restrict__ gW, float* __restrict__ gV,
-                               uint8_t* __restrict__ touched, float l2, int64_t rb, double* partial, unsigned int* done,
-                               double* out_slot, int do_stats, int CR /* rows per chunk */) {
+                               uint8_t* __restrict__ touched, float l2_arg, int64_t rb, double* partial, unsigned int* done,
+                               double* out_slot, int do_stats, int CR /* rows per chunk */, const float* __restrict__ rw) {
     extern __shared__ __align__(16) unsigned char smem_raw[];  // (dynamic shared memory starts 1024 B aligned)
     const int A = Fc * k / 4;     // 16 B slots per row
     const int PPF = k / 4;        // slots per field
@@ -412,7 +416,8 @@ __global__ void ffm_tma_kernel(const int64_t* __restrict__ row_ptr, const uint32
     const float p = red[64];
     double loss = 0.0, correct = 0.0;
     const float y = label[r];
-    const float d = p - y;
+    const float d = row_head<RW>(p, y, rw, r);
+    const float l2 = row_l2<RW>(l2_arg, rw, r);
     if (d != 0.f) {  // train_ffm_algo.cpp:81-83: rows with pred == label contribute nothing at all
         if (t == 0 && do_stats) loss_terms(p, y, loss, correct);
         // ---- phase 3: gradients, from the rows still in shared memory (one chunk) or streamed a second time -----------
@@ -500,13 +505,15 @@ int launch_ffm_predict_inorder(lctr_ctx* c, Slot& s) {
 
 // the CTA-per-sample kernel's instance (bulk: the TMA bulk reduce-add of the gradient rows, 4-wide training rows only)
 template <int VEC, bool HV, bool TR>
-static auto ffm_kernel(bool bulk) {
+static auto ffm_kernel(bool bulk, bool rw) {
+    if (TR && rw)
+        return bulk ? ffm_fused_kernel<VEC, HV, TR, (VEC == 4) && TR, false, TR> : ffm_fused_kernel<VEC, HV, TR, false, false, TR>;
     return bulk ? ffm_fused_kernel<VEC, HV, TR, (VEC == 4) && TR> : ffm_fused_kernel<VEC, HV, TR, false>;
 }
 template <int VEC>
-static auto ffm_kernel(bool hv, bool train, bool bulk) {
-    return hv ? (train ? ffm_kernel<VEC, true, true>(bulk) : ffm_kernel<VEC, true, false>(bulk))
-              : (train ? ffm_kernel<VEC, false, true>(bulk) : ffm_kernel<VEC, false, false>(bulk));
+static auto ffm_kernel(bool hv, bool train, bool bulk, bool rw) {
+    return hv ? (train ? ffm_kernel<VEC, true, true>(bulk, rw) : ffm_kernel<VEC, true, false>(bulk, rw))
+              : (train ? ffm_kernel<VEC, false, true>(bulk, rw) : ffm_kernel<VEC, false, false>(bulk, rw));
 }
 
 // step_kernel: the kernel a train step chooses, otherwise the plain CTA-per-sample kernel; train (implies step_kernel): that
@@ -532,9 +539,10 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool step_ke
     if (grouped) {
         LCTR_CHECK(train && vec == 4 && c->ffm_T && c->ffm_cnt, "grouped FFM step needs k %% 4 == 0 and the tile buffer");
         return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream},
-                      s.has_val ? ffm_fused_kernel<4, true, true, false, true> : ffm_fused_kernel<4, false, true, false, true>,
+                      s.has_rw ? (s.has_val ? ffm_fused_kernel<4, true, true, false, true, true> : ffm_fused_kernel<4, false, true, false, true, true>)
+                               : (s.has_val ? ffm_fused_kernel<4, true, true, false, true> : ffm_fused_kernel<4, false, true, false, true>),
                       s.row_ptr, s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, nullptr, c->cfg.l2_reg, rb,
-                      c->stat_partial, c->stat_done, out_slot, train ? 1 : 0, c->ffm_T, c->ffm_cnt);
+                      c->stat_partial, c->stat_done, out_slot, train ? 1 : 0, c->ffm_T, c->ffm_cnt, row_weights(s));
     }
     // LCTR_FFM_TMA=1 selects the TMA-staged kernel (cp.async.bulk rows + mbarrier).  It is parity-green but NOT the
     // default: both kernels are issue-bound rather than memory-bound, and staging whole rows in shared memory cuts the
@@ -554,11 +562,12 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool step_ke
         LCTR_CHECK(CR >= 8, "FFM field-pair tile + row buffer do not fit 227 KB shared memory: Fc=%d k=%d", Fc, k);
         const size_t smem2 = (size_t)CR * (stage_bytes + 14) + fixed;
         const int tpb2 = std::max(64, (A + 31) / 32 * 32);
-        auto tma = s.has_val ? (train ? ffm_tma_kernel<true, true> : ffm_tma_kernel<true, false>)
-                             : (train ? ffm_tma_kernel<false, true> : ffm_tma_kernel<false, false>);
+        const bool rw = train && s.has_rw;
+        auto tma = s.has_val ? (train ? (rw ? ffm_tma_kernel<true, true, true> : ffm_tma_kernel<true, true>) : ffm_tma_kernel<true, false>)
+                             : (train ? (rw ? ffm_tma_kernel<false, true, true> : ffm_tma_kernel<false, true>) : ffm_tma_kernel<false, false>);
         return launch(c, {(unsigned)rows, (unsigned)tpb2, smem2, c->stream}, tma, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW,
                       c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot,
-                      train ? 1 : 0, CR);
+                      train ? 1 : 0, CR, row_weights(s));
     }
     // default for k % 4 == 0: the warp-per-sample kernel of ffm_warp.cu (LCTR_FFM_WARP=0 keeps the CTA-per-sample kernel below)
     if (step_kernel && !bulk && vec == 4) {
@@ -566,11 +575,12 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool step_ke
         if (rc >= 0) return rc;
     }
     // (a forward-only instance of the bulk kernel is the plain one: ffm_kernel takes the bulk path with training only)
-    auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, train, bulk) : vec == 2 ? ffm_kernel<2>(s.has_val, train, bulk)
-                                                                    : ffm_kernel<1>(s.has_val, train, bulk);
+    const bool rw = train && s.has_rw;
+    auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, train, bulk, rw) : vec == 2 ? ffm_kernel<2>(s.has_val, train, bulk, rw)
+                                                                        : ffm_kernel<1>(s.has_val, train, bulk, rw);
     return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid,
                   s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(),
-                  c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, train ? 1 : 0, nullptr, nullptr);
+                  c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, train ? 1 : 0, nullptr, nullptr, row_weights(s));
 }
 
 // the train step: forward + backward are one fused kernel

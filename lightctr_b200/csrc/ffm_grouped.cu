@@ -46,9 +46,10 @@ struct FfmParams {
 // the task's entries on its own -- the NS = ceil(A/32) warps of a task never synchronise (the entry metadata they all
 // read is 10 B per entry against a 16 B x 32 lane tile slice).  One float4 slot per lane keeps the register count low
 // enough for 16 warps per SM with kFfmU = 8 entries (8 x 512 B per warp) in flight.
-template <bool HAS_VAL, bool FUSE>
+// RW: the slot's row weights rw scale each entry's head d and its per-pair L2 coefficient by its row's weight
+template <bool HAS_VAL, bool FUSE, bool RW = false>
 __global__ void __launch_bounds__(128, 4)
-ffm_backward_grouped_kernel(FfmView C, FfmParams T, int Fc, int k, int NS, float l2, OptParams P) {
+ffm_backward_grouped_kernel(FfmView C, FfmParams T, int Fc, int k, int NS, float l2, OptParams P, const float* __restrict__ rw) {
     const int lane = threadIdx.x & 31;
     const int A = Fc * k / 4, PPF = k / 4;
     const size_t rowlen = (size_t)Fc * k;
@@ -109,12 +110,13 @@ ffm_backward_grouped_kernel(FfmView C, FfmParams T, int Fc, int k, int NS, float
             const int my_a = a_n;
             const float my_x = x_n;
             if (base + 32 < n) meta(base + 32, r_n, a_n, x_n);
-            const float my_d = base + lane < n ? __ldg(C.pred + my_r) - __ldg(C.label + my_r) : 0.f;
+            const float my_d = base + lane < n ? row_head<RW>(__ldg(C.pred + my_r), __ldg(C.label + my_r), rw, my_r) : 0.f;
+            const float my_l2 = RW && base + lane < n ? row_l2<RW>(l2, rw, my_r) : l2;
             const int m = min(32, n - base);
             for (int j0 = 0; j0 < m; j0 += kFfmU) {
                 float4 tt[kFfmU];
                 int cb[kFfmU], a[kFfmU];
-                float x[kFfmU], d[kFfmU];
+                float x[kFfmU], d[kFfmU], l2e[kFfmU];
 #pragma unroll
                 for (int uu = 0; uu < kFfmU; uu++) {
                     const int j = min(j0 + uu, 31);
@@ -122,6 +124,7 @@ ffm_backward_grouped_kernel(FfmView C, FfmParams T, int Fc, int k, int NS, float
                     a[uu] = __shfl_sync(kFull, my_a, j);
                     x[uu] = HAS_VAL ? __shfl_sync(kFull, my_x, j) : 1.f;
                     d[uu] = __shfl_sync(kFull, my_d, j);
+                    if (RW) l2e[uu] = __shfl_sync(kFull, my_l2, j);
                     if (j0 + uu >= m) d[uu] = 0.f;  // train_ffm_algo.cpp:81-83: d == 0 contributes nothing at all
                     // unconditional loads (row 0 / stale tiles are valid addresses): not behind the pred/label gather
                     if (own) {
@@ -137,11 +140,12 @@ ffm_backward_grouped_kernel(FfmView C, FfmParams T, int Fc, int k, int NS, float
                     if (d[uu] == 0.f) continue;
                     nvalid++;
                     const float sx = d[uu] * x[uu];
-                    gws += (double)(sx + l2 * w);  // train_ffm_algo.cpp:98
+                    const float l2u = RW ? l2e[uu] : l2;
+                    gws += (double)(sx + l2u * w);  // train_ffm_algo.cpp:98
                     const bool self = fq == a[uu];
                     const int c_ib = cb[uu] - (self ? 1 : 0);
                     if (c_ib <= 0) continue;
-                    const float lc = l2 * (float)c_ib;
+                    const float lc = l2u * (float)c_ib;
                     float4 tv = tt[uu];
                     if (self) { tv.x -= x[uu] * v.x; tv.y -= x[uu] * v.y; tv.z -= x[uu] * v.z; tv.w -= x[uu] * v.w; }
                     u0 += (double)(sx * tv.x + lc * v.x);
@@ -244,9 +248,11 @@ int launch_ffm_backward_grouped(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     const unsigned grid = (unsigned)c->sm_count * 8;
     ProfScope prof(c, PROF_FM_BWD_CSC);
     LCTR_CHECK(NS >= 1 && NS <= 4, "grouped FFM backward: row of %d floats exceeds 512", Fc * k);
-    auto kern = s.has_val ? (fuse ? ffm_backward_grouped_kernel<true, true> : ffm_backward_grouped_kernel<true, false>)
-                          : (fuse ? ffm_backward_grouped_kernel<false, true> : ffm_backward_grouped_kernel<false, false>);
-    return launch(c, {grid, 128, 0, c->stream}, kern, C, T, Fc, k, NS, c->cfg.l2_reg, P);
+    auto kern = s.has_rw ? (s.has_val ? (fuse ? ffm_backward_grouped_kernel<true, true, true> : ffm_backward_grouped_kernel<true, false, true>)
+                                      : (fuse ? ffm_backward_grouped_kernel<false, true, true> : ffm_backward_grouped_kernel<false, false, true>))
+                         : (s.has_val ? (fuse ? ffm_backward_grouped_kernel<true, true> : ffm_backward_grouped_kernel<true, false>)
+                                      : (fuse ? ffm_backward_grouped_kernel<false, true> : ffm_backward_grouped_kernel<false, false>));
+    return launch(c, {grid, 128, 0, c->stream}, kern, C, T, Fc, k, NS, c->cfg.l2_reg, P, row_weights(s));
 }
 
 }  // namespace lctr

@@ -39,14 +39,15 @@ __device__ __forceinline__ void acc4(float4& acc, const float4& v, float x) {
 
 constexpr int max_warps(int passes) { return passes <= 2 ? 10 : 5; }  // 3-4 passes keep kU rows of 3-4 x 16 B per lane: 255 registers
 
-// TRAIN = false: the forward-only instance of lctr_score (phases 1 and 2, the pCTR; no statistics, no gradient)
-template <int PASSES, bool HAS_VAL, bool TRAIN>
+// TRAIN = false: the forward-only instance of lctr_score (phases 1 and 2, the pCTR; no statistics, no gradient).  RW: the
+// slot's row weights rw scale the head and the per-pair L2 terms of each row
+template <int PASSES, bool HAS_VAL, bool TRAIN, bool RW = false>
 __global__ void __launch_bounds__(max_warps(PASSES) * 32, 1)
 ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ fid, const uint16_t* __restrict__ field,
                 const float* __restrict__ val, const float* __restrict__ label, const float* __restrict__ W,
                 const float* __restrict__ V, int Fc, int k, float* __restrict__ pred, float* __restrict__ gW,
                 float* __restrict__ gV, uint8_t* __restrict__ touched, float l2, int64_t rb, int64_t rows, int tile_bytes,
-                double* partial, unsigned int* done, double* out_slot, int do_stats) {
+                double* partial, unsigned int* done, double* out_slot, int do_stats, const float* __restrict__ rw) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int KU = group_size(PASSES);
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
@@ -208,7 +209,7 @@ ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
         const float y = label[r];
         if (lane == 0) pred[r] = pr;
         if (!TRAIN) continue;
-        const float d = pr - y;
+        const float d = row_head<RW>(pr, y, rw, r);
         if (d == 0.f) continue;  // train_ffm_algo.cpp:81-83: rows with pred == label contribute nothing at all
         if (lane == 0 && do_stats) {
             double l1, c1;
@@ -220,9 +221,10 @@ ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
         // g[i][b] = d x_i (T[b][a_i] - [b == a_i] x_i v) + l2 c_ib v,  c_ib = cnt[b] - [b == a_i]; nothing at all when c_ib == 0
         float lc0[PASSES], lc1[PASSES];  // l2 * c_ib for an entry of another field / of the slot's own field
         bool go0[PASSES], go1[PASSES];
+        const float l2r = row_l2<RW>(l2, rw, r);
 #pragma unroll
         for (int p = 0; p < PASSES; p++) {
-            lc0[p] = l2 * (float)cntf[p]; lc1[p] = l2 * (float)(cntf[p] - 1);
+            lc0[p] = l2r * (float)cntf[p]; lc1[p] = l2r * (float)(cntf[p] - 1);
             go0[p] = sb[p] >= 0 && cntf[p] > 0; go1[p] = sb[p] >= 0 && cntf[p] > 1;
         }
         for (int64_t s0 = b0; s0 < e0; s0 += 128) {
@@ -230,7 +232,7 @@ ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
 #pragma unroll
           for (int c = 0; c < 4; c++)
               if (s0 + 32 * c + lane < e0) {
-                  red_add_f32(gW + f_c[c], fmaf(l2, w_c[c], d * x_c[c]));  // train_ffm_algo.cpp:98
+                  red_add_f32(gW + f_c[c], fmaf(l2r, w_c[c], d * x_c[c]));  // train_ffm_algo.cpp:98
                   if (touched) touched[f_c[c]] = 1;
               }
 #pragma unroll 1
@@ -288,7 +290,8 @@ ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
 // returns 0 when launched, -1 when the shape is not covered (caller falls back to ffm.cu), 1 on error.  train = false: the
 // forward-only instance (stats unused)
 template <int PASSES>
-static auto warp_kernel(bool hv, bool train) {
+static auto warp_kernel(bool hv, bool train, bool rw) {
+    if (train && rw) return hv ? ffm_warp_kernel<PASSES, true, true, true> : ffm_warp_kernel<PASSES, false, true, true>;
     return hv ? (train ? ffm_warp_kernel<PASSES, true, true> : ffm_warp_kernel<PASSES, true, false>)
               : (train ? ffm_warp_kernel<PASSES, false, true> : ffm_warp_kernel<PASSES, false, false>);
 }
@@ -312,11 +315,12 @@ int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats, bo
     ProfScope prof(c, PROF_FFM_FUSED);
     const uint32_t* ids = c->cfg.world > 1 ? s.ent_pslot : s.fid;
     uint8_t* touched = c->cfg.world > 1 ? nullptr : c->touched.get();
-    auto kern = passes == 1 ? warp_kernel<1>(s.has_val, train) : passes == 2 ? warp_kernel<2>(s.has_val, train)
-              : passes == 3 ? warp_kernel<3>(s.has_val, train) : warp_kernel<4>(s.has_val, train);
+    const bool rw = s.has_rw;
+    auto kern = passes == 1 ? warp_kernel<1>(s.has_val, train, rw) : passes == 2 ? warp_kernel<2>(s.has_val, train, rw)
+              : passes == 3 ? warp_kernel<3>(s.has_val, train, rw) : warp_kernel<4>(s.has_val, train, rw);
     return launch(c, {grid, (unsigned)warps * 32, smem, c->stream}, kern, s.row_ptr, ids, s.field, s.val, s.label, c->cW, c->cV, Fc,
                   k, s.pred, c->cgW, c->cgV, touched, c->cfg.l2_reg, rb, rows, (int)tile, c->stat_partial, c->stat_done, out_slot,
-                  stats ? 1 : 0);
+                  stats ? 1 : 0, row_weights(s));
 }
 
 }  // namespace lctr

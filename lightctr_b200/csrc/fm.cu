@@ -178,13 +178,15 @@ fm_forward_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restric
 // ------------------------------------------------------------------------------------------------
 // backward: scatter-add into the dense update_g (W part, V part) with vector REDs + touched marks
 // ------------------------------------------------------------------------------------------------
-template <int LPR, int VEC, bool HAS_VAL, bool NFM>
+// RW: the slot's row weights rw scale the head and the per-occurrence L2 terms
+template <int LPR, int VEC, bool HAS_VAL, bool NFM, bool RW = false>
 __global__ void __launch_bounds__(256)
 fm_backward_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ fid,
                    const float* __restrict__ val, const float* __restrict__ label, const float* __restrict__ W,
                    const float* __restrict__ V, int k, const float* __restrict__ pred,
                    const float* __restrict__ sumvx, const float* __restrict__ dz, float* __restrict__ gW,
-                   float* __restrict__ gV, uint8_t* __restrict__ touched, float l2, int64_t rb, int64_t re) {
+                   float* __restrict__ gV, uint8_t* __restrict__ touched, float l2_arg, int64_t rb, int64_t re,
+                   const float* __restrict__ rw) {
     constexpr int G = 32 / LPR;
     const int lane = threadIdx.x & 31;
     const int q = lane % LPR, g = lane / LPR;
@@ -192,7 +194,8 @@ fm_backward_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restri
     if (r >= re) return;
     const bool qa = q * VEC < k;
     const int64_t b = row_ptr[r], e = row_ptr[r + 1];
-    const float d = pred[r] - label[r];  // LogisticGradW: (pred - label) * x  (fm_algo_abst.h:159-161)
+    const float d = row_head<RW>(pred[r], label[r], rw, r);  // LogisticGradW: (pred - label) * x  (fm_algo_abst.h:159-161)
+    const float l2 = row_l2<RW>(l2_arg, rw, r);
     float s[VEC], dzv[VEC];
 #pragma unroll
     for (int c = 0; c < VEC; c++) {
@@ -251,21 +254,21 @@ static bool pick_shape(int k, Shape& sh) {
 }
 
 // the instance of fm_backward_kernel for the row shape
-template <int VEC, bool HV, bool NF>
+template <int VEC, bool HV, bool NF, bool RW>
 static auto backward_lpr(int lpr) {
     switch (lpr) {
-        case 1: return fm_backward_kernel<1, VEC, HV, NF>;
-        case 2: return fm_backward_kernel<2, VEC, HV, NF>;
-        case 4: return fm_backward_kernel<4, VEC, HV, NF>;
-        case 8: return fm_backward_kernel<8, VEC, HV, NF>;
-        case 16: return fm_backward_kernel<16, VEC, HV, NF>;
-        default: return fm_backward_kernel<32, VEC, HV, NF>;
+        case 1: return fm_backward_kernel<1, VEC, HV, NF, RW>;
+        case 2: return fm_backward_kernel<2, VEC, HV, NF, RW>;
+        case 4: return fm_backward_kernel<4, VEC, HV, NF, RW>;
+        case 8: return fm_backward_kernel<8, VEC, HV, NF, RW>;
+        case 16: return fm_backward_kernel<16, VEC, HV, NF, RW>;
+        default: return fm_backward_kernel<32, VEC, HV, NF, RW>;
     }
 }
-template <int VEC>
+template <int VEC, bool RW>
 static auto backward_kernel(int lpr, bool hv, bool nfm) {
-    return hv ? (nfm ? backward_lpr<VEC, true, true>(lpr) : backward_lpr<VEC, true, false>(lpr))
-              : (nfm ? backward_lpr<VEC, false, true>(lpr) : backward_lpr<VEC, false, false>(lpr));
+    return hv ? (nfm ? backward_lpr<VEC, true, true, RW>(lpr) : backward_lpr<VEC, true, false, RW>(lpr))
+              : (nfm ? backward_lpr<VEC, false, true, RW>(lpr) : backward_lpr<VEC, false, false, RW>(lpr));
 }
 
 // Coalesced variant for K % 8 == 0: LPR = K/4 lanes cover one V row with float4 loads (a 64 B row is ONE request of two
@@ -456,10 +459,11 @@ int launch_fm_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
     if (rows <= 0) return 0;
     const unsigned grid = (unsigned)((rows + 7) / 8);
     ProfScope prof(c, PROF_FM_BWD_RED);
-    return launch(c, {grid, 256, 0, c->stream},
-                  sh.vec == 4 ? backward_kernel<4>(sh.lpr, s.has_val, nfm) : backward_kernel<1>(sh.lpr, s.has_val, nfm), s.row_ptr,
-                  c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val, s.label, c->cW, c->cV, k, s.pred, s.sumvx, c->dz, c->cgW, c->cgV,
-                  c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb, re);
+    auto kern = s.has_rw ? (sh.vec == 4 ? backward_kernel<4, true>(sh.lpr, s.has_val, nfm) : backward_kernel<1, true>(sh.lpr, s.has_val, nfm))
+                         : (sh.vec == 4 ? backward_kernel<4, false>(sh.lpr, s.has_val, nfm) : backward_kernel<1, false>(sh.lpr, s.has_val, nfm));
+    return launch(c, {grid, 256, 0, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val, s.label, c->cW,
+                  c->cV, k, s.pred, s.sumvx, c->dz, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb,
+                  re, row_weights(s));
 }
 
 
@@ -472,14 +476,15 @@ int launch_fm_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
 // so the summed gradient equals the reference's canonical single-thread result bit for bit (given equal
 // inputs).  The updater then runs on the register-resident gradient: no update_g traffic, no atomics,
 // no touched map.
-template <int LR, bool HAS_VAL, bool NFM>
+// RW: the slot's row weights rw scale each entry's head and L2 terms by its row's weight
+template <int LR, bool HAS_VAL, bool NFM, bool RW = false>
 __global__ void __launch_bounds__(256)
 fm_backward_csc_kernel(const int64_t* __restrict__ seg_ptr, const uint32_t* __restrict__ seg_fid,
                        const uint32_t* __restrict__ ent_row, const float* __restrict__ ent_x, int64_t seg_begin,
                        int64_t seg_end, const float* __restrict__ label, const float* __restrict__ pred,
                        const float* __restrict__ sumvx, const float* __restrict__ dz, int64_t rb, float* __restrict__ W,
                        float* __restrict__ V, float* __restrict__ s1W, float* __restrict__ s1V, float* __restrict__ s2W,
-                       float* __restrict__ s2V, int k, float l2, OptParams P) {
+                       float* __restrict__ s2V, int k, float l2, OptParams P, const float* __restrict__ rw) {
     constexpr int SPW = 32 / LR;
     const int lane = threadIdx.x & 31;
     const int c = lane % LR, grp = lane / LR;
@@ -498,13 +503,14 @@ fm_backward_csc_kernel(const int64_t* __restrict__ seg_ptr, const uint32_t* __re
         const int cnt = n - base;
         const uint32_t my_row = c < cnt ? __ldg(ent_row + eb + base + c) : 0u;
         const float my_x = HAS_VAL ? (c < cnt ? __ldg(ent_x + eb + base + c) : 0.f) : 1.f;
-        float sv_[LR], d_[LR], dz_[LR];
+        float sv_[LR], d_[LR], dz_[LR], l2_[LR];
 #pragma unroll
         for (int j = 0; j < LR; j++) {
             const uint32_t row = __shfl_sync(kFull, my_row, j, LR);
             const bool ok = j < cnt;
             sv_[j] = (ok && act) ? __ldg(sumvx + (size_t)row * k + c) : 0.f;
-            d_[j] = ok ? (__ldg(pred + row) - __ldg(label + row)) : 0.f;  // LogisticGradW  fm_algo_abst.h:159-161
+            d_[j] = ok ? row_head<RW>(__ldg(pred + row), __ldg(label + row), rw, row) : 0.f;  // LogisticGradW  fm_algo_abst.h:159-161
+            if (RW) l2_[j] = ok ? row_l2<true>(l2, rw, row) : 0.f;
             dz_[j] = (NFM && ok && act) ? __ldg(dz + (size_t)(row - rb) * k + c) : 0.f;
         }
 #pragma unroll
@@ -512,12 +518,13 @@ fm_backward_csc_kernel(const int64_t* __restrict__ seg_ptr, const uint32_t* __re
             if (j >= nmax - base) break;  // warp-uniform
             const float x = __shfl_sync(kFull, my_x, j, LR);
             if (j < cnt) {
-                const float gw = d_[j] * x + l2 * w;         // train_fm_algo.cpp:108 / train_nfm_algo.cpp:135
+                const float l2j = RW ? l2_[j] : l2;
+                const float gw = d_[j] * x + l2j * w;        // train_fm_algo.cpp:108 / train_nfm_algo.cpp:135
                 gwsum = gwsum + gw;                          // *update_W(fid) += gradW            :109
                 const float t = sv_[j] + v * (-x);           // avx_vecScalerAdd(sumVX, V, tmp, -x) :112-113
                 if (NFM) u = u + t * (dz_[j] * x);           // train_nfm_algo.cpp:154-156
                 else u = u + t * gw;                         // avx_vecScalerAdd(ptr, tmp, ptr, gradW) :114
-                u = u + v * l2;                              // avx_vecScalerAdd(ptr, V, ptr, L2)      :115
+                u = u + v * l2j;                             // avx_vecScalerAdd(ptr, V, ptr, L2)      :115
             }
         }
     }
@@ -538,10 +545,14 @@ fm_backward_csc_kernel(const int64_t* __restrict__ seg_ptr, const uint32_t* __re
     }
 }
 
-template <int LR>
+template <int LR, bool RW>
 static auto backward_csc_kernel(bool hv, bool nfm) {
-    return hv ? (nfm ? fm_backward_csc_kernel<LR, true, true> : fm_backward_csc_kernel<LR, true, false>)
-              : (nfm ? fm_backward_csc_kernel<LR, false, true> : fm_backward_csc_kernel<LR, false, false>);
+    return hv ? (nfm ? fm_backward_csc_kernel<LR, true, true, RW> : fm_backward_csc_kernel<LR, true, false, RW>)
+              : (nfm ? fm_backward_csc_kernel<LR, false, true, RW> : fm_backward_csc_kernel<LR, false, false, RW>);
+}
+template <int LR>
+static auto backward_csc_kernel(bool hv, bool nfm, bool rw) {
+    return rw ? backward_csc_kernel<LR, true>(hv, nfm) : backward_csc_kernel<LR, false>(hv, nfm);
 }
 
 int launch_fm_backward_csc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
@@ -560,10 +571,11 @@ int launch_fm_backward_csc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nf
     const int segs_per_cta = 8 * (32 / lr);
     const unsigned grid = (unsigned)((se - sb + segs_per_cta - 1) / segs_per_cta);
     ProfScope prof(c, PROF_FM_BWD_CSC);
-    auto kern = lr == 4 ? backward_csc_kernel<4>(s.has_val, nfm) : lr == 8 ? backward_csc_kernel<8>(s.has_val, nfm)
-              : lr == 16 ? backward_csc_kernel<16>(s.has_val, nfm) : backward_csc_kernel<32>(s.has_val, nfm);
+    const bool rw = s.has_rw;
+    auto kern = lr == 4 ? backward_csc_kernel<4>(s.has_val, nfm, rw) : lr == 8 ? backward_csc_kernel<8>(s.has_val, nfm, rw)
+              : lr == 16 ? backward_csc_kernel<16>(s.has_val, nfm, rw) : backward_csc_kernel<32>(s.has_val, nfm, rw);
     return launch(c, {grid, 256, 0, c->stream}, kern, s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, sb, se, s.label, s.pred, s.sumvx,
-                  c->dz, rb, c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, k, c->cfg.l2_reg, P);
+                  c->dz, rb, c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, k, c->cfg.l2_reg, P, row_weights(s));
 }
 
 // FM_Predict quirk mode (predict/fm_predict.cpp:20-33): pred = sum w x - 0.5 sum|vx|^2 + 0.5|sumVX_train[rid]|^2, evaluated

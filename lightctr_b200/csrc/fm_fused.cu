@@ -107,9 +107,11 @@ int launch_slotmap_compact(lctr_ctx* c, uint8_t* mark, size_t T, uint32_t* uniq,
     return launch(c, {cg, 256, 0, st}, slotmap_compact_kernel, mark, T, uniq, n_uniq, nullptr);
 }
 
-// mode 1: FM forward + backward;  2: NFM forward (z, wide part);  3: NFM backward from dz
+// mode 1: FM forward + backward;  2: NFM forward (z, wide part);  3: NFM backward from dz.  rw: the weighted instances of
+// the modes that form a head (the NFM forward has none)
 template <int K, bool HV>
-static auto fused_kernel(int mode) {
+static auto fused_kernel(int mode, bool rw) {
+    if (rw && mode != 2) return mode == 1 ? fm_fused_kernel<K, HV, 1, false, 4, true> : fm_fused_kernel<K, HV, 3, false, 4, true>;
     return mode == 1 ? fm_fused_kernel<K, HV, 1, false>
          : mode == 2 ? fm_fused_kernel<K, HV, 2, false> : fm_fused_kernel<K, HV, 3, false>;
 }
@@ -128,10 +130,11 @@ static int fused_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, dou
     // dependent launches: MODE 1 on several GPUs behind my own serve kernel (it polls the owners' flags at its head); the NFM
     // backward on one GPU behind the dense kernels in front of it (it requests its batch data before their end)
     const bool dependent = mode == 1 ? multi : mode == 3 && !multi;
-    return launch(c, {grid, 128, 0, c->stream, dependent}, s.has_val ? fused_kernel<K, true>(mode) : fused_kernel<K, false>(mode),
+    const bool rw = s.has_rw;
+    return launch(c, {grid, 128, 0, c->stream, dependent}, s.has_val ? fused_kernel<K, true>(mode, rw) : fused_kernel<K, false>(mode, rw),
                   s.row_ptr, multi ? s.ent_pslot : s.fid, s.ent_slot, s.val, s.label, c->cW, c->cV, s.pred, s.sumvx, nullptr, f->G,
                   f->Ghot, f->GS, c->cfg.l2_reg, rb, re, hdr, c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep,
-                  mode == 2 ? c->z : mode == 3 ? c->dz.get() : nullptr, mode == 2 ? s.wide.get() : nullptr);
+                  mode == 2 ? c->z : mode == 3 ? c->dz.get() : nullptr, mode == 2 ? s.wide.get() : nullptr, row_weights(s));
 }
 
 // FM k in {4, 8, 16, 32}: go<K>(args...) for the context's k (32 for any other)
@@ -183,7 +186,7 @@ static int fwd_tree_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, 
     return launch(c, {grid, 128, 0, c->stream, multi}, s.has_val ? fm_fused_kernel<K, true, 0, true> : fm_fused_kernel<K, false, 0, true>,
                   s.row_ptr, fid, fid, s.val, s.label, multi ? c->cW : c->W, multi ? c->cV : c->V, s.pred, s.sumvx, nullptr, nullptr,
                   nullptr, grad_stride(K), c->cfg.l2_reg, rb, re, nullptr, c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep,
-                  nullptr, nullptr);
+                  nullptr, nullptr, nullptr);
 }
 int launch_fm_forward_tree(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats) {
     if (re - rb <= 0) return 0;

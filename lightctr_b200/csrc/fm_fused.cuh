@@ -203,7 +203,8 @@ slotmap_assign_kernel(const uint32_t* __restrict__ fid, const int64_t* __restric
 // are fetched with one load, and the index loads of sample t+1 are issued before sample t's rows are consumed, so that
 // per sample only ONE dependent round trip (the row gather itself) is exposed instead of three (row_ptr -> indices ->
 // rows).
-template <int K, bool HAS_VAL, int MODE, bool SAME_IDX, int MINB = 4>
+// RW: the slot's row weights rw scale the head and the per-occurrence L2 terms of MODE 1 and MODE 3
+template <int K, bool HAS_VAL, int MODE, bool SAME_IDX, int MINB = 4, bool RW = false>
 __global__ void __launch_bounds__(128, MINB)
 fm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ pidx, const uint32_t* __restrict__ gidx,
                 const float* __restrict__ val, const float* __restrict__ label, const float* __restrict__ W,
@@ -212,7 +213,8 @@ fm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
                 const int64_t* __restrict__ hdr, double* partial, unsigned int* done, double* out_slot, int do_stats,
                 const unsigned long long* wait_flags = nullptr, int n_wait = 0, unsigned long long wait_epoch = 0,
                 float* __restrict__ zbuf = nullptr /* MODE 2: z out, MODE 3: dz in; [re - rb][K] */,
-                float* __restrict__ wide = nullptr /* MODE 2: wide part out [rows] */) {
+                float* __restrict__ wide = nullptr /* MODE 2: wide part out [rows] */,
+                const float* __restrict__ rw = nullptr /* RW: [rows] */) {
     constexpr bool FWD = MODE != 3, BWD = MODE == 1 || MODE == 3, NFM = MODE >= 2;
     static_assert(K % 4 == 0 && K <= 32 && (K / 4 & (K / 4 - 1)) == 0, "fused FM step: K in {4, 8, 16, 32}");
     // programmatic dependent launch: a kernel launched behind this one with the serialisation attribute (the compact
@@ -377,7 +379,7 @@ fm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
                 const float fm = wsum - 0.5f * sq + 0.5f * dot;             // :78, :82
                 const float pr = ref_sigmoid(fm);                           // :84
                 const float y = __ldg(label + r);
-                d = pr - y;                                                 // LogisticGradW  fm_algo_abst.h:159-161
+                d = row_head<RW>(pr, y, rw, r);                             // LogisticGradW  fm_algo_abst.h:159-161
                 if (lane == 0) {
                     pred[r] = pr;
                     if (dvec) dvec[r] = d;
@@ -399,9 +401,10 @@ fm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
             } else {  // MODE 3
                 s = __ldg(reinterpret_cast<const float4*>(sumvx + (size_t)r * K + 4 * q));
                 dz4 = __ldg(reinterpret_cast<const float4*>(zbuf + (size_t)(r - rb) * K + 4 * q));
-                d = __ldg(pred + r) - __ldg(label + r);
+                d = row_head<RW>(__ldg(pred + r), __ldg(label + r), rw, r);
             }
             if (BWD) {
+                const float l2r = row_l2<RW>(l2, rw, r);
                 // ---- backward from the register-resident rows (train_fm_algo.cpp:101-116; NFM: train_nfm_algo.cpp:126-159),
                 // vector REDs into G / Ghot.  FM: gV = (sumVX - xV) gradW + l2 V;  NFM: gV = (sumVX - xV) (dz x) + l2 V
 #pragma unroll
@@ -414,14 +417,14 @@ fm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
                             const float wj = __shfl_sync(kFull, ws[p], j);
                             const uint32_t sj = __shfl_sync(kFull, gs[p], j);
                             if (p * 32 + j < n) {
-                                const float gw = __fmaf_rn(d, xj, l2 * wj);                       // :108
+                                const float gw = __fmaf_rn(d, xj, l2r * wj);                       // :108
                                 const float4 vv = v[p][it];
                                 const float4 mu = NFM ? make_float4(dz4.x * xj, dz4.y * xj, dz4.z * xj, dz4.w * xj) : make_float4(gw, gw, gw, gw);
                                 float4 gv;
-                                gv.x = __fmaf_rn(__fmaf_rn(-xj, vv.x, s.x), mu.x, l2 * vv.x);     // :112-115
-                                gv.y = __fmaf_rn(__fmaf_rn(-xj, vv.y, s.y), mu.y, l2 * vv.y);
-                                gv.z = __fmaf_rn(__fmaf_rn(-xj, vv.z, s.z), mu.z, l2 * vv.z);
-                                gv.w = __fmaf_rn(__fmaf_rn(-xj, vv.w, s.w), mu.w, l2 * vv.w);
+                                gv.x = __fmaf_rn(__fmaf_rn(-xj, vv.x, s.x), mu.x, l2r * vv.x);     // :112-115
+                                gv.y = __fmaf_rn(__fmaf_rn(-xj, vv.y, s.y), mu.y, l2r * vv.y);
+                                gv.z = __fmaf_rn(__fmaf_rn(-xj, vv.z, s.z), mu.z, l2r * vv.z);
+                                gv.w = __fmaf_rn(__fmaf_rn(-xj, vv.w, s.w), mu.w, l2r * vv.w);
                                 float* dst = (sj & kHotBit) ? Ghot + ((size_t)(sj & ~kHotBit) * kHotRep + rep) * GS
                                                             : G + (size_t)sj * GS;
                                 red_add_v4(dst + 4 * q, gv);
@@ -446,13 +449,13 @@ fm_fused_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
                         const float wj = __shfl_sync(kFull, w, j);
                         if (base + j < n) {
                             const float4 vv = ldg_f4(V + (size_t)fj * K + 4 * q);
-                            const float gw = __fmaf_rn(d, xj, l2 * wj);
+                            const float gw = __fmaf_rn(d, xj, l2r * wj);
                             const float4 mu = NFM ? make_float4(dz4.x * xj, dz4.y * xj, dz4.z * xj, dz4.w * xj) : make_float4(gw, gw, gw, gw);
                             float4 gv;
-                            gv.x = __fmaf_rn(__fmaf_rn(-xj, vv.x, s.x), mu.x, l2 * vv.x);
-                            gv.y = __fmaf_rn(__fmaf_rn(-xj, vv.y, s.y), mu.y, l2 * vv.y);
-                            gv.z = __fmaf_rn(__fmaf_rn(-xj, vv.z, s.z), mu.z, l2 * vv.z);
-                            gv.w = __fmaf_rn(__fmaf_rn(-xj, vv.w, s.w), mu.w, l2 * vv.w);
+                            gv.x = __fmaf_rn(__fmaf_rn(-xj, vv.x, s.x), mu.x, l2r * vv.x);
+                            gv.y = __fmaf_rn(__fmaf_rn(-xj, vv.y, s.y), mu.y, l2r * vv.y);
+                            gv.z = __fmaf_rn(__fmaf_rn(-xj, vv.z, s.z), mu.z, l2r * vv.z);
+                            gv.w = __fmaf_rn(__fmaf_rn(-xj, vv.w, s.w), mu.w, l2r * vv.w);
                             float* dst = (sj & kHotBit) ? Ghot + ((size_t)(sj & ~kHotBit) * kHotRep + rep) * GS
                                                         : G + (size_t)sj * GS;
                             red_add_v4(dst + 4 * q, gv);

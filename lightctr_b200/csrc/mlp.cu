@@ -87,10 +87,13 @@ __global__ void fc_weight_grad_kernel(const float* __restrict__ x, const float* 
     }
 }
 
-// p = sigmoid(wide + mlp_out); loss/acc; delta_L = p - y  (train_nfm_algo.cpp:101-116)
+// p = sigmoid(wide + mlp_out); loss/acc; delta_L = p - y  (train_nfm_algo.cpp:101-116); RW: delta_L = w (p - y) with the
+// slot's row weights rw (the layers' clip then applies to the weighted delta)
+template <bool RW = false>
 __global__ void nfm_loss_kernel(const float* __restrict__ wide, const float* __restrict__ out,
                                 const float* __restrict__ label, float* __restrict__ pred, float* __restrict__ delta,
-                                int64_t rb, int64_t n, double* partial, unsigned int* done, double* out_slot) {
+                                int64_t rb, int64_t n, double* partial, unsigned int* done, double* out_slot,
+                                const float* __restrict__ rw) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     double loss = 0.0, correct = 0.0;
     if (i < n) {
@@ -98,7 +101,7 @@ __global__ void nfm_loss_kernel(const float* __restrict__ wide, const float* __r
         pred[rb + i] = p;
         const float y = label[rb + i];
         loss_terms(p, y, loss, correct);
-        delta[i] = p - y;
+        delta[i] = row_head<RW>(p, y, rw, rb + i);
     }
     publish_stats(loss, correct, partial, done, out_slot, false);
 }
@@ -257,8 +260,8 @@ int launch_nfm_mlp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int64_t rows_di
         double* out_slot = c->stats + 2 * (c->step % kStatRing);
         MlpLayer& last = c->layers[nl - 1];
         if (mlp_forward_dev(c, B) ||
-            launch(c, {mlp_blocks(B), 256, 0, c->stream}, nfm_loss_kernel, s.wide, last.act, s.label, s.pred, last.delta, rb, B,
-                   c->stat_partial, c->stat_done, out_slot) ||
+            launch(c, {mlp_blocks(B), 256, 0, c->stream}, s.has_rw ? nfm_loss_kernel<true> : nfm_loss_kernel<false>, s.wide,
+                   last.act, s.label, s.pred, last.delta, rb, B, c->stat_partial, c->stat_done, out_slot, row_weights(s)) ||
             mlp_backward_dev(c, B))
             return 1;
     }

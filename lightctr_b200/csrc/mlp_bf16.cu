@@ -140,12 +140,13 @@ __device__ __forceinline__ void warp_gemm_tn(uint32_t d_base, int d_stride, int 
 }
 
 // TRAIN = false: the forward-only instance of lctr_score -- the same staging, forward and output layer, then the pCTR
-// alone: no labels, loss, statistics, deltas or dW / db (dz, label and the statistics arguments are unused).
-template <int TM, bool TRAIN>
+// alone: no labels, loss, statistics, deltas or dW / db (dz, label and the statistics arguments are unused).  RW: the output
+// delta is the clip of w (p - y) with the slot's row weights rw
+template <int TM, bool TRAIN, bool RW = false>
 __global__ void __launch_bounds__(TM * 2, 1)
 nfm_mlp_fused_kernel(MlpDev P, const float* __restrict__ z, float* __restrict__ dz, const float* __restrict__ wide,
                      const float* __restrict__ label, float* __restrict__ pred, int64_t rb, int B, double* partial,
-                     unsigned int* done, double* out_slot) {
+                     unsigned int* done, double* out_slot, const float* __restrict__ rw) {
     extern __shared__ __align__(16) unsigned char smem[];
     const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, g = lane >> 2, t = lane & 3;
@@ -253,7 +254,7 @@ nfm_mlp_fused_kernel(MlpDev P, const float* __restrict__ z, float* __restrict__ 
                     loss_terms(p, yv, l1, c1);
                     loss += l1; correct += c1;
                 }
-                d3 = clip15(p - yv);
+                d3 = clip15(row_head<RW>(p, yv, rw, gi));
             }
             if (!TRAIN) continue;
             dbl += d3;
@@ -458,10 +459,11 @@ static int launch_mlp_bf16_kernel(lctr_ctx* c, Slot& s, int64_t rb, int B, bool 
     P.w32_last = c->layers[nh].w;
     const unsigned grid = (unsigned)((B + c->mlp_tm - 1) / c->mlp_tm);
     const bool t128 = c->mlp_tm == 128;
-    auto kern = train ? (t128 ? nfm_mlp_fused_kernel<128, true> : nfm_mlp_fused_kernel<64, true>)
+    auto kern = train ? (s.has_rw ? (t128 ? nfm_mlp_fused_kernel<128, true, true> : nfm_mlp_fused_kernel<64, true, true>)
+                                  : (t128 ? nfm_mlp_fused_kernel<128, true> : nfm_mlp_fused_kernel<64, true>))
                       : (t128 ? nfm_mlp_fused_kernel<128, false> : nfm_mlp_fused_kernel<64, false>);
     return launch(c, {grid, t128 ? 256u : 128u, c->mlp_smem, c->stream}, kern, P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
-                  c->stat_partial, c->stat_done, out_slot);
+                  c->stat_partial, c->stat_done, out_slot, row_weights(s));
 }
 
 int launch_mlp_bf16_forward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {

@@ -266,12 +266,13 @@ __device__ __forceinline__ void backward_layer(const Dev& P, unsigned char* smem
 }
 
 // TRAIN = false: the forward-only instance of lctr_score -- the same staging, forward passes and output layer, then the
-// pCTR alone: no labels, loss, statistics, deltas or dW / db (dz, label and the statistics arguments are unused).
-template <int ACT, bool TRAIN>
+// pCTR alone: no labels, loss, statistics, deltas or dW / db (dz, label and the statistics arguments are unused).  RW: the
+// output delta is the clip of w (p - y) with the slot's row weights row_w, loaded next to the labels
+template <int ACT, bool TRAIN, bool RW = false>
 __global__ void __launch_bounds__(kThreads, 1)
 nfm_mlp_umma_kernel(Dev P, const float* __restrict__ z, float* __restrict__ dz, const float* __restrict__ wide,
                     const float* __restrict__ label, float* __restrict__ pred, int64_t rb, int B, double* partial,
-                    unsigned int* done, double* out_slot) {
+                    unsigned int* done, double* out_slot, const float* __restrict__ row_w) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_addr(smem);
     int ns = 0;
@@ -307,12 +308,13 @@ nfm_mlp_umma_kernel(Dev P, const float* __restrict__ z, float* __restrict__ dz, 
     // kernel has finished.  (No-op for an ordinary launch.)
     cudaGridDependencySynchronize();
     // the rows' wide terms and labels: requested now, used after the forward pass
-    float wide_r[2], label_r[2];
+    float wide_r[2], label_r[2], weight_r[2];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
         const bool ok = r0 + 8 * h < valid;
         wide_r[h] = ok ? wide[rb + row0 + r0 + 8 * h] : 0.f;
         label_r[h] = TRAIN && ok ? label[rb + row0 + r0 + 8 * h] : 0.f;
+        weight_r[h] = RW && TRAIN && ok ? row_w[rb + row0 + r0 + 8 * h] : 0.f;
     }
     {   // z tile -> bf16, chunk-major
         const int k = P.in[0], chunks = k / 8;
@@ -394,7 +396,7 @@ nfm_mlp_umma_kernel(Dev P, const float* __restrict__ z, float* __restrict__ dz, 
                     loss += lt;
                     correct += ct;
                 }
-                d3[h] = clip15(p - label_r[h]);
+                d3[h] = clip15(RW ? weight_r[h] * (p - label_r[h]) : p - label_r[h]);
             }
         }
         if constexpr (!TRAIN) return;
@@ -513,10 +515,11 @@ int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot, b
     const unsigned grid = (unsigned)((B + umma::kTM - 1) / umma::kTM);
     // one GPU: dependent on the embedding forward in front of it (fm_fused.cu, MODE 2), in a train step and in a score alike
     const bool sig = P.act == LCTR_ACT_SIGMOID;
-    auto kern = train ? (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, true> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, true>)
+    auto kern = train ? (s.has_rw ? (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, true, true> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, true, true>)
+                                  : (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, true> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, true>))
                       : (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, false> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, false>);
     if (launch(c, {grid, (unsigned)umma::kThreads, c->mlp_umma_smem, c->stream, c->cfg.world == 1}, kern, P, c->z, c->dz, s.wide,
-               s.label, s.pred, rb, B, c->stat_partial, c->stat_done, out_slot))
+               s.label, s.pred, rb, B, c->stat_partial, c->stat_done, out_slot, row_weights(s)))
         return 1;
     if (trace) {  // phase boundaries of CTA 0: setup | per layer (mma, epilogue) | output | per layer backward | stats
         unsigned long long h[64];

@@ -64,16 +64,20 @@ wnd_forward_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restri
     if (lane == 0) wide_out[r] = wide;
 }
 
-// warp = row: wide gradients of every entry, tensor gradients of the first-of-field entries
+// warp = row: wide gradients of every entry, tensor gradients of the first-of-field entries.  RW: the slot's row weights rw
+// scale the wide head and its L2 term (the tensor gradients arrive weighted in dz)
+template <bool RW = false>
 __global__ void __launch_bounds__(256)
 wnd_backward_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict__ fid, const float* __restrict__ val,
                     const float* __restrict__ label, const float* __restrict__ pred, const float* __restrict__ W,
                     const uint32_t* __restrict__ zsrc, const float* __restrict__ dz, int Fc, int d, float* __restrict__ gW,
-                    float* __restrict__ gE, uint8_t* __restrict__ touched, float l2, int64_t rb, int64_t re) {
+                    float* __restrict__ gE, uint8_t* __restrict__ touched, float l2_arg, int64_t rb, int64_t re,
+                    const float* __restrict__ rw) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int64_t r = rb + (int64_t)blockIdx.x * (blockDim.x >> 5) + wid;
     if (r >= re) return;
-    const float lossv = pred[r] - label[r];  // :248
+    const float lossv = row_head<RW>(pred[r], label[r], rw, r);  // :248
+    const float l2 = row_l2<RW>(l2_arg, rw, r);
     const int64_t b = row_ptr[r], e = row_ptr[r + 1];
     for (int64_t i = b + lane; i < e; i += 32) {
         const uint32_t f = __ldg(fid + i);
@@ -124,10 +128,10 @@ int launch_wnd_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     const int64_t rows = re - rb;
     if (rows <= 0) return 0;
     ProfScope prof(c, PROF_FM_BWD_RED);
-    return launch(c, {(unsigned)((rows + 7) / 8), 256, 0, c->stream}, wnd_backward_kernel, s.row_ptr,
+    return launch(c, {(unsigned)((rows + 7) / 8), 256, 0, c->stream}, s.has_rw ? wnd_backward_kernel<true> : wnd_backward_kernel<false>, s.row_ptr,
                   c->cfg.world > 1 ? s.ent_pslot : s.fid, s.has_val ? s.val.get() : nullptr, s.label, s.pred, c->cW, c->wnd_src, c->dz,
                   (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(),
-                  c->cfg.l2_reg, rb, re);
+                  c->cfg.l2_reg, rb, re, row_weights(s));
 }
 
 }  // namespace lctr
