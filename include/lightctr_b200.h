@@ -284,13 +284,13 @@ int lctr_train_step(lctr_ctx* ctx, int slot, int64_t row_begin, int64_t row_end,
  *   - loss_sum = sum w_r loss_r and acc_cnt = sum w_r [correct_r].
  * So w = 1 everywhere is bit for bit an unweighted step; a row of w = 0 is an absent row, except that its entries still
  * mark rows for change tracking; an integer w equals w copies of the row (fixed minibatch_size) up to re-association and
- * the clip.  Weights change gradients and statistics, not pCTR: lctr_score, lctr_predict and lctr_eval / lctr_eval_pred
- * ignore them (a weighted AUC needs non-integer buckets and is not offered).  They are batch data: any later upload into
+ * the clip.  Weights change gradients and statistics, not pCTR: lctr_score, lctr_predict, lctr_eval and lctr_eval_pred
+ * ignore them; lctr_eval_weighted evaluates the slot with them.  They are batch data: any later upload into
  * the slot (lctr_upload_batch, lctr_upload_batch_keys with insert 0 or 1, lctr_upload_libffm, lctr_train_batch) drops
  * them, and checkpoints do not carry them.  Key admission removes entries, never rows, so weights stay aligned with the
  * rows of a keyed slot.  On several GPUs each rank weights its own rows (no collective).
  * Every model, deterministic mode and world trains weighted slots.  The statistics cost one more launch, and only when
- * loss_sum or acc_cnt is requested.  Not covered: the streamed pipeline (lctr_train_batch_async takes no weights). */
+ * loss_sum or acc_cnt is requested.  The streamed pipeline takes weights through lctr_train_batch_weighted_async. */
 int lctr_set_row_weights(lctr_ctx* ctx, int slot, int64_t rows, const float* weight);
 /* End-to-end convenience: upload_batch(slot 0) + train_step + result readback, host buffers in. */
 int lctr_train_batch(lctr_ctx* ctx, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
@@ -305,6 +305,17 @@ int lctr_train_batch(lctr_ctx* ctx, int64_t rows, int64_t nnz, const int64_t* ro
 #define LCTR_PIPE_DEPTH 3
 int lctr_train_batch_async(lctr_ctx* ctx, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
                            const uint16_t* field, const float* val, const int32_t* label, uint64_t* ticket);
+/* lctr_train_batch_async plus one weight per row; weight = NULL is lctr_train_batch_async exactly.  The ticket's step
+ * trains exactly as lctr_upload_batch + lctr_set_row_weights + lctr_train_step(0, rows) would (the rule of
+ * lctr_set_row_weights), and lctr_wait returns its weighted statistics (sum w loss, sum w [correct]).  The weights are
+ * checked on the host as lctr_set_row_weights checks them before anything is enqueued: a refused call issues no ticket and
+ * leaves the pipeline usable.  `weight` must stay valid until the ticket has been waited for, like the other buffers.
+ * Every model and world (each rank weights its own rows); on the captured-graph path (FM, cfg.deterministic 0 with a
+ * compact gradient or 2, one GPU) a pipeline slot captures a weighted variant of its step graph the first time it streams a
+ * weighted batch after an unweighted one, and the other way round, so a stream of one kind never recaptures. */
+int lctr_train_batch_weighted_async(lctr_ctx* ctx, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
+                                    const uint16_t* field, const float* val, const int32_t* label, const float* weight,
+                                    uint64_t* ticket);
 int lctr_wait(lctr_ctx* ctx, uint64_t ticket, float* loss_sum, float* acc_cnt);
 /* Forward only on a resident slot; pctr (rows floats, host; may be NULL) receives sigmoid(pred).
  * quirk_sumvx_slot >= 0 reproduces FM_Predict's use of the TRAINING sumVX of the same row index
@@ -472,6 +483,24 @@ int lctr_eval(lctr_ctx* ctx, int slot, float* loss_sum, int64_t* correct, float*
  * slot. */
 int lctr_eval_pred(lctr_ctx* ctx, int64_t n, const float* pctr, const int32_t* label, float* loss_sum, int64_t* correct,
                    float* auc);
+/* Weighted test-set metrics: lctr_eval over the slot's row weights (lctr_set_row_weights); refused when the slot has none
+ * or no rows.  THE RULE, deterministic, and lctr_eval bit for bit when every w = 1:
+ *   - loss: in row order, loss = (float)((double)loss + (double)w_i * term_i) over the rows with w_i != 0 (so no 0 * inf at
+ *     p in {0, 1}), term_i being lctr_eval's term;
+ *   - correct: sum w_i [correct_i] in double, in row order;
+ *   - AUC: lctr_eval's bucket, (p * (2^24 - 1)) truncated.  With M = max w_i and 2^(E-1) <= M < 2^E, row i adds the
+ *     integer q_i = rint(w_i 2^(32-E)) in [0, 2^32] to its bucket's u64 sum P_b (label 1) or N_b (otherwise), exact and
+ *     independent of row order for n < 2^31; the fp32 trapezoid walk then runs over (fl32(P_b), fl32(N_b)) in place of the
+ *     counts.  The walk runs in units of 2^(E-32), a power-of-two scale that commutes with each of its fp32 operations and
+ *     that auc / totPos / totNeg divides out.  So integer weights give the AUC of the rows duplicated w times bit for bit,
+ *     scaling every weight by 2^k changes no bit, and weights below 2^(E-33) round to q = 0 and leave the AUC alone (they
+ *     still count in loss and correct).  M = 0 gives AUC 0.
+ * The first weighted evaluation allocates 256 MB of histograms (not counted by lctr_device_bytes, like lctr_eval's 128 MB). */
+int lctr_eval_weighted(lctr_ctx* ctx, int slot, float* loss_sum, double* correct, float* auc);
+/* the same over n host (pCTR, label, weight) triples in row order, on any context and any world; each weight must be finite
+ * and >= 0 (checked before anything is launched) */
+int lctr_eval_pred_weighted(lctr_ctx* ctx, int64_t n, const float* pctr, const int32_t* label, const float* weight,
+                            float* loss_sum, double* correct, float* auc);
 /* test hook: overwrite the slot's pCTR array with host values */
 int lctr_upload_pred(lctr_ctx* ctx, int slot, const float* pctr);
 

@@ -35,7 +35,8 @@ SYMBOLS = [
     "lctr_load_libffm_keys", "lctr_free_keyed_dataset", "lctr_evict_keys", "lctr_load_checkpoint_shards", "lctr_eval_pred",
     "lctr_download_host_tier", "lctr_evict_host_tier", "lctr_set_key_admission", "lctr_decay_key_admission",
     "lctr_key_admission_stats", "lctr_upload_libffm", "lctr_download_batch", "lctr_track_changes", "lctr_save_checkpoint_delta",
-    "lctr_load_checkpoint_chain", "lctr_checkpoint_hash", "lctr_set_row_weights",
+    "lctr_load_checkpoint_chain", "lctr_checkpoint_hash", "lctr_set_row_weights", "lctr_train_batch_weighted_async",
+    "lctr_eval_weighted", "lctr_eval_pred_weighted",
 ]
 NO_LIMIT = (1 << 64) - 1  # lctr_evict_keys: UINT64_MAX = no limit
 TEXT_BEGIN, TEXT_END, TEXT_LOOKUP = 1, 2, 4  # lctr_upload_libffm flags
@@ -102,6 +103,7 @@ def load_library():
     L.lctr_set_row_weights.argtypes = [vp, C.c_int, i64, f32p]
     L.lctr_train_batch.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     L.lctr_train_batch_async.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp, C.POINTER(C.c_uint64)]
+    L.lctr_train_batch_weighted_async.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp, vp, C.POINTER(C.c_uint64)]
     L.lctr_wait.argtypes = [vp, C.c_uint64, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     L.lctr_predict.argtypes = [vp, C.c_int, C.c_int, f32p]
     L.lctr_score.argtypes = [vp, C.c_int, i64, i64, f32p]
@@ -118,6 +120,9 @@ def load_library():
     L.lctr_eval.argtypes = [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int64), C.POINTER(C.c_float)]
     L.lctr_upload_pred.argtypes = [vp, C.c_int, f32p]
     L.lctr_eval_pred.argtypes = [vp, i64, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_int64), C.POINTER(C.c_float)]
+    L.lctr_eval_weighted.argtypes = [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_double), C.POINTER(C.c_float)]
+    L.lctr_eval_pred_weighted.argtypes = [vp, i64, vp, vp, vp, C.POINTER(C.c_float), C.POINTER(C.c_double),
+                                          C.POINTER(C.c_float)]
     L.lctr_save_checkpoint.argtypes = [vp, C.c_char_p]
     L.lctr_load_checkpoint.argtypes = [vp, C.c_char_p]
     L.lctr_load_checkpoint_shards.argtypes = [vp, C.c_int, C.POINTER(C.c_char_p)]
@@ -506,10 +511,18 @@ class Context:
                                      _p(label), C.byref(loss), C.byref(acc)))
         return loss.value, acc.value
 
-    def train_batch_async(self, row_ptr, fid, field, val, label):
+    def train_batch_async(self, row_ptr, fid, field, val, label, weight=None):
+        """Streamed step on host buffers; returns the ticket for wait().  weight (float32, one per row) trains the batch
+        weighted (lctr_train_batch_weighted_async).  Every buffer must stay alive until the ticket has been waited for."""
         t = C.c_uint64()
-        _chk(self.L.lctr_train_batch_async(self.h, len(row_ptr) - 1, len(fid), _p(row_ptr), _p(fid), _p(field), _p(val),
-                                           _p(label), C.byref(t)))
+        if weight is None:
+            _chk(self.L.lctr_train_batch_async(self.h, len(row_ptr) - 1, len(fid), _p(row_ptr), _p(fid), _p(field), _p(val),
+                                               _p(label), C.byref(t)))
+            return t.value
+        if len(weight) != len(row_ptr) - 1:
+            raise ValueError("train_batch_async: %d weights for %d rows" % (len(weight), len(row_ptr) - 1))
+        _chk(self.L.lctr_train_batch_weighted_async(self.h, len(row_ptr) - 1, len(fid), _p(row_ptr), _p(fid), _p(field),
+                                                    _p(val), _p(label), _p(weight), C.byref(t)))
         return t.value
 
     def wait(self, ticket):
@@ -577,14 +590,30 @@ class Context:
         _chk(self.L.lctr_eval(self.h, slot, C.byref(loss), C.byref(correct), C.byref(auc)))
         return loss.value, correct.value, auc.value
 
-    def eval_pred(self, pctr, labels):
-        """eval_metrics over host arrays: (summed logloss, correct count, AUC) of pctr against labels, in row order."""
+    def eval_pred(self, pctr, labels, weights=None):
+        """eval_metrics over host arrays: (summed logloss, correct count, AUC) of pctr against labels, in row order.  With
+        weights (one per row) the weighted metrics of lctr_eval_pred_weighted, the correct count then a float."""
         p = np.ascontiguousarray(pctr, np.float32)
         y = np.ascontiguousarray(labels, np.int32)
         if len(p) != len(y):
             raise ValueError("eval_pred: %d pCTR values for %d labels" % (len(p), len(y)))
+        if weights is not None:
+            w = np.ascontiguousarray(weights, np.float32)
+            if len(w) != len(p):
+                raise ValueError("eval_pred: %d weights for %d rows" % (len(w), len(p)))
+            loss, correct, auc = C.c_float(), C.c_double(), C.c_float()
+            _chk(self.L.lctr_eval_pred_weighted(self.h, len(p), _p(p), _p(y), _p(w), C.byref(loss), C.byref(correct),
+                                                C.byref(auc)))
+            return loss.value, correct.value, auc.value
         loss, correct, auc = C.c_float(), C.c_int64(), C.c_float()
         _chk(self.L.lctr_eval_pred(self.h, len(p), _p(p), _p(y), C.byref(loss), C.byref(correct), C.byref(auc)))
+        return loss.value, correct.value, auc.value
+
+    def eval_weighted(self, slot):
+        """(summed weighted logloss, weighted correct count, weighted AUC) of the slot's pCTR / labels under the row weights
+        set with set_row_weights (lctr_eval_weighted)."""
+        loss, correct, auc = C.c_float(), C.c_double(), C.c_float()
+        _chk(self.L.lctr_eval_weighted(self.h, slot, C.byref(loss), C.byref(correct), C.byref(auc)))
         return loss.value, correct.value, auc.value
 
     def upload_pred(self, slot, pctr):

@@ -74,9 +74,9 @@ __global__ void label_to_float_kernel(const int32_t* in, float* out, int64_t n_a
 // the slot and the same loss_terms as the unweighted kernels, written over the ring slot those kernels published to.
 // A zero-weight row is absent; FFM (skip_zero_head) also leaves out every row whose weighted head fl(w (p - y)) is zero,
 // as its kernels do
-__global__ void weighted_stats_kernel(const float* __restrict__ pred, const float* __restrict__ label, const float* __restrict__ rw,
-                                      int64_t rb, int64_t re, int skip_zero_head, double* partial, unsigned int* done,
-                                      double* out_slot) {
+__device__ __forceinline__ void weighted_stats_rows(const float* __restrict__ pred, const float* __restrict__ label,
+                                                    const float* __restrict__ rw, int64_t rb, int64_t re, int skip_zero_head,
+                                                    double* partial, unsigned int* done, double* out_slot) {
     double loss = 0.0, correct = 0.0;
     for (int64_t r = rb + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < re; r += (int64_t)gridDim.x * blockDim.x) {
         const float w = rw[r];
@@ -87,6 +87,17 @@ __global__ void weighted_stats_kernel(const float* __restrict__ pred, const floa
         correct += (double)w * c1;
     }
     publish_stats(loss, correct, partial, done, out_slot, false);
+}
+__global__ void weighted_stats_kernel(const float* __restrict__ pred, const float* __restrict__ label, const float* __restrict__ rw,
+                                      int64_t rb, int64_t re, int skip_zero_head, double* partial, unsigned int* done,
+                                      double* out_slot) {
+    weighted_stats_rows(pred, label, rw, rb, re, skip_zero_head, partial, done, out_slot);
+}
+// the streamed step graph's instance: rows [0, hdr[0]) of the batch in the pipeline slot, read from its device header
+__global__ void weighted_stats_hdr_kernel(const float* __restrict__ pred, const float* __restrict__ label,
+                                          const float* __restrict__ rw, const int64_t* __restrict__ hdr, int skip_zero_head,
+                                          double* partial, unsigned int* done, double* out_slot) {
+    weighted_stats_rows(pred, label, rw, 0, hdr[0], skip_zero_head, partial, done, out_slot);
 }
 
 int launch_weighted_stats(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
@@ -699,7 +710,9 @@ static int check_slot(lctr_ctx* c, const char* who, int slot, int64_t rb, int64_
     return 0;
 }
 
-int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_sum, float* acc_cnt) {
+// one train step over rows [rb, re) of the slot, statistics into the ring slot of the step; a weighted slot launches its
+// weighted statistics when weighted_stats is set (the caller reads them)
+static int train_step_on(lctr_ctx* c, int slot, int64_t rb, int64_t re, bool weighted_stats) {
     if (check_slot(c, "train_step", slot, rb, re, true)) return 1;
     Slot& s = c->slots[slot];
     LCTR_CHECK(c->cfg.world == 1 || c->cfg.minibatch_size > 0,
@@ -757,11 +770,17 @@ int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_s
     }
     // a weighted slot's statistics are the weighted sums, computed from the step's predictions once its kernels are done,
     // when the caller reads them
-    if (!rc && s.has_rw && (loss_sum || acc_cnt)) rc = launch_weighted_stats(c, s, rb, re);
+    if (!rc && s.has_rw && weighted_stats) rc = launch_weighted_stats(c, s, rb, re);
     // change tracking: the rows the stepped entries name, behind the updater (several GPUs: the owner marks the rows it
     // served, dist_post_step)
     if (rc || (!multi && track_mark_entries(c, s, rb, re, nullptr, c->stream))) return 1;
     c->step++;
+    return 0;
+}
+
+int lctr_train_step(lctr_ctx* c, int slot, int64_t rb, int64_t re, float* loss_sum, float* acc_cnt) {
+    const uint64_t step = c ? c->step : 0;
+    if (train_step_on(c, slot, rb, re, loss_sum || acc_cnt)) return 1;
     return read_stats(c, step, loss_sum, acc_cnt);
 }
 
@@ -861,7 +880,9 @@ static int count_kernel_nodes(cudaGraph_t graph, int* n) {
     return 0;
 }
 
-static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
+// weighted: the step graph takes the weighted kernel instances and ends with a weighted-statistics node over s.rw, which
+// must hold cap_rows floats before the capture
+static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val, bool weighted) {
     PipeGraph& g = c->pipe_graph[p];
     Slot& s = c->slots[kNumSlots - kPipe + p];
     if (g.build) { cudaGraphExecDestroy(g.build); g.build = nullptr; }
@@ -870,6 +891,7 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
                       g.h_stat.alloc(2)))
         return 1;
     s.has_val = has_val;
+    s.has_rw = weighted;
     // the launchers pick their updater instance from the host copy at capture time: give it the context's updater
     memset(g.h_opt, 0, sizeof(OptParams));
     g.h_opt[0].opt = c->cfg.optimizer;
@@ -902,6 +924,9 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
         else
             rc = launch_fm_forward_ex(c, s, 0, s.cap_rows, false, true, g.d_hdr, g.d_stat) ||
                  launch_fm_backward_devcsc_ex(c, s, 0, s.cap_rows, g.h_opt, g.d_opt);
+        if (!rc && weighted)  // over what the forward wrote into d_stat
+            rc = launch(c, {(unsigned)std::min<int64_t>((s.cap_rows + 255) / 256, (int64_t)c->sm_count * 4), 256, 0, c->stream},
+                        weighted_stats_hdr_kernel, s.pred, s.label, s.rw, g.d_hdr, 0, c->stat_partial, c->stat_done, g.d_stat);
         if (!rc) rc = track_mark_entries(c, s, 0, 0, g.d_hdr, c->stream);
     }
     if (!rc) rc = cudaMemcpyAsync(g.h_stat, g.d_stat, 2 * sizeof(double), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess;
@@ -911,33 +936,41 @@ static int pipe_graph_capture(lctr_ctx* c, int p, bool has_val) {
     LCTR_CUDA(cudaGraphInstantiate(&g.step, graph, 0));
     cudaGraphDestroy(graph);
     g.cap_rows = s.cap_rows; g.cap_nnz = s.cap_nnz; g.has_val = has_val; g.tracked = c->changed;
+    g.weighted = weighted; g.rw = weighted ? s.rw.get() : nullptr;
     return 0;
 }
 
 static int train_batch_async_graph(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
-                                   const float* val, const int32_t* label, uint64_t* ticket) {
+                                   const float* val, const int32_t* label, const float* weight, uint64_t* ticket) {
     const int p = (int)(c->pipe_issued % kPipe);
     const int slot = kNumSlots - kPipe + p;
     Slot& s = c->slots[slot];
     PipeGraph& g = c->pipe_graph[p];
     const bool fused = c->grad_path == GRAD_COMPACT;
+    const bool weighted = weight != nullptr;
     if (rows > s.cap_rows || nnz > s.cap_nnz || !g.build || g.has_val != (val != nullptr) || g.cap_rows != s.cap_rows ||
-        g.cap_nnz != s.cap_nnz || g.tracked != c->changed.get()) {
+        g.cap_nnz != s.cap_nnz || g.tracked != c->changed.get() || g.weighted != weighted || (weighted && g.rw != s.rw.get())) {
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
         LCTR_CUDA(cudaStreamSynchronize(c->copy_stream));
         LCTR_CUDA(cudaStreamSynchronize(c->build_stream));
         if (rows > s.cap_rows || nnz > s.cap_nnz)  // head-room so that slightly larger batches do not re-capture
             if (slot_reserve(c, s, std::max(rows, s.cap_rows) + rows / 8 + 64, std::max(nnz, s.cap_nnz) + nnz / 8 + 1024)) return 1;
         if (fused ? fused_reserve(c, s, s.cap_nnz) : csc_reserve(c, s, s.cap_nnz)) return 1;
+        if (weighted && s.cap_rw < s.cap_rows) {  // the graph captures the pointer: room for any batch the slot fits
+            s.cap_rw = 0;
+            if (alloc_group(sized(s.rw, (size_t)s.cap_rows))) return 1;
+            s.cap_rw = s.cap_rows;
+        }
         LCTR_CUDA(cudaStreamSynchronize(c->stream));
-        if (pipe_graph_capture(c, p, val != nullptr)) return 1;
+        if (pipe_graph_capture(c, p, val != nullptr, weighted)) return 1;
     }
-    s.rows = rows; s.nnz = nnz; s.has_val = val != nullptr; s.has_field = false; s.has_rw = false;
+    s.rows = rows; s.nnz = nnz; s.has_val = val != nullptr; s.has_field = false; s.has_rw = weighted;
     if (c->pipe_issued >= (uint64_t)kPipe) LCTR_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_computed[p], 0));
     LCTR_CUDA(cudaMemcpyAsync(s.row_ptr, row_ptr, (size_t)(rows + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, c->copy_stream));
     LCTR_CUDA(cudaMemcpyAsync(s.fid, fid, (size_t)nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, c->copy_stream));
     if (val) LCTR_CUDA(cudaMemcpyAsync(s.val, val, (size_t)nnz * sizeof(float), cudaMemcpyHostToDevice, c->copy_stream));
     LCTR_CUDA(cudaMemcpyAsync(s.pred, label, (size_t)rows * sizeof(int32_t), cudaMemcpyHostToDevice, c->copy_stream));
+    if (weighted) LCTR_CUDA(cudaMemcpyAsync(s.rw, weight, (size_t)rows * sizeof(float), cudaMemcpyHostToDevice, c->copy_stream));
     g.h_hdr[0] = rows; g.h_hdr[1] = nnz;
     // the batch's slot map is built on its own stream: the copy engine moves batch t+1 while the SMs build batch t's map (the
     // build kernels share scratch buffers, so they stay serialised among themselves -- on this one stream)
@@ -957,26 +990,46 @@ static int train_batch_async_graph(lctr_ctx* c, int64_t rows, int64_t nnz, const
     return 0;
 }
 
-int lctr_train_batch_async(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
-                           const uint16_t* field, const float* val, const int32_t* label, uint64_t* ticket) {
+// lctr_train_batch_async, weighted when weight is not null
+static int train_batch_async(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
+                             const uint16_t* field, const float* val, const int32_t* label, const float* weight,
+                             uint64_t* ticket) {
     LCTR_CHECK(c && ticket, "null argument");
     LCTR_CHECK(!c->keys, "lctr_train_batch_async: the streamed pipeline takes no keyed batches (lctr_upload_batch_keys + lctr_train_step)");
     LCTR_CHECK(c->cfg.deterministic != 1, "streamed batches need cfg.deterministic 0 (RED scatter) or 2 (device grouping)");
     if (pipe_init(c)) return 1;
     LCTR_CHECK(c->pipe_issued - c->pipe_waited < (uint64_t)kPipe, "more than %d streamed batches outstanding: call lctr_wait first", kPipe);
+    if (weight) {  // before anything is enqueued: a refused batch issues no ticket
+        for (int64_t r = 0; r < rows; r++)
+            LCTR_CHECK(std::isfinite(weight[r]) && weight[r] >= 0.f, "lctr_train_batch_weighted_async: weight %g of row %lld is "
+                       "not a finite value >= 0", (double)weight[r], (long long)r);
+    }
     if (c->cfg.model == LCTR_MODEL_FM && c->grad_path != GRAD_DENSE && c->cfg.world == 1 && !c->profiling && rows > 0 && nnz > 0)
-        return train_batch_async_graph(c, rows, nnz, row_ptr, fid, val, label, ticket);
+        return train_batch_async_graph(c, rows, nnz, row_ptr, fid, val, label, weight, ticket);
     const int p = (int)(c->pipe_issued % kPipe);
     const int slot = kNumSlots - kPipe + p;
+    Slot& s = c->slots[slot];
+    if (weight && rows > s.cap_rw) {  // room for the weights first (a step may still read the old array)
+        LCTR_CUDA(cudaStreamSynchronize(c->stream));
+        s.cap_rw = 0;
+        const int64_t cap = std::max(rows, s.cap_rows);
+        if (alloc_group(sized(s.rw, (size_t)cap))) return 1;
+        s.cap_rw = cap;
+    }
     // the copy may only overwrite the slot once the step that last used it has finished
     if (c->pipe_issued >= (uint64_t)kPipe) LCTR_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_computed[p], 0));
     if (c->pipe_issued >= 1) LCTR_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_copied[(p + kPipe - 1) % kPipe], 0));  // a graph-path build of the
                                                                    // other slot (build_stream) shares the slot-map scratch
     if (upload_batch_on(c, c->copy_stream, slot, rows, nnz, row_ptr, fid, field, val, label)) return 1;
+    if (weight && rows > 0) {
+        LCTR_CUDA(cudaMemcpyAsync(s.rw, weight, (size_t)rows * sizeof(float), cudaMemcpyHostToDevice, c->copy_stream));
+        s.has_rw = true;
+    }
     LCTR_CUDA(cudaEventRecord(c->ev_copied[p], c->copy_stream));
     LCTR_CUDA(cudaStreamWaitEvent(c->stream, c->ev_copied[p], 0));
     const uint64_t step = c->step;
-    if (lctr_train_step(c, slot, 0, rows, nullptr, nullptr)) return 1;
+    // the ticket's statistics come from the ring: a weighted slot always writes its weighted ones there
+    if (train_step_on(c, slot, 0, rows, true)) return 1;
     LCTR_CUDA(cudaEventRecord(c->ev_computed[p], c->stream));
     const int ri = (int)(step % kStatRing);
     LCTR_CUDA(cudaMemcpyAsync(c->h_stat_ring + 2 * ri, c->stats + 2 * ri, 2 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
@@ -985,6 +1038,17 @@ int lctr_train_batch_async(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t
     *ticket = step;
     c->pipe_issued++;
     return 0;
+}
+
+int lctr_train_batch_async(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
+                           const uint16_t* field, const float* val, const int32_t* label, uint64_t* ticket) {
+    return train_batch_async(c, rows, nnz, row_ptr, fid, field, val, label, nullptr, ticket);
+}
+
+int lctr_train_batch_weighted_async(lctr_ctx* c, int64_t rows, int64_t nnz, const int64_t* row_ptr, const uint32_t* fid,
+                                    const uint16_t* field, const float* val, const int32_t* label, const float* weight,
+                                    uint64_t* ticket) {
+    return train_batch_async(c, rows, nnz, row_ptr, fid, field, val, label, weight, ticket);
 }
 
 int lctr_wait(lctr_ctx* c, uint64_t ticket, float* loss_sum, float* acc_cnt) {

@@ -211,6 +211,8 @@ struct PipeGraph {
     uint64_t ticket = ~0ull;
     int build_kernels = 0, step_kernels = 0;  // kernel nodes of each graph: the launches its replay counts
     const uint8_t* tracked = nullptr;         // the change map the step graph ends by marking (lctr_track_changes)
+    bool weighted = false;                    // captured with the weighted instances and statistics over rw
+    const float* rw = nullptr;                // the slot's weight array the weighted graph reads
 };
 
 struct MlpLayer {
