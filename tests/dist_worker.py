@@ -27,9 +27,10 @@ def run_gpu(args, rank, world):
                           **(dict(optimizer=capi.OPT_PS_SGD, lr=float(world * args.rows)) if args.probe else {}))
     ctx.upload_params(W0, V0)
     ldist.connect(ctx)
-    if args.model == "nfm":
+    if args.model in ("nfm", "wnd"):
         for l, (w, b) in enumerate(mr.dense_layers(args.model, args.k)):
             ctx.mlp_upload(l, w, b)
+    if args.model == "nfm":  # Wide&Deep without the hook: every rank trains its own dense layers
         ldist.attach_dense_allreduce(ctx)
     stats, preds = [], []
     for b in batches:

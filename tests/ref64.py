@@ -1,17 +1,20 @@
-"""Float64 restatement of the FM / NFM / FFM forward and per-feature gradients, written from each operation's definition
-(not from any kernel's arithmetic order).  The GPU shape and gradient tests (tests/test_kernel_shapes_gpu.py,
-tests/test_gradients_gpu.py) compare the CUDA kernels with it; tests/test_ref64_cpu.py holds it against the CPU oracle first.
+"""Float64 restatement of the FM / NFM / FFM / Wide&Deep forward and per-feature gradients, written from each operation's
+definition (not from any kernel's arithmetic order).  The GPU shape and gradient tests (tests/test_kernel_shapes_gpu.py,
+tests/test_gradients_gpu.py, tests/test_wnd_gpu.py) compare the CUDA kernels with it; tests/test_ref64_cpu.py holds it
+against the CPU oracle first.
 
 Every function takes a CSR batch (row_ptr, fid, val; val None = all ones) and returns float64 arrays.  Next to each value
 it returns a condition figure: the same expression evaluated on absolute values, so a tolerance can be stated as
 `|got - want| <= rtol * cond + atol` and hold for any fp32 summation order.
 
-nfm_head restates NFM's dense layers (forward, pCTR and the input delta dz that the embedding backward consumes), and
-probe_excess is the bound of tests/test_gradients_gpu.py, which recovers each kernel's gradient from one unit SGD step.
+nfm_head restates the dense layers of NFM and Wide&Deep (forward, pCTR and the input delta dz that the embedding backward
+consumes, and on request each layer's dW / db), and probe_excess is the bound of tests/test_gradients_gpu.py, which
+recovers each kernel's gradient from one unit SGD step.
 
 Reference quirks kept on purpose:
 - FM: gV = (sumVX - x V) * gradW + l2 V per entry, with gradW = (p - y) x + l2 W (the W regulariser leaks into gV).
 - FFM: l2 V is added once per PAIR an entry takes part in, and rows whose prediction equals the label contribute nothing.
+- Wide&Deep: only the first entry of each field feeds the deep part, and L2 applies to the wide weights, never the tensors.
 - the sigmoid clamps to 1e-7 / 1 - 1e-7 outside [-16, 16] (activations.h)."""
 import numpy as np
 
@@ -87,6 +90,58 @@ def nfm_grad(row_ptr, fid, val, label, W, V, k, pred, sumvx, dz, l2, dz_cond=Non
     return _fm_like_grad(row_ptr, fid, val, label, W, V, k, pred, sumvx, l2, dz, dz_cond)
 
 
+def _wnd_first(row_ptr, fid, field, Fc):
+    """(rows [m], fields [m], entries [m]) of the first entry of each (row, field) pair present, in entry order"""
+    r = _rows(row_ptr)
+    key = r * Fc + np.asarray(field, np.int64)
+    _u, first = np.unique(key, return_index=True)  # the index of each key's first occurrence
+    return r[first], np.asarray(field, np.int64)[first], first
+
+
+def wnd_forward(row_ptr, fid, field, val, W, E, Fc, d):
+    """Wide&Deep embedding side (the per-field concat input): z[r, a d : (a + 1) d] = E[f] for the first entry f of field
+    a in row r's entry order, 0 for a field the row lacks; wide[r] = sum_i w_i x_i over every entry.
+    Returns (z [rows, Fc d], first [rows, Fc] (the first entry's fid, -1 for an absent field), wide [rows], z_cond
+    [rows, Fc d] (zeros: z is copied, not computed), wide_cond [rows])."""
+    rows = len(row_ptr) - 1
+    f = np.asarray(fid, np.int64)
+    r = _rows(row_ptr)
+    wx = np.asarray(W, np.float64)[f] * _val(val, len(f))
+    rr, aa, ii = _wnd_first(row_ptr, fid, field, Fc)
+    first = np.full((rows, Fc), -1, np.int64)
+    first[rr, aa] = f[ii]
+    z = np.zeros((rows, Fc, d))
+    z[rr, aa] = np.asarray(E, np.float64).reshape(-1, d)[f[ii]]
+    z = z.reshape(rows, Fc * d)
+    return z, first, np.bincount(r, wx, rows), np.zeros_like(z), np.bincount(r, np.abs(wx), rows)
+
+
+def wnd_grad(row_ptr, fid, field, val, label, W, E, Fc, d, pred, dz, l2, weights=None, dz_cond=None):
+    """Per-feature Wide&Deep gradient: gW[f] = sum_entries w_r (p_r - y_r) x + w_r l2 W_f (the head unclipped);
+    gE[f] = sum of dz[r, a d : (a + 1) d] over the (row, field) pairs whose first entry is f, with no L2 on the tensors.
+    weights: per-row w (None = 1); dz already carries them (nfm_head's weighted delta).  dz_cond (nfm_head's figure for
+    dz) is folded into gE's condition.  Returns (gW [F], gE [F, d], gW_cond [F], gE_cond [F, d])."""
+    f = np.asarray(fid, np.int64)
+    x = _val(val, len(f))
+    r = _rows(row_ptr)
+    W = np.asarray(W, np.float64)
+    F = len(W)
+    rw = np.ones(len(row_ptr) - 1) if weights is None else np.asarray(weights, np.float64)
+    head = rw * (np.asarray(pred, np.float64) - np.asarray(label, np.float64))
+    gw, cl2 = head[r] * x, rw[r] * l2 * W[f]
+    gW = np.bincount(f, gw + cl2, F)
+    gW_c = np.bincount(f, np.abs(gw) + np.abs(cl2), F)
+    rr, aa, ii = _wnd_first(row_ptr, fid, field, Fc)
+    dz3 = np.asarray(dz, np.float64).reshape(len(rw), Fc, d)
+    gE, gE_c = np.zeros((F, d)), np.zeros((F, d))
+    np.add.at(gE, f[ii], dz3[rr, aa])
+    c = np.abs(dz3[rr, aa])
+    if dz_cond is not None:
+        c = c + np.asarray(dz_cond, np.float64).reshape(len(rw), Fc, d)[rr, aa]
+    np.add.at(gE_c, f[ii], c)
+    return gW, gE, gW_c, gE_c
+
+
 def _act(h, act):
     """hidden activation and its derivative as a function of the output (activations.h): 0 sigmoid, 1 tanh"""
     if act == 0:
@@ -96,19 +151,24 @@ def _act(h, act):
     return o, 1 - o * o, 2 * np.abs(o)
 
 
-def nfm_head(z, wide, layers, act, masks, label, z_cond=None, wide_cond=None):
+def nfm_head(z, wide, layers, act, masks, label, z_cond=None, wide_cond=None, weights=None, grads=False):
     """The Fully_Conn_Layer chain of NFM in float64 (the oracle's orc_mlp_forward / orc_mlp_backward): layers = [(weight
     [out, in], bias [out])...], the last one linear with one output; every hidden output is masked (mask 0 -> 0) and then
     activated (masked ones included); p = sigmoid(wide + out); the delta p - y runs back with a +-15 clip per layer and the
     hidden masks on the weights, and dz is the first layer's input delta.  masks: one array per layer (None = all ones).
-    z_cond / wide_cond: nfm_forward's figures for z and the wide part.
+    z_cond / wide_cond: nfm_forward's figures for z and the wide part.  weights: per-row weights w, the output delta is then
+    w (p - y) before its clip.  Any input width works: Wide&Deep's chain is this one on wnd_forward's z.
     Returns (pctr [rows], dz [rows, k], dz_cond [rows, k], logit_cond [rows]); the figures carry the fp32 rounding of
-    every dot product, activation and input through the chain, so that |dz - dz64| <= 1e-5 * dz_cond for an fp32 chain."""
+    every dot product, activation and input through the chain, so that |dz - dz64| <= 1e-5 * dz_cond for an fp32 chain.
+    grads=True appends the per-layer batch gradients [(dW [out, in], db [out], dW_cond, db_cond)...]: dW = delta^T x and
+    db = the column sums of delta, with the layer's unmasked, clipped delta and its input x."""
     a = np.asarray(z, np.float64)
     c = np.zeros_like(a) if z_cond is None else np.asarray(z_cond, np.float64)
     n = len(layers)
+    ins = []   # (input, its figure) per layer
     acts = []  # (output, its figure, activation', |d act' / d output|) per hidden layer
     for l, (w, b) in enumerate(layers):
+        ins.append((a, c))
         w = np.asarray(w, np.float64).reshape(len(b), -1)
         b = np.asarray(b, np.float64)
         h = a @ w.T + b
@@ -125,18 +185,24 @@ def nfm_head(z, wide, layers, act, masks, label, z_cond=None, wide_cond=None):
     logit = np.asarray(wide, np.float64) + out
     logit_cond = (np.zeros_like(logit) if wide_cond is None else np.asarray(wide_cond, np.float64)) + cout
     p = sigmoid(logit)
-    delta = np.clip(p - np.asarray(label, np.float64), -15, 15)[:, None]
-    cd = (p * (1 - p) * logit_cond + np.abs(p))[:, None]
+    rw = np.ones_like(p) if weights is None else np.asarray(weights, np.float64)
+    delta = np.clip(rw * (p - np.asarray(label, np.float64)), -15, 15)[:, None]
+    cd = (np.abs(rw) * (p * (1 - p) * logit_cond + np.abs(p)))[:, None]
+    dense = [None] * n
     for l in range(n - 1, -1, -1):
         w, b = layers[l]
         w = np.asarray(w, np.float64).reshape(len(b), -1)
         if l + 1 < n and masks is not None and masks[l] is not None:
             w = w * np.asarray(masks[l], np.float64)[:, None]
         delta = np.clip(delta, -15, 15)
+        if grads:
+            x, cx = ins[l]
+            ad = np.abs(delta)
+            dense[l] = (delta.T @ x, delta.sum(0), cd.T @ np.abs(x) + ad.T @ cx + ad.T @ np.abs(x), cd.sum(0) + ad.sum(0))
         idl = delta @ w
         cidl = cd @ np.abs(w) + np.abs(delta) @ np.abs(w)
         if l == 0:
-            return p, idl, cidl, logit_cond
+            return (p, idl, cidl, logit_cond) + ((dense,) if grads else ())
         o, co, d1, d2 = acts[l - 1]
         delta = idl * d1
         cd = d1 * cidl + np.abs(idl) * d2 * co + np.abs(delta)

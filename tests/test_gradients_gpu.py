@@ -8,7 +8,8 @@ size of every coordinate's gradient, the heavy ones included.  Checks, per step:
 - |g - g64| <= 1e-5 * cond + spacing(w1) (ref64.probe_excess), with ref64's gradient and condition figure evaluated at the
   kernel's own pCTR, which is itself held to ref64's forward;
 - exactly the ids of the rows stepped moved (W), and no V row outside them.
-NFM: ref64.nfm_head restates the dense layers; the error of the fp32 dz is folded into gV's condition.
+NFM: ref64.nfm_head restates the dense layers; the error of the fp32 dz is folded into gV's condition.  Wide&Deep has
+tests/test_wnd_gpu.py, which shares these checks.
 Two ranks on one device: the merged shards against ref64 on the concatenated batch and the concatenated per-rank pCTR."""
 import os
 import subprocess
@@ -45,14 +46,16 @@ def _check_grad(what, w0, w1, g64, cond):
     assert ex[at] <= 0, (what, float(ex[at]), at, float(got[at]), float(g64.ravel()[at]), float(cond.ravel()[at]))
 
 
-def _check_moved(W0, W1, V0, V1, rowlen, fid, exact_v=True):
+def _check_moved(W0, W1, V0, V1, rowlen, fid, exact_v=True, v_fid=None):
+    """W moved on exactly the ids of fid; V on exactly those of v_fid (default fid), or only inside them (exact_v False)"""
     ids = np.unique(fid)
+    v_ids = ids if v_fid is None else np.unique(v_fid)
     moved_w = np.flatnonzero(W1 != W0)
     moved_v = np.flatnonzero(np.any((V1 != V0).reshape(-1, rowlen), 1))
     assert np.array_equal(moved_w, ids), ("W moved", len(moved_w), len(ids), np.setxor1d(moved_w, ids)[:8])
-    assert np.all(np.isin(moved_v, ids)), ("V moved outside the batch", np.setdiff1d(moved_v, ids)[:8])
+    assert np.all(np.isin(moved_v, v_ids)), ("V moved outside the batch", np.setdiff1d(moved_v, v_ids)[:8])
     if exact_v:
-        assert np.array_equal(moved_v, ids), ("V rows that did not move", np.setdiff1d(ids, moved_v)[:8])
+        assert np.array_equal(moved_v, v_ids), ("V rows that did not move", np.setdiff1d(v_ids, moved_v)[:8])
 
 
 def _rows(batch, rb, re):
@@ -96,10 +99,10 @@ def _check_ffm(batch, W0, V0, W1, V1, pred, Fc, k, l2):
 # ------------------------------------------------------------------------------------------------------------------------
 # probes
 # ------------------------------------------------------------------------------------------------------------------------
-def _unit_sgd_context(model, F, k, Fc=0, **kw):
+def _unit_sgd_context(model, F, k, Fc=0, l2=L2, **kw):
     """a context whose step is w -= g: OPT_PS_SGD with minibatch_size = lr = 1"""
     from lightctr_b200 import capi
-    return capi.Context(model, F, k, Fc, optimizer=capi.OPT_PS_SGD, lr=1.0, minibatch_size=1, l2=L2, **kw)
+    return capi.Context(model, F, k, Fc, optimizer=capi.OPT_PS_SGD, lr=1.0, minibatch_size=1, l2=l2, **kw)
 
 
 def _step(ctx, W0, V0, slot, rb, re):
@@ -369,6 +372,7 @@ def test_ffm_other_kernels_gradient_vs_ref64(tmp_path, Fc, k, det, env, l2):
     pytest.param("fm", 20000, 16, 2048, id="push_rows_kernel-hot+merge_apply_kernel-FM-K16"),
     pytest.param("nfm", 20000, 16, 1024, id="push_rows_kernel+merge_apply_kernel-NFM-K16"),
     pytest.param("ffm", 6000, 4, 256, id="merge_kernel+apply-FFM-Fc39-K4"),
+    pytest.param("wnd", 20000, 4, 512, id="wnd_backward_kernel-ent_pslot+merge_kernel+apply-WND-Fc39-d4"),
 ])
 def test_two_ranks_gradient_vs_ref64(tmp_path, model, F, k, rows):
     """lr = minibatch_size = the global batch; 2048 Criteo-shaped rows per rank put the frequent ids of the FM case over
@@ -387,5 +391,8 @@ def test_two_ranks_gradient_vs_ref64(tmp_path, model, F, k, rows):
         _check_fm(batch, W0, V0, W1, V1, pred, k)
     elif model == "nfm":
         _check_nfm(batch, W0, V0, W1, V1, pred, k, mr.dense_layers(model, k))
+    elif model == "wnd":  # every rank's own dense layers, equal at the first step
+        from test_wnd_gpu import check_wnd
+        check_wnd(batch, W0, V0, W1, V1, pred, 39, k, mr.dense_layers(model, k), 0, L2)
     else:
         _check_ffm(batch, W0, V0, W1, V1, pred, 39, k, L2)

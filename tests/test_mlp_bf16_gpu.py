@@ -1,4 +1,4 @@
-"""NFM dense layers in tensor-core mode (mlp_precision = BF16, lightctr_b200/csrc/mlp_bf16.cu).
+"""NFM and Wide&Deep dense layers in tensor-core mode (mlp_precision = BF16, lightctr_b200/csrc/mlp_bf16.cu, mlp_umma.cu).
 
 This mode is not a 1e-5 trajectory mode: operands are rounded to bf16 (fp32 accumulation, fp32 masters).  It is checked
   (1) against a plain PyTorch fp32 emulation of Fully_Conn_Layer (fullyconnLayer.h:80-180) that rounds at exactly the
@@ -12,6 +12,8 @@ import os
 
 import numpy as np
 import pytest
+
+import ref64
 
 pytestmark = pytest.mark.gpu
 
@@ -48,9 +50,8 @@ def _ctx(capi, prec, F, k, hidden, act, mb, W, V, layers, masks=None, lr=0.05):
     return c
 
 
-def _emulate(torch, capi, rp, fid, label, W, V, k, layers, act, masks):
-    """fp32 PyTorch reference with the kernel's bf16 rounding points."""
-    bf = lambda x: x.to(torch.bfloat16).to(torch.float32)
+def _nfm_embed(torch, rp, fid, W, V, k):
+    """NFM's embedding side in fp32: the bi-interaction z [rows, k] and the wide part [rows]"""
     rows = len(rp) - 1
     Vt = torch.from_numpy(V.reshape(-1, k))
     z = torch.zeros(rows, k)
@@ -61,6 +62,18 @@ def _emulate(torch, capi, rp, fid, label, W, V, k, layers, act, masks):
         s = t.sum(0)
         z[r] = 0.5 * s * s - 0.5 * (t * t).sum(0)  # train_nfm_algo.cpp:87-94
         wide[r] = torch.from_numpy(W)[ids].sum()
+    return z, wide
+
+
+def _wnd_embed(torch, rp, fid, fld, val, W, E, Fc, d):
+    """Wide&Deep's embedding side: z [rows, Fc d] (copies of the first-entry tensors: exact in fp32) and the wide part"""
+    z, _first, wide, _zc, _wc = ref64.wnd_forward(rp, fid, fld, val, W, E, Fc, d)
+    return torch.from_numpy(z.astype(np.float32)), torch.from_numpy(wide.astype(np.float32))
+
+
+def _emulate(torch, capi, z, wide, label, layers, act, masks):
+    """the dense chain on the embedding side's (z, wide): fp32 PyTorch with the kernel's bf16 rounding points"""
+    bf = lambda x: x.to(torch.bfloat16).to(torch.float32)
     y = torch.from_numpy(label.astype(np.float32))
     fwd = (lambda v: torch.sigmoid(v)) if act == capi.ACT_SIGMOID else (lambda v: torch.tanh(v))
     dact = (lambda a: a * (1 - a)) if act == capi.ACT_SIGMOID else (lambda a: 1 - a * a)
@@ -117,7 +130,7 @@ def test_bf16_mlp_matches_emulation(hidden, act_name, rows, masked, kernel, capf
     loss, acc = c.train_step(0)
     pred = c.download_pred(0)
     assert ("[mlp_umma trace" in capfd.readouterr().err) == (kernel == "umma")
-    p_ref, g_ref, _ = _emulate(torch, capi, rp, fid, label, W, V, k, layers, act, masks)
+    p_ref, g_ref, _ = _emulate(torch, capi, *_nfm_embed(torch, rp, fid, W, V, k), label, layers, act, masks)
     assert np.max(np.abs(pred - p_ref)) < 3e-3, np.max(np.abs(pred - p_ref))  # bf16-ulp flips of single activations
     y = label.astype(np.float64)
     loss_ref = float(-(y * np.log(p_ref.astype(np.float64)) + (1 - y) * np.log(1 - p_ref.astype(np.float64))).sum())
@@ -131,6 +144,81 @@ def test_bf16_mlp_matches_emulation(hidden, act_name, rows, masked, kernel, capf
             assert err < 1e-2, (l, name, err)  # max-norm relative; typical measured value is ~1e-3
             # and the bulk of the entries is much tighter than the max
             assert np.median(np.abs(got - ref)) / scale < 1e-3, (l, name)
+    c.close()
+
+
+def _mma_sync_tile(in0, hidden):
+    """the rows per CTA of the mma.sync kernel, by mlp_bf16_prepare's arithmetic: bf16_layout's shared memory (every
+    layer input as [TM][in + 8] bf16, the hidden weights as [out][in + 8] bf16, the fp32 output weights and hidden biases,
+    the bf16 masks, each 16-byte aligned) at TM = 128, or TM = 64 when that exceeds 227 KB - 1 KB"""
+    dims = [in0] + list(hidden) + [1]
+    a16 = lambda b: (b + 15) // 16 * 16
+
+    def need(tm):
+        return (sum(a16(tm * (dims[l] + 8) * 2) for l in range(len(dims) - 1)) +
+                sum(a16(dims[l + 1] * (dims[l] + 8) * 2) for l in range(len(hidden))) +
+                a16(hidden[-1] * 4) + a16(sum(hidden) * 4) + a16(sum(hidden) * 2))
+    return 128 if need(128) <= 227 * 1024 - 1024 else 64
+
+
+# Wide&Deep's first layer is Fc * d wide: (Fc, d, hidden, activation, rows, kernel, LCTR_MLP_UMMA, mma.sync tile).  Fc * d =
+# 208 is not a multiple of 64: the mma.sync kernel's dz store and dW tiles take their NC = 16 path
+WND_BF16 = [
+    pytest.param(16, 4, (64,), "sigmoid", 300, "umma", None, None, id="nfm_mlp_umma_kernel-WND-in64-H64"),
+    pytest.param(32, 8, (128, 64), "tanh", 257, "umma", None, None, id="nfm_mlp_umma_kernel-WND-in256-H128-64"),
+    pytest.param(52, 4, (64,), "sigmoid", 300, "umma", None, None, id="nfm_mlp_umma_kernel-WND-in208-H64"),
+    pytest.param(52, 4, (64,), "tanh", 300, "mma", "0", 128,
+                 id="nfm_mlp_fused_kernel-TM128-NC16-WND-in208-H64-LCTR_MLP_UMMA0"),
+    pytest.param(64, 8, (64,), "sigmoid", 300, "mma", None, 128, id="nfm_mlp_fused_kernel-TM128-WND-in512-H64"),
+    pytest.param(64, 8, (128,), "tanh", 200, "mma", None, 64, id="nfm_mlp_fused_kernel-TM64-WND-in512-H128"),
+]
+
+
+@pytest.mark.parametrize("Fc,d,hidden,act_name,rows,kernel,umma_env,tm", WND_BF16)
+def test_wnd_bf16_mlp_matches_emulation(Fc, d, hidden, act_name, rows, kernel, umma_env, tm, capfd, monkeypatch):
+    """Wide&Deep on the tensor-core dense layers, one unit SGD step (OPT_PS_SGD, lr = minibatch_size = 1: g = w0 - w1):
+    pred and every dW / db against the emulation on wnd_forward's z at the bars of the NFM rows; the tensor gradient
+    against the emulated dz scattered by first-entry fid, at the dW bar; the wide gradient against ref64 at the kernel's
+    own pCTR."""
+    torch = pytest.importorskip("torch")
+    from lightctr_b200 import capi
+    from test_gradients_gpu import L2, _check_grad
+    from test_wnd_gpu import F, wnd_batch
+    if tm is not None:
+        assert _mma_sync_tile(Fc * d, hidden) == tm
+    monkeypatch.setenv("LCTR_MLP_UMMA_TRACE", "1")
+    monkeypatch.setenv("LCTR_MLP_SKIP_UPDATE", "1")
+    if umma_env is not None:
+        monkeypatch.setenv("LCTR_MLP_UMMA", umma_env)
+    act = capi.ACT_SIGMOID if act_name == "sigmoid" else capi.ACT_TANH
+    dims = [Fc * d] + list(hidden) + [1]
+    rp, fid, fld, val, label = wnd_batch(8000 + Fc * d, Fc, rows, True)
+    W, E, layers = _params(8100 + Fc * d, F, d, dims)
+    masks = [np.ones(h, np.float32) for h in hidden]
+    c = capi.Context(capi.MODEL_WND, F, d, Fc, hidden=hidden, activation=act, mlp_precision=capi.MLP_BF16,
+                     optimizer=capi.OPT_PS_SGD, lr=1.0, minibatch_size=1, l2=L2)
+    c.upload_params(W, E)
+    for l, (w, b) in enumerate(layers):
+        c.mlp_upload(l, w, b)
+    c.upload_batch(0, rp, fid, fld, val, label)
+    c.train_step(0)
+    pred = c.download_pred(0)
+    W1, E1 = c.download_params()
+    assert ("[mlp_umma trace" in capfd.readouterr().err) == (kernel == "umma")
+    p_ref, g_ref, dz = _emulate(torch, capi, *_wnd_embed(torch, rp, fid, fld, val, W, E, Fc, d), label, layers, act, masks)
+    assert np.max(np.abs(pred - p_ref)) < 3e-3, np.max(np.abs(pred - p_ref))
+    got = [c.mlp_download_grad(l, dims[l], dims[l + 1]) for l in range(len(dims) - 1)]
+    gW, gE, gW_c, _ = ref64.wnd_grad(rp, fid, fld, val, label, W, E, Fc, d, pred, dz, L2)
+    first = np.unique(ref64.wnd_forward(rp, fid, fld, val, W, E, Fc, d)[1])
+    first = first[first >= 0]
+    pairs = [(l, "dW", g[0].reshape(r[0].shape), r[0]) for l, (g, r) in enumerate(zip(got, g_ref))]
+    pairs += [(l, "db", g[1], r[1]) for l, (g, r) in enumerate(zip(got, g_ref))]
+    pairs.append((0, "gE", (E.astype(np.float64) - E1).reshape(-1, d)[first], gE[first]))
+    for l, name, g, ref in pairs:
+        scale = np.max(np.abs(ref)) + 1e-12
+        assert np.max(np.abs(g - ref)) / scale < 1e-2, (l, name, np.max(np.abs(g - ref)) / scale)
+        assert np.median(np.abs(g - ref)) / scale < 1e-3, (l, name)
+    _check_grad("W", W, W1, gW, gW_c)
     c.close()
 
 

@@ -178,6 +178,114 @@ def test_nfm_head_and_gradient_match_the_oracle(oracle_api, act, hidden):
     assert np.count_nonzero(gV) > F  # the batch touches most features
 
 
+def _wnd_batch(rng, F, rows, Fc, with_val=True):
+    """_batch's rows (0, 1, 63, 64 and 65 entries first, fields unsorted and repeated, fields absent), plus: in the
+    63-entry row a fid repeated and one fid that is the first entry of two fields; in the 64-entry row a field whose
+    entries all lie past the 32nd"""
+    rp, fid, fld, val, lab = _batch(rng, F, rows, Fc, with_val)
+    b = rp[2]
+    fid[b + 40] = fid[b + 3]                                         # the same fid twice in a row
+    fld[b:b + 63][fld[b:b + 63] == (fld[b] + 1) % Fc] = (fld[b] + 2) % Fc
+    fid[b + 1], fld[b + 1] = fid[b], (fld[b] + 1) % Fc               # fid of entry 0 first of a second field
+    b = rp[3]
+    late = (fld[b] + 1) % Fc
+    fld[b:b + 32][fld[b:b + 32] == late] = fld[b]
+    fld[b + 50] = late                                               # field `late` only past entry 31
+    return rp, fid, fld, val, lab
+
+
+def _wnd_layers(rng, dims):
+    return [((rng.random((dims[i + 1], dims[i])) - 0.5).astype(np.float32) * np.float32(2 / np.sqrt(dims[i])),
+             (rng.standard_normal(dims[i + 1]) * 0.1).astype(np.float32)) for i in range(len(dims) - 1)]
+
+
+@pytest.mark.parametrize("Fc,d,act,hidden,with_val", [(13, 4, 0, [8], True), (6, 3, 1, [8], False),
+                                                      (40, 2, 0, [7, 5], True)],
+                         ids=["Fc13-d4-sigmoid-H8", "Fc6-d3-tanh-H8", "Fc40-d2-sigmoid-H7-5"])
+def test_wnd_forward_gradient_and_dense_gradients_match_the_oracle(oracle_api, Fc, d, act, hidden, with_val):
+    """One minibatch of WNDOracle with the parameter-server SGD rule and lr = minibatch, so that g = w0 - w1 for W and E
+    (ref64.probe_excess), and its dense layers from a zero Adagrad state (masks all 1) recovered as in the NFM test; the
+    loss from nfm_head's pCTR on wnd_forward's z."""
+    rng = np.random.default_rng(40 + Fc + d)
+    F, rows = 300, 40
+    rp, fid, fld, val, lab = _wnd_batch(rng, F, rows, Fc, with_val)
+    W = (rng.standard_normal(F) * 0.05).astype(np.float32)
+    E = (rng.standard_normal(F * d) * 0.3).astype(np.float32)
+    ds = oracle_api.Dataset(rp, fid, fld, val, lab, F, Fc)
+    o = oracle_api.WNDOracle(ds, d, hidden, W, E, lr=float(rows), batch_size=rows, minibatch=rows, act=act,
+                             optimizer="ps_sgd")
+    dims = [Fc * d] + hidden + [1]
+    layers = _wnd_layers(rng, dims)
+    for l, (w, b) in enumerate(layers):
+        o.mlp.arrays("mask", l)[:] = 1.0
+        o.mlp.arrays("weight", l)[:] = w.ravel()
+        o.mlp.arrays("bias", l)[:] = b
+    loss, _ = o.epoch()
+    z, first, wide, z_c, w_c = ref64.wnd_forward(rp, fid, fld, val, W, E, Fc, d)
+    assert np.sum(first[2] == fid[rp[2]]) == 2                       # one fid first of two fields
+    p, dz, dz_c, _lc, dense = ref64.nfm_head(z, wide, layers, act, None, lab, z_c, w_c, grads=True)
+    loss64 = float(np.sum(np.where(lab == 1, -np.log(p), -np.log(1 - p))))
+    assert abs(loss - loss64) <= 1e-5 * loss64, (loss, loss64)
+    gW, gE, gW_c, gE_c = ref64.wnd_grad(rp, fid, fld, val, lab, W, E, Fc, d, p, dz, float(o.l2), dz_cond=dz_c)
+    for name, w0, w1, g, c in (("W", W, o.W, gW, gW_c), ("E", E, o.E, gE.ravel(), gE_c.ravel())):
+        ex = ref64.probe_excess(w0.astype(np.float64) - w1, g, c, w1)
+        assert np.all(ex <= 0), (name, float(np.max(ex)), int(np.argmax(ex)))
+    moved = np.flatnonzero(np.any(o.E.reshape(F, d) != E.reshape(F, d), 1))
+    assert np.array_equal(moved, np.unique(first[first >= 0]))      # only first-of-field tensors move
+    for l in range(len(dims) - 1):
+        acc = o.mlp.arrays("accum", l)
+        out = dims[l + 1]
+        dW, db, dW_c, db_c = dense[l]
+        for w0, w1, a, g, c in ((layers[l][1], o.mlp.arrays("bias", l), acc[:out], db, db_c),
+                                (layers[l][0].ravel(), o.mlp.arrays("weight", l), acc[out:], dW.ravel(), dW_c.ravel())):
+            got, known = _adagrad_recovered(w0, w1, a, rows)
+            err = np.where(known, np.abs(got - g), np.minimum(np.abs(got - g), np.abs(-got - g)))
+            bound = 1e-5 * c + 1e-7
+            assert np.all(err <= bound), (l, float(np.max(err - bound)))
+
+
+def test_wnd_gradients_are_the_derivatives():
+    """With l2 = 0, for the weighted loss L = sum_r w_r logloss(p_r) of the whole float64 Wide&Deep model (wnd_forward +
+    nfm_head, no delta reaching the +-15 clip): wnd_grad's gW and gE and nfm_head's dense gradients agree with central
+    differences of L to 1e-6 relative, on rows with repeated fields and fids."""
+    rng = np.random.default_rng(12)
+    F, rows, Fc, d = 100, 10, 5, 3
+    rp, fid, fld, val, lab = _wnd_batch(rng, F, rows, Fc)
+    val = val.astype(np.float64)
+    W = rng.standard_normal(F) * 0.1
+    E = rng.standard_normal(F * d) * 0.3
+    layers = [(w.astype(np.float64), b.astype(np.float64)) for w, b in _wnd_layers(rng, [Fc * d, 6, 4, 1])]
+    rw = 0.25 + 2 * rng.random(rows)
+
+    def loss(W_, E_, layers_):
+        z, _f, wide, _zc, _wc = ref64.wnd_forward(rp, fid, fld, val, W_, E_, Fc, d)
+        p = ref64.nfm_head(z, wide, layers_, 1, None, lab)[0]
+        return float(np.sum(rw * np.where(lab == 1, -np.log(p), -np.log(1 - p))))
+
+    z, first, wide, _zc, _wc = ref64.wnd_forward(rp, fid, fld, val, W, E, Fc, d)
+    p, dz, _dc, _lc, dense = ref64.nfm_head(z, wide, layers, 1, None, lab, weights=rw, grads=True)
+    gW, gE, _, _ = ref64.wnd_grad(rp, fid, fld, val, lab, W, E, Fc, d, p, dz, 0.0, weights=rw)
+    firsts = np.unique(first[first >= 0])
+    seen_late = np.setdiff1d(np.unique(fid), firsts)                 # fids never first of a field: gE = 0
+    assert len(seen_late) > 0 and np.all(gE[seen_late] == 0)
+    idxE = (firsts[:8, None] * d + np.arange(d)).ravel()
+    numE = _num_grad(lambda e: loss(W, e, layers), E, idxE)
+    assert np.allclose(gE.ravel()[idxE], numE, rtol=1e-6, atol=1e-8)
+    ids = np.unique(fid)[:8]
+    assert np.allclose(gW[ids], _num_grad(lambda w: loss(w, E, layers), W, ids), rtol=1e-6, atol=1e-8)
+    for l in range(len(layers)):
+        def with_layer(wb, l=l, part=0):
+            out = list(layers)
+            out[l] = (wb.reshape(layers[l][0].shape), layers[l][1]) if part == 0 else (layers[l][0], wb)
+            return out
+        w, b = layers[l]
+        iw = np.arange(0, w.size, max(1, w.size // 7))
+        numw = _num_grad(lambda v: loss(W, E, with_layer(v)), w.ravel(), iw)
+        assert np.allclose(dense[l][0].ravel()[iw], numw, rtol=1e-6, atol=1e-8), l
+        numb = _num_grad(lambda v: loss(W, E, with_layer(v, part=1)), b, np.arange(len(b)))
+        assert np.allclose(dense[l][1], numb, rtol=1e-6, atol=1e-8), l
+
+
 def _hot_fm_problem(rows=2000, F=500, k=8, seed=31):
     """every row holds id 0; returns the batch, parameters, the float64 forward and gradient"""
     rng = np.random.default_rng(seed)

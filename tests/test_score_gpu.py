@@ -15,7 +15,7 @@ import pytest
 
 import ref64
 from test_kernel_shapes_gpu import _check_pctr
-from test_mlp_bf16_gpu import _emulate
+from test_mlp_bf16_gpu import _emulate, _nfm_embed
 
 pytestmark = pytest.mark.gpu
 
@@ -227,8 +227,8 @@ def test_nfm_bf16_score_vs_emulation(name, monkeypatch):
     c, info = _make(capi, monkeypatch, name, 300)
     s = c.score(0)
     rp, fid, _, _, label = info["batch"]
-    p_ref, _, _ = _emulate(torch, capi, rp, fid, label, info["W"], info["V"], info["k"], info["layers"], capi.ACT_SIGMOID,
-                           info["masks"])
+    p_ref, _, _ = _emulate(torch, capi, *_nfm_embed(torch, rp, fid, info["W"], info["V"], info["k"]), label, info["layers"],
+                           capi.ACT_SIGMOID, info["masks"])
     assert np.max(np.abs(s - p_ref)) < 3e-3, np.max(np.abs(s - p_ref))  # bf16-ulp flips of single activations
     c.close()
 
