@@ -477,17 +477,16 @@ int csc_build_device(lctr_ctx* c, Slot& s, cudaStream_t st, const int32_t* label
     return 0;
 }
 
+using DevCscK = Built<4, 8, 16, 32>;  // the factor counts of the device feature-major backward
+
 template <int K>
 static int bwd_go(lctr_ctx* c, Slot& s, const OptParams& P, const OptParams* dP) {
     const unsigned grid = (unsigned)c->sm_count * 4;
     const CscView C{s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, s.label, s.pred, s.sumvx};
     const ParamView T{c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V};
     const uint2* longs = s.long_list;
-    const bool rw = s.has_rw;
-    auto lk = s.has_val ? (rw ? csc_backward_long_kernel<K, true, true> : csc_backward_long_kernel<K, true>)
-                        : (rw ? csc_backward_long_kernel<K, false, true> : csc_backward_long_kernel<K, false>);
-    auto sk = s.has_val ? (rw ? csc_backward_short_kernel<K, true, true> : csc_backward_short_kernel<K, true>)
-                        : (rw ? csc_backward_short_kernel<K, false, true> : csc_backward_short_kernel<K, false>);
+    auto lk = by_flags([](auto hv, auto rw) { return csc_backward_long_kernel<K, hv, rw>; }, s.has_val, s.has_rw);
+    auto sk = by_flags([](auto hv, auto rw) { return csc_backward_short_kernel<K, hv, rw>; }, s.has_val, s.has_rw);
     return launch(c, {grid, 256, 0, c->stream}, lk, longs, s.csc_totals, C, T, s.csc_acc, s.csc_arrived, c->cfg.l2_reg, P, dP,
                   row_weights(s)) ||
            launch(c, {grid, 256, 0, c->stream}, sk, s.short_list, s.csc_totals, C, T, c->cfg.l2_reg, P, dP, row_weights(s));
@@ -503,15 +502,11 @@ int launch_fm_backward_devcsc_ex(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, c
     if (P_host) P = *P_host; else P = make_opt_params(c, re - rb);
     ProfScope prof(c, PROF_FM_BWD_CSC);
     const OptParams* d = reinterpret_cast<const OptParams*>(dP);
-    switch (k) {
-        case 4: return bwd_go<4>(c, s, P, d);
-        case 8: return bwd_go<8>(c, s, P, d);
-        case 16: return bwd_go<16>(c, s, P, d);
-        case 32: return bwd_go<32>(c, s, P, d);
-        default:
-            set_error("device feature-major backward is built for k in {4, 8, 16, 32} (k=%d)", k);
-            return 1;
+    if (!DevCscK::has(k)) {
+        set_error("device feature-major backward is built for k in {4, 8, 16, 32} (k=%d)", k);
+        return 1;
     }
+    return DevCscK::pick(k, [&](auto K) { return bwd_go<K>(c, s, P, d); });
 }
 
 int launch_fm_backward_devcsc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
@@ -527,7 +522,7 @@ void csc_opt_params(lctr_ctx* c, int64_t rows, void* out) {
 bool csc_device_supported(const lctr_ctx* c) {
     const int k = (int)c->cfg.factor_cnt;
     if (c->cfg.model == LCTR_MODEL_FFM) return ffm_grouped_supported(c);
-    return c->cfg.model == LCTR_MODEL_FM && (k == 4 || k == 8 || k == 16 || k == 32);
+    return c->cfg.model == LCTR_MODEL_FM && DevCscK::has(k);
 }
 
 }  // namespace lctr

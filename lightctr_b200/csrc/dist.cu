@@ -717,11 +717,6 @@ merge_apply_kernel(PeerTable P, ArenaLayout A, int me, int world, unsigned long 
     }
 }
 
-template <int K>
-static auto merge_apply_instance(int opt) {
-    return by_opt(opt, [](auto o) { return merge_apply_kernel<K, o.value>; });
-}
-
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 int dist_alloc(lctr_ctx* c) {
@@ -1055,9 +1050,9 @@ int dist_post_step(lctr_ctx* c, Slot& s, int slot, int64_t rows_divisor) {
         }
         ProfScope prof(c, PROF_DIST_MERGE);
         const OptParams Pp = make_opt_params(c, rows_divisor);
-        const int k = (int)c->cfg.factor_cnt;
-        auto kern = k == 4 ? merge_apply_instance<4>(Pp.opt) : k == 8 ? merge_apply_instance<8>(Pp.opt)
-                  : k == 16 ? merge_apply_instance<16>(Pp.opt) : merge_apply_instance<32>(Pp.opt);
+        auto kern = by_value<4, 8, 16, 32>((int)c->cfg.factor_cnt, [&](auto K) {
+            return by_opt(Pp.opt, [&](auto o) { return merge_apply_kernel<K, o>; });
+        });
         // dependent: behind my push kernel
         if (launch(c, {(unsigned)c->sm_count * 4, 256, 0, c->stream, true}, kern, d->peers, d->A, d->rank, d->world,
                    d->epoch, d->recw, d->own_uniq + (size_t)slot * d->cap_own, d->n_own + slot,

@@ -503,19 +503,6 @@ int launch_ffm_predict_inorder(lctr_ctx* c, Slot& s) {
                   s.row_ptr, s.fid, s.field, s.val, c->cW, c->cV, (int)c->cfg.field_cnt, (int)c->cfg.factor_cnt, s.pred, s.rows);
 }
 
-// the CTA-per-sample kernel's instance (bulk: the TMA bulk reduce-add of the gradient rows, 4-wide training rows only)
-template <int VEC, bool HV, bool TR>
-static auto ffm_kernel(bool bulk, bool rw) {
-    if (TR && rw)
-        return bulk ? ffm_fused_kernel<VEC, HV, TR, (VEC == 4) && TR, false, TR> : ffm_fused_kernel<VEC, HV, TR, false, false, TR>;
-    return bulk ? ffm_fused_kernel<VEC, HV, TR, (VEC == 4) && TR> : ffm_fused_kernel<VEC, HV, TR, false>;
-}
-template <int VEC>
-static auto ffm_kernel(bool hv, bool train, bool bulk, bool rw) {
-    return hv ? (train ? ffm_kernel<VEC, true, true>(bulk, rw) : ffm_kernel<VEC, true, false>(bulk, rw))
-              : (train ? ffm_kernel<VEC, false, true>(bulk, rw) : ffm_kernel<VEC, false, false>(bulk, rw));
-}
-
 // step_kernel: the kernel a train step chooses, otherwise the plain CTA-per-sample kernel; train (implies step_kernel): that
 // kernel's forward + backward instance with the step's statistics, otherwise its forward-only instance
 static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool step_kernel, bool train, bool grouped = false) {
@@ -538,10 +525,9 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool step_ke
     ProfScope prof(c, PROF_FFM_FUSED);
     if (grouped) {
         LCTR_CHECK(train && vec == 4 && c->ffm_T && c->ffm_cnt, "grouped FFM step needs k %% 4 == 0 and the tile buffer");
-        return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream},
-                      s.has_rw ? (s.has_val ? ffm_fused_kernel<4, true, true, false, true, true> : ffm_fused_kernel<4, false, true, false, true, true>)
-                               : (s.has_val ? ffm_fused_kernel<4, true, true, false, true> : ffm_fused_kernel<4, false, true, false, true>),
-                      s.row_ptr, s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, nullptr, c->cfg.l2_reg, rb,
+        auto kern = by_flags([](auto hv, auto rw) { return ffm_fused_kernel<4, hv, true, false, true, rw>; }, s.has_val, s.has_rw);
+        return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream}, kern, s.row_ptr, s.fid, s.field, s.val, s.label, c->cW,
+                      c->cV, Fc, k, s.pred, c->cgW, c->cgV, nullptr, c->cfg.l2_reg, rb,
                       c->stat_partial, c->stat_done, out_slot, train ? 1 : 0, c->ffm_T, c->ffm_cnt, row_weights(s));
     }
     // LCTR_FFM_TMA=1 selects the TMA-staged kernel (cp.async.bulk rows + mbarrier).  It is parity-green but NOT the
@@ -562,9 +548,7 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool step_ke
         LCTR_CHECK(CR >= 8, "FFM field-pair tile + row buffer do not fit 227 KB shared memory: Fc=%d k=%d", Fc, k);
         const size_t smem2 = (size_t)CR * (stage_bytes + 14) + fixed;
         const int tpb2 = std::max(64, (A + 31) / 32 * 32);
-        const bool rw = train && s.has_rw;
-        auto tma = s.has_val ? (train ? (rw ? ffm_tma_kernel<true, true, true> : ffm_tma_kernel<true, true>) : ffm_tma_kernel<true, false>)
-                             : (train ? (rw ? ffm_tma_kernel<false, true, true> : ffm_tma_kernel<false, true>) : ffm_tma_kernel<false, false>);
+        auto tma = by_flags([](auto hv, auto tr, auto rw) { return ffm_tma_kernel<hv, tr, tr && rw>; }, s.has_val, train, s.has_rw);
         return launch(c, {(unsigned)rows, (unsigned)tpb2, smem2, c->stream}, tma, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW,
                       c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot,
                       train ? 1 : 0, CR, row_weights(s));
@@ -574,10 +558,12 @@ static int ffm_launch(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool step_ke
         const int rc = launch_ffm_warp(c, s, rb, re, train, train);
         if (rc >= 0) return rc;
     }
-    // (a forward-only instance of the bulk kernel is the plain one: ffm_kernel takes the bulk path with training only)
-    const bool rw = train && s.has_rw;
-    auto kern = vec == 4 ? ffm_kernel<4>(s.has_val, train, bulk, rw) : vec == 2 ? ffm_kernel<2>(s.has_val, train, bulk, rw)
-                                                                        : ffm_kernel<1>(s.has_val, train, bulk, rw);
+    // bulk: the TMA bulk reduce-add of the gradient rows, on 4-wide training rows only (a forward-only instance of the bulk
+    // kernel is the plain one); weighted rows: training instances only
+    auto kern = by_value<4, 2, 1>(vec, [&](auto V) {
+        return by_flags([&](auto hv, auto tr, auto bk, auto rw) { return ffm_fused_kernel<V, hv, tr, bk && V == 4 && tr, false, tr && rw>; },
+                        s.has_val, train, bulk, s.has_rw);
+    });
     return launch(c, {(unsigned)rows, (unsigned)tpb, smem, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid,
                   s.field, s.val, s.label, c->cW, c->cV, Fc, k, s.pred, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(),
                   c->cfg.l2_reg, rb, c->stat_partial, c->stat_done, out_slot, train ? 1 : 0, nullptr, nullptr, row_weights(s));

@@ -248,10 +248,7 @@ int launch_ffm_backward_grouped(lctr_ctx* c, Slot& s, int64_t rb, int64_t re) {
     const unsigned grid = (unsigned)c->sm_count * 8;
     ProfScope prof(c, PROF_FM_BWD_CSC);
     LCTR_CHECK(NS >= 1 && NS <= 4, "grouped FFM backward: row of %d floats exceeds 512", Fc * k);
-    auto kern = s.has_rw ? (s.has_val ? (fuse ? ffm_backward_grouped_kernel<true, true, true> : ffm_backward_grouped_kernel<true, false, true>)
-                                      : (fuse ? ffm_backward_grouped_kernel<false, true, true> : ffm_backward_grouped_kernel<false, false, true>))
-                         : (s.has_val ? (fuse ? ffm_backward_grouped_kernel<true, true> : ffm_backward_grouped_kernel<true, false>)
-                                      : (fuse ? ffm_backward_grouped_kernel<false, true> : ffm_backward_grouped_kernel<false, false>));
+    auto kern = by_flags([](auto hv, auto fu, auto rw) { return ffm_backward_grouped_kernel<hv, fu, rw>; }, s.has_val, fuse, s.has_rw);
     return launch(c, {grid, 128, 0, c->stream}, kern, C, T, Fc, k, NS, c->cfg.l2_reg, P, row_weights(s));
 }
 

@@ -288,14 +288,7 @@ ffm_warp_kernel(const int64_t* __restrict__ row_ptr, const uint32_t* __restrict_
 }  // namespace
 
 // returns 0 when launched, -1 when the shape is not covered (caller falls back to ffm.cu), 1 on error.  train = false: the
-// forward-only instance (stats unused)
-template <int PASSES>
-static auto warp_kernel(bool hv, bool train, bool rw) {
-    if (train && rw) return hv ? ffm_warp_kernel<PASSES, true, true, true> : ffm_warp_kernel<PASSES, false, true, true>;
-    return hv ? (train ? ffm_warp_kernel<PASSES, true, true> : ffm_warp_kernel<PASSES, true, false>)
-              : (train ? ffm_warp_kernel<PASSES, false, true> : ffm_warp_kernel<PASSES, false, false>);
-}
-
+// forward-only instance (stats unused); the weighted instance exists for training only
 int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats, bool train) {
     static const bool off = getenv("LCTR_FFM_WARP") && atoi(getenv("LCTR_FFM_WARP")) == 0;
     const int k = (int)c->cfg.factor_cnt, Fc = (int)c->cfg.field_cnt;
@@ -315,9 +308,9 @@ int launch_ffm_warp(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats, bo
     ProfScope prof(c, PROF_FFM_FUSED);
     const uint32_t* ids = c->cfg.world > 1 ? s.ent_pslot : s.fid;
     uint8_t* touched = c->cfg.world > 1 ? nullptr : c->touched.get();
-    const bool rw = s.has_rw;
-    auto kern = passes == 1 ? warp_kernel<1>(s.has_val, train, rw) : passes == 2 ? warp_kernel<2>(s.has_val, train, rw)
-              : passes == 3 ? warp_kernel<3>(s.has_val, train, rw) : warp_kernel<4>(s.has_val, train, rw);
+    auto kern = by_value<1, 2, 3, 4>(passes, [&](auto P) {
+        return by_flags([&](auto hv, auto tr, auto rw) { return ffm_warp_kernel<P, hv, tr, tr && rw>; }, s.has_val, train, s.has_rw);
+    });
     return launch(c, {grid, (unsigned)warps * 32, smem, c->stream}, kern, s.row_ptr, ids, s.field, s.val, s.label, c->cW, c->cV, Fc,
                   k, s.pred, c->cgW, c->cgV, touched, c->cfg.l2_reg, rb, rows, (int)tile, c->stat_partial, c->stat_done, out_slot,
                   stats ? 1 : 0, row_weights(s));

@@ -253,24 +253,6 @@ static bool pick_shape(int k, Shape& sh) {
     return false;
 }
 
-// the instance of fm_backward_kernel for the row shape
-template <int VEC, bool HV, bool NF, bool RW>
-static auto backward_lpr(int lpr) {
-    switch (lpr) {
-        case 1: return fm_backward_kernel<1, VEC, HV, NF, RW>;
-        case 2: return fm_backward_kernel<2, VEC, HV, NF, RW>;
-        case 4: return fm_backward_kernel<4, VEC, HV, NF, RW>;
-        case 8: return fm_backward_kernel<8, VEC, HV, NF, RW>;
-        case 16: return fm_backward_kernel<16, VEC, HV, NF, RW>;
-        default: return fm_backward_kernel<32, VEC, HV, NF, RW>;
-    }
-}
-template <int VEC, bool RW>
-static auto backward_kernel(int lpr, bool hv, bool nfm) {
-    return hv ? (nfm ? backward_lpr<VEC, true, true, RW>(lpr) : backward_lpr<VEC, true, false, RW>(lpr))
-              : (nfm ? backward_lpr<VEC, false, true, RW>(lpr) : backward_lpr<VEC, false, false, RW>(lpr));
-}
-
 // Coalesced variant for K % 8 == 0: LPR = K/4 lanes cover one V row with float4 loads (a 64 B row is ONE request of two
 // fully used sectors instead of four scattered 16 B requests), so a warp gathers G = 32/LPR rows per load instruction.
 // The avx-ordered self dot runs across the LPR lanes (chunk sums, then the hsum tree), the shared tile is
@@ -401,11 +383,6 @@ fm_forward_coalesced_kernel(const int64_t* __restrict__ row_ptr, const uint32_t*
     if (!NFM && do_stats) publish_stats(loss, correct, partial, done, out_slot, false);
 }
 
-template <int K, bool HV, bool NF>
-static auto forward_kernel(bool co) {
-    return co ? fm_forward_coalesced_kernel<(K % 8 == 0) && K <= 32 ? K : 8, HV, NF> : fm_forward_kernel<K, HV, NF>;
-}
-
 template <int K>
 static int fwd_go(lctr_ctx* c, Slot& s, bool nfm, int64_t rb, int64_t re, double* out_slot, int stats, const int64_t* hdr) {
     constexpr bool kCoalesced = (K % 8 == 0) && K <= 32;
@@ -416,8 +393,9 @@ static int fwd_go(lctr_ctx* c, Slot& s, bool nfm, int64_t rb, int64_t re, double
     const int wpb = co ? 4 : 8;
     const unsigned grid = (unsigned)((re - rb + wpb - 1) / wpb);
     const size_t smem = co ? (size_t)wpb * (K + 2) * 68 * sizeof(float) : (size_t)wpb * 64 * (K + 4) * sizeof(float);
-    auto kern = s.has_val ? (nfm ? forward_kernel<K, true, true>(co) : forward_kernel<K, true, false>(co))
-                          : (nfm ? forward_kernel<K, false, true>(co) : forward_kernel<K, false, false>(co));
+    auto kern = by_flags([co](auto hv, auto nf) {
+        return co ? fm_forward_coalesced_kernel<kCoalesced ? K : 8, hv, nf> : fm_forward_kernel<K, hv, nf>;
+    }, s.has_val, nfm);
     return launch(c, {grid, (unsigned)wpb * 32, smem, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val,
                   s.label, c->cW, c->cV, s.pred, s.sumvx, c->z, s.wide, rb, re, c->stat_partial, c->stat_done, out_slot, stats, hdr,
                   c->fwd_quirk_sumvx, c->fwd_quirk_rows);
@@ -436,18 +414,16 @@ int launch_fm_forward_ex(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm,
     double* out_slot = out_slot_override ? out_slot_override : c->stats + 2 * (c->step % kStatRing);
     const int st = stats ? 1 : 0;
     ProfScope prof(c, PROF_FM_FWD);
+    // the factor count is a compile-time constant of the kernel (register-resident rows)
+    using FwdK = Built<1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 16, 20, 24, 32>;
+    if (!FwdK::has(k)) {
+        set_error("factor_cnt=%d is not instantiated (built: 1-8, 10, 12, 16, 20, 24, 32)", k);
+        return 1;
+    }
     int rc = 0;
     static const int dbg_repeat = getenv("LCTR_DBG_FWD_REPEAT") ? atoi(getenv("LCTR_DBG_FWD_REPEAT")) : 1;
     for (int rep = 0; rep < dbg_repeat && !rc; rep++)
-    switch (k) {  // the factor count is a compile-time constant of the kernel (register-resident rows)
-#define FWD_CASE(KK) case KK: rc = fwd_go<KK>(c, s, nfm, rb, re, out_slot, st, hdr); break;
-        FWD_CASE(1) FWD_CASE(2) FWD_CASE(3) FWD_CASE(4) FWD_CASE(5) FWD_CASE(6) FWD_CASE(7) FWD_CASE(8)
-        FWD_CASE(10) FWD_CASE(12) FWD_CASE(16) FWD_CASE(20) FWD_CASE(24) FWD_CASE(32)
-#undef FWD_CASE
-        default:
-            set_error("factor_cnt=%d is not instantiated (built: 1-8, 10, 12, 16, 20, 24, 32)", k);
-            return 1;
-    }
+        rc = FwdK::pick(k, [&](auto K) { return fwd_go<K>(c, s, nfm, rb, re, out_slot, st, hdr); });
     return rc;
 }
 
@@ -459,8 +435,11 @@ int launch_fm_backward(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
     if (rows <= 0) return 0;
     const unsigned grid = (unsigned)((rows + 7) / 8);
     ProfScope prof(c, PROF_FM_BWD_RED);
-    auto kern = s.has_rw ? (sh.vec == 4 ? backward_kernel<4, true>(sh.lpr, s.has_val, nfm) : backward_kernel<1, true>(sh.lpr, s.has_val, nfm))
-                         : (sh.vec == 4 ? backward_kernel<4, false>(sh.lpr, s.has_val, nfm) : backward_kernel<1, false>(sh.lpr, s.has_val, nfm));
+    auto kern = by_value<1, 2, 4, 8, 16, 32>(sh.lpr, [&](auto lpr) {
+        return by_value<4, 1>(sh.vec, [&](auto vec) {
+            return by_flags([&](auto hv, auto nf, auto rw) { return fm_backward_kernel<lpr, vec, hv, nf, rw>; }, s.has_val, nfm, s.has_rw);
+        });
+    });
     return launch(c, {grid, 256, 0, c->stream}, kern, s.row_ptr, c->cfg.world > 1 ? s.ent_pslot : s.fid, s.val, s.label, c->cW,
                   c->cV, k, s.pred, s.sumvx, c->dz, c->cgW, c->cgV, c->cfg.world > 1 ? nullptr : c->touched.get(), c->cfg.l2_reg, rb,
                   re, row_weights(s));
@@ -545,16 +524,6 @@ fm_backward_csc_kernel(const int64_t* __restrict__ seg_ptr, const uint32_t* __re
     }
 }
 
-template <int LR, bool RW>
-static auto backward_csc_kernel(bool hv, bool nfm) {
-    return hv ? (nfm ? fm_backward_csc_kernel<LR, true, true, RW> : fm_backward_csc_kernel<LR, true, false, RW>)
-              : (nfm ? fm_backward_csc_kernel<LR, false, true, RW> : fm_backward_csc_kernel<LR, false, false, RW>);
-}
-template <int LR>
-static auto backward_csc_kernel(bool hv, bool nfm, bool rw) {
-    return rw ? backward_csc_kernel<LR, true>(hv, nfm) : backward_csc_kernel<LR, false>(hv, nfm);
-}
-
 int launch_fm_backward_csc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nfm) {
     const int k = (int)c->cfg.factor_cnt;
     LCTR_CHECK(k <= 32, "factor_cnt=%d unsupported by the feature-major backward (need k <= 32)", k);
@@ -571,9 +540,9 @@ int launch_fm_backward_csc(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool nf
     const int segs_per_cta = 8 * (32 / lr);
     const unsigned grid = (unsigned)((se - sb + segs_per_cta - 1) / segs_per_cta);
     ProfScope prof(c, PROF_FM_BWD_CSC);
-    const bool rw = s.has_rw;
-    auto kern = lr == 4 ? backward_csc_kernel<4>(s.has_val, nfm, rw) : lr == 8 ? backward_csc_kernel<8>(s.has_val, nfm, rw)
-              : lr == 16 ? backward_csc_kernel<16>(s.has_val, nfm, rw) : backward_csc_kernel<32>(s.has_val, nfm, rw);
+    auto kern = by_value<4, 8, 16, 32>(lr, [&](auto LR) {
+        return by_flags([&](auto hv, auto nf, auto rw) { return fm_backward_csc_kernel<LR, hv, nf, rw>; }, s.has_val, nfm, s.has_rw);
+    });
     return launch(c, {grid, 256, 0, c->stream}, kern, s.seg_ptr, s.seg_fid, s.ent_row, s.ent_x, sb, se, s.label, s.pred, s.sumvx,
                   c->dz, rb, c->W, c->V, c->s1W, c->s1V, c->s2W, c->s2V, k, c->cfg.l2_reg, P, row_weights(s));
 }

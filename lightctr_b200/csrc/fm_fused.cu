@@ -107,15 +107,6 @@ int launch_slotmap_compact(lctr_ctx* c, uint8_t* mark, size_t T, uint32_t* uniq,
     return launch(c, {cg, 256, 0, st}, slotmap_compact_kernel, mark, T, uniq, n_uniq, nullptr);
 }
 
-// mode 1: FM forward + backward;  2: NFM forward (z, wide part);  3: NFM backward from dz.  rw: the weighted instances of
-// the modes that form a head (the NFM forward has none)
-template <int K, bool HV>
-static auto fused_kernel(int mode, bool rw) {
-    if (rw && mode != 2) return mode == 1 ? fm_fused_kernel<K, HV, 1, false, 4, true> : fm_fused_kernel<K, HV, 3, false, 4, true>;
-    return mode == 1 ? fm_fused_kernel<K, HV, 1, false>
-         : mode == 2 ? fm_fused_kernel<K, HV, 2, false> : fm_fused_kernel<K, HV, 3, false>;
-}
-
 template <int K>
 static int fused_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, double* out_slot, const int64_t* hdr, int mode) {
     FusedState* f = c->fused.get();
@@ -130,29 +121,25 @@ static int fused_go(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, int stats, dou
     // dependent launches: MODE 1 on several GPUs behind my own serve kernel (it polls the owners' flags at its head); the NFM
     // backward on one GPU behind the dense kernels in front of it (it requests its batch data before their end)
     const bool dependent = mode == 1 ? multi : mode == 3 && !multi;
-    const bool rw = s.has_rw;
-    return launch(c, {grid, 128, 0, c->stream, dependent}, s.has_val ? fused_kernel<K, true>(mode, rw) : fused_kernel<K, false>(mode, rw),
-                  s.row_ptr, multi ? s.ent_pslot : s.fid, s.ent_slot, s.val, s.label, c->cW, c->cV, s.pred, s.sumvx, nullptr, f->G,
+    // mode 1: FM forward + backward;  2: NFM forward (z, wide part);  3: NFM backward from dz.  Weighted rows: the weighted
+    // instances of the modes that form a head (the NFM forward has none)
+    auto kern = by_value<1, 2, 3>(mode, [&](auto m) {
+        return by_flags([&](auto hv, auto rw) { return fm_fused_kernel<K, hv, m, false, 4, rw && m != 2>; }, s.has_val, s.has_rw);
+    });
+    return launch(c, {grid, 128, 0, c->stream, dependent}, kern, s.row_ptr, multi ? s.ent_pslot : s.fid, s.ent_slot, s.val, s.label, c->cW, c->cV, s.pred, s.sumvx, nullptr, f->G,
                   f->Ghot, f->GS, c->cfg.l2_reg, rb, re, hdr, c->stat_partial, c->stat_done, out_slot, stats, wf, nw, ep,
                   mode == 2 ? c->z : mode == 3 ? c->dz.get() : nullptr, mode == 2 ? s.wide.get() : nullptr, row_weights(s));
 }
 
-// FM k in {4, 8, 16, 32}: go<K>(args...) for the context's k (32 for any other)
-#define K_DISPATCH(go, ...)                                                                                                      \
-    switch ((int)c->cfg.factor_cnt) {                                                                                            \
-        case 4: return go<4>(__VA_ARGS__);                                                                                       \
-        case 8: return go<8>(__VA_ARGS__);                                                                                       \
-        case 16: return go<16>(__VA_ARGS__);                                                                                     \
-        default: return go<32>(__VA_ARGS__);                                                                                     \
-    }
-
+// the launchers below are built for FM k in {4, 8, 16, 32} and take 32 for any other k
 static int launch_fused_mode(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool stats, const int64_t* hdr, double* out_slot_override,
                              int mode, int prof_id) {
     if (re - rb <= 0) return 0;
     LCTR_CHECK(s.fused_valid, "fused FM step on a slot without its slot map (uploaded before the context supported it?)");
     double* out_slot = out_slot_override ? out_slot_override : c->stats + 2 * (c->step % kStatRing);
     ProfScope prof(c, prof_id);
-    K_DISPATCH(fused_go, c, s, rb, re, stats ? 1 : 0, out_slot, hdr, mode)
+    return by_value<4, 8, 16, 32>((int)c->cfg.factor_cnt,
+                                  [&](auto K) { return fused_go<K>(c, s, rb, re, stats ? 1 : 0, out_slot, hdr, mode); });
 }
 
 // forward + RED backward of rows [rb, re) of the slot.  hdr != nullptr: `re` only sizes the grid, the row count comes
@@ -192,7 +179,8 @@ int launch_fm_forward_tree(lctr_ctx* c, Slot& s, int64_t rb, int64_t re, bool st
     if (re - rb <= 0) return 0;
     double* out_slot = c->stats + 2 * (c->step % kStatRing);
     ProfScope prof(c, PROF_FM_FWD);
-    K_DISPATCH(fwd_tree_go, c, s, rb, re, stats ? 1 : 0, out_slot)
+    return by_value<4, 8, 16, 32>((int)c->cfg.factor_cnt,
+                                  [&](auto K) { return fwd_tree_go<K>(c, s, rb, re, stats ? 1 : 0, out_slot); });
 }
 
 template <int K>
@@ -210,9 +198,8 @@ static int apply_go(lctr_ctx* c, Slot& s, const OptParams& P, const OptParams* P
 int launch_apply_compact(lctr_ctx* c, Slot& s, int64_t rows_in_step, const OptParams* P_host, const OptParams* dP) {
     const OptParams P = P_host ? *P_host : make_opt_params(c, rows_in_step);
     ProfScope prof(c, PROF_APPLY_COMPACT);
-    K_DISPATCH(apply_go, c, s, P, dP)
+    return by_value<4, 8, 16, 32>((int)c->cfg.factor_cnt, [&](auto K) { return apply_go<K>(c, s, P, dP); });
 }
-#undef K_DISPATCH
 
 void fused_opt_params(lctr_ctx* c, int64_t rows, void* out) { *reinterpret_cast<OptParams*>(out) = make_opt_params(c, rows); }
 void* fused_dev_opt(lctr_ctx* c) { return c->fused ? c->fused->d_opt.get() : nullptr; }

@@ -104,12 +104,9 @@ static unsigned warp_grid(const lctr_ctx* c, size_t m) {
 static unsigned stride_grid(const lctr_ctx* c, size_t n) {
     return (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
 }
-// the instance of a row kernel for the context's rows: 16-byte accesses when rowlen % 4 == 0 (FM / NFM k % 4 == 0,
+// the VEC4 instance of a row kernel for the context's rows: 16-byte accesses when rowlen % 4 == 0 (FM / NFM k % 4 == 0,
 // FFM Fc * k % 4 == 0), scalar ones otherwise
-template <class K>
-static K by_rowlen(const lctr_ctx* c, K vec4, K scalar) {
-    return (c->rowlen & 3) == 0 ? vec4 : scalar;
-}
+static bool rows_vec4(const lctr_ctx* c) { return (c->rowlen & 3) == 0; }
 
 // the per-row arrays that move with a row
 struct RowArrays {
@@ -802,7 +799,7 @@ static bool tier_live(const KeyTable* t) { return t->tier && t->tier->n > 0; }
 int init_new_rows(lctr_ctx* c, int64_t max_new) {
     KeyTable* t = c->keys.get();
     const bool tiered = tier_live(t);
-    const auto kernel = tiered ? by_rowlen(c, key_init_kernel<true, true>, key_init_kernel<true, false>) : key_init_kernel<false, false>;
+    const auto kernel = by_flags([](auto tr, auto v4) { return key_init_kernel<tr, tr && v4>; }, tiered, rows_vec4(c));
     HostTier* h = tiered ? t->tier.get() : nullptr;
     if (launch(c, {warp_grid(c, (size_t)max_new), 256, 0, c->stream}, kernel, view(t), h ? view(h) : KeyView{}, device_rows(c),
                h ? h->a : RowArrays{}, c->rowlen, h ? h->rel.get() : nullptr, initial_s1(c->cfg), t->seed, t->scale)) return 1;
@@ -910,7 +907,7 @@ static int tier_rebuild(lctr_ctx* c) {
 
 // survivors at or above n_live into the holes below it, for the rows of one table (wscan, holes: evict_move_kernel)
 static int launch_move(lctr_ctx* c, const RowArrays& a, size_t n_live, size_t n, const uint32_t* wscan, const uint32_t* holes) {
-    if (launch(c, {warp_grid(c, n - n_live), 256, 0, c->stream}, by_rowlen(c, evict_move_kernel<true>, evict_move_kernel<false>),
+    if (launch(c, {warp_grid(c, n - n_live), 256, 0, c->stream}, rows_vec4(c) ? evict_move_kernel<true> : evict_move_kernel<false>,
                a, c->rowlen, n_live, n, wscan, holes)) return 1;
     return 0;
 }
@@ -1089,7 +1086,7 @@ int flags_to_list(lctr_ctx* c, const uint8_t* flags, size_t n, uint32_t* list, s
 
 int keys_reset_rows(lctr_ctx* c, size_t lo, size_t hi) {
     if (hi <= lo) return 0;
-    return launch(c, {warp_grid(c, hi - lo), 256, 0, c->stream}, by_rowlen(c, evict_reset_kernel<true>, evict_reset_kernel<false>),
+    return launch(c, {warp_grid(c, hi - lo), 256, 0, c->stream}, rows_vec4(c) ? evict_reset_kernel<true> : evict_reset_kernel<false>,
                   device_rows(c), c->rowlen, lo, hi, initial_s1(c->cfg));
 }
 
@@ -1255,7 +1252,7 @@ static int tier_spill(lctr_ctx* c, const EvTable& dev, size_t m) {
     HostTier* h = c->keys->tier.get();
     KeyIndex& ix = h->ix;
     LCTR_CUDA(cudaMemsetAsync(ix.flags, 0, 3 * sizeof(unsigned int), c->stream));
-    if (launch(c, {warp_grid(c, m), 256, 0, c->stream}, by_rowlen(c, tier_spill_kernel<true>, tier_spill_kernel<false>), dev.rows,
+    if (launch(c, {warp_grid(c, m), 256, 0, c->stream}, rows_vec4(c) ? tier_spill_kernel<true> : tier_spill_kernel<false>, dev.rows,
                m, dev.a, h->a, h->n, c->rowlen, view(h))) return 1;
     LCTR_CUDA(cudaMemcpyAsync(ix.h_flags, ix.flags, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     LCTR_CUDA(cudaStreamSynchronize(c->stream));
@@ -1489,7 +1486,7 @@ int lctr_evict_keys(lctr_ctx* c, uint64_t max_idle, uint64_t max_rows, uint64_t*
     if (launch_move(c, tb.a, n_live, n, t->ev_scan + n_live, t->ev_rows)) return 1;
     // change tracking: the move's destinations, the E(n_live) rows that left from below n_live (the head of ev_rows)
     if (track_mark_rows(c, t->ev_rows, t->ev_scan + n_live, m)) return 1;
-    if (launch(c, {warp_grid(c, m), 256, 0, c->stream}, by_rowlen(c, evict_reset_kernel<true>, evict_reset_kernel<false>), tb.a,
+    if (launch(c, {warp_grid(c, m), 256, 0, c->stream}, rows_vec4(c) ? evict_reset_kernel<true> : evict_reset_kernel<false>, tb.a,
                c->rowlen, n_live, n, initial_s1(c->cfg))) return 1;
     const unsigned long long cnt = n_live;
     LCTR_CUDA(cudaMemcpyAsync(t->count, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, c->stream));

@@ -3,11 +3,42 @@
 #include <map>
 #include <mutex>
 #include <stdlib.h>
+#include <type_traits>
 #include <utility>
 
 #include "common.cuh"
 
 namespace lctr {
+
+// Run-time values to kernel template instances.  pick names the instance (or runs the launch) for compile-time constants;
+// every branch returns the same type, a kernel pointer or a launch's status.  A combination that is not built is folded
+// into the template arguments inside pick, so that it names an instance that is.
+
+// pick(std::bool_constant<b0>(), std::bool_constant<b1>(), ...) for the run-time flags b0, b1, ...
+template <typename Pick>
+auto by_flags(Pick&& pick) {
+    return pick();
+}
+template <typename Pick, typename... B>
+auto by_flags(Pick&& pick, bool b, B... rest) {
+    return b ? by_flags([&](auto... f) { return pick(std::true_type(), f...); }, rest...)
+             : by_flags([&](auto... f) { return pick(std::false_type(), f...); }, rest...);
+}
+
+// pick(std::integral_constant<int, v>()) for v in V0, V1, ..., Vn; any other v takes Vn
+template <int V, int... Vs, typename Pick>
+auto by_value(int v, Pick&& pick) {
+    if constexpr (sizeof...(Vs) == 0) return pick(std::integral_constant<int, V>());
+    else return v == V ? pick(std::integral_constant<int, V>()) : by_value<Vs...>(v, pick);
+}
+
+// the values a kernel is built for, written once for the check that refuses the others and the dispatch among them
+template <int... V>
+struct Built {
+    static bool has(int v) { return ((v == V) || ...); }
+    template <typename Pick>
+    static auto pick(int v, Pick&& p) { return by_value<V...>(v, p); }
+};
 
 // programmatic dependent launches (updater behind the gradient kernel; dense kernels and the NFM backward behind their
 // predecessors): LCTR_PDL=0 turns them off; read per launch, the tests toggle it

@@ -459,9 +459,7 @@ static int launch_mlp_bf16_kernel(lctr_ctx* c, Slot& s, int64_t rb, int B, bool 
     P.w32_last = c->layers[nh].w;
     const unsigned grid = (unsigned)((B + c->mlp_tm - 1) / c->mlp_tm);
     const bool t128 = c->mlp_tm == 128;
-    auto kern = train ? (s.has_rw ? (t128 ? nfm_mlp_fused_kernel<128, true, true> : nfm_mlp_fused_kernel<64, true, true>)
-                                  : (t128 ? nfm_mlp_fused_kernel<128, true> : nfm_mlp_fused_kernel<64, true>))
-                      : (t128 ? nfm_mlp_fused_kernel<128, false> : nfm_mlp_fused_kernel<64, false>);
+    auto kern = by_flags([](auto t, auto tr, auto rw) { return nfm_mlp_fused_kernel<t ? 128 : 64, tr, tr && rw>; }, t128, train, s.has_rw);
     return launch(c, {grid, t128 ? 256u : 128u, c->mlp_smem, c->stream}, kern, P, c->z, c->dz, s.wide, s.label, s.pred, rb, B,
                   c->stat_partial, c->stat_done, out_slot, row_weights(s));
 }

@@ -514,10 +514,9 @@ int launch_mlp_umma(lctr_ctx* c, Slot& s, int64_t rb, int B, double* out_slot, b
     }
     const unsigned grid = (unsigned)((B + umma::kTM - 1) / umma::kTM);
     // one GPU: dependent on the embedding forward in front of it (fm_fused.cu, MODE 2), in a train step and in a score alike
-    const bool sig = P.act == LCTR_ACT_SIGMOID;
-    auto kern = train ? (s.has_rw ? (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, true, true> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, true, true>)
-                                  : (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, true> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, true>))
-                      : (sig ? umma::nfm_mlp_umma_kernel<LCTR_ACT_SIGMOID, false> : umma::nfm_mlp_umma_kernel<LCTR_ACT_TANH, false>);
+    auto kern = by_value<LCTR_ACT_SIGMOID, LCTR_ACT_TANH>(P.act, [&](auto act) {
+        return by_flags([&](auto tr, auto rw) { return umma::nfm_mlp_umma_kernel<act, tr, tr && rw>; }, train, s.has_rw);
+    });
     if (launch(c, {grid, (unsigned)umma::kThreads, c->mlp_umma_smem, c->stream, c->cfg.world == 1}, kern, P, c->z, c->dz, s.wide,
                s.label, s.pred, rb, B, c->stat_partial, c->stat_done, out_slot, row_weights(s)))
         return 1;

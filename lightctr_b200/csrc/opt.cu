@@ -179,34 +179,6 @@ apply_kernel(const uint32_t* __restrict__ list, unsigned int* __restrict__ n_lis
     }
 }
 
-// the sparse apply's instance: Adagrad, FTRL, Adam, RMSprop and Adadelta are specialised on 4-wide rows, every other
-// updater and row shape takes OPT = -1
-template <int LPR, int VEC, int SPL, int U>
-static auto apply_instance(int opt) {
-    if (VEC != 4) return apply_kernel<LPR, VEC, SPL, U, -1>;
-    switch (opt) {
-        case LCTR_OPT_ADAGRAD: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_ADAGRAD>;
-        case LCTR_OPT_FTRL: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_FTRL>;
-        case LCTR_OPT_ADAM: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_ADAM>;
-        case LCTR_OPT_RMSPROP: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_RMSPROP>;
-        case LCTR_OPT_ADADELTA: return apply_kernel<LPR, VEC, SPL, U, LCTR_OPT_ADADELTA>;
-        default: return apply_kernel<LPR, VEC, SPL, U, -1>;
-    }
-}
-template <int VEC>
-static auto apply_pick(int lpr, int spl, int opt) {
-    switch (lpr) {
-        case 1: return apply_instance<1, VEC, 1, 4>(opt);
-        case 2: return apply_instance<2, VEC, 1, 4>(opt);
-        case 4: return apply_instance<4, VEC, 1, 4>(opt);
-        case 8: return apply_instance<8, VEC, 1, 4>(opt);
-        case 16: return apply_instance<16, VEC, 1, 4>(opt);
-        default:
-            return spl == 1 ? apply_instance<32, VEC, 1, 4>(opt) : spl == 2 ? apply_instance<32, VEC, 2, 2>(opt)
-                 : spl == 3 ? apply_instance<32, VEC, 3, 1>(opt) : apply_instance<32, VEC, 4, 1>(opt);
-    }
-}
-
 int launch_apply(lctr_ctx* c, int64_t rows_in_step) {
     OptParams P = make_opt_params(c, rows_in_step);
     const int rowlen = (int)c->rowlen;
@@ -222,8 +194,20 @@ int launch_apply(lctr_ctx* c, int64_t rows_in_step) {
     const unsigned grid = (unsigned)c->sm_count * 2;
     ProfScope prof(c, PROF_APPLY);
     if (launch(c, {grid_a, 256, 0, c->stream}, compact_touched_kernel, c->touched, c->Fl, c->touch_list, c->n_touch)) return 1;
-    return launch(c, {grid, 256, 0, c->stream}, vec == 4 ? apply_pick<4>(lpr, spl, P.opt) : apply_pick<1>(lpr, spl, P.opt),
-                  c->touch_list, c->n_touch, c->apply_done, rowlen, c->W, c->V, c->gW, c->gV, c->s1W, c->s1V, c->s2W, c->s2V, P);
+    // several slices per lane (SPL, unrolled by U = 4 / SPL) only on rows longer than 32 lanes.  Adagrad, FTRL, Adam, RMSprop
+    // and Adadelta are specialised on 4-wide rows; every other updater and row shape takes OPT = -1.
+    auto kern = by_value<1, 2, 4, 8, 16, 32>(lpr, [&](auto L) {
+        return by_value<1, 2, 3, 4>(spl, [&](auto S) {
+            return by_value<4, 1>(vec, [&](auto V) {
+                return by_opt(vec == 4 ? P.opt : -1, [&](auto o) {
+                    constexpr int SPL = L == 32 ? S : 1;
+                    return apply_kernel<L, V, SPL, 4 / SPL, o <= LCTR_OPT_ADADELTA ? o : -1>;
+                });
+            });
+        });
+    });
+    return launch(c, {grid, 256, 0, c->stream}, kern, c->touch_list, c->n_touch, c->apply_done, rowlen, c->W, c->V, c->gW, c->gV,
+                  c->s1W, c->s1V, c->s2W, c->s2V, P);
 }
 
 }  // namespace lctr

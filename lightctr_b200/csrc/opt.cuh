@@ -140,18 +140,9 @@ __device__ __forceinline__ void update_one(const OptParams& P, float corr, float
 // host: snapshot of the hyper-parameters for one step (advances the Adam call counter)
 // pick(std::integral_constant<int, OPT>()) for the updater opt: the instance of a kernel specialised per optimizer
 template <typename Pick>
-auto by_opt(int opt, Pick pick) {
-    switch (opt) {
-        case LCTR_OPT_ADAGRAD: return pick(std::integral_constant<int, LCTR_OPT_ADAGRAD>());
-        case LCTR_OPT_FTRL: return pick(std::integral_constant<int, LCTR_OPT_FTRL>());
-        case LCTR_OPT_ADAM: return pick(std::integral_constant<int, LCTR_OPT_ADAM>());
-        case LCTR_OPT_RMSPROP: return pick(std::integral_constant<int, LCTR_OPT_RMSPROP>());
-        case LCTR_OPT_ADADELTA: return pick(std::integral_constant<int, LCTR_OPT_ADADELTA>());
-        case LCTR_OPT_PS_SGD: return pick(std::integral_constant<int, LCTR_OPT_PS_SGD>());
-        case LCTR_OPT_PS_ADAGRAD: return pick(std::integral_constant<int, LCTR_OPT_PS_ADAGRAD>());
-        case LCTR_OPT_PS_DCASGD: return pick(std::integral_constant<int, LCTR_OPT_PS_DCASGD>());
-        default: return pick(std::integral_constant<int, LCTR_OPT_PS_DCASGDA>());
-    }
+auto by_opt(int opt, Pick&& pick) {
+    return by_value<LCTR_OPT_ADAGRAD, LCTR_OPT_FTRL, LCTR_OPT_ADAM, LCTR_OPT_RMSPROP, LCTR_OPT_ADADELTA, LCTR_OPT_PS_SGD,
+                    LCTR_OPT_PS_ADAGRAD, LCTR_OPT_PS_DCASGD, LCTR_OPT_PS_DCASGDA>(opt, pick);
 }
 
 inline OptParams make_opt_params(lctr_ctx* c, int64_t rows_in_step) {
